@@ -1,4 +1,4 @@
-"""3dobjecttracking_b200 — B200-native (sm_100a) implementation of M3T's per-frame pose-optimisation
+"""3dobjecttracking_b200 — H100-native (sm_90a) implementation of M3T's per-frame pose-optimisation
 hot path behind a C ABI (include/m3t_b200.h), plus the host-side mirrors of the reference interface.
 
 The package name starts with a digit, so import it with

@@ -1,4 +1,4 @@
-"""In-tree builds: the CUDA C-ABI library (sm_100a) and the synthetic-data helper library."""
+"""In-tree builds: the CUDA C-ABI library (sm_90a) and the synthetic-data helper library."""
 from __future__ import annotations
 
 import os
@@ -9,7 +9,7 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 _ROOT = os.path.dirname(_HERE)
 
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++17",
+    "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
     # IEEE single-rounding arithmetic in the order written: keeps control flow (int truncations, line
     # validity) bit-identical to the reference restatement (DESIGN.md "Numerics").
     "-fmad=false", "-prec-div=true", "-prec-sqrt=true", "-ftz=false",

@@ -254,7 +254,7 @@ class Context:
         h = C.c_void_p()
         rc = self.L.m3tb_create(device, max_bodies, max_cameras, max_models, C.byref(h))
         if rc != 0:
-            raise M3TBError(f"m3tb_create failed with status {rc} (no usable sm_100 CUDA device?)")
+            raise M3TBError(f"m3tb_create failed with status {rc} (no usable sm_90 CUDA device?)")
         self.h = h
         self.n_bodies = 0
         if stream is not None:

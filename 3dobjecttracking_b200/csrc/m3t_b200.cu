@@ -105,7 +105,7 @@ struct m3tb_ctx {
   RoiRecord* d_roi = nullptr;             // [max_bodies][2]
   unsigned long long* d_ingest_bytes = nullptr;  // [2]: one counter per ingest launch in flight
   int ingest_bytes_slot = 0;              // the counter of the last ingest launch
-  int sm_count = 148;
+  int sm_count = 132;
   bool ingest_pending = false;            // a pinned frame was handed over since the last k_ingest launch
   // frame prefetch (m3tb_prefetch_frames): second set of image pools / camera tables / ROI records, side stream
   ImagePool color_pool_alt, depth_pool_alt;
@@ -617,7 +617,7 @@ int LaunchTrack(m3tb_ctx* ctx, int iteration, int corr_begin, int corr_end, int 
   } while (0)
   if (cluster > 0) {
     // cluster-fused structures: 256-thread CTAs without ROI tiles, so that two CTAs share an SM and every cluster of
-    // a 32-chain shard is resident at once (with 220 KB tiles only 15 clusters of 8 fit on the 148 SMs)
+    // a 32-chain shard is resident at once (with 220 KB tiles at most 16 clusters of 8 fit on the 132 SMs)
     if (items <= 256) { if (lut_smem) M3TB_LAUNCH_CLUSTER(256, 1, true); else M3TB_LAUNCH_CLUSTER(256, 1, false); }
     else if (items <= 512) { if (lut_smem) M3TB_LAUNCH_CLUSTER(256, 2, true); else M3TB_LAUNCH_CLUSTER(256, 2, false); }
     else return Fail(ctx, M3TB_ERR_UNSUPPORTED, "cluster-fused structures: n_lines_max / n_points_max above 512");
@@ -1212,7 +1212,7 @@ int m3tb_create(int device, int max_bodies, int max_cameras, int max_models, m3t
   if (cudaGetDeviceCount(&n_dev) != cudaSuccess || device < 0 || device >= n_dev) return M3TB_ERR_CUDA;
   cudaDeviceProp prop;
   if (cudaGetDeviceProperties(&prop, device) != cudaSuccess) return M3TB_ERR_CUDA;
-  if (prop.major != 10) return M3TB_ERR_CUDA;  // sm_100a cubin only: no other architecture can run it
+  if (prop.major != 9 || prop.minor != 0) return M3TB_ERR_CUDA;  // sm_90a cubin only: no other architecture can run it
   m3tb_ctx* ctx = new m3tb_ctx();
   ctx->device = device;
   ctx->sm_count = prop.multiProcessorCount;
@@ -1963,8 +1963,8 @@ int m3tb_prefetch_frames(m3tb_ctx* ctx) {
   std::swap(ctx->d_dcams, ctx->d_dcams_alt);
   std::swap(ctx->d_roi, ctx->d_roi_alt);
   // Stream plan. The ingest stream runs the ingests back to back: anything queued on it in front of k_ingest would sit
-  // between two PCIe-bound kernels (r02: two pageable table copies + a memset + the wait for the pose snapshot were
-  // ~45 us of a 0.53 ms step). So the set-up goes to a third stream, beside the ingest in flight: wait for the pose
+  // between two PCIe-bound kernels (two pageable table copies, a memset and the wait for the pose snapshot would
+  // lengthen every end-to-end step). So the set-up goes to a third stream, beside the ingest in flight: wait for the pose
   // snapshot of the last tracking launch (which also orders it behind every reader of the buffers swapped in above: they
   // precede that launch on the main stream), camera tables from pinned staging, counter reset; the ingest stream then
   // waits for one event that is normally long past.
@@ -2002,11 +2002,9 @@ int m3tb_prefetch_frames(m3tb_ctx* ctx) {
   a.n_bodies = ctx->n_bodies;
   // Grid of the prefetch ingest: a quarter of the SMs, CTAs looping over the bodies. k_track2 takes a whole SM per body
   // (1024 threads x 64 registers), so an ingest CTA that sits on an SM keeps a body waiting for as long as the ingest
-  // lasts (~0.5 ms), and whichever kernel is dispatched first wins: with one CTA per body the end-to-end step alternated
-  // between 0.36 and 0.92 ms once both kernels became ready at the same moment. The link does not need more: ~80 KB in
-  // flight saturate it (scripts/probes/pcie_probe.cu), one CTA keeps 16 KB in flight. Measured on the bench workload
-  // (128 bodies, ms per end-to-end step): 12 CTAs 0.65, 20 0.585, 24 0.567, 32 0.518, 37 0.517, 40 0.526, 48 0.546,
-  // 64 0.532, 80 0.546, 128 0.541 - 0.575 (M3TB_INGEST_CTAS overrides).
+  // lasts, and whichever kernel is dispatched first wins: with one CTA per body the end-to-end step time swings widely
+  // once both kernels become ready at the same moment. One CTA keeps 16 KB in flight; a few dozen keep the link busy
+  // (scripts/probes/pcie_probe.cu measures it). M3TB_INGEST_CTAS overrides the grid.
   static const int forced_ctas = [] { const char* e = std::getenv("M3TB_INGEST_CTAS"); return e ? std::atoi(e) : 0; }();
   int ingest_ctas = std::max(16, ctx->sm_count / 4);
   if (forced_ctas > 0) ingest_ctas = forced_ctas;

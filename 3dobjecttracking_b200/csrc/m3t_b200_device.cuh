@@ -1,4 +1,4 @@
-// m3t_b200_device.cuh — device-side data layout and math of the B200 pose-optimisation path.
+// m3t_b200_device.cuh — device-side data layout and math of the H100 pose-optimisation path.
 //
 // One CTA owns one body for a whole tracking step (all correspondence iterations x update
 // iterations); warps own groups of correspondence lines / surface points, lanes own lines.

@@ -13,10 +13,10 @@
 //     local-mode gradient reads its two entries from there by index.
 //   * GetClosestView is the exact pruned search of m3t_b200_views.cuh (~200 instead of 2 x 2562 dot products per
 //     iteration), done by the last warp of each group while the other warps wait at the group's named barrier
-//     (measured: every warp searching redundantly costs 6.4 k cycles of issue slots, one warp ~1.3 k).
+//     (every warp searching redundantly would spend the issue slots of the whole group on the same search).
 //   * CalculateOptimization (6 x 6) runs thread-serially in registers on warp 0 (every lane the same work, no
 //     shuffles in the dependent chain): pivot order from the original diagonal, gather of the permuted matrix,
-//     unrolled left-looking LDL^T, substitutions, Rodrigues, pose products; ~4x shorter than the lane-parallel form.
+//     unrolled left-looking LDL^T, substitutions, Rodrigues, pose products; shorter than the lane-parallel form.
 //
 // Serves the fused entry points (m3tb_tracking_step, m3tb_corr_iteration) and the plain correspondence calls for
 // bodies with <= 512 lines and <= 512 points, no measured occlusion handling, function lookups identical across the
@@ -538,7 +538,7 @@ __global__ void __launch_bounds__(T, 1) k_track2(const __grid_constant__ TrackAr
   if (!gbody.set) return;
   // Per-body parameters, cameras and model headers are read all over the iteration loops. With 225 KB of the SM's
   // 228 KB configured as shared memory the L1 cache is ~3 KB, so from global memory each of those reads is an L2 round
-  // trip (long-scoreboard stalls: 2.6 cycles per issue in the r02 capture); one copy into shared memory instead.
+  // trip (long-scoreboard stalls); one copy into shared memory instead.
   __shared__ BodyDev s_body;
   __shared__ CameraDev s_cams[2];
   __shared__ ModelDev s_models[2];
@@ -916,7 +916,7 @@ __global__ void __launch_bounds__(T, 1) k_track2(const __grid_constant__ TrackAr
         __syncwarp();
         M3TB_STAMP2(stamp_base);  // cross-warp sum + normal equations
         // with two warp groups the depth camera's pose products are left to the point group's leader (below): they are
-        // off the critical path there, and the serial section every warp waits for gets ~700 cycles shorter
+        // off the critical path there, and the serial section every warp waits for gets shorter
         SolveAndUpdateSerial(sh, ccam != nullptr, dcam != nullptr && T == kGroup);
         M3TB_STAMP2(stamp_base);  // solve + pose update + pose products
       }

@@ -56,7 +56,7 @@ class Batch {
   Batch(int device, int max_bodies, int max_cameras, int max_models) {
     if (m3tb_create(device, max_bodies, max_cameras, max_models, &ctx_) != M3TB_OK) {
       ctx_ = nullptr;
-      std::cerr << "m3t_b200::Batch: no usable sm_100 CUDA device / context creation failed" << std::endl;
+      std::cerr << "m3t_b200::Batch: no usable sm_90 CUDA device / context creation failed" << std::endl;
     }
     max_bodies_ = max_bodies;
   }

@@ -1,13 +1,14 @@
 #!/usr/bin/env python
-"""bench.py — pose-opt iterations/s (bodies x corr_iters) of the M3T pose-optimisation hot path on B200.
+"""bench.py — pose-opt iterations/s (bodies x corr_iters) of the M3T pose-optimisation hot path on H100.
 
   python bench.py --gpus N --steps K --warmup W            (N>1: launched by torch.distributed.run, one rank per GPU)
   python bench.py --impl reference ...                      (the CPU arm: the oracle port on the host cores)
+  python bench.py ... --dump-outputs DIR                    (also writes the last timed step's poses to DIR)
 
 A "step" is one Tracker::ExecuteTrackingStep pass (n_corr correspondence iterations x n_update update
 iterations, tracker.cpp:344-361) over this GPU's batch of bodies = ONE launch of the fused kernel k_track.
 Default workload: the per-GPU shard of BASELINE.json configs[3] ("1024 bodies Region+Depth, 512 lines each,
-640x480 RGB-D, sharded 8xB200" -> 128 bodies per GPU, weak scaling), the configuration the metric's
+640x480 RGB-D, sharded 8xH100" -> 128 bodies per GPU, weak scaling), the configuration the metric's
 1/2/4/8-GPU numbers are quoted on; `--workload c2|c3` selects the other configs.
 
 value : whole-job throughput, frames already resident in HBM, timed with CUDA events around each step on the
@@ -64,6 +65,9 @@ def parse_args():
     ap.add_argument("--no-e2e", action="store_true")
     ap.add_argument("--no-parity-check", action="store_true")
     ap.add_argument("--no-secondary", action="store_true", help="skip the short runs of the other BASELINE configs")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the solved poses of the last timed step as DIR/poses.npy (float32, [bodies, 3, 4]; "
+                         "DIR/poses_rank<r>.npy per rank under torchrun), to compare two builds output for output")
     return ap.parse_args()
 
 
@@ -167,9 +171,8 @@ def parity_check(ctx, wl, n_sample=4):
 
 def bind_to_gpu_numa_node(torch, local_rank):
     """Pin this rank's host threads (and therefore, by first touch, the pinned frame buffers it allocates next) to the
-    NUMA node its GPU hangs off. Unbound, the 8 ranks' zero-copy frame reads cross the socket interconnect for half of
-    the GPUs (GPUs 0-3 on node 0, 4-7 on node 1 on the 8-GPU boxes) and the end-to-end step time rose from 0.71 to
-    0.99 ms at N = 8 (SCALE_r01). Returns a description for the JSON line."""
+    NUMA node its GPU hangs off. Unbound, the ranks' zero-copy frame reads cross the socket interconnect for the GPUs
+    attached to the other node, which lengthens the end-to-end step. Returns a description for the JSON line."""
     try:
         prop = torch.cuda.get_device_properties(local_rank)
         bdf = f"{prop.pci_domain_id:04x}:{prop.pci_bus_id:02x}:{prop.pci_device_id:02x}.0"
@@ -194,7 +197,7 @@ def secondary_measurements(args, torch, dist, dev, stream, flush, rank, world):
     step, L2 flushed in between, max over ranks), so that the driver's record carries them next to the headline workload.
     One GPU: configs[1], configs[2] and the per-GPU shard of configs[4] in both joint formulations. N GPUs: configs[4]
     weak-scaled like the headline (32 chains x 8 links per GPU; at N = 8 that is BASELINE's "256 instances sharded
-    8 x B200"; whole chains per rank, no collective on the data path). Short runs: 10 steps each. Called by ALL ranks."""
+    8 x H100"; whole chains per rank, no collective on the data path). Short runs: 10 steps each. Called by ALL ranks."""
     import copy
     pkg = importlib.import_module("3dobjecttracking_b200")
     capi = importlib.import_module("3dobjecttracking_b200.capi")
@@ -262,7 +265,7 @@ def build_workload(args, rank, n_shards=1):
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons while the GPU is under load (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks / throttle reasons while the GPU is under load."""
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.active,clocks_event_reasons.hw_slowdown,"
          "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,"
          "clocks_event_reasons.sw_power_cap")
@@ -319,7 +322,7 @@ def measured_peak_gbs():
         with open(p) as f:
             return float(json.load(f)["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
     except Exception:
-        return 6650.0, "fallback (B200_PROFILING.md 6.65 TB/s)"
+        return 3350.0, "fallback (H100 SXM data sheet, 3.35 TB/s HBM3)"
 
 
 _THREADS = {}
@@ -433,7 +436,7 @@ def run_b200(args):
         os.environ.setdefault("MASTER_ADDR", "127.0.0.1")
         dist.init_process_group("nccl", device_id=torch.device("cuda", local_rank))
     if not torch.cuda.is_available():
-        raise SystemExit("bench.py: no CUDA device - the B200 path has no CPU fallback")
+        raise SystemExit("bench.py: no CUDA device - the H100 path has no CPU fallback")
     torch.cuda.set_device(local_rank)
     dev = torch.device("cuda", local_rank)
     numa = bind_to_gpu_numa_node(torch, local_rank) if world > 1 else {"numa_node": None, "note": "single rank: unbound"}
@@ -453,7 +456,7 @@ def run_b200(args):
     its_per_step = nb * n_corr
     start_poses = torch.from_numpy(np.ascontiguousarray(wl.start_body2world.reshape(nb, 12))).pin_memory()
     poses_np = start_poses.numpy()
-    flush = torch.empty(256 * 1024 * 1024, dtype=torch.uint8, device=dev)  # > 126 MB L2
+    flush = torch.empty(256 * 1024 * 1024, dtype=torch.uint8, device=dev)  # > 50 MB L2
 
     def step():
         ctx.tracking_step(0, n_corr, n_upd)
@@ -483,6 +486,8 @@ def run_b200(args):
         evs.append((e0, e1))
     torch.cuda.synchronize(dev)
     launches = ctx.launch_count - launches0
+    # what the timed path computed in its last step, read before the e2e loop below overwrites the poses
+    last_poses = ctx.get_poses() if args.dump_outputs else None
     barrier()
     total_ms = sum(a.elapsed_time(b) for a, b in evs)
     t = torch.tensor([total_ms], dtype=torch.float64, device=dev)
@@ -630,6 +635,10 @@ def run_b200(args):
                                    "best_step_value": r["best_step_value"], "single_thread_value": r1["value"],
                                    "phase_split_cpu_seconds": r["phase_split_cpu_seconds"]}
         emit(json.dumps(out))
+    if last_poses is not None:
+        os.makedirs(args.dump_outputs, exist_ok=True)
+        name = "poses.npy" if world == 1 else f"poses_rank{rank}.npy"
+        np.save(os.path.join(args.dump_outputs, name), last_poses)
     ctx.close()
     if world > 1:
         dist.destroy_process_group()

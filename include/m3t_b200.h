@@ -1,4 +1,4 @@
-/* m3t_b200.h — C ABI of libm3t_b200: the B200-native (sm_100a) implementation of M3T's
+/* m3t_b200.h — C ABI of libm3t_b200: the H100-native (sm_90a) implementation of M3T's
  * per-frame pose-optimisation hot path (RegionModality correspondence lines + DepthModality
  * point-to-plane -> per-body 6x6 Hessian / 6-gradient -> Tikhonov Gauss-Newton solve -> SE(3) update).
  *
@@ -22,7 +22,7 @@
  *  - one host thread per context (the reference's Calculate* methods are single-threaded as well,
  *    tracker.cpp:251-255). Contexts are independent.
  *  - there is NO CPU fallback: every compute entry point fails with M3TB_ERR_CUDA when no
- *    sm_100-class device is usable.
+ *    sm_90 (H100-class) device is usable.
  */
 #ifndef M3T_B200_H_
 #define M3T_B200_H_
@@ -309,7 +309,7 @@ int m3tb_start_modalities(m3tb_ctx* ctx, int iteration);
 int m3tb_calculate_results(m3tb_ctx* ctx, int iteration);
 
 /* ---- the hot path, fine-grained: mirrors the Modality / Optimizer methods 1:1 (parity, debugging,
- * and the B200 Modality adapters driven by an unmodified m3t::Tracker). g/H may be NULL. ------- */
+ * and the CUDA Modality adapters driven by an unmodified m3t::Tracker). g/H may be NULL. ------- */
 /* RegionModality::CalculateCorrespondences (region_modality.cpp:390-465), all bodies. */
 int m3tb_region_correspondences(m3tb_ctx* ctx, int iteration, int corr_iteration);
 /* RegionModality::CalculateGradientAndHessian (region_modality.cpp:485-558): g[n_bodies][6], H[n_bodies][36]. */

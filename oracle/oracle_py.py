@@ -152,21 +152,33 @@ class Structure(C.Structure):
 _libs = {}
 
 
-def build(native=False):
+def build(native=False, native_lib=None):
     target = "native" if native else "all"
-    subprocess.run(["make", "-C", _HERE, target], check=True, capture_output=True)
+    extra = [f"NATIVE_LIB={native_lib}"] if native_lib else []
+    subprocess.run(["make", "-C", _HERE, target] + extra, check=True, capture_output=True)
 
 
 def lib(native=False):
-    """native=True: the -O3 -march=native build (timing only; built on the machine it runs on)."""
+    """native=True: the -O3 -march=native build (timing only; built on the machine it runs on, in a temporary
+    directory, so that a read-only source tree can run the timed CPU baseline)."""
     key = "native" if native else "strict"
     if key in _libs:
         return _libs[key]
-    name = "libm3t_oracle_native.so" if native else "libm3t_oracle.so"
-    path = os.path.join(_HERE, name)
-    if native or not os.path.exists(path):
-        build(native)
-    L = C.CDLL(path)
+    if native:
+        import shutil
+        import tempfile
+        tmp = tempfile.mkdtemp(prefix="m3t_oracle_native_")
+        try:
+            path = os.path.join(tmp, "libm3t_oracle_native.so")
+            build(True, path)
+            L = C.CDLL(path)
+        finally:
+            shutil.rmtree(tmp, ignore_errors=True)  # the loaded library stays mapped
+    else:
+        path = os.path.join(_HERE, "libm3t_oracle.so")
+        if not os.path.exists(path):
+            build()
+        L = C.CDLL(path)
     L.orc_region_params_default.argtypes = [C.POINTER(RegionParams)]
     L.orc_depth_params_default.argtypes = [C.POINTER(DepthParams)]
     L.orc_pose_multiply.argtypes = [fp, fp, fp]

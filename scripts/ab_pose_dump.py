@@ -1,5 +1,5 @@
 """Runs three frames of the c4 workload through the library M3TB_LIB names (default: the in-tree build) and dumps the poses
-and the per-line / per-point state: variants that claim to be bit-exact must produce identical files (scripts/gpu_ab2.sh)."""
+and the per-line / per-point state: variants that claim to be bit-exact must produce identical files."""
 import os, sys, importlib
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import numpy as np

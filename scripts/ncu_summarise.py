@@ -1,15 +1,16 @@
-"""Turns one `ncu --set full --import-source on` capture of the fused kernel into the tracked evidence files:
+"""Turns one `ncu --set full --import-source on` capture of the fused kernel into evidence files (kept out of git):
   profiles/<tag>_ncu_full_summary.json   key metrics of the captured launch
   profiles/<tag>_ncu_raw.csv             the full --page raw export
   profiles/<tag>_source_hotspots.txt     warp-stall samples and executed instructions per CUDA source line (top 40)
   profiles/traffic.json                  dram bytes per launch, tied to the sha of the kernel sources (bench.py reads it)
-usage: python scripts/ncu_summarise.py gpurun_out/prof_k_track2.ncu-rep r02_k_track2 [workload-key]"""
+usage: python scripts/ncu_summarise.py <capture>.ncu-rep <tag> [workload-key]"""
 import csv, io, json, os, subprocess, sys, collections
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 rep, tag = sys.argv[1], sys.argv[2]
 key = sys.argv[3] if len(sys.argv) > 3 else "c4"
+os.makedirs(os.path.join(ROOT, "profiles"), exist_ok=True)
 raw = subprocess.run(["ncu", "-i", rep, "--page", "raw", "--csv"], capture_output=True, text=True).stdout
 open(os.path.join(ROOT, "profiles", f"{tag}_ncu_raw.csv"), "w").write(raw)
 rows = list(csv.reader(io.StringIO(raw)))

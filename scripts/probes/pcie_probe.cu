@@ -1,7 +1,7 @@
 // PCIe probe for the ROI ingest (k_ingest): what the link gives to (1) the copy engine, (2) a zero-copy kernel reading a
 // contiguous pinned buffer, (3) the ROI pattern of configs[3] (128 bodies x one 608 B x 202 row colour rectangle + one 256 B
 // x 128 row depth rectangle out of 640x480 frames) with several launch shapes, (4) 256 cudaMemcpy2DAsync calls.
-// build: nvcc -O3 -gencode arch=compute_100a,code=sm_100a -o scripts/probes/pcie_probe scripts/probes/pcie_probe.cu
+// build: nvcc -O3 -gencode arch=compute_90a,code=sm_90a -o scripts/probes/pcie_probe scripts/probes/pcie_probe.cu
 #include <cstdio>
 #include <cstdlib>
 #include <vector>
@@ -74,7 +74,7 @@ int main() {
   }
   {  // (2) zero-copy contiguous
     const size_t n = (64u << 20) / 16;
-    const int grids[3] = {148, 296, 592};
+    const int grids[3] = {132, 264, 528};  // 1, 2, 4 CTAs per SM of an H100 SXM
     for (int g : grids) {
       k_contig<4><<<g, 256, 0, s>>>(reinterpret_cast<const uint4*>(h), reinterpret_cast<uint4*>(d), n);
       CK(cudaEventRecord(e0, s));

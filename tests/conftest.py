@@ -11,7 +11,7 @@ for p in (ROOT, os.path.join(ROOT, "oracle"), os.path.join(ROOT, "tests")):
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a B200 (run by `pytest -m gpu` on the GPU box)")
+    config.addinivalue_line("markers", "gpu: needs an H100 (sm_90a); `pytest -m gpu` runs them")
 
 
 @pytest.fixture(scope="session")

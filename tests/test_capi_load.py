@@ -13,7 +13,7 @@ def _header_symbols():
 
 
 def test_library_exports_every_declared_symbol(pkg, capi):
-    pkg._build.build_cuda()  # in-tree nvcc build (cross-compiles for sm_100a without a GPU)
+    pkg._build.build_cuda()  # in-tree nvcc build (cross-compiles for sm_90a without a GPU)
     lib = ctypes.CDLL(capi.LIB_PATH)
     declared = _header_symbols()
     assert len(declared) >= 35
@@ -38,7 +38,7 @@ def test_defaults_through_the_abi_match_the_oracle(capi, oracle):
 
 
 def test_no_cpu_fallback_without_a_device(capi):
-    """On a box without a usable sm_100 device context creation fails loudly instead of computing on the CPU."""
+    """On a machine without a usable sm_90 device context creation fails loudly instead of computing on the CPU."""
     import torch
     if torch.cuda.is_available():
         import pytest
@@ -48,8 +48,8 @@ def test_no_cpu_fallback_without_a_device(capi):
         capi.Context(0, 1, 1, 1)
 
 
-def test_cuda_library_contains_sm100a_tma_bulk_copy():
-    """The shipped cubin is sm_100a and uses the TMA bulk-copy path (UBLKCP) + mbarrier (SYNCS) for staging."""
+def test_cuda_library_contains_sm90a_tma_bulk_copy():
+    """The shipped cubin is sm_90a and uses the TMA bulk-copy path (UBLKCP) + mbarrier (SYNCS) for staging."""
     import shutil
     import subprocess
     if not shutil.which("cuobjdump"):
@@ -57,5 +57,5 @@ def test_cuda_library_contains_sm100a_tma_bulk_copy():
         pytest.skip("cuobjdump not available")
     so = os.path.join(ROOT, "3dobjecttracking_b200", "csrc", "libm3t_b200.so")
     out = subprocess.run(["cuobjdump", "-sass", so], capture_output=True, text=True).stdout
-    assert "sm_100a" in out
+    assert "sm_90a" in out
     assert "UBLKCP" in out and "SYNCS" in out

@@ -1,6 +1,6 @@
 """Multi-GPU result equality on real devices (VERDICT r01 weak #4): N NCCL ranks, each tracking its shard through the
-C ABI, gathered poses == the single-GPU run of the whole job, bit for bit. Needs >= 2 GPUs (gpurun --gpus 2);
-skipped on a 1-GPU box. The host-side sharding logic alone is covered on CPU by test_sharding_gloo.py."""
+C ABI, gathered poses == the single-GPU run of the whole job, bit for bit. Needs >= 2 GPUs;
+skipped on a 1-GPU machine. The host-side sharding logic alone is covered on CPU by test_sharding_gloo.py."""
 import os
 import subprocess
 import sys
