@@ -52,11 +52,11 @@ for body in (0, slow):
     if both:
         b = c[128:][c[128:] > 0]
         e = np.diff(b)
-        per = 2 + 2 * nu
+        per = 2 + 3 * nu  # view, points; per update: accumulate + reduce, all warps arrived, released
         rows = e[1:1 + nc * per].reshape(nc, per)
         labels = ["view_d", "points"]
         for u in range(nu):
-            labels += [f"acc{u}", f"wait{u}"]
+            labels += [f"acc{u}", f"wait{u}", f"rel{u}"]
         print(f"   point warp: total {b[-1]-b[0]}, start offset vs warp 0 {b[0]-a[0]}; prologue {e[0]}")
         print("   " + " ".join(f"{l:>7}" for l in labels))
         for row in rows:
