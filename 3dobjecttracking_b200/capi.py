@@ -102,7 +102,8 @@ SYMBOLS = [
     "m3tb_n_structures", "m3tb_calculate_consistent_poses", "m3tb_get_link_poses", "m3tb_get_structure_theta",
     "m3tb_set_gradient_hessian", "m3tb_reset_joint_poses", "m3tb_prefetch_frames", "m3tb_detach_frames",
     "m3tb_debug_closest_view", "m3tb_upload_depth_rendering", "m3tb_upload_silhouette_rendering",
-    "m3tb_share_color_histograms", "m3tb_debug_last_launch",
+    "m3tb_share_color_histograms", "m3tb_debug_last_launch", "m3tb_set_body_geometry", "m3tb_set_focused_renderer",
+    "m3tb_attach_renderer", "m3tb_render", "m3tb_get_rendering",
 ]
 
 KERNEL_NAMES = {0: None, 1: "k_track", 2: "k_track2", 3: "k_track_cluster"}
@@ -192,6 +193,11 @@ def lib():
     L.m3tb_get_structure_theta.argtypes = [vp, ci, fp, ci, C.POINTER(ci), C.POINTER(ci)]
     L.m3tb_set_gradient_hessian.argtypes = [vp, ci, fp, fp]
     L.m3tb_debug_last_launch.argtypes = [vp, C.POINTER(LaunchInfo)]
+    L.m3tb_set_body_geometry.argtypes = [vp, ci, fp, ci, fp, C.c_float, ci, ci, ci]
+    L.m3tb_set_focused_renderer.argtypes = [vp, ci, ci, ci, ci, C.c_float, C.c_float, ci, ip, ci, ip, ci]
+    L.m3tb_attach_renderer.argtypes = [vp, ci, ci, ci, ci]
+    L.m3tb_render.argtypes = [vp]
+    L.m3tb_get_rendering.argtypes = [vp, ci, vp, vp, fp, fp, fp, fp, fp, ip]
     _lib = L
     return L
 
@@ -349,6 +355,55 @@ class Context:
         modality = 0 if key.startswith("region") else 1
         f = self.L.m3tb_upload_depth_rendering if key.endswith("depth") else self.L.m3tb_upload_silhouette_rendering
         self._ck(f(self.h, body, modality, C.byref(a)))
+
+    def set_body_geometry(self, body, triangles, geometry2body=None, maximum_body_diameter=None, enable_culling=True,
+                          body_id=0, region_id=0):
+        """Body + RendererGeometry::AddBody: triangles [n,3,3] (metres, geometry frame, counter-clockwise seen from
+        outside). The diameter defaults to twice the largest vertex distance from the body origin."""
+        t = _f32(triangles).reshape(-1, 9)
+        g2b = _f32(np.eye(4)[:3] if geometry2body is None else geometry2body).reshape(12)
+        if maximum_body_diameter is None:
+            v = t.reshape(-1, 3).astype(np.float64) @ g2b.reshape(3, 4)[:, :3].T.astype(np.float64) + g2b.reshape(3, 4)[:, 3]
+            maximum_body_diameter = 2.0 * float(np.linalg.norm(v, axis=1).max())
+        self._ck(self.L.m3tb_set_body_geometry(self.h, body, _p(t), t.shape[0], _p(g2b), maximum_body_diameter,
+                                               int(enable_culling), int(body_id), int(region_id)))
+
+    def set_focused_renderer(self, renderer, camera_kind, camera, geometry_bodies, referenced_bodies, image_size=200,
+                             z_min=0.02, z_max=10.0, id_type="body"):
+        """camera_kind: "color" | "depth" (or 0 | 1); id_type: "body" | "region" (or 0 | 1)."""
+        kind = {"color": 0, "depth": 1}.get(camera_kind, camera_kind)
+        idt = {"body": 0, "region": 1}.get(id_type, id_type)
+        g = np.ascontiguousarray(geometry_bodies, np.int32)
+        r = np.ascontiguousarray(referenced_bodies, np.int32)
+        ip = C.POINTER(C.c_int)
+        self._ck(self.L.m3tb_set_focused_renderer(self.h, renderer, int(kind), camera, image_size, z_min, z_max, int(idt),
+                                                  g.ctypes.data_as(ip), g.size, r.ctypes.data_as(ip), r.size))
+        self._renderer_refs = getattr(self, "_renderer_refs", {})
+        self._renderer_refs[renderer] = (image_size, r.size)
+
+    def attach_renderer(self, body, key, renderer):
+        """key: "region_depth" | "region_silhouette" | "depth_depth" | "depth_silhouette"; renderer -1 detaches."""
+        modality = 0 if key.startswith("region") else 1
+        kind = 0 if key.endswith("depth") else 1
+        self._ck(self.L.m3tb_attach_renderer(self.h, body, modality, kind, renderer))
+
+    def render(self):
+        self._ck(self.L.m3tb_render(self.h))
+
+    def get_rendering(self, renderer):
+        """dict(depth [S,S] u16, silhouette [S,S] u8, corner_u, corner_v, scale, projection_term_a / b (float32),
+        visible [n_referenced] int32)."""
+        S, n_ref = self._renderer_refs[renderer]
+        depth = np.zeros((S, S), np.uint16)
+        sil = np.zeros((S, S), np.uint8)
+        f = [C.c_float(0.0) for _ in range(5)]
+        vis = np.zeros(n_ref, np.int32)
+        self._ck(self.L.m3tb_get_rendering(self.h, renderer, depth.ctypes.data, sil.ctypes.data, *[C.byref(x) for x in f],
+                                           vis.ctypes.data_as(C.POINTER(C.c_int))))
+        out = dict(zip(("corner_u", "corner_v", "scale", "projection_term_a", "projection_term_b"),
+                       (np.float32(x.value) for x in f)))
+        out.update(depth=depth, silhouette=sil, visible=vis)
+        return out
 
     def set_body(self, body, region, depth, optimizer, region_model=0, depth_model=0, color_camera=0, depth_camera=0):
         self._ck(self.L.m3tb_set_body(self.h, body, C.byref(region) if region is not None else None,

@@ -8,10 +8,12 @@
 #include <cstddef>
 #include <cstdio>
 #include <cstdlib>
+#include <array>
 #include <cstring>
 #include <string>
 #include <vector>
 
+#include "m3t_b200_render.cuh"
 #include "m3t_b200_structures.cuh"
 #include "m3t_b200_kernels.cuh"
 #include "m3t_b200_views.cuh"
@@ -69,6 +71,9 @@ struct ModelAlloc {
   float4* cluster_info = nullptr;
   float4* sorted_views = nullptr;
 };
+
+// which device renderers one k_render launch draws
+enum RenderList { kRenderAll = 0, kRenderAttached, kRenderRegion, kRenderLists };
 
 }  // namespace
 
@@ -163,6 +168,31 @@ struct m3tb_ctx {
   float* d_theta = nullptr;
   int* d_struct_status = nullptr;
   size_t struct_smem = 0;
+
+  // device renderers (m3tb_set_body_geometry / m3tb_set_focused_renderer / m3tb_attach_renderer, k_render)
+  std::vector<GeometryDev> h_geometry;       // [max_bodies]
+  std::vector<float*> geometry_alloc;        // [max_bodies] device triangle soups
+  GeometryDev* d_geometry = nullptr;
+  struct RendererHost {
+    RendererDev dev;
+    std::vector<int> geometry, referenced;
+    bool rendered = false;  // images / records exist (m3tb_get_rendering)
+  };
+  std::vector<RendererHost> renderers;       // dense ids
+  std::vector<std::array<int, RS_COUNT>> attached;  // per body and renderer slot: the device renderer feeding it, or -1
+  std::vector<std::array<char, RS_COUNT>> attach_uploaded;  // the slot's record went to d_bodies once (k_render owns it)
+  bool render_dirty = true;                  // the renderer / geometry / attachment tables changed
+  RendererDev* d_renderers = nullptr;
+  int* d_render_lists = nullptr;             // geometry_bodies | referenced_bodies | render_list
+  int* d_visible = nullptr;
+  RenderOutDev* d_render_out = nullptr;
+  RenderAttachDev* d_attach = nullptr;
+  int n_attached = 0;                        // slots with a device renderer (0: every launch is as without renderers)
+  int n_attach = 0, n_geometry_list = 0, n_referenced_list = 0;
+  int render_n[kRenderLists] = {};           // renderers in each RenderList
+  size_t render_smem[kRenderLists] = {};     // z-buffer bytes of the largest renderer of each list
+  std::vector<int> render_list[kRenderLists];  // host copies of the lists
+  size_t render_capacity[4] = {0, 0, 0, 0};  // renderers, list ints, attachments, visible flags
 };
 
 namespace {
@@ -257,9 +287,30 @@ int EnsureState(m3tb_ctx* ctx) {
 }
 
 int SyncTables(m3tb_ctx* ctx) {
-  if (ctx->bodies_dirty) {
+  if (ctx->bodies_dirty && ctx->n_attached == 0) {
     CU(cudaMemcpyAsync(ctx->d_bodies, ctx->h_bodies.data(), sizeof(BodyDev) * ctx->max_bodies, cudaMemcpyHostToDevice,
                        ctx->stream));
+    ctx->bodies_dirty = false;
+  } else if (ctx->bodies_dirty) {
+    // k_render writes the records of the slots a device renderer feeds: after their first upload (image pointer, size,
+    // pitch; visible = 0 until rendered) the host copy, which never learns corner / scale / visible, must not replace them
+    for (int b = 0; b < ctx->max_bodies; ++b) {
+      const auto& at = ctx->attached[b];
+      auto& up = ctx->attach_uploaded[b];
+      bool keep_any = false;
+      for (int s = 0; s < RS_COUNT; ++s) keep_any = keep_any || (at[s] >= 0 && up[s]);
+      BodyDev* dst = ctx->d_bodies + b;
+      const BodyDev* src = ctx->h_bodies.data() + b;
+      if (!keep_any) {
+        CU(cudaMemcpyAsync(dst, src, sizeof(BodyDev), cudaMemcpyHostToDevice, ctx->stream));
+      } else {
+        CU(cudaMemcpyAsync(dst, src, offsetof(BodyDev, rend), cudaMemcpyHostToDevice, ctx->stream));
+        for (int s = 0; s < RS_COUNT; ++s)
+          if (!(at[s] >= 0 && up[s]))
+            CU(cudaMemcpyAsync(&dst->rend[s], &src->rend[s], sizeof(RenderingDev), cudaMemcpyHostToDevice, ctx->stream));
+      }
+      for (int s = 0; s < RS_COUNT; ++s) up[s] = at[s] >= 0;
+    }
     ctx->bodies_dirty = false;
   }
   if (ctx->cams_dirty) {
@@ -335,6 +386,7 @@ int LaunchIngestIfPending(m3tb_ctx* ctx) {
 }
 
 int SyncStructures(m3tb_ctx* ctx);
+int LaunchRender(m3tb_ctx* ctx, int which);
 
 // cuTensorMapEncodeTiled through the runtime (libcuda is not linked: the library must load on machines without a driver)
 PFN_cuTensorMapEncodeTiled_v12000 TensorMapEncoder() {
@@ -823,7 +875,8 @@ int ClusterLinks(m3tb_ctx* ctx) {
 int StructureStep(m3tb_ctx* ctx, int iteration, int corr_begin, int corr_end, int n_update) {
   int rc0 = SyncStructures(ctx);
   if (rc0) return rc0;
-  if (const int nl = ClusterLinks(ctx)) {
+  const bool render = ctx->n_attached > 0;  // device renderers refresh their images before every correspondence iteration
+  if (const int nl = render ? 0 : ClusterLinks(ctx)) {
     // fused: the whole corr x update loop nest in ONE launch, one cluster per structure, CalculateOptimization over
     // distributed shared memory
     if (n_update > 0)
@@ -833,6 +886,10 @@ int StructureStep(m3tb_ctx* ctx, int iteration, int corr_begin, int corr_end, in
                          nl);
   }
   for (int corr = corr_begin; corr < corr_end; ++corr) {
+    if (render) {
+      int rc = LaunchRender(ctx, kRenderAttached);
+      if (rc) return rc;
+    }
     if (n_update == 0) {
       int rc = LaunchTrack(ctx, iteration, corr, corr + 1, 0, 0, PH_REGION_CORR | PH_DEPTH_CORR | PH_STORE_REGION | PH_STORE_DEPTH);
       if (rc) return rc;
@@ -940,6 +997,117 @@ int LaunchHistogram(m3tb_ctx* ctx, int mode, int iteration) {
     CU(cudaGetLastError());
     ctx->launches++;
   }
+  return M3TB_OK;
+}
+
+// Grows a device table to hold `n` elements (contents are rewritten by the caller).
+template <typename T>
+int EnsureCapacity(m3tb_ctx* ctx, T*& ptr, size_t& capacity, size_t n) {
+  if (n <= capacity && ptr) return M3TB_OK;
+  CU(cudaStreamSynchronize(ctx->stream));  // a launch in flight may still read the old table
+  cudaFree(ptr);
+  ptr = nullptr;
+  capacity = std::max<size_t>(n, 16);
+  CU(cudaMalloc(&ptr, sizeof(T) * capacity));
+  return M3TB_OK;
+}
+
+// Flattens the renderer, list and attachment tables and uploads them with the geometry table.
+int SyncRenderTables(m3tb_ctx* ctx) {
+  if (!ctx->render_dirty) return M3TB_OK;
+  const int nr = int(ctx->renderers.size());
+  std::vector<RendererDev> devs(nr);
+  std::vector<int> geo, ref;
+  for (int r = 0; r < nr; ++r) {
+    auto& h = ctx->renderers[r];
+    h.dev.first_geometry = int(geo.size());
+    h.dev.n_geometry = int(h.geometry.size());
+    h.dev.first_referenced = int(ref.size());
+    h.dev.n_referenced = int(h.referenced.size());
+    geo.insert(geo.end(), h.geometry.begin(), h.geometry.end());
+    ref.insert(ref.end(), h.referenced.begin(), h.referenced.end());
+    devs[r] = h.dev;
+  }
+  std::vector<RenderAttachDev> att;
+  for (int b = 0; b < ctx->max_bodies; ++b)
+    for (int s = 0; s < RS_COUNT; ++s) {
+      const int r = ctx->attached[b][s];
+      if (r < 0) continue;
+      const auto& L = ctx->renderers[r].referenced;
+      const int k = int(std::find(L.begin(), L.end(), b) - L.begin());
+      att.push_back({b, s, r, k});
+    }
+  // lists: geometry_bodies | referenced_bodies | the three render lists (RenderList)
+  std::vector<int> lists(geo);
+  lists.insert(lists.end(), ref.begin(), ref.end());
+  for (int pass = 0; pass < kRenderLists; ++pass) {
+    ctx->render_smem[pass] = 0;
+    ctx->render_n[pass] = 0;
+    ctx->render_list[pass].clear();
+  }
+  for (int pass = 0; pass < kRenderLists; ++pass)
+    for (int r = 0; r < nr; ++r) {
+      bool use = pass == kRenderAll;
+      for (const auto& x : att)
+        use = use || (x.renderer == r && (pass == kRenderAttached || x.slot == RS_REGION_DEPTH || x.slot == RS_REGION_SILHOUETTE));
+      if (!use) continue;
+      lists.push_back(r);
+      ctx->render_list[pass].push_back(r);
+      ctx->render_n[pass]++;
+      ctx->render_smem[pass] = std::max(ctx->render_smem[pass], size_t(devs[r].image_size) * devs[r].image_size * sizeof(uint32_t));
+    }
+  int rc = EnsureCapacity(ctx, ctx->d_renderers, ctx->render_capacity[0], size_t(std::max(nr, 1)));
+  if (!rc) rc = EnsureCapacity(ctx, ctx->d_render_lists, ctx->render_capacity[1], std::max<size_t>(lists.size(), 1));
+  if (!rc) rc = EnsureCapacity(ctx, ctx->d_attach, ctx->render_capacity[2], std::max<size_t>(att.size(), 1));
+  if (!rc) rc = EnsureCapacity(ctx, ctx->d_visible, ctx->render_capacity[3], std::max<size_t>(ref.size(), 1));
+  if (rc) return rc;
+  if (!ctx->d_render_out) CU(cudaMalloc(&ctx->d_render_out, sizeof(RenderOutDev) * size_t(4 * ctx->max_bodies)));
+  if (!ctx->d_geometry) CU(cudaMalloc(&ctx->d_geometry, sizeof(GeometryDev) * ctx->max_bodies));
+  CU(cudaStreamSynchronize(ctx->stream));  // the host vectors below are temporaries (set-up path, not per step)
+  if (nr) CU(cudaMemcpy(ctx->d_renderers, devs.data(), sizeof(RendererDev) * nr, cudaMemcpyHostToDevice));
+  if (!lists.empty()) CU(cudaMemcpy(ctx->d_render_lists, lists.data(), sizeof(int) * lists.size(), cudaMemcpyHostToDevice));
+  if (!att.empty()) CU(cudaMemcpy(ctx->d_attach, att.data(), sizeof(RenderAttachDev) * att.size(), cudaMemcpyHostToDevice));
+  CU(cudaMemcpy(ctx->d_geometry, ctx->h_geometry.data(), sizeof(GeometryDev) * ctx->max_bodies, cudaMemcpyHostToDevice));
+  ctx->n_attach = int(att.size());
+  for (auto& h : ctx->renderers) h.rendered = false;  // offsets / visible flags moved: read-back waits for the next render
+  ctx->n_geometry_list = int(geo.size());
+  ctx->n_referenced_list = int(ref.size());
+  ctx->render_dirty = false;
+  return M3TB_OK;
+}
+
+// FocusedRenderer::StartRendering of the renderers of one RenderList: every device renderer (m3tb_render), those attached
+// to a modality (Modality::correspondence_renderer_ptrs, before each correspondence iteration) or those attached to a
+// region modality (RegionModality::start_modality_renderer_ptrs / results_renderer_ptrs; DepthModality has none there).
+// One k_render launch; the images and the attached slots' records are current when the launch has run.
+int LaunchRender(m3tb_ctx* ctx, int which) {
+  int rc = SyncTables(ctx);  // pending body-table uploads go first: k_render then owns the attached records
+  if (!rc) rc = SyncRenderTables(ctx);
+  if (rc) return rc;
+  const int n = ctx->render_n[which];
+  const size_t smem = ctx->render_smem[which];
+  if (n == 0) return M3TB_OK;
+  const int* d_list = ctx->d_render_lists + ctx->n_geometry_list + ctx->n_referenced_list;
+  for (int k = 0; k < which; ++k) d_list += ctx->render_n[k];
+  RenderArgs a;
+  a.renderers = ctx->d_renderers;
+  a.render_list = d_list;
+  a.geometry = ctx->d_geometry;
+  a.geometry_bodies = ctx->d_render_lists;
+  a.referenced_bodies = ctx->d_render_lists + ctx->n_geometry_list;
+  a.poses = ctx->d_poses;
+  a.color_cams = ctx->d_ccams;
+  a.depth_cams = ctx->d_dcams;
+  a.out = ctx->d_render_out;
+  a.visible = ctx->d_visible;
+  a.bodies = ctx->d_bodies;
+  a.attach = ctx->d_attach;
+  a.n_attach = ctx->n_attach;
+  CU(cudaFuncSetAttribute(k_render, cudaFuncAttributeMaxDynamicSharedMemorySize, int(smem)));
+  k_render<<<unsigned(n), kRenderThreads, smem, ctx->stream>>>(a);
+  CU(cudaGetLastError());
+  ctx->launches++;
+  for (int r : ctx->render_list[which]) ctx->renderers[r].rendered = true;
   return M3TB_OK;
 }
 
@@ -1240,6 +1408,11 @@ int m3tb_create(int device, int max_bodies, int max_cameras, int max_models, m3t
   ctx->private_color.assign(max_cameras, nullptr);
   ctx->private_depth.assign(max_cameras, nullptr);
   ctx->bin_stale.assign(max_cameras, 1);
+  ctx->h_geometry.assign(max_bodies, GeometryDev());
+  std::memset(ctx->h_geometry.data(), 0, sizeof(GeometryDev) * max_bodies);
+  ctx->geometry_alloc.assign(max_bodies, nullptr);
+  ctx->attached.assign(max_bodies, std::array<int, RS_COUNT>{-1, -1, -1, -1});
+  ctx->attach_uploaded.assign(max_bodies, std::array<char, RS_COUNT>{0, 0, 0, 0});
   if (const char* e = std::getenv("M3TB_NO_TILES")) ctx->use_tiles = !(e[0] == '1');
   if (const char* e = std::getenv("M3TB_NO_ROI_INGEST")) ctx->roi_ingest = !(e[0] == '1');
   if (const char* e = std::getenv("M3TB_CLUSTER")) ctx->use_clusters = e[0] == '1';
@@ -1317,6 +1490,10 @@ int m3tb_destroy(m3tb_ctx* ctx) {
   cudaFree(ctx->d_structures); cudaFree(ctx->d_links); cudaFree(ctx->d_links_default); cudaFree(ctx->d_constraints);
   cudaFree(ctx->d_gh_link);
   cudaFree(ctx->d_theta); cudaFree(ctx->d_struct_status); cudaFree(ctx->d_hist_owner); cudaFree(ctx->d_hist_groups);
+  for (auto p : ctx->geometry_alloc) cudaFree(p);
+  for (auto& r : ctx->renderers) { cudaFree(r.dev.depth); cudaFree(r.dev.silhouette); }
+  cudaFree(ctx->d_geometry); cudaFree(ctx->d_renderers); cudaFree(ctx->d_render_lists); cudaFree(ctx->d_visible);
+  cudaFree(ctx->d_render_out); cudaFree(ctx->d_attach);
   delete ctx;
   return M3TB_OK;
 }
@@ -1609,15 +1786,26 @@ int m3tb_tracking_step(m3tb_ctx* ctx, int iteration, int n_corr_iterations, int 
   CHECK_CTX();
   if (n_corr_iterations < 0 || n_update_iterations < 0) return Fail(ctx, M3TB_ERR_INVALID, "negative iteration count");
   if (HasStructures(ctx)) return StructureStep(ctx, iteration, 0, n_corr_iterations, n_update_iterations);
-  return LaunchTrack(ctx, iteration, 0, n_corr_iterations, n_update_iterations, 0,
-                     PH_REGION_CORR | PH_DEPTH_CORR | PH_REGION_GH | PH_DEPTH_GH | PH_SOLVE | PH_STORE_REGION |
-                         PH_STORE_DEPTH);
+  const unsigned phases = PH_REGION_CORR | PH_DEPTH_CORR | PH_REGION_GH | PH_DEPTH_GH | PH_SOLVE | PH_STORE_REGION |
+                          PH_STORE_DEPTH;
+  if (ctx->n_attached == 0) return LaunchTrack(ctx, iteration, 0, n_corr_iterations, n_update_iterations, 0, phases);
+  // device renderers: Tracker::CalculateCorrespondences renders before every correspondence iteration (tracker.cpp:447-456)
+  for (int corr = 0; corr < n_corr_iterations; ++corr) {
+    int rc = LaunchRender(ctx, kRenderAttached);
+    if (!rc) rc = LaunchTrack(ctx, iteration, corr, corr + 1, n_update_iterations, 0, phases);
+    if (rc) return rc;
+  }
+  return M3TB_OK;
 }
 
 int m3tb_corr_iteration(m3tb_ctx* ctx, int iteration, int corr_iteration, int n_update_iterations) {
   CHECK_CTX();
   if (corr_iteration < 0 || n_update_iterations < 0) return Fail(ctx, M3TB_ERR_INVALID, "negative iteration count");
   if (HasStructures(ctx)) return StructureStep(ctx, iteration, corr_iteration, corr_iteration + 1, n_update_iterations);
+  if (ctx->n_attached > 0) {
+    int rc = LaunchRender(ctx, kRenderAttached);
+    if (rc) return rc;
+  }
   return LaunchTrack(ctx, iteration, corr_iteration, corr_iteration + 1, n_update_iterations, 0,
                      PH_REGION_CORR | PH_DEPTH_CORR | PH_REGION_GH | PH_DEPTH_GH | PH_SOLVE | PH_STORE_REGION |
                          PH_STORE_DEPTH);
@@ -1627,11 +1815,19 @@ int m3tb_start_modalities(m3tb_ctx* ctx, int iteration) {
   CHECK_CTX();
   for (int b = 0; b < ctx->n_bodies; ++b) ctx->h_bodies[b].first_iteration = iteration;
   ctx->bodies_dirty = true;
+  if (ctx->n_attached > 0) {  // Tracker::StartModalities renders first (tracker.cpp:430-434)
+    int rc = LaunchRender(ctx, kRenderRegion);
+    if (rc) return rc;
+  }
   return LaunchHistogram(ctx, 0, iteration);
 }
 
 int m3tb_calculate_results(m3tb_ctx* ctx, int iteration) {
   CHECK_CTX();
+  if (ctx->n_attached > 0) {  // Tracker::CalculateResults renders first (tracker.cpp:503-506)
+    int rc = LaunchRender(ctx, kRenderRegion);
+    if (rc) return rc;
+  }
   return LaunchHistogram(ctx, 1, iteration);
 }
 
@@ -2029,6 +2225,8 @@ static int UploadRendering(m3tb_ctx* ctx, int body, int slot, const m3tb_renderi
   if (body < 0 || body >= ctx->max_bodies || !r || !r->image || r->image_size <= 0 ||
       r->pitch < size_t(r->image_size) * bytes_per_pixel || !(r->scale > 0.0f))
     return Fail(ctx, M3TB_ERR_INVALID, "bad rendering arguments");
+  if (ctx->attached[body][slot] >= 0)
+    return Fail(ctx, M3TB_ERR_INVALID, "a device renderer is attached to this slot (m3tb_attach_renderer(..., -1) detaches it)");
   RenderingDev& d = ctx->h_bodies[body].rend[slot];
   const unsigned pitch = unsigned(Align(size_t(r->image_size) * bytes_per_pixel, 16));
   if (!d.image || d.image_size != r->image_size) {
@@ -2068,6 +2266,179 @@ int m3tb_upload_silhouette_rendering(m3tb_ctx* ctx, int body, int modality, cons
   CHECK_CTX();
   if (modality != 0 && modality != 1) return Fail(ctx, M3TB_ERR_INVALID, "modality must be 0 (region) or 1 (depth)");
   return UploadRendering(ctx, body, modality == 0 ? RS_REGION_SILHOUETTE : RS_DEPTH_SILHOUETTE, rendering, 1);
+}
+
+int m3tb_set_body_geometry(m3tb_ctx* ctx, int body, const float* triangles, int n_triangles,
+                           const float geometry2body[12], float maximum_body_diameter, int enable_culling, int body_id,
+                           int region_id) {
+  CHECK_CTX();
+  if (body < 0 || body >= ctx->max_bodies) return Fail(ctx, M3TB_ERR_INVALID, "body index out of range");
+  if (!triangles || n_triangles < 1 || !geometry2body || !(maximum_body_diameter > 0.0f) ||
+      !std::isfinite(maximum_body_diameter))
+    return Fail(ctx, M3TB_ERR_INVALID, "bad geometry arguments");
+  if (body_id < 0 || body_id > 255 || region_id < 0 || region_id > 255)
+    return Fail(ctx, M3TB_ERR_INVALID, "body_id / region_id must be uint8 values");
+  GeometryDev& G = ctx->h_geometry[body];
+  if (ctx->geometry_alloc[body] && G.n_triangles != n_triangles) {
+    CU(cudaStreamSynchronize(ctx->stream));  // a render in flight may still read the old soup
+    cudaFree(ctx->geometry_alloc[body]);
+    ctx->geometry_alloc[body] = nullptr;
+  }
+  if (!ctx->geometry_alloc[body]) CU(cudaMalloc(&ctx->geometry_alloc[body], sizeof(float) * 9 * size_t(n_triangles)));
+  CU(cudaMemcpyAsync(ctx->geometry_alloc[body], triangles, sizeof(float) * 9 * size_t(n_triangles), cudaMemcpyHostToDevice,
+                     ctx->stream));
+  CU(cudaStreamSynchronize(ctx->stream));  // the caller's triangles are free again
+  G.triangles = ctx->geometry_alloc[body];
+  G.n_triangles = n_triangles;
+  std::memcpy(G.geometry2body, geometry2body, sizeof(G.geometry2body));
+  G.radius = 0.5f * maximum_body_diameter;  // FocusedRenderer::CalculateProjectionMatrix (renderer.cpp:356)
+  G.enable_culling = enable_culling ? 1 : 0;
+  G.body_id = body_id;
+  G.region_id = region_id;
+  G.set = 1;
+  ctx->render_dirty = true;
+  return M3TB_OK;
+}
+
+int m3tb_set_focused_renderer(m3tb_ctx* ctx, int renderer, int camera_kind, int camera, int image_size, float z_min,
+                              float z_max, int id_type, const int* geometry_bodies, int n_geometry,
+                              const int* referenced_bodies, int n_referenced) {
+  CHECK_CTX();
+  if (renderer < 0 || renderer > int(ctx->renderers.size()) || renderer >= 4 * ctx->max_bodies)
+    return Fail(ctx, M3TB_ERR_INVALID, "renderer ids must be dense (0..n) and below 4 * max_bodies");
+  if (camera_kind != 0 && camera_kind != 1) return Fail(ctx, M3TB_ERR_INVALID, "camera_kind must be 0 (colour) or 1 (depth)");
+  if (camera < 0 || camera >= ctx->max_cameras || !(camera_kind == 0 ? ctx->h_ccams : ctx->h_dcams)[camera].set)
+    return Fail(ctx, M3TB_ERR_INVALID, "camera not set");
+  if (image_size > kRenderMaxImageSize)
+    return Fail(ctx, M3TB_ERR_UNSUPPORTED, "image_size above " + std::to_string(kRenderMaxImageSize) +
+                                               " (the z-buffer lives in shared memory)");
+  if (image_size < 1 || !(z_min > 0.0f) || !(z_max > z_min) || !std::isfinite(z_max))
+    return Fail(ctx, M3TB_ERR_INVALID, "bad image_size / z_min / z_max");
+  if (id_type != RID_BODY && id_type != RID_REGION) return Fail(ctx, M3TB_ERR_INVALID, "id_type must be 0 (BODY) or 1 (REGION)");
+  if (!geometry_bodies || n_geometry < 1 || n_geometry > 65535 || !referenced_bodies || n_referenced < 1)
+    return Fail(ctx, M3TB_ERR_INVALID, "a renderer needs geometry bodies and referenced bodies");
+  for (int pass = 0; pass < 2; ++pass) {
+    const int* L = pass == 0 ? geometry_bodies : referenced_bodies;
+    const int n = pass == 0 ? n_geometry : n_referenced;
+    for (int k = 0; k < n; ++k) {
+      if (L[k] < 0 || L[k] >= ctx->max_bodies || !ctx->h_geometry[L[k]].set)
+        return Fail(ctx, M3TB_ERR_INVALID, "body " + std::to_string(L[k]) + " has no geometry (m3tb_set_body_geometry)");
+      for (int q = 0; q < k; ++q)
+        if (L[q] == L[k]) return Fail(ctx, M3TB_ERR_INVALID, "body listed twice");
+    }
+  }
+  if (renderer < int(ctx->renderers.size()))
+    for (const auto& at : ctx->attached)
+      for (int r : at)
+        if (r == renderer) return Fail(ctx, M3TB_ERR_INVALID, "renderer is attached to a modality: detach it first");
+  if (renderer == int(ctx->renderers.size())) {
+    m3tb_ctx::RendererHost h;
+    std::memset(&h.dev, 0, sizeof(h.dev));
+    ctx->renderers.push_back(h);
+  }
+  auto& h = ctx->renderers[renderer];
+  RendererDev& R = h.dev;
+  if (R.image_size != image_size) {
+    CU(cudaStreamSynchronize(ctx->stream));
+    cudaFree(R.depth);
+    cudaFree(R.silhouette);
+    R.depth = nullptr;
+    R.silhouette = nullptr;
+    R.depth_pitch = unsigned(Align(size_t(image_size) * 2, 16));
+    R.silhouette_pitch = unsigned(Align(size_t(image_size), 16));
+    CU(cudaMalloc(&R.depth, size_t(R.depth_pitch) * image_size));
+    CU(cudaMalloc(&R.silhouette, size_t(R.silhouette_pitch) * image_size));
+    CU(cudaMemsetAsync(R.depth, 0xff, size_t(R.depth_pitch) * image_size, ctx->stream));  // cleared: depth 1.0
+    CU(cudaMemsetAsync(R.silhouette, 0, size_t(R.silhouette_pitch) * image_size, ctx->stream));
+  }
+  R.camera_kind = camera_kind;
+  R.camera = camera;
+  R.image_size = image_size;
+  R.id_type = id_type;
+  R.z_min = z_min;
+  R.z_max = z_max;
+  R.set = 1;
+  h.geometry.assign(geometry_bodies, geometry_bodies + n_geometry);
+  h.referenced.assign(referenced_bodies, referenced_bodies + n_referenced);
+  h.rendered = false;
+  ctx->render_dirty = true;
+  return M3TB_OK;
+}
+
+int m3tb_attach_renderer(m3tb_ctx* ctx, int body, int modality, int kind, int renderer) {
+  CHECK_CTX();
+  if (body < 0 || body >= ctx->n_bodies || !ctx->h_bodies[body].set) return Fail(ctx, M3TB_ERR_INVALID, "body not set");
+  if (modality != 0 && modality != 1) return Fail(ctx, M3TB_ERR_INVALID, "modality must be 0 (region) or 1 (depth)");
+  if (kind != 0 && kind != 1) return Fail(ctx, M3TB_ERR_INVALID, "kind must be 0 (depth) or 1 (silhouette)");
+  BodyDev& B = ctx->h_bodies[body];
+  if (!(modality == 0 ? B.has_region : B.has_depth)) return Fail(ctx, M3TB_ERR_INVALID, "body has no such modality");
+  const int slot = modality == 0 ? (kind == 0 ? RS_REGION_DEPTH : RS_REGION_SILHOUETTE)
+                                 : (kind == 0 ? RS_DEPTH_DEPTH : RS_DEPTH_SILHOUETTE);
+  int& cur = ctx->attached[body][slot];
+  if (renderer == -1) {  // DoNotModelOcclusions / DoNotUseRegionChecking / DoNotUseSilhouetteChecking
+    if (cur >= 0) {
+      std::memset(&B.rend[slot], 0, sizeof(RenderingDev));
+      cur = -1;
+      ctx->n_attached--;
+      ctx->bodies_dirty = true;
+      ctx->render_dirty = true;
+    }
+    return M3TB_OK;
+  }
+  if (renderer < 0 || renderer >= int(ctx->renderers.size())) return Fail(ctx, M3TB_ERR_INVALID, "renderer not set");
+  const auto& h = ctx->renderers[renderer];
+  const RendererDev& R = h.dev;
+  // what RegionModality / DepthModality::SetUp require of the renderer (region_modality.cpp:66-86, depth_modality.cpp:56-76)
+  if (R.camera_kind != modality || R.camera != (modality == 0 ? B.color_camera : B.depth_camera))
+    return Fail(ctx, M3TB_ERR_INVALID, "the renderer does not render the modality's camera");
+  if (std::find(h.referenced.begin(), h.referenced.end(), body) == h.referenced.end())
+    return Fail(ctx, M3TB_ERR_INVALID, "the renderer does not reference the body");
+  if (kind == 1 && R.id_type != (modality == 0 ? RID_REGION : RID_BODY))
+    return Fail(ctx, M3TB_ERR_INVALID, modality == 0 ? "region checking needs a silhouette renderer of id_type REGION"
+                                                     : "silhouette checking needs a silhouette renderer of id_type BODY");
+  RenderingDev& d = B.rend[slot];
+  std::memset(&d, 0, sizeof(d));  // visible = 0: the checks stay off until the first render
+  d.image = kind == 1 ? R.silhouette : reinterpret_cast<const uint8_t*>(R.depth);
+  d.image_size = R.image_size;
+  d.pitch = kind == 1 ? R.silhouette_pitch : R.depth_pitch;
+  if (cur < 0) ctx->n_attached++;
+  cur = renderer;
+  ctx->attach_uploaded[body][slot] = 0;
+  ctx->bodies_dirty = true;
+  ctx->render_dirty = true;
+  return M3TB_OK;
+}
+
+int m3tb_render(m3tb_ctx* ctx) {
+  CHECK_CTX();
+  if (ctx->renderers.empty()) return Fail(ctx, M3TB_ERR_NOT_SET_UP, "no device renderer set");
+  return LaunchRender(ctx, kRenderAll);
+}
+
+int m3tb_get_rendering(m3tb_ctx* ctx, int renderer, void* depth_u16, void* silhouette_u8, float* corner_u, float* corner_v,
+                       float* scale, float* projection_term_a, float* projection_term_b, int* visible_flags) {
+  CHECK_CTX();
+  if (renderer < 0 || renderer >= int(ctx->renderers.size())) return Fail(ctx, M3TB_ERR_INVALID, "renderer not set");
+  const auto& h = ctx->renderers[renderer];
+  if (!h.rendered) return Fail(ctx, M3TB_ERR_NOT_SET_UP, "renderer has not rendered since it was set");
+  const RendererDev& R = h.dev;
+  const size_t S = size_t(R.image_size);
+  if (depth_u16)
+    CU(cudaMemcpy2DAsync(depth_u16, S * 2, R.depth, R.depth_pitch, S * 2, S, cudaMemcpyDeviceToHost, ctx->stream));
+  if (silhouette_u8)
+    CU(cudaMemcpy2DAsync(silhouette_u8, S, R.silhouette, R.silhouette_pitch, S, S, cudaMemcpyDeviceToHost, ctx->stream));
+  RenderOutDev o;
+  CU(cudaMemcpyAsync(&o, ctx->d_render_out + renderer, sizeof(o), cudaMemcpyDeviceToHost, ctx->stream));
+  if (visible_flags)
+    CU(cudaMemcpyAsync(visible_flags, ctx->d_visible + R.first_referenced, sizeof(int) * R.n_referenced,
+                       cudaMemcpyDeviceToHost, ctx->stream));
+  CU(cudaStreamSynchronize(ctx->stream));
+  if (corner_u) *corner_u = o.corner_u;
+  if (corner_v) *corner_v = o.corner_v;
+  if (scale) *scale = o.scale;
+  if (projection_term_a) *projection_term_a = o.projection_term_a;
+  if (projection_term_b) *projection_term_b = o.projection_term_b;
+  return M3TB_OK;
 }
 
 int m3tb_detach_frames(m3tb_ctx* ctx) {

@@ -10,7 +10,8 @@
 //   m3t::Optimizer::CalculateOptimization              -> m3tb_calculate_optimization
 //   m3t::Tracker::ExecuteTrackingStep                  -> m3tb_tracking_step + m3tb_calculate_results (fast path)
 //
-// Everything the reference has outside this path (renderers, detectors, viewers, texture modality, YAML metafiles,
+// Focused depth / silhouette renderers exist as device renderers (k_render). Everything else the reference has outside
+// this path (full-frame and normal renderers, detectors, viewers, texture modality, YAML metafiles,
 // kinematic constraints) is out of scope here (DESIGN.md). Poses use a minimal Transform3fA (row-major 3x4).
 #ifndef M3T_B200_HPP_
 #define M3T_B200_HPP_
@@ -68,7 +69,7 @@ class Batch {
   m3tb_ctx* ctx() const { return ctx_; }
   bool ok() const { return ctx_ != nullptr; }
 
-  enum PhaseKind { kRegionCorr, kDepthCorr, kRegionGH, kDepthGH, kOptimize, kStart, kResults, kNPhases };
+  enum PhaseKind { kRegionCorr, kDepthCorr, kRegionGH, kDepthGH, kOptimize, kStart, kResults, kRender, kNPhases };
   struct Key {
     int iteration = -1, corr = -1, opt = -1;
     long pose_version = -1;
@@ -85,6 +86,7 @@ class Batch {
   }
   void MarkDone(PhaseKind k, int iteration, int corr, int opt) { done_[k] = Key{iteration, corr, opt, pose_version_}; }
   void PosesChanged() { ++pose_version_; }
+  int NextRenderer() { return n_renderers_++; }
   int NextBody() { return n_bodies_++; }
   int NextColorCamera() { return n_color_++; }
   int NextDepthCamera() { return n_depth_++; }
@@ -97,7 +99,7 @@ class Batch {
 
  private:
   m3tb_ctx* ctx_ = nullptr;
-  int max_bodies_ = 0, n_bodies_ = 0, n_color_ = 0, n_depth_ = 0, n_rmodels_ = 0, n_dmodels_ = 0, n_structures_ = 0;
+  int max_bodies_ = 0, n_bodies_ = 0, n_renderers_ = 0, n_color_ = 0, n_depth_ = 0, n_rmodels_ = 0, n_dmodels_ = 0, n_structures_ = 0;
   long pose_version_ = 0;
   Key done_[kNPhases];
 };
@@ -121,17 +123,46 @@ class Body {
     Check(batch_->ctx(), m3tb_get_poses(batch_->ctx(), index_, 1, body2world_pose_.data()), "Body::body2world_pose");
     return body2world_pose_;
   }
+  // geometry setters (body.h:57-66). The mesh is handed over as the triangle soup Body::SetUp would load from
+  // geometry_path: [n][3][3] floats in metres, geometry frame, counter-clockwise seen from outside.
+  void set_geometry_triangles(const std::vector<float>& triangles) { triangles_ = triangles; }
+  void set_geometry2body_pose(const Transform3fA& p) { geometry2body_pose_ = p; }
+  void set_geometry_enable_culling(bool v) { geometry_enable_culling_ = v; }
+  void set_maximum_body_diameter(float v) { maximum_body_diameter_ = v; }
+  void set_body_id(uint8_t v) { body_id_ = v; }
+  void set_region_id(uint8_t v) { region_id_ = v; }
+  float maximum_body_diameter() const { return maximum_body_diameter_; }
+  uint8_t body_id() const { return body_id_; }
+  uint8_t region_id() const { return region_id_; }
+  // the geometry part of Body::SetUp (body.cpp:201-249): uploads the soup (RendererGeometry::AddBody calls it)
+  bool SetUpGeometry() {
+    if (triangles_.empty() || triangles_.size() % 9 != 0) {
+      std::cerr << "Body " << name_ << " has no geometry" << std::endl;
+      return false;
+    }
+    return Check(batch_->ctx(),
+                 m3tb_set_body_geometry(batch_->ctx(), index_, triangles_.data(), int(triangles_.size() / 9),
+                                        geometry2body_pose_.data(), maximum_body_diameter_, geometry_enable_culling_ ? 1 : 0,
+                                        body_id_, region_id_),
+                 "Body::SetUp");
+  }
 
  private:
   std::string name_;
   std::shared_ptr<Batch> batch_;
   int index_ = 0;
   Transform3fA body2world_pose_;
+  std::vector<float> triangles_;
+  Transform3fA geometry2body_pose_;
+  bool geometry_enable_culling_ = true;
+  float maximum_body_diameter_ = 0.0f;
+  uint8_t body_id_ = 0, region_id_ = 0;
 };
 
 // ---- camera.h --------------------------------------------------------------------------------------------------------
 class Camera {
  public:
+  virtual ~Camera() = default;
   const std::string& name() const { return name_; }
   const Intrinsics& intrinsics() const { return intrinsics_; }
   const Transform3fA& world2camera_pose() const { return world2camera_pose_; }
@@ -286,6 +317,163 @@ class DepthModel : public Model {
   }
 };
 
+// ---- renderer_geometry.h / renderer.h / basic_depth_renderer.h / silhouette_renderer.h: device renderers (k_render) ----
+class RendererGeometry {
+ public:
+  RendererGeometry(const std::string& name, const std::shared_ptr<Batch>& batch) : name_(name), batch_(batch) {}
+  // RendererGeometry::AddBody: uploads the body's triangle soup; bodies are drawn in the order they were added
+  bool AddBody(const std::shared_ptr<Body>& body_ptr) {
+    for (auto& b : body_ptrs_)
+      if (b->name() == body_ptr->name()) {
+        std::cerr << "Body " << body_ptr->name() << " already exists" << std::endl;
+        return false;
+      }
+    if (!body_ptr->SetUpGeometry()) return false;
+    body_ptrs_.push_back(body_ptr);
+    return true;
+  }
+  bool SetUp() { set_up_ = true; return true; }
+  bool set_up() const { return set_up_; }
+  const std::string& name() const { return name_; }
+  const std::vector<std::shared_ptr<Body>>& body_ptrs() const { return body_ptrs_; }
+
+ private:
+  std::string name_;
+  std::shared_ptr<Batch> batch_;
+  std::vector<std::shared_ptr<Body>> body_ptrs_;
+  bool set_up_ = false;
+};
+
+enum class IDType { BODY = 0, REGION = 1 };  // body.h
+
+// FocusedDepthRenderer (renderer.h:199-230). Every device renderer also produces the silhouette image, so the two
+// focused renderer classes below only differ in their defaults.
+class FocusedDepthRenderer {
+ public:
+  virtual ~FocusedDepthRenderer() = default;
+  bool AddReferencedBody(const std::shared_ptr<Body>& body_ptr) {
+    for (auto& b : referenced_body_ptrs_)
+      if (b->name() == body_ptr->name()) {
+        std::cerr << "Body " << body_ptr->name() << " already exists" << std::endl;
+        return false;
+      }
+    referenced_body_ptrs_.push_back(body_ptr);
+    set_up_ = false;
+    return true;
+  }
+  bool SetUp() {
+    set_up_ = false;
+    std::vector<int> geo, ref;
+    for (auto& b : renderer_geometry_ptr_->body_ptrs()) geo.push_back(b->index());
+    for (auto& b : referenced_body_ptrs_) ref.push_back(b->index());
+    const int kind = std::dynamic_pointer_cast<ColorCamera>(camera_ptr_) ? 0 : 1;
+    if (!Check(batch_->ctx(),
+               m3tb_set_focused_renderer(batch_->ctx(), index_, kind, camera_ptr_->index(), image_size_, z_min_, z_max_,
+                                         int(id_type_), geo.data(), int(geo.size()), ref.data(), int(ref.size())),
+               "FocusedRenderer::SetUp"))
+      return false;
+    set_up_ = true;
+    return true;
+  }
+  // FocusedRenderer::StartRendering: one k_render launch for every device renderer of the batch (the renderers a
+  // Tracker starts one after another at the same poses share it)
+  bool StartRendering() {
+    if (!set_up_) {
+      std::cerr << "Set up renderer " << name_ << " first" << std::endl;
+      return false;
+    }
+    fetched_ = false;
+    if (!batch_->Claim(Batch::kRender, 0, 0, 0)) return true;
+    return Check(batch_->ctx(), m3tb_render(batch_->ctx()), "FocusedRenderer::StartRendering");
+  }
+  bool FetchDepthImage() { return Fetch(); }
+  bool IsBodyVisible(const std::string& body_name) {
+    if (!Fetch()) return false;
+    for (size_t k = 0; k < referenced_body_ptrs_.size(); ++k)
+      if (referenced_body_ptrs_[k]->name() == body_name) return visible_[k] != 0;
+    return false;
+  }
+  bool IsBodyReferenced(const std::string& body_name) const {
+    for (auto& b : referenced_body_ptrs_)
+      if (b->name() == body_name) return true;
+    return false;
+  }
+  const std::vector<uint16_t>& focused_depth_image() { Fetch(); return depth_; }
+  float corner_u() { Fetch(); return corner_u_; }
+  float corner_v() { Fetch(); return corner_v_; }
+  float scale() { Fetch(); return scale_; }
+  float projection_term_a() { Fetch(); return projection_term_a_; }
+  float projection_term_b() { Fetch(); return projection_term_b_; }
+  int image_size() const { return image_size_; }
+  float z_min() const { return z_min_; }
+  float z_max() const { return z_max_; }
+  IDType id_type() const { return id_type_; }
+  void set_image_size(int v) { image_size_ = v; set_up_ = false; }
+  void set_z_min(float v) { z_min_ = v; set_up_ = false; }
+  void set_z_max(float v) { z_max_ = v; set_up_ = false; }
+  bool set_up() const { return set_up_; }
+  int index() const { return index_; }
+  const std::string& name() const { return name_; }
+  const std::shared_ptr<Camera>& camera_ptr() const { return camera_ptr_; }
+  const std::vector<std::shared_ptr<Body>>& referenced_body_ptrs() const { return referenced_body_ptrs_; }
+
+ protected:
+  FocusedDepthRenderer(const std::string& name, const std::shared_ptr<Batch>& batch,
+                       const std::shared_ptr<RendererGeometry>& renderer_geometry_ptr, const std::shared_ptr<Camera>& camera_ptr,
+                       IDType id_type, int image_size, float z_min, float z_max)
+      : name_(name), batch_(batch), renderer_geometry_ptr_(renderer_geometry_ptr), camera_ptr_(camera_ptr), id_type_(id_type),
+        image_size_(image_size), z_min_(z_min), z_max_(z_max) {
+    index_ = batch->NextRenderer();
+  }
+  // FetchDepthImage / FetchSilhouetteImage: one read-back of the last rendering (debug / display)
+  bool Fetch() {
+    if (fetched_) return true;
+    const size_t n = size_t(image_size_) * image_size_;
+    depth_.resize(n);
+    silhouette_.resize(n);
+    visible_.assign(referenced_body_ptrs_.size(), 0);
+    fetched_ = Check(batch_->ctx(),
+                     m3tb_get_rendering(batch_->ctx(), index_, depth_.data(), silhouette_.data(), &corner_u_, &corner_v_,
+                                        &scale_, &projection_term_a_, &projection_term_b_, visible_.data()),
+                     "FocusedRenderer::FetchImage");
+    return fetched_;
+  }
+  std::string name_;
+  std::shared_ptr<Batch> batch_;
+  std::shared_ptr<RendererGeometry> renderer_geometry_ptr_;
+  std::shared_ptr<Camera> camera_ptr_;
+  std::vector<std::shared_ptr<Body>> referenced_body_ptrs_;
+  IDType id_type_;
+  int image_size_;
+  float z_min_, z_max_;
+  int index_ = 0;
+  bool set_up_ = false, fetched_ = false;
+  std::vector<uint16_t> depth_;
+  std::vector<uint8_t> silhouette_;
+  std::vector<int> visible_;
+  float corner_u_ = 0, corner_v_ = 0, scale_ = 0, projection_term_a_ = 0, projection_term_b_ = 0;
+};
+
+class FocusedBasicDepthRenderer : public FocusedDepthRenderer {
+ public:
+  FocusedBasicDepthRenderer(const std::string& name, const std::shared_ptr<Batch>& batch,
+                            const std::shared_ptr<RendererGeometry>& renderer_geometry_ptr,
+                            const std::shared_ptr<Camera>& camera_ptr, int image_size = 200, float z_min = 0.02f,
+                            float z_max = 10.0f)
+      : FocusedDepthRenderer(name, batch, renderer_geometry_ptr, camera_ptr, IDType::BODY, image_size, z_min, z_max) {}
+};
+
+class FocusedSilhouetteRenderer : public FocusedDepthRenderer {
+ public:
+  FocusedSilhouetteRenderer(const std::string& name, const std::shared_ptr<Batch>& batch,
+                            const std::shared_ptr<RendererGeometry>& renderer_geometry_ptr,
+                            const std::shared_ptr<Camera>& camera_ptr, IDType id_type = IDType::BODY, int image_size = 200,
+                            float z_min = 0.02f, float z_max = 10.0f)
+      : FocusedDepthRenderer(name, batch, renderer_geometry_ptr, camera_ptr, id_type, image_size, z_min, z_max) {}
+  bool FetchSilhouetteImage() { return Fetch(); }
+  const std::vector<uint8_t>& focused_silhouette_image() { Fetch(); return silhouette_; }
+};
+
 // ---- modality.h ----------------------------------------------------------------------------------------------------
 class Modality {
  public:
@@ -300,8 +488,38 @@ class Modality {
   const std::string& name() const { return name_; }
   const std::shared_ptr<Body>& body_ptr() const { return body_ptr_; }
   bool set_up() const { return set_up_; }
+  // Modality::correspondence_renderer_ptrs (modality.h): what Tracker renders before CalculateCorrespondences
+  std::vector<std::shared_ptr<FocusedDepthRenderer>> correspondence_renderer_ptrs() const {
+    std::vector<std::shared_ptr<FocusedDepthRenderer>> out;
+    if (depth_renderer_ptr_) out.push_back(depth_renderer_ptr_);
+    if (silhouette_renderer_ptr_) out.push_back(silhouette_renderer_ptr_);
+    return out;
+  }
+  const std::shared_ptr<FocusedDepthRenderer>& depth_renderer_ptr() const { return depth_renderer_ptr_; }
+  const std::shared_ptr<FocusedSilhouetteRenderer>& silhouette_renderer_ptr() const { return silhouette_renderer_ptr_; }
 
  protected:
+  // RegionModality / DepthModality::SetUp checks on the renderers (region_modality.cpp:50-86, depth_modality.cpp:45-76)
+  bool CheckRenderers(IDType silhouette_id_type) const {
+    for (auto& r : correspondence_renderer_ptrs()) {
+      if (!r->set_up()) {
+        std::cerr << "Focused renderer " << r->name() << " was not set up" << std::endl;
+        return false;
+      }
+      if (!r->IsBodyReferenced(body_ptr_->name())) {
+        std::cerr << "Focused renderer " << r->name() << " does not reference body " << body_ptr_->name() << std::endl;
+        return false;
+      }
+    }
+    if (silhouette_renderer_ptr_ && silhouette_renderer_ptr_->id_type() != silhouette_id_type) {
+      std::cerr << "Focused silhouette renderer " << silhouette_renderer_ptr_->name() << " does not use id_type "
+                << (silhouette_id_type == IDType::REGION ? "REGION" : "BODY") << std::endl;
+      return false;
+    }
+    return true;
+  }
+  std::shared_ptr<FocusedDepthRenderer> depth_renderer_ptr_;
+  std::shared_ptr<FocusedSilhouetteRenderer> silhouette_renderer_ptr_;
   Modality(const std::string& name, const std::shared_ptr<Batch>& batch, const std::shared_ptr<Body>& body_ptr)
       : name_(name), batch_(batch), body_ptr_(body_ptr) {}
   bool IsSetup() const {
@@ -380,6 +598,16 @@ class RegionModality : public Modality {
     set_up_ = false;
   }
   void DoNotUseSharedColorHistograms() { color_histograms_ptr_ = nullptr; set_up_ = false; }
+  // region_modality.cpp:230-267 with a device renderer (DESIGN.md "k_render")
+  void ModelOcclusions(const std::shared_ptr<FocusedDepthRenderer>& depth_renderer_ptr) {
+    depth_renderer_ptr_ = depth_renderer_ptr; params_.model_occlusions = 1; set_up_ = false;
+  }
+  void DoNotModelOcclusions() { depth_renderer_ptr_ = nullptr; params_.model_occlusions = 0; set_up_ = false; }
+  void UseRegionChecking(const std::shared_ptr<FocusedSilhouetteRenderer>& silhouette_renderer_ptr) {
+    silhouette_renderer_ptr_ = silhouette_renderer_ptr; params_.use_region_checking = 1; set_up_ = false;
+  }
+  void DoNotUseRegionChecking() { silhouette_renderer_ptr_ = nullptr; params_.use_region_checking = 0; set_up_ = false; }
+  void set_n_unoccluded_iterations(int v) { params_.n_unoccluded_iterations = v; set_up_ = false; }
   const std::shared_ptr<ColorHistograms>& color_histograms_ptr() const { return color_histograms_ptr_; }
   bool set_n_histogram_bins(int v) {
     if (color_histograms_ptr_) { std::cerr << "Modality " << name_ << " uses shared color histograms" << std::endl; return false; }
@@ -400,6 +628,7 @@ class RegionModality : public Modality {
   const std::shared_ptr<RegionModel>& region_model_ptr() const { return region_model_ptr_; }
 
   bool SetUp() override {  // the body's device record is written by Optimizer::SetUp
+    if (!CheckRenderers(IDType::REGION)) return false;
     if (color_histograms_ptr_) {
       if (!color_histograms_ptr_->set_up()) {
         std::cerr << "Color histograms " << color_histograms_ptr_->name() << " was not set up" << std::endl;
@@ -471,11 +700,25 @@ class DepthModality : public Modality {
     for (size_t i = 0; i < v.size() && i < M3TB_MAX_SCHEDULE; ++i) params_.standard_deviations[i] = v[i];
     set_up_ = false;
   }
+  // depth_modality.cpp:128-161 with a device renderer (DESIGN.md "k_render")
+  void ModelOcclusions(const std::shared_ptr<FocusedDepthRenderer>& depth_renderer_ptr) {
+    depth_renderer_ptr_ = depth_renderer_ptr; params_.model_occlusions = 1; set_up_ = false;
+  }
+  void DoNotModelOcclusions() { depth_renderer_ptr_ = nullptr; params_.model_occlusions = 0; set_up_ = false; }
+  void UseSilhouetteChecking(const std::shared_ptr<FocusedSilhouetteRenderer>& silhouette_renderer_ptr) {
+    silhouette_renderer_ptr_ = silhouette_renderer_ptr; params_.use_silhouette_checking = 1; set_up_ = false;
+  }
+  void DoNotUseSilhouetteChecking() { silhouette_renderer_ptr_ = nullptr; params_.use_silhouette_checking = 0; set_up_ = false; }
+  void set_n_unoccluded_iterations(int v) { params_.n_unoccluded_iterations = v; set_up_ = false; }
   const m3tb_depth_params& params() const { return params_; }
   const std::shared_ptr<DepthCamera>& depth_camera_ptr() const { return depth_camera_ptr_; }
   const std::shared_ptr<DepthModel>& depth_model_ptr() const { return depth_model_ptr_; }
 
-  bool SetUp() override { set_up_ = true; return true; }
+  bool SetUp() override {
+    if (!CheckRenderers(IDType::BODY)) return false;
+    set_up_ = true;
+    return true;
+  }
   bool StartModality(int, int) override { return IsSetup(); }  // depth_modality.cpp:248-250
   bool CalculateCorrespondences(int iteration, int corr_iteration) override {
     if (!IsSetup()) return false;
@@ -804,6 +1047,15 @@ class Optimizer {
     const int body = link.body_ptr()->index();
     if (!Check(batch_->ctx(), m3tb_set_body(batch_->ctx(), body, rp, dp, &params_, rmodel, dmodel, ccam, dcam), "Optimizer::SetUp"))
       return false;
+    // the modalities' renderers feed the body's renderer slots (-1: none, detaches an earlier one)
+    for (auto& m : link.modality_ptrs()) {
+      const int modality = std::dynamic_pointer_cast<RegionModality>(m) ? 0 : 1;
+      const int dr = m->depth_renderer_ptr() ? m->depth_renderer_ptr()->index() : -1;
+      const int sr = m->silhouette_renderer_ptr() ? m->silhouette_renderer_ptr()->index() : -1;
+      if (!Check(batch_->ctx(), m3tb_attach_renderer(batch_->ctx(), body, modality, 0, dr), "Modality::ModelOcclusions") ||
+          !Check(batch_->ctx(), m3tb_attach_renderer(batch_->ctx(), body, modality, 1, sr), "Modality::UseSilhouetteChecking"))
+        return false;
+    }
     if (rp && shared) {  // UseSharedColorHistograms: the first body the object was given to owns it on the device
       shared->claim_owner(body);
       if (!Check(batch_->ctx(), m3tb_share_color_histograms(batch_->ctx(), body, shared->owner_body()),
@@ -936,6 +1188,10 @@ class Tracker {
   // them out (tracker.cpp:447-517); used to show that the adapters compose and for step-wise debugging.
   bool ExecuteTrackingStepObjectWise(int iteration) {
     for (int corr = 0; corr < n_corr_iterations_; ++corr) {
+      // Tracker::CalculateCorrespondences renders first (tracker.cpp:447-456)
+      for (auto& m : modality_ptrs_)
+        for (auto& r : m->correspondence_renderer_ptrs())
+          if (!r->StartRendering()) return false;
       for (auto& m : modality_ptrs_)
         if (!m->CalculateCorrespondences(iteration, corr)) return false;
       for (int upd = 0; upd < n_update_iterations_; ++upd) {

@@ -422,6 +422,46 @@ def add_renderings(wl: Workload, image_size=200, z_min=0.02, z_max=5.0, occluder
     return wl
 
 
+# ---- triangle soups for the device renderers (m3tb_set_body_geometry) -------------------------------------------------
+# the reference's triangle prism in the body frame (synth/m3t_synth.cpp kVerts / kFaces: data/_body/triangle.obj with
+# geometry2body's z offset applied)
+PRISM_VERTICES = np.array([[-0.038305, 0.0, -0.006], [-0.038305, 0.0, 0.006], [0.019152, -0.033231, -0.006],
+                           [0.019152, -0.033231, 0.006], [0.019152, 0.033231, -0.006], [0.019152, 0.033231, 0.006]])
+PRISM_FACES = np.array([[0, 2, 3], [2, 4, 3], [3, 5, 1], [4, 0, 1], [0, 4, 2], [1, 0, 3], [4, 5, 3], [5, 4, 1]])
+
+
+def _outward(vertices, faces):
+    """[n,3,3] float32 soup of a convex body around the origin, every triangle counter-clockwise seen from outside."""
+    tri = np.asarray(vertices, np.float64)[np.asarray(faces)]
+    n = np.cross(tri[:, 1] - tri[:, 0], tri[:, 2] - tri[:, 0])
+    flip = np.einsum("ij,ij->i", n, tri.mean(axis=1)) < 0
+    tri[flip] = tri[flip][:, [0, 2, 1]]
+    return tri.astype(np.float32)
+
+
+def prism_triangles():
+    """The prism (8 triangles) and its maximum body diameter (twice the largest vertex distance, as float32)."""
+    return _outward(PRISM_VERTICES, PRISM_FACES), float(np.float32(2.0 * np.linalg.norm(PRISM_VERTICES, axis=1).max()))
+
+
+def icosphere_triangles(radius=0.04, n_divides=4):
+    """A closed subdivided icosahedron (20 * 4^n_divides triangles; 5120 at the default) and its diameter."""
+    t = (1.0 + 5.0 ** 0.5) / 2.0
+    v = [(-1, t, 0), (1, t, 0), (-1, -t, 0), (1, -t, 0), (0, -1, t), (0, 1, t), (0, -1, -t), (0, 1, -t), (t, 0, -1),
+         (t, 0, 1), (-t, 0, -1), (-t, 0, 1)]
+    f = [(0, 11, 5), (0, 5, 1), (0, 1, 7), (0, 7, 10), (0, 10, 11), (1, 5, 9), (5, 11, 4), (11, 10, 2), (10, 7, 6),
+         (7, 1, 8), (3, 9, 4), (3, 4, 2), (3, 2, 6), (3, 6, 8), (3, 8, 9), (4, 9, 5), (2, 4, 11), (6, 2, 10), (8, 6, 7),
+         (9, 8, 1)]
+    tri = np.array([[v[i] for i in face] for face in f], np.float64)
+    tri /= np.linalg.norm(tri, axis=2, keepdims=True)
+    for _ in range(n_divides):
+        a, b, c = tri[:, 0], tri[:, 1], tri[:, 2]
+        ab, bc, ca = [m / np.linalg.norm(m, axis=1, keepdims=True) for m in (a + b, b + c, c + a)]
+        tri = np.concatenate([np.stack(x, 1) for x in ((a, ab, ca), (ab, b, bc), (ca, bc, c), (ab, bc, ca))])
+    tri *= radius
+    return _outward(tri.reshape(-1, 3), np.arange(tri.shape[0] * 3).reshape(-1, 3)), float(np.float32(2.0 * radius))
+
+
 PRESETS = {
     # name: (n_bodies, n_lines, n_points, rbot_shape)
     "c1": dict(n_bodies=1, n_lines=200, n_points=0, rbot=False),

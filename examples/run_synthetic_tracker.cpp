@@ -4,6 +4,10 @@
 // object through the Modality / Optimizer methods; prints both pose sets as JSON for tests/test_gpu_host_mirror.py.
 //
 //   usage: run_synthetic_tracker [n_bodies=3] [n_lines=200] [n_points=200] [n_divides=2] [seed=1] [links_per_structure=1]
+//                                [renderers=0]
+// With renderers = 1 every body's modalities model occlusions and check regions / silhouettes with device renderers
+// (one FocusedSilhouetteRenderer per camera over all bodies of one RendererGeometry), and the same scene is also run
+// through the plain C ABI ("c_abi" poses), which the fused Tracker path must reproduce bit for bit.
 // With links_per_structure > 1 the bodies are grouped into serial kinematic chains (root link with 6 DoF, every further
 // link a revolute-x child at Tx(0.01) of the previous one, as in the reference's examples/optimization_time.cpp) that
 // are tracked by one Optimizer each; the children's start poses come from Optimizer::CalculateConsistentPoses.
@@ -45,8 +49,30 @@ Transform3fA JointPose(float tx, float angle_x_deg) {  // Tx(tx) * Rx(angle)
   return r;
 }
 
+// the reference's triangle prism (data/_body/triangle.obj, geometry2body applied), counter-clockwise seen from outside
+std::vector<float> PrismTriangles(float* diameter) {
+  const float v[6][3] = {{-0.038305f, 0.0f, -0.006f}, {-0.038305f, 0.0f, 0.006f}, {0.019152f, -0.033231f, -0.006f},
+                         {0.019152f, -0.033231f, 0.006f}, {0.019152f, 0.033231f, -0.006f}, {0.019152f, 0.033231f, 0.006f}};
+  const int f[8][3] = {{0, 2, 3}, {2, 4, 3}, {3, 5, 1}, {4, 0, 1}, {0, 4, 2}, {1, 0, 3}, {4, 5, 3}, {5, 4, 1}};
+  std::vector<float> out;
+  for (auto& t : f) {
+    const float* a = v[t[0]];
+    const float* b = v[t[1]];
+    const float* c = v[t[2]];
+    const float e1[3] = {b[0] - a[0], b[1] - a[1], b[2] - a[2]}, e2[3] = {c[0] - a[0], c[1] - a[1], c[2] - a[2]};
+    const float n[3] = {e1[1] * e2[2] - e1[2] * e2[1], e1[2] * e2[0] - e1[0] * e2[2], e1[0] * e2[1] - e1[1] * e2[0]};
+    const bool outward = n[0] * (a[0] + b[0] + c[0]) + n[1] * (a[1] + b[1] + c[1]) + n[2] * (a[2] + b[2] + c[2]) > 0.0f;
+    for (const float* p : {a, outward ? b : c, outward ? c : b}) out.insert(out.end(), p, p + 3);
+  }
+  float r = 0.0f;
+  for (auto& p : v) r = std::max(r, std::sqrt(p[0] * p[0] + p[1] * p[1] + p[2] * p[2]));
+  *diameter = 2.0f * r;
+  return out;
+}
+
 struct Scene {
   std::shared_ptr<Batch> batch;
+  std::vector<std::shared_ptr<FocusedSilhouetteRenderer>> renderers;
   std::vector<std::shared_ptr<Body>> bodies;
   std::vector<std::shared_ptr<ColorCamera>> color_cameras;
   std::vector<std::shared_ptr<DepthCamera>> depth_cameras;
@@ -74,6 +100,9 @@ int main(int argc, char** argv) {
   const int n_divides = argc > 4 ? std::atoi(argv[4]) : 2;
   const uint64_t seed = argc > 5 ? std::strtoull(argv[5], nullptr, 10) : 1;
   const int chain = argc > 6 ? std::max(1, std::atoi(argv[6])) : 1;
+  const bool with_renderers = argc > 7 && std::atoi(argv[7]) != 0;
+  float prism_diameter = 0.0f;
+  const std::vector<float> prism = PrismTriangles(&prism_diameter);
   if (n_bodies % chain != 0) {
     std::cerr << "n_bodies must be a multiple of links_per_structure" << std::endl;
     return 1;
@@ -131,8 +160,19 @@ int main(int argc, char** argv) {
     if (!region_model->SetUp() || !depth_model->SetUp()) return false;
     s.tracker = std::make_shared<Tracker>("tracker", s.batch, 7, 2);
     std::vector<std::shared_ptr<Link>> links;  // links of the chain being assembled
+    auto geometry = std::make_shared<RendererGeometry>("renderer_geometry", s.batch);
+    std::vector<std::shared_ptr<Body>> all_bodies;
     for (int b = 0; b < n_bodies; ++b) {
-      auto body = std::make_shared<Body>("triangle_" + std::to_string(b), s.batch);
+      all_bodies.push_back(std::make_shared<Body>("triangle_" + std::to_string(b), s.batch));
+      all_bodies.back()->set_geometry_triangles(prism);
+      all_bodies.back()->set_maximum_body_diameter(prism_diameter);
+      all_bodies.back()->set_body_id(uint8_t(b + 1));
+      all_bodies.back()->set_region_id(7);
+      if (with_renderers && !geometry->AddBody(all_bodies.back())) return false;
+    }
+    if (!geometry->SetUp()) return false;
+    for (int b = 0; b < n_bodies; ++b) {
+      auto body = all_bodies[b];
       auto cc = std::make_shared<ColorCamera>("color_camera_" + std::to_string(b), s.batch, ci, color_w2c);
       auto dc = std::make_shared<DepthCamera>("depth_camera_" + std::to_string(b), s.batch, di, depth_w2c, 0.001f);
       if (!cc->SetUp() || !dc->SetUp()) return false;
@@ -140,6 +180,21 @@ int main(int argc, char** argv) {
       rm->set_n_lines_max(n_lines);
       auto dm = std::make_shared<DepthModality>("depth_modality_" + std::to_string(b), s.batch, body, dc, depth_model);
       dm->set_n_points_max(n_points);
+      if (with_renderers) {
+        auto cr = std::make_shared<FocusedSilhouetteRenderer>("color_renderer_" + std::to_string(b), s.batch, geometry, cc,
+                                                              IDType::REGION);
+        auto dr = std::make_shared<FocusedSilhouetteRenderer>("depth_renderer_" + std::to_string(b), s.batch, geometry, dc,
+                                                              IDType::BODY);
+        if (!cr->AddReferencedBody(body) || !dr->AddReferencedBody(body) || !cr->SetUp() || !dr->SetUp()) return false;
+        rm->ModelOcclusions(cr);
+        rm->UseRegionChecking(cr);
+        rm->set_n_unoccluded_iterations(0);
+        dm->ModelOcclusions(dr);
+        dm->UseSilhouetteChecking(dr);
+        dm->set_n_unoccluded_iterations(0);
+        s.renderers.push_back(cr);
+        s.renderers.push_back(dr);
+      }
       auto link = std::make_shared<Link>("link_" + std::to_string(b), body);
       link->AddModality(rm);
       link->AddModality(dm);
@@ -176,6 +231,46 @@ int main(int argc, char** argv) {
     std::cerr << "setup failed" << std::endl;
     return 2;
   }
+  // the same renderer scene through the plain C ABI (rigid bodies only)
+  std::vector<float> c_abi(size_t(12) * n_bodies, 0.0f);
+  if (with_renderers && chain == 1) {
+    m3tb_ctx* raw = nullptr;
+    bool ok = m3tb_create(0, n_bodies, n_bodies, 1, &raw) == M3TB_OK;
+    m3tb_region_params rp;
+    m3tb_depth_params dp;
+    m3tb_region_params_default(&rp);
+    m3tb_depth_params_default(&dp);
+    rp.n_lines_max = n_lines;
+    dp.n_points_max = n_points;
+    rp.model_occlusions = rp.use_region_checking = 1;
+    dp.model_occlusions = dp.use_silhouette_checking = 1;
+    rp.n_unoccluded_iterations = dp.n_unoccluded_iterations = 0;
+    const m3tb_optimizer_params op{1000.0f, 30000.0f};
+    ok = ok && m3tb_set_region_model(raw, 0, nv, n_lines, r_ori.data(), r_len.data(), r_pts.data(), 0.002f, 0.05f) == 0 &&
+         m3tb_set_depth_model(raw, 0, nv, n_points, d_ori.data(), d_area.data(), d_pts.data(), 0.002f, 0.05f) == 0;
+    std::vector<int> all(n_bodies);
+    for (int b = 0; b < n_bodies; ++b) all[b] = b;
+    const Transform3fA identity;
+    for (int b = 0; b < n_bodies && ok; ++b)
+      ok = m3tb_set_color_camera(raw, b, &ci, color_w2c.data()) == 0 &&
+           m3tb_set_depth_camera(raw, b, &di, depth_w2c.data(), 0.001f) == 0 &&
+           m3tb_upload_color(raw, b, color[b].data(), cpitch) == 0 && m3tb_upload_depth(raw, b, depth[b].data(), dpitch) == 0 &&
+           m3tb_set_body(raw, b, &rp, &dp, &op, 0, 0, b, b) == 0 && m3tb_set_poses(raw, b, 1, start[b].data()) == 0 &&
+           m3tb_set_body_geometry(raw, b, prism.data(), int(prism.size() / 9), identity.data(), prism_diameter, 1, b + 1, 7) == 0;
+    for (int b = 0; b < n_bodies && ok; ++b)
+      ok = m3tb_set_focused_renderer(raw, 2 * b, 0, b, 200, 0.02f, 10.0f, 1, all.data(), n_bodies, &b, 1) == 0 &&
+           m3tb_set_focused_renderer(raw, 2 * b + 1, 1, b, 200, 0.02f, 10.0f, 0, all.data(), n_bodies, &b, 1) == 0;
+    for (int b = 0; b < n_bodies && ok; ++b)
+      for (int m = 0; m < 2 && ok; ++m)
+        for (int k = 0; k < 2 && ok; ++k) ok = m3tb_attach_renderer(raw, b, m, k, 2 * b + m) == 0;
+    ok = ok && m3tb_start_modalities(raw, 0) == 0 && m3tb_tracking_step(raw, 0, 7, 2) == 0 &&
+         m3tb_calculate_results(raw, 0) == 0 && m3tb_get_poses(raw, 0, n_bodies, c_abi.data()) == 0;
+    if (!ok) {
+      std::cerr << "C ABI run failed: " << (raw ? m3tb_last_error(raw) : "no context") << std::endl;
+      return 6;
+    }
+    m3tb_destroy(raw);
+  }
   // an unset-up tracker must refuse to run, like the reference (tracker.cpp:224-228)
   Tracker not_set_up("not_set_up", fused.batch);
   const bool refused = !not_set_up.ExecuteTrackingStep(0);
@@ -198,6 +293,19 @@ int main(int argc, char** argv) {
   std::printf("\"n_bodies\": %d, \"refused_without_setup\": %s, \"launches_fused\": %lld, \"launches_object_wise\": %lld, ",
               n_bodies, refused ? "true" : "false", (long long)m3tb_launch_count(fused.batch->ctx()),
               (long long)m3tb_launch_count(object_wise.batch->ctx()));
+  if (with_renderers) {
+    bool visible = true;
+    for (int b = 0; b < n_bodies; ++b)
+      visible = visible && fused.renderers[2 * b]->IsBodyVisible(fused.bodies[b]->name()) &&
+                fused.renderers[2 * b + 1]->IsBodyVisible(fused.bodies[b]->name());
+    std::printf("\"renderers_visible\": %s, \"c_abi\": [", visible ? "true" : "false");
+    for (int b = 0; b < n_bodies; ++b) {
+      std::printf("%s[", b ? ", " : "");
+      for (int k = 0; k < 12; ++k) std::printf("%s%.9g", k ? ", " : "", c_abi[12 * b + k]);
+      std::printf("]");
+    }
+    std::printf("], ");
+  }
   std::printf("\"start\": [");
   for (int b = 0; b < n_bodies; ++b) {
     std::printf("%s[", b ? ", " : "");

@@ -259,6 +259,47 @@ typedef struct m3tb_rendering {
 int m3tb_upload_depth_rendering(m3tb_ctx* ctx, int body, int modality, const m3tb_rendering* rendering);
 int m3tb_upload_silhouette_rendering(m3tb_ctx* ctx, int body, int modality, const m3tb_rendering* rendering);
 
+/* ---- device renderers: the focused renderers of the checks above, rendered on the device (k_render, DESIGN.md §3) so
+ * that no OpenGL renderer and no image upload is needed. Rasterisation contract: DESIGN.md §3 "k_render".
+ *
+ * Body + RendererGeometry::AddBody (body.h, renderer_geometry.cpp): `triangles` is the body's triangle soup,
+ * [n_triangles][3][3] floats in metres in the geometry frame, as RendererGeometry uploads it (after Body's unit scaling
+ * and winding normalisation, body.cpp:201-249: counter-clockwise seen from outside); `geometry2body` the
+ * Body::geometry2body_pose(); `enable_culling` Body::geometry_enable_culling(); body_id / region_id Body::body_id() /
+ * region_id() (0..255). Independent of m3tb_set_body: a body that is only drawn (an occluder) needs only this and a pose. */
+int m3tb_set_body_geometry(m3tb_ctx* ctx, int body, const float* triangles, int n_triangles,
+                           const float geometry2body[12], float maximum_body_diameter, int enable_culling, int body_id,
+                           int region_id);
+/* FocusedBasicDepthRenderer / FocusedSilhouetteRenderer (basic_depth_renderer.h, silhouette_renderer.h; every device
+ * renderer produces both images) of the colour (camera_kind 0) or depth (1) camera `camera`. `geometry_bodies` are drawn
+ * in that order (RendererGeometry::render_data_bodies), `referenced_bodies` are the bodies the image focuses on
+ * (FocusedRenderer::AddReferencedBody). Defaults (renderer.h:112-113,222): image_size 200, z_min 0.02, z_max 10.
+ * id_type: 0 = IDType::BODY, 1 = IDType::REGION (the silhouette value). Renderer ids are dense (0..n). image_size above
+ * 240 returns M3TB_ERR_UNSUPPORTED (the z-buffer lives in shared memory). A renderer attached to a modality cannot be
+ * set again before it is detached. */
+int m3tb_set_focused_renderer(m3tb_ctx* ctx, int renderer, int camera_kind, int camera, int image_size, float z_min,
+                              float z_max, int id_type, const int* geometry_bodies, int n_geometry,
+                              const int* referenced_bodies, int n_referenced);
+/* RegionModality::ModelOcclusions / UseRegionChecking (region_modality.cpp:230-267) and DepthModality::ModelOcclusions /
+ * UseSilhouetteChecking (depth_modality.cpp:128-161) with a device renderer: `modality` 0 region / 1 depth, `kind`
+ * 0 depth image / 1 silhouette image; renderer -1 detaches (DoNot...). The renderer must render the modality's camera
+ * and reference the body; a silhouette renderer must use id_type REGION for the region and BODY for the depth modality
+ * (region_modality.cpp:66-86, depth_modality.cpp:56-76). The parameter flags (model_occlusions, use_region_checking,
+ * use_silhouette_checking) still switch the checks. While a slot is attached, m3tb_upload_*_rendering on it fails.
+ * With at least one slot attached, m3tb_tracking_step / m3tb_corr_iteration render every attached renderer before each
+ * correspondence iteration (Tracker::CalculateCorrespondences, tracker.cpp:447-456), and m3tb_start_modalities /
+ * m3tb_calculate_results first render the renderers attached to region modalities (tracker.cpp:430-434, 503-506).
+ * Contexts without attached slots launch exactly what they launched before. */
+int m3tb_attach_renderer(m3tb_ctx* ctx, int body, int modality, int kind, int renderer);
+/* FocusedRenderer::StartRendering of every device renderer from the current poses (the fine-grained path calls it where
+ * Tracker does). One kernel launch. */
+int m3tb_render(m3tb_ctx* ctx);
+/* Debug / parity read-back of one device renderer's last rendering: focused depth image (u16) and silhouette image (u8),
+ * image_size x image_size, rows packed; corner_u / corner_v / scale, projection terms, and one
+ * FocusedRenderer::IsBodyVisible flag per referenced body. Any pointer may be NULL. */
+int m3tb_get_rendering(m3tb_ctx* ctx, int renderer, void* depth_u16, void* silhouette_u8, float* corner_u, float* corner_v,
+                       float* scale, float* projection_term_a, float* projection_term_b, int* visible_flags);
+
 /* Loader-style batch ingest: `count` frames for cameras [first_cam, first_cam+count), frame k at
  * base + k*frame_stride bytes. Cameras of equal size share one device pool, so this is a single
  * host->device copy when the host frames are contiguous (frame_stride == height*pitch). */
