@@ -103,7 +103,8 @@ SYMBOLS = [
     "m3tb_set_gradient_hessian", "m3tb_reset_joint_poses", "m3tb_prefetch_frames", "m3tb_detach_frames",
     "m3tb_debug_closest_view", "m3tb_upload_depth_rendering", "m3tb_upload_silhouette_rendering",
     "m3tb_share_color_histograms", "m3tb_debug_last_launch", "m3tb_set_body_geometry", "m3tb_set_focused_renderer",
-    "m3tb_attach_renderer", "m3tb_render", "m3tb_get_rendering",
+    "m3tb_attach_renderer", "m3tb_render", "m3tb_get_rendering", "m3tb_model_params_default", "m3tb_model_views",
+    "m3tb_generate_depth_model", "m3tb_get_depth_model", "m3tb_debug_render_model_view",
 ]
 
 KERNEL_NAMES = {0: None, 1: "k_track", 2: "k_track2", 3: "k_track_cluster"}
@@ -113,6 +114,14 @@ class LaunchInfo(C.Structure):
     """m3tb_launch_info: the tracking-kernel variant of the last tracking launch."""
     _fields_ = [("kernel", C.c_int32), ("threads", C.c_int32), ("items_per_thread", C.c_int32), ("lut_smem", C.c_int32),
                 ("occ", C.c_int32), ("tiles", C.c_int32), ("tma_mode", C.c_int32)]
+
+
+class ModelParams(C.Structure):
+    """m3tb_model_params (model.h:161-167)."""
+    _fields_ = [("sphere_radius", C.c_float), ("n_divides", C.c_int32), ("n_points", C.c_int32),
+                ("max_radius_depth_offset", C.c_float), ("stride_depth_offset", C.c_float),
+                ("use_random_seed", C.c_int32), ("image_size", C.c_int32)]
+
 
 _lib = None
 
@@ -198,6 +207,11 @@ def lib():
     L.m3tb_attach_renderer.argtypes = [vp, ci, ci, ci, ci]
     L.m3tb_render.argtypes = [vp]
     L.m3tb_get_rendering.argtypes = [vp, ci, vp, vp, fp, fp, fp, fp, fp, ip]
+    L.m3tb_model_params_default.argtypes = [C.POINTER(ModelParams)]
+    L.m3tb_model_views.argtypes = [C.POINTER(ModelParams), fp, ci, ip]
+    L.m3tb_generate_depth_model.argtypes = [vp, ci, ci, ip, ci, C.POINTER(ModelParams)]
+    L.m3tb_get_depth_model.argtypes = [vp, ci, ip, ip, fp, fp, vp, fp, fp]
+    L.m3tb_debug_render_model_view.argtypes = [vp, ci, ip, ci, C.POINTER(ModelParams), ci, vp, vp, vp]
     _lib = L
     return L
 
@@ -208,6 +222,31 @@ def _f32(a):
 
 def _p(a):
     return a.ctypes.data_as(fp)
+
+
+def model_params(**kw) -> ModelParams:
+    """m3tb_model_params_default with the given fields replaced (sphere_radius, n_divides, n_points,
+    max_radius_depth_offset, stride_depth_offset, use_random_seed, image_size)."""
+    p = ModelParams()
+    lib().m3tb_model_params_default(C.byref(p))
+    for k, v in kw.items():
+        if k not in dict(ModelParams._fields_):
+            raise TypeError(f"unknown model parameter {k}")
+        setattr(p, k, v)
+    return p
+
+
+def model_views(params=None):
+    """Geodesic camera2body poses [n,3,4] float32 of a model (m3tb_model_views, host only); the view orientation is
+    column 2."""
+    p = params if params is not None else model_params()
+    n = C.c_int(0)
+    ip = C.POINTER(C.c_int)
+    if lib().m3tb_model_views(C.byref(p), None, 0, C.cast(C.byref(n), ip)) != 0:
+        raise M3TBError("m3tb_model_views: bad parameters")
+    out = np.zeros((n.value, 3, 4), np.float32)
+    lib().m3tb_model_views(C.byref(p), _p(out), n.value, C.cast(C.byref(n), ip))
+    return out
 
 
 def region_params(settings=None) -> RegionParams:
@@ -404,6 +443,44 @@ class Context:
                        (np.float32(x.value) for x in f)))
         out.update(depth=depth, silhouette=sil, visible=vis)
         return out
+
+    def generate_depth_model(self, model_id, body, occlusion_bodies=(), params=None):
+        """DepthModel::GenerateModel on the device from the geometry of m3tb_set_body_geometry (params: ModelParams,
+        default model_params())."""
+        p = params if params is not None else model_params()
+        occ = np.ascontiguousarray(occlusion_bodies, np.int32)
+        self._ck(self.L.m3tb_generate_depth_model(self.h, model_id, body, occ.ctypes.data_as(C.POINTER(C.c_int)),
+                                                  occ.size, C.byref(p)))
+
+    def get_depth_model(self, model_id):
+        """A generated depth model as synth.Model (orientations, surface areas, [nv, np, 36] DataPoints, and the
+        stride_depth_offset / max_radius_depth_offset it was generated with)."""
+        from .synth import Model
+        nv, npt = C.c_int(0), C.c_int(0)
+        stride, radius = C.c_float(0.0), C.c_float(0.0)
+        ip = C.POINTER(C.c_int)
+        self._ck(self.L.m3tb_get_depth_model(self.h, model_id, C.cast(C.byref(nv), ip), C.cast(C.byref(npt), ip),
+                                             None, None, None, C.byref(stride), C.byref(radius)))
+        ori = np.zeros((nv.value, 3), np.float32)
+        area = np.zeros(nv.value, np.float32)
+        pts = np.zeros((nv.value, npt.value, 36), np.float32)
+        self._ck(self.L.m3tb_get_depth_model(self.h, model_id, None, None, _p(ori), _p(area), pts.ctypes.data, None,
+                                             None))
+        return Model("depth", ori, area, pts, stride_depth_offset=float(np.float32(stride.value)),
+                     max_radius_depth_offset=float(np.float32(radius.value)))
+
+    def debug_render_model_view(self, body, view, occlusion_bodies=(), params=None):
+        """dict(normal [S,S,4] u8 BGRA, depth [S,S] u16, silhouette [S,S] u8) of one generation view."""
+        p = params if params is not None else model_params()
+        S = p.image_size
+        occ = np.ascontiguousarray(occlusion_bodies, np.int32)
+        normal = np.zeros((S, S, 4), np.uint8)
+        depth = np.zeros((S, S), np.uint16)
+        sil = np.zeros((S, S), np.uint8)
+        self._ck(self.L.m3tb_debug_render_model_view(self.h, body, occ.ctypes.data_as(C.POINTER(C.c_int)), occ.size,
+                                                     C.byref(p), view, normal.ctypes.data, depth.ctypes.data,
+                                                     sil.ctypes.data))
+        return dict(normal=normal, depth=depth, silhouette=sil)
 
     def set_body(self, body, region, depth, optimizer, region_model=0, depth_model=0, color_camera=0, depth_camera=0):
         self._ck(self.L.m3tb_set_body(self.h, body, C.byref(region) if region is not None else None,

@@ -9,10 +9,12 @@
 #include <cstdio>
 #include <cstdlib>
 #include <array>
+#include <set>
 #include <cstring>
 #include <string>
 #include <vector>
 
+#include "m3t_b200_model.cuh"
 #include "m3t_b200_render.cuh"
 #include "m3t_b200_structures.cuh"
 #include "m3t_b200_kernels.cuh"
@@ -193,6 +195,14 @@ struct m3tb_ctx {
   size_t render_smem[kRenderLists] = {};     // z-buffer bytes of the largest renderer of each list
   std::vector<int> render_list[kRenderLists];  // host copies of the lists
   size_t render_capacity[4] = {0, 0, 0, 0};  // renderers, list ints, attachments, visible flags
+
+  // host copies of the depth models made by m3tb_generate_depth_model (m3tb_get_depth_model); empty: not generated
+  struct GeneratedModel {
+    int n_views = 0, n_points = 0;
+    float stride_depth_offset = 0.0f, max_radius_depth_offset = 0.0f;
+    std::vector<float> orientations, surface_areas, points;
+  };
+  std::vector<GeneratedModel> dmodel_generated;
 };
 
 namespace {
@@ -1321,6 +1331,269 @@ int UploadBatch(m3tb_ctx* ctx, bool color, int first, int count, const void* src
   return M3TB_OK;
 }
 
+// ---- depth-model generation (m3tb_generate_depth_model) -------------------------------------------------------------
+// Host side: parameters, geodesic views and the per-view transforms, in float32 with the reference's expressions.
+
+constexpr int kImageSizeSafetyBoundary = 20;    // model.h:57
+constexpr float kMinimumClipSpaceRatio = 0.2f;  // model.h:59
+constexpr unsigned kModelSeed = 7;              // std::mt19937 generator{7} (depth_model.cpp:317)
+constexpr int kModelMaxImageSize = 8192;        // two 8192^2 z-buffers of 8 B are the whole scratch bound
+constexpr int kModelMaxDivides = 8;
+
+using Vec3 = std::array<float, 3>;
+
+struct SmallerVec3 {  // Model::CompareSmallerVector3f (model.h:62-67)
+  bool operator()(const Vec3& a, const Vec3& b) const {
+    return a[0] < b[0] || (a[0] == b[0] && a[1] < b[1]) || (a[0] == b[0] && a[1] == b[1] && a[2] < b[2]);
+  }
+};
+
+Vec3 Normalized(const Vec3& v) {  // Eigen normalized(): v / sqrt(squaredNorm), unchanged if the norm is 0
+  const float n = v[0] * v[0] + v[1] * v[1] + v[2] * v[2];
+  if (!(n > 0.0f)) return v;
+  const float s = std::sqrt(n);
+  return {v[0] / s, v[1] / s, v[2] / s};
+}
+
+Vec3 Cross(const Vec3& a, const Vec3& b) {
+  return {a[1] * b[2] - a[2] * b[1], a[2] * b[0] - a[0] * b[2], a[0] * b[1] - a[1] * b[0]};
+}
+
+void SubdivideTriangle(const Vec3& v1, const Vec3& v2, const Vec3& v3, int n, std::set<Vec3, SmallerVec3>& points) {
+  if (n == 0) {
+    points.insert(v1);
+    points.insert(v2);
+    points.insert(v3);
+    return;
+  }
+  const Vec3 v12 = Normalized({v1[0] + v2[0], v1[1] + v2[1], v1[2] + v2[2]});
+  const Vec3 v13 = Normalized({v1[0] + v3[0], v1[1] + v3[1], v1[2] + v3[2]});
+  const Vec3 v23 = Normalized({v2[0] + v3[0], v2[1] + v3[1], v2[2] + v3[2]});
+  SubdivideTriangle(v1, v12, v13, n - 1, points);
+  SubdivideTriangle(v2, v12, v23, n - 1, points);
+  SubdivideTriangle(v3, v13, v23, n - 1, points);
+  SubdivideTriangle(v12, v13, v23, n - 1, points);
+}
+
+// Model::GenerateGeodesicPoints / GenerateGeodesicPoses (model.cpp:386-454): camera2body [n][12], row-major 3x4
+std::vector<float> GeodesicPoses(int n_divides, float sphere_radius) {
+  const float x = 0.525731112119133606f, z = 0.850650808352039932f;
+  const Vec3 ico[12] = {{-x, 0.0f, z}, {x, 0.0f, z},  {-x, 0.0f, -z}, {x, 0.0f, -z}, {0.0f, z, x},  {0.0f, z, -x},
+                        {0.0f, -z, x}, {0.0f, -z, -x}, {z, x, 0.0f},  {-z, x, 0.0f}, {z, -x, 0.0f}, {-z, -x, 0.0f}};
+  const int ids[20][3] = {{0, 4, 1},  {0, 9, 4},  {9, 5, 4},  {4, 5, 8},  {4, 8, 1},  {8, 10, 1}, {8, 3, 10},
+                          {5, 3, 8},  {5, 2, 3},  {2, 7, 3},  {7, 10, 3}, {7, 6, 10}, {7, 11, 6}, {11, 0, 6},
+                          {0, 1, 6},  {6, 1, 10}, {9, 0, 11}, {9, 11, 2}, {9, 2, 5},  {7, 2, 11}};
+  std::set<Vec3, SmallerVec3> points;
+  for (const auto& t : ids) SubdivideTriangle(ico[t[0]], ico[t[1]], ico[t[2]], n_divides, points);
+  std::vector<float> poses;
+  poses.reserve(points.size() * 12);
+  for (const Vec3& p : points) {
+    const Vec3 c2 = {-p[0], -p[1], -p[2]};
+    const Vec3 c0 = (p[0] == 0.0f && p[2] == 0.0f) ? Vec3{1.0f, 0.0f, 0.0f} : Normalized(Cross({0.0f, 1.0f, 0.0f}, c2));
+    const Vec3 c1 = Cross(c2, c0);
+    for (int r = 0; r < 3; ++r) {
+      const float row[4] = {c0[r], c1[r], c2[r], p[r] * sphere_radius};
+      poses.insert(poses.end(), row, row + 4);
+    }
+  }
+  return poses;
+}
+
+// Checks the model parameters (Model::DepthOffsetVariablesValid, model.cpp:325-336)
+int CheckModelParams(m3tb_ctx* ctx, const m3tb_model_params* p) {
+  if (!p) return Fail(ctx, M3TB_ERR_INVALID, "null model parameters");
+  if (p->use_random_seed) return Fail(ctx, M3TB_ERR_UNSUPPORTED, "use_random_seed: the reference seeds from the clock");
+  if (!(p->sphere_radius > 0.0f) || !std::isfinite(p->sphere_radius) || p->n_divides < 0 ||
+      p->n_divides > kModelMaxDivides || p->n_points < 1 || !(p->stride_depth_offset > 0.0f) ||
+      !(p->max_radius_depth_offset >= 0.0f) || !std::isfinite(p->max_radius_depth_offset) ||
+      p->image_size <= kImageSizeSafetyBoundary || p->image_size > kModelMaxImageSize)
+    return Fail(ctx, M3TB_ERR_INVALID, "bad model parameters");
+  if (int(p->max_radius_depth_offset / p->stride_depth_offset + 1.0f) > kModelMaxOffsets)
+    return Fail(ctx, M3TB_ERR_INVALID, "max_radius_depth_offset / stride_depth_offset is above 30");
+  return M3TB_OK;
+}
+
+// What one generation renders: the full renderers' intrinsics and projection, and per view the camera2body pose, the
+// clip-space matrices of every drawn body and the main renderer's world2camera * geometry2world rotation.
+struct ModelSetup {
+  int S = 0, n_views = 0, n_occlusion = 0, n_renderers = 1, n_slots = 2, max_triangles = 0;
+  float fu = 0.0f, pp = 0.0f, projection_term_a = 0.0f, projection_term_b = 0.0f;
+  std::vector<float> camera2body, M, rot, face_normals;
+  std::vector<ModelBodyDev> bodies;
+};
+
+int PrepareModel(m3tb_ctx* ctx, int body, const int* occlusion_bodies, int n_occlusion, const m3tb_model_params* p,
+                 ModelSetup& st) {
+  int rc = CheckModelParams(ctx, p);
+  if (rc) return rc;
+  if (body < 0 || body >= ctx->max_bodies || !ctx->h_geometry[body].set)
+    return Fail(ctx, M3TB_ERR_INVALID, "body has no geometry (m3tb_set_body_geometry)");
+  if (n_occlusion < 0 || (n_occlusion > 0 && !occlusion_bodies) || n_occlusion >= 65535)
+    return Fail(ctx, M3TB_ERR_INVALID, "bad occlusion body list");
+  for (int k = 0; k < n_occlusion; ++k) {
+    const int b = occlusion_bodies[k];
+    if (b < 0 || b >= ctx->max_bodies || !ctx->h_geometry[b].set)
+      return Fail(ctx, M3TB_ERR_INVALID, "occlusion body " + std::to_string(b) + " has no geometry");
+    if (b == body) return Fail(ctx, M3TB_ERR_INVALID, "the body is its own occlusion body");
+    for (int q = 0; q < k; ++q)
+      if (occlusion_bodies[q] == b) return Fail(ctx, M3TB_ERR_INVALID, "occlusion body listed twice");
+  }
+  // Model::SetUpRenderer / AddBodiesToRenderer (model.cpp:120-196); the radius is 0.5f * diameter, exactly
+  const float r = p->sphere_radius;
+  const GeometryDev& G = ctx->h_geometry[body];
+  const float z_min = r - G.radius, z_max = r + G.radius;
+  if (z_min < r * kMinimumClipSpaceRatio) return Fail(ctx, M3TB_ERR_INVALID, "z_min of the body below 0.2 * sphere_radius");
+  float zo_min = z_min, zo_max = z_max;
+  for (int k = 0; k < n_occlusion; ++k) {
+    const float rad = ctx->h_geometry[occlusion_bodies[k]].radius;
+    const float lo = r - rad, hi = r + rad;
+    if (lo < r * kMinimumClipSpaceRatio)
+      return Fail(ctx, M3TB_ERR_INVALID, "z_min of an occlusion body below 0.2 * sphere_radius");
+    zo_min = std::min(lo, zo_min);
+    zo_max = std::max(hi, zo_max);
+  }
+  st.S = p->image_size;
+  st.n_occlusion = n_occlusion;
+  st.n_renderers = n_occlusion > 0 ? 2 : 1;
+  st.n_slots = 2 + n_occlusion;
+  st.fu = 0.5f * float(st.S - kImageSizeSafetyBoundary) / tanf(asinf(G.radius / r));
+  st.pp = float(st.S) / 2.0f;
+  st.projection_term_a = z_max * z_min * 65535.0f / (z_max - z_min);  // FullDepthRenderer (renderer.cpp:476-477)
+  st.projection_term_b = z_max * 65535.0f / (z_max - z_min);
+  // FullRenderer::CalculateProjectionMatrix (renderer.cpp:257-263) of the main and the occlusion renderer
+  const float fS = float(st.S);
+  const float P00 = 2.0f * st.fu / fS, P02 = 2.0f * (st.pp + 0.5f) / fS - 1.0f;
+  const float P11 = P00, P12 = P02;  // fv = fu, ppv = ppu, height = width
+  const float P22[2] = {(z_max + z_min) / (z_max - z_min), (zo_max + zo_min) / (zo_max - zo_min)};
+  const float P23[2] = {-2.0f * z_max * z_min / (z_max - z_min), -2.0f * zo_max * zo_min / (zo_max - zo_min)};
+
+  st.bodies.assign(1 + n_occlusion, ModelBodyDev());
+  for (int g = 0; g <= n_occlusion; ++g) {
+    const GeometryDev& B = ctx->h_geometry[g == 0 ? body : occlusion_bodies[g - 1]];
+    st.bodies[g] = {B.triangles, B.n_triangles, B.enable_culling};
+    st.max_triangles = std::max(st.max_triangles, B.n_triangles);
+  }
+  // face normals of the body (RendererGeometry::AssembleVertexData, renderer_geometry.cpp:199-200)
+  std::vector<float> tri(size_t(G.n_triangles) * 9);
+  CU(cudaMemcpy(tri.data(), G.triangles, sizeof(float) * tri.size(), cudaMemcpyDeviceToHost));
+  st.face_normals.resize(size_t(G.n_triangles) * 3);
+  for (int t = 0; t < G.n_triangles; ++t) {
+    const float* v = tri.data() + 9 * size_t(t);
+    const Vec3 a = {v[6] - v[3], v[7] - v[4], v[8] - v[5]}, b = {v[0] - v[3], v[1] - v[4], v[2] - v[5]};
+    const Vec3 n = Normalized(Cross(a, b));
+    std::memcpy(st.face_normals.data() + 3 * size_t(t), n.data(), sizeof(float) * 3);
+  }
+
+  st.camera2body = GeodesicPoses(p->n_divides, r);
+  st.n_views = int(st.camera2body.size() / 12);
+  st.M.assign(size_t(st.n_views) * st.n_slots * 16, 0.0f);
+  st.rot.assign(size_t(st.n_views) * 9, 0.0f);
+  for (int v = 0; v < st.n_views; ++v) {
+    float w2c[12];
+    PoseInverse(st.camera2body.data() + 12 * size_t(v), w2c);  // Renderer::set_camera2world_pose, body2world = I
+    for (int slot = 0; slot < st.n_slots; ++slot) {
+      const int g = slot == 0 ? 0 : slot - 1;
+      const int pr = slot == 0 ? 0 : 1;
+      const GeometryDev& B = ctx->h_geometry[g == 0 ? body : occlusion_bodies[g - 1]];
+      float T[12];
+      PoseMul(w2c, B.geometry2body, T);  // world2camera * geometry2world
+      float* M = st.M.data() + (size_t(v) * st.n_slots + slot) * 16;
+      for (int c = 0; c < 4; ++c) {  // P * [T; 0 0 0 1] without the products with P's zero entries, as k_render
+        M[c] = P00 * T[c] + P02 * T[8 + c];
+        M[4 + c] = P11 * T[4 + c] + P12 * T[8 + c];
+        M[8 + c] = P22[pr] * T[8 + c];
+        M[12 + c] = T[8 + c];
+      }
+      M[11] = M[11] + P23[pr];
+      if (slot == 0)
+        for (int i = 0; i < 3; ++i)
+          for (int j = 0; j < 3; ++j) st.rot[9 * size_t(v) + 3 * i + j] = T[4 * i + j];
+    }
+  }
+  return M3TB_OK;
+}
+
+// Device buffers of one generation call, freed when it returns
+struct ModelBuffers {
+  uint64_t* zbuf = nullptr;
+  float *M = nullptr, *rot = nullptr, *camera2body = nullptr, *face_normals = nullptr, *points = nullptr,
+        *surface_area = nullptr;
+  int* coords = nullptr;
+  ModelBodyDev* bodies = nullptr;
+  int batch = 0;
+  ~ModelBuffers() {
+    cudaFree(zbuf); cudaFree(M); cudaFree(rot); cudaFree(camera2body); cudaFree(face_normals); cudaFree(points);
+    cudaFree(surface_area); cudaFree(coords); cudaFree(bodies);
+  }
+};
+
+// Allocates the buffers for views [first, first + n_views) of `st` (points only when n_points > 0) and uploads their
+// tables; view k of the buffers is view first + k of `st`
+int AllocModel(m3tb_ctx* ctx, const ModelSetup& st, int first, int n_views, int n_points, ModelBuffers& b) {
+  const size_t view_bytes = size_t(st.n_renderers) * st.S * st.S * sizeof(uint64_t);
+  b.batch = int(std::max<size_t>(1, std::min<size_t>({size_t(n_views), kModelScratchBytes / view_bytes, 65535})));
+  const size_t nm = size_t(n_views) * st.n_slots * 16, nr = size_t(n_views) * 9, nc = size_t(n_views) * 12;
+  CU(cudaMalloc(&b.zbuf, view_bytes * b.batch));
+  CU(cudaMalloc(&b.M, sizeof(float) * nm));
+  CU(cudaMalloc(&b.rot, sizeof(float) * nr));
+  CU(cudaMalloc(&b.camera2body, sizeof(float) * nc));
+  CU(cudaMalloc(&b.face_normals, sizeof(float) * st.face_normals.size()));
+  CU(cudaMalloc(&b.bodies, sizeof(ModelBodyDev) * st.bodies.size()));
+  CU(cudaMemcpy(b.M, st.M.data() + size_t(first) * st.n_slots * 16, sizeof(float) * nm, cudaMemcpyHostToDevice));
+  CU(cudaMemcpy(b.rot, st.rot.data() + size_t(first) * 9, sizeof(float) * nr, cudaMemcpyHostToDevice));
+  CU(cudaMemcpy(b.camera2body, st.camera2body.data() + size_t(first) * 12, sizeof(float) * nc, cudaMemcpyHostToDevice));
+  CU(cudaMemcpy(b.face_normals, st.face_normals.data(), sizeof(float) * st.face_normals.size(), cudaMemcpyHostToDevice));
+  CU(cudaMemcpy(b.bodies, st.bodies.data(), sizeof(ModelBodyDev) * st.bodies.size(), cudaMemcpyHostToDevice));
+  if (n_points > 0) {
+    CU(cudaMalloc(&b.coords, sizeof(int) * size_t(b.batch) * n_points));
+    CU(cudaMalloc(&b.points, sizeof(float) * 36 * size_t(n_views) * n_points));
+    CU(cudaMalloc(&b.surface_area, sizeof(float) * n_views));
+  }
+  return M3TB_OK;
+}
+
+// Renders views [first, first + count) into the z-buffers (k_model_raster)
+int RenderModelViews(m3tb_ctx* ctx, const ModelSetup& st, const ModelBuffers& b, int first, int count) {
+  const size_t view_bytes = size_t(st.n_renderers) * st.S * st.S * sizeof(uint64_t);
+  CU(cudaMemsetAsync(b.zbuf, 0xff, view_bytes * count, ctx->stream));  // glClear
+  ModelRasterArgs ra;
+  ra.bodies = b.bodies;
+  ra.n_occlusion = st.n_occlusion;
+  ra.M = b.M + size_t(first) * st.n_slots * 16;
+  ra.zbuf = b.zbuf;
+  ra.n_renderers = st.n_renderers;
+  ra.image_size = st.S;
+  const dim3 grid(unsigned((st.max_triangles + kModelTrianglesPerCta - 1) / kModelTrianglesPerCta), unsigned(count),
+                  unsigned(st.n_renderers));
+  k_model_raster<<<grid, kModelThreads, 0, ctx->stream>>>(ra);
+  CU(cudaGetLastError());
+  ctx->launches++;
+  return M3TB_OK;
+}
+
+ModelPointArgs PointArgs(const ModelSetup& st, const ModelBuffers& b, const m3tb_model_params* p, int first) {
+  ModelPointArgs a;
+  a.zbuf = b.zbuf;
+  a.n_renderers = st.n_renderers;
+  a.image_size = st.S;
+  a.face_normals = b.face_normals;
+  a.rot = b.rot + 9 * size_t(first);
+  a.camera2body = b.camera2body + 12 * size_t(first);
+  a.fu = a.fv = st.fu;
+  a.ppu = a.ppv = st.pp;
+  a.projection_term_a = st.projection_term_a;
+  a.projection_term_b = st.projection_term_b;
+  a.sphere_radius = p->sphere_radius;
+  a.stride_depth_offset = p->stride_depth_offset;
+  a.n_values = int(p->max_radius_depth_offset / p->stride_depth_offset + 1.0f);  // model.cpp:343
+  a.n_points = p->n_points;
+  a.seed = kModelSeed;
+  a.coords = b.coords;
+  a.points = b.points ? b.points + 36 * size_t(first) * p->n_points : nullptr;
+  a.surface_area = b.surface_area ? b.surface_area + first : nullptr;
+  return a;
+}
+
 }  // namespace
 
 extern "C" {
@@ -1528,8 +1801,10 @@ int m3tb_set_depth_model(m3tb_ctx* ctx, int model_id, int n_views, int n_points,
                          const float* surface_areas, const void* points, float stride_depth_offset,
                          float max_radius_depth_offset) {
   CHECK_CTX();
-  return SetModel(ctx, false, model_id, n_views, n_points, orientations, surface_areas, points, stride_depth_offset,
-                  max_radius_depth_offset);
+  const int rc = SetModel(ctx, false, model_id, n_views, n_points, orientations, surface_areas, points,
+                          stride_depth_offset, max_radius_depth_offset);
+  if (!rc && model_id < int(ctx->dmodel_generated.size())) ctx->dmodel_generated[model_id] = {};  // replaced
+  return rc;
 }
 
 int m3tb_set_color_camera(m3tb_ctx* ctx, int cam, const m3tb_intrinsics* intrinsics, const float world2camera[12]) {
@@ -2525,6 +2800,121 @@ int m3tb_get_closest_views(m3tb_ctx* ctx, int body, int* region_view, int* depth
   if (region_view) *region_view = counts[2];
   if (depth_view) *depth_view = counts[3];
   return M3TB_OK;
+}
+
+void m3tb_model_params_default(m3tb_model_params* p) {
+  if (!p) return;
+  p->sphere_radius = 0.8f;  // model.h:161-167
+  p->n_divides = 4;
+  p->n_points = 200;
+  p->max_radius_depth_offset = 0.05f;
+  p->stride_depth_offset = 0.002f;
+  p->use_random_seed = 0;
+  p->image_size = 2000;
+}
+
+int m3tb_model_views(const m3tb_model_params* params, float* camera2body, int capacity, int* n_views) {
+  if (!params || !n_views || capacity < 0 || params->n_divides < 0 || params->n_divides > kModelMaxDivides)
+    return M3TB_ERR_INVALID;
+  const std::vector<float> poses = GeodesicPoses(params->n_divides, params->sphere_radius);
+  *n_views = int(poses.size() / 12);
+  if (camera2body) std::memcpy(camera2body, poses.data(), sizeof(float) * 12 * size_t(std::min(capacity, *n_views)));
+  return M3TB_OK;
+}
+
+int m3tb_generate_depth_model(m3tb_ctx* ctx, int model_id, int body, const int* occlusion_bodies, int n_occlusion_bodies,
+                              const m3tb_model_params* params) {
+  CHECK_CTX();
+  if (model_id < 0 || model_id >= ctx->max_models) return Fail(ctx, M3TB_ERR_INVALID, "model id out of range");
+  ModelSetup st;
+  int rc = PrepareModel(ctx, body, occlusion_bodies, n_occlusion_bodies, params, st);
+  if (rc) return rc;
+  const int n_points = params->n_points;
+  ModelBuffers b;
+  rc = AllocModel(ctx, st, 0, st.n_views, n_points, b);
+  if (rc) return rc;
+  for (int first = 0; first < st.n_views; first += b.batch) {
+    const int count = std::min(b.batch, st.n_views - first);
+    rc = RenderModelViews(ctx, st, b, first, count);
+    if (rc) return rc;
+    k_model_points<<<unsigned(count), kModelThreads, 0, ctx->stream>>>(PointArgs(st, b, params, first));
+    CU(cudaGetLastError());
+    ctx->launches++;
+  }
+  m3tb_ctx::GeneratedModel gm;
+  gm.n_views = st.n_views;
+  gm.n_points = n_points;
+  gm.stride_depth_offset = params->stride_depth_offset;
+  gm.max_radius_depth_offset = params->max_radius_depth_offset;
+  gm.points.resize(size_t(st.n_views) * n_points * 36);
+  gm.surface_areas.resize(st.n_views);
+  CU(cudaMemcpyAsync(gm.points.data(), b.points, sizeof(float) * gm.points.size(), cudaMemcpyDeviceToHost, ctx->stream));
+  CU(cudaMemcpyAsync(gm.surface_areas.data(), b.surface_area, sizeof(float) * st.n_views, cudaMemcpyDeviceToHost,
+                     ctx->stream));
+  CU(cudaStreamSynchronize(ctx->stream));
+  gm.orientations.resize(size_t(st.n_views) * 3);
+  for (int v = 0; v < st.n_views; ++v)  // views_[i].orientation = camera2body.matrix().col(2)
+    for (int r = 0; r < 3; ++r) gm.orientations[3 * size_t(v) + r] = st.camera2body[12 * size_t(v) + 4 * r + 2];
+  // the same path as m3tb_set_depth_model: repacking, depth-offset table, cluster tables of the closest-view search
+  rc = SetModel(ctx, false, model_id, gm.n_views, gm.n_points, gm.orientations.data(), gm.surface_areas.data(),
+                gm.points.data(), params->stride_depth_offset, params->max_radius_depth_offset);
+  if (rc) return rc;
+  if (int(ctx->dmodel_generated.size()) < ctx->max_models) ctx->dmodel_generated.resize(ctx->max_models);
+  ctx->dmodel_generated[model_id] = std::move(gm);
+  return M3TB_OK;
+}
+
+int m3tb_get_depth_model(m3tb_ctx* ctx, int model_id, int* n_views, int* n_points, float* orientations,
+                         float* surface_areas, void* points, float* stride_depth_offset, float* max_radius_depth_offset) {
+  if (!ctx) return M3TB_ERR_INVALID;
+  if (model_id < 0 || model_id >= ctx->max_models) return Fail(ctx, M3TB_ERR_INVALID, "model id out of range");
+  if (model_id >= int(ctx->dmodel_generated.size()) || ctx->dmodel_generated[model_id].n_views == 0)
+    return Fail(ctx, M3TB_ERR_NOT_SET_UP, "depth model was not generated by m3tb_generate_depth_model");
+  const auto& gm = ctx->dmodel_generated[model_id];
+  if (n_views) *n_views = gm.n_views;
+  if (n_points) *n_points = gm.n_points;
+  if (orientations) std::memcpy(orientations, gm.orientations.data(), sizeof(float) * gm.orientations.size());
+  if (surface_areas) std::memcpy(surface_areas, gm.surface_areas.data(), sizeof(float) * gm.surface_areas.size());
+  if (points) std::memcpy(points, gm.points.data(), sizeof(float) * gm.points.size());
+  if (stride_depth_offset) *stride_depth_offset = gm.stride_depth_offset;
+  if (max_radius_depth_offset) *max_radius_depth_offset = gm.max_radius_depth_offset;
+  return M3TB_OK;
+}
+
+int m3tb_debug_render_model_view(m3tb_ctx* ctx, int body, const int* occlusion_bodies, int n_occlusion_bodies,
+                                 const m3tb_model_params* params, int view, uint8_t* normal_bgra, uint16_t* depth,
+                                 uint8_t* silhouette) {
+  CHECK_CTX();
+  ModelSetup st;
+  int rc = PrepareModel(ctx, body, occlusion_bodies, n_occlusion_bodies, params, st);
+  if (rc) return rc;
+  if (view < 0 || view >= st.n_views) return Fail(ctx, M3TB_ERR_INVALID, "view index out of range");
+  ModelBuffers b;
+  rc = AllocModel(ctx, st, view, 1, 0, b);  // one view: its z-buffers and tables only
+  if (!rc) rc = RenderModelViews(ctx, st, b, 0, 1);
+  if (rc) return rc;
+  const size_t n_pix = size_t(st.S) * st.S;
+  uint8_t *d_normal = nullptr, *d_sil = nullptr;
+  uint16_t* d_depth = nullptr;
+  auto run = [&]() -> int {
+    CU(cudaMalloc(&d_normal, 4 * n_pix));
+    CU(cudaMalloc(&d_depth, 2 * n_pix));
+    CU(cudaMalloc(&d_sil, n_pix));
+    k_model_images<<<unsigned((n_pix + 255) / 256), 256, 0, ctx->stream>>>(PointArgs(st, b, params, 0), 0, d_normal,
+                                                                            d_depth, d_sil);
+    CU(cudaGetLastError());
+    ctx->launches++;
+    if (normal_bgra) CU(cudaMemcpyAsync(normal_bgra, d_normal, 4 * n_pix, cudaMemcpyDeviceToHost, ctx->stream));
+    if (depth) CU(cudaMemcpyAsync(depth, d_depth, 2 * n_pix, cudaMemcpyDeviceToHost, ctx->stream));
+    if (silhouette) CU(cudaMemcpyAsync(silhouette, d_sil, n_pix, cudaMemcpyDeviceToHost, ctx->stream));
+    CU(cudaStreamSynchronize(ctx->stream));
+    return M3TB_OK;
+  };
+  rc = run();
+  cudaFree(d_normal);
+  cudaFree(d_depth);
+  cudaFree(d_sil);
+  return rc;
 }
 
 }  // extern "C"

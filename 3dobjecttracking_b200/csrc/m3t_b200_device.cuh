@@ -205,7 +205,7 @@ struct TrackArgs {
 // ---------------------------------------------------------------------------------------------
 // pose helpers: float[12] row-major 3x4, same expressions as the reference's Eigen calls
 // ---------------------------------------------------------------------------------------------
-__device__ __forceinline__ void PoseMul(const float* a, const float* b, float* o) {
+__host__ __device__ __forceinline__ void PoseMul(const float* a, const float* b, float* o) {
 #pragma unroll
   for (int i = 0; i < 3; ++i) {
 #pragma unroll
@@ -222,7 +222,7 @@ __device__ __forceinline__ void PoseApply(const float* p, float vx, float vy, fl
 }
 
 // Transform3fA::inverse() (Affine): 3x3 cofactor inverse, translation = -inv * t  (depth_modality.cpp:644)
-__device__ __forceinline__ void PoseInverse(const float* p, float* o) {
+__host__ __device__ __forceinline__ void PoseInverse(const float* p, float* o) {
   float m[9] = {p[0], p[1], p[2], p[4], p[5], p[6], p[8], p[9], p[10]};
   float inv[9];
 #define M3TB_COF(i, j) (m[3 * (((i) + 1) % 3) + (((j) + 1) % 3)] * m[3 * (((i) + 2) % 3) + (((j) + 2) % 3)] - \

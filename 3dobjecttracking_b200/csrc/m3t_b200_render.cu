@@ -5,81 +5,10 @@
 // the contract and tests/render_reference.py restates it.
 #include <cfloat>
 
+#include "m3t_b200_raster.cuh"
 #include "m3t_b200_render.cuh"
 
 namespace m3tb {
-
-namespace {
-
-struct ClipVertex {
-  float x, y, z, w;
-};
-struct WinVertex {
-  float x, y, z;
-};
-
-// E(a -> b, p) with the endpoints taken in a fixed (x, then y) order, so that the two triangles sharing an edge
-// evaluate it with the same operations and get values of opposite sign (negation is exact)
-__device__ __forceinline__ float EdgeValue(const WinVertex& a, const WinVertex& b, float px, float py) {
-  const bool fwd = a.x < b.x || (a.x == b.x && a.y < b.y);
-  const WinVertex& s = fwd ? a : b;
-  const WinVertex& t = fwd ? b : a;
-  const float e = (t.x - s.x) * (py - s.y) - (t.y - s.y) * (px - s.x);
-  return fwd ? e : -e;
-}
-
-// inside test of one edge of a positively oriented triangle, top-left style tie rule for centres on the edge
-__device__ __forceinline__ bool EdgeCovers(float e, const WinVertex& a, const WinVertex& b) {
-  if (e > 0.0f) return true;
-  if (e < 0.0f) return false;
-  const float dy = b.y - a.y, dx = b.x - a.x;
-  return dy > 0.0f || (dy == 0.0f && dx < 0.0f);
-}
-
-__device__ __forceinline__ ClipVertex Intersect(const ClipVertex& in, float d_in, const ClipVertex& out, float d_out) {
-  const float t = d_in / (d_in - d_out);
-  return {in.x + t * (out.x - in.x), in.y + t * (out.y - in.y), in.z + t * (out.z - in.z), in.w + t * (out.w - in.w)};
-}
-
-__device__ __forceinline__ WinVertex Window(const ClipVertex& c, float half) {
-  return {(c.x / c.w + 1.0f) * half, (c.y / c.w + 1.0f) * half, (c.z / c.w + 1.0f) * 0.5f};
-}
-
-// one (clipped) triangle, the 32 lanes of a warp stride over its pixel bounding box
-__device__ void RasterTriangle(WinVertex v0, WinVertex v1, WinVertex v2, int culling, int S, unsigned draw_index,
-                               uint32_t* zbuf, int lane) {
-  float A = (v1.x - v0.x) * (v2.y - v0.y) - (v2.x - v0.x) * (v1.y - v0.y);
-  if (!(A != 0.0f)) return;             // zero area (or NaN): no fragments
-  if (culling && A > 0.0f) return;      // glFrontFace(GL_CCW) + glCullFace(GL_FRONT)
-  if (A < 0.0f) {
-    const WinVertex t = v1; v1 = v2; v2 = t;
-    A = -A;
-  }
-  const float fS = float(S);
-  const float lo_x = fminf(fmaxf(ceilf(fminf(fminf(v0.x, v1.x), v2.x) - 0.5f), 0.0f), fS);
-  const float hi_x = fminf(fmaxf(floorf(fmaxf(fmaxf(v0.x, v1.x), v2.x) - 0.5f), -1.0f), fS - 1.0f);
-  const float lo_y = fminf(fmaxf(ceilf(fminf(fminf(v0.y, v1.y), v2.y) - 0.5f), 0.0f), fS);
-  const float hi_y = fminf(fmaxf(floorf(fmaxf(fmaxf(v0.y, v1.y), v2.y) - 0.5f), -1.0f), fS - 1.0f);
-  const int i0 = int(lo_x), j0 = int(lo_y);
-  const int nx = int(hi_x) - i0 + 1, ny = int(hi_y) - j0 + 1;
-  if (nx <= 0 || ny <= 0) return;
-  const int n = nx * ny;
-  for (int k = lane; k < n; k += 32) {
-    const int i = i0 + k % nx, j = j0 + k / nx;
-    const float px = float(i) + 0.5f, py = float(j) + 0.5f;
-    const float e0 = EdgeValue(v1, v2, px, py);
-    const float e1 = EdgeValue(v2, v0, px, py);
-    const float e2 = EdgeValue(v0, v1, px, py);
-    if (!EdgeCovers(e0, v1, v2) || !EdgeCovers(e1, v2, v0) || !EdgeCovers(e2, v0, v1)) continue;
-    const float z = (e0 * v0.z + e1 * v1.z + e2 * v2.z) / A;
-    const float q = rintf(z * 65535.0f);   // DEPTH_COMPONENT16
-    if (!(q < 65535.0f)) continue;         // GL_LESS against the cleared 1.0 (and beyond the far plane)
-    const unsigned d16 = unsigned(fmaxf(q, 0.0f));
-    atomicMin(zbuf + j * S + i, (d16 << 16) | draw_index);
-  }
-}
-
-}  // namespace
 
 __global__ void __launch_bounds__(kRenderThreads) k_render(const __grid_constant__ RenderArgs a) {
   extern __shared__ uint32_t zbuf[];
@@ -173,35 +102,10 @@ __global__ void __launch_bounds__(kRenderThreads) k_render(const __grid_constant
       float M[16];
 #pragma unroll
       for (int k = 0; k < 16; ++k) M[k] = sM[k];
-      for (int t = warp; t < G.n_triangles; t += n_warps) {
-        const float* tv = G.triangles + 9 * t;
-        ClipVertex c[3];
-        float dist[3];
-#pragma unroll
-        for (int k = 0; k < 3; ++k) {
-          const float vx = tv[3 * k], vy = tv[3 * k + 1], vz = tv[3 * k + 2];
-          c[k].x = M[0] * vx + M[1] * vy + M[2] * vz + M[3];
-          c[k].y = M[4] * vx + M[5] * vy + M[6] * vz + M[7];
-          c[k].z = M[8] * vx + M[9] * vy + M[10] * vz + M[11];
-          c[k].w = M[12] * vx + M[13] * vy + M[14] * vz + M[15];
-          dist[k] = c[k].z + c[k].w;  // near plane: z_clip >= -w_clip
-        }
-        // Sutherland-Hodgman against the near plane: 0, 3 or 4 vertices, fanned from the first
-        ClipVertex poly[4];
-        int n = 0;
-#pragma unroll
-        for (int e = 0; e < 3; ++e) {
-          const int e1 = e == 2 ? 0 : e + 1;
-          const bool in0 = dist[e] >= 0.0f, in1 = dist[e1] >= 0.0f;
-          if (in0) poly[n++] = c[e];
-          if (in0 != in1)  // computed from the inside vertex, so that both triangles of the edge get the same point
-            poly[n++] = in0 ? Intersect(c[e], dist[e], c[e1], dist[e1]) : Intersect(c[e1], dist[e1], c[e], dist[e]);
-        }
-        if (n < 3) continue;
-        const WinVertex w0 = Window(poly[0], half), w1 = Window(poly[1], half), w2 = Window(poly[2], half);
-        RasterTriangle(w0, w1, w2, G.enable_culling, S, unsigned(g), zbuf, lane);
-        if (n == 4) RasterTriangle(w0, w2, Window(poly[3], half), G.enable_culling, S, unsigned(g), zbuf, lane);
-      }
+      const unsigned draw_index = unsigned(g);
+      auto frag = [&](int i, int j, unsigned d16) { atomicMin(zbuf + j * S + i, (d16 << 16) | draw_index); };
+      for (int t = warp; t < G.n_triangles; t += n_warps)
+        DrawTriangle(M, G.triangles + 9 * t, G.enable_culling, S, half, frag, lane);
       __syncthreads();  // sM is rewritten for the next body
     }
   }

@@ -10,7 +10,8 @@
 //   m3t::Optimizer::CalculateOptimization              -> m3tb_calculate_optimization
 //   m3t::Tracker::ExecuteTrackingStep                  -> m3tb_tracking_step + m3tb_calculate_results (fast path)
 //
-// Focused depth / silhouette renderers exist as device renderers (k_render). Everything else the reference has outside
+// Focused depth / silhouette renderers exist as device renderers (k_render), depth-model generation as
+// DepthModel::GenerateModel (k_model_raster / k_model_points). Everything else the reference has outside
 // this path (full-frame and normal renderers, detectors, viewers, texture modality, YAML metafiles,
 // kinematic constraints) is out of scope here (DESIGN.md). Poses use a minimal Transform3fA (row-major 3x4).
 #ifndef M3T_B200_HPP_
@@ -131,6 +132,16 @@ class Body {
   void set_maximum_body_diameter(float v) { maximum_body_diameter_ = v; }
   void set_body_id(uint8_t v) { body_id_ = v; }
   void set_region_id(uint8_t v) { region_id_ = v; }
+  // what a saved model records about the mesh (Model::SaveBodyData, model.cpp:301-323); the soup above is already
+  // scaled and wound, these only describe where it came from
+  void set_geometry_path(const std::string& v) { geometry_path_ = v; }
+  void set_geometry_unit_in_meter(float v) { geometry_unit_in_meter_ = v; }
+  void set_geometry_counterclockwise(bool v) { geometry_counterclockwise_ = v; }
+  const std::string& geometry_path() const { return geometry_path_; }
+  float geometry_unit_in_meter() const { return geometry_unit_in_meter_; }
+  bool geometry_counterclockwise() const { return geometry_counterclockwise_; }
+  bool geometry_enable_culling() const { return geometry_enable_culling_; }
+  const Transform3fA& geometry2body_pose() const { return geometry2body_pose_; }
   float maximum_body_diameter() const { return maximum_body_diameter_; }
   uint8_t body_id() const { return body_id_; }
   uint8_t region_id() const { return region_id_; }
@@ -157,6 +168,9 @@ class Body {
   bool geometry_enable_culling_ = true;
   float maximum_body_diameter_ = 0.0f;
   uint8_t body_id_ = 0, region_id_ = 0;
+  std::string geometry_path_;
+  float geometry_unit_in_meter_ = 1.0f;
+  bool geometry_counterclockwise_ = true;
 };
 
 // ---- camera.h --------------------------------------------------------------------------------------------------------
@@ -303,6 +317,12 @@ class DepthModel : public Model {
  public:
   DepthModel(const std::string& name, const std::shared_ptr<Batch>& batch) : Model(name, batch, M3TB_DEPTH_POINT_BYTES) {
     index_ = batch->NextDepthModel();
+    m3tb_model_params_default(&params_);
+  }
+  // DepthModel(name, body_ptr, model_path, ...) with the body whose model is generated (depth_model.h:108-114)
+  DepthModel(const std::string& name, const std::shared_ptr<Batch>& batch, const std::shared_ptr<Body>& body_ptr)
+      : DepthModel(name, batch) {
+    body_ptr_ = body_ptr;
   }
   bool SetUp() {
     if (n_views_ == 0) {
@@ -311,10 +331,120 @@ class DepthModel : public Model {
     }
     set_up_ = Check(batch_->ctx(),
                     m3tb_set_depth_model(batch_->ctx(), index_, n_views_, n_points_, orientations_.data(), scalars_.data(),
-                                         points_.data(), 0.002f, 0.05f),
+                                         points_.data(), params_.stride_depth_offset, params_.max_radius_depth_offset),
                     "DepthModel::SetUp");
     return set_up_;
   }
+
+  // model.h setters (model.h:161-167)
+  void set_sphere_radius(float v) { params_.sphere_radius = v; }
+  void set_n_divides(int v) { params_.n_divides = v; }
+  void set_n_points(int v) { params_.n_points = v; }
+  void set_max_radius_depth_offset(float v) { params_.max_radius_depth_offset = v; }
+  void set_stride_depth_offset(float v) { params_.stride_depth_offset = v; }
+  void set_use_random_seed(bool v) { params_.use_random_seed = v ? 1 : 0; }
+  void set_image_size(int v) { params_.image_size = v; }
+  const m3tb_model_params& params() const { return params_; }
+
+  // DepthModel::AddOcclusionBody (depth_model.cpp:61-69)
+  bool AddOcclusionBody(const std::shared_ptr<Body>& body_ptr) {
+    for (auto& b : occlusion_body_ptrs_)
+      if (b->name() == body_ptr->name()) {
+        std::cerr << "Occlusion body " << body_ptr->name() << " already exists" << std::endl;
+        return false;
+      }
+    occlusion_body_ptrs_.push_back(body_ptr);
+    return true;
+  }
+
+  // DepthModel::GenerateModel (depth_model.cpp:144-213) on the device: uploads the meshes, generates, installs the
+  // model for tracking and keeps its views so that SaveModel can write them
+  bool GenerateModel() {
+    if (!body_ptr_) {
+      std::cerr << "Depth model " << name_ << " has no body" << std::endl;
+      return false;
+    }
+    if (!body_ptr_->SetUpGeometry()) return false;
+    std::vector<int> occ;
+    for (auto& b : occlusion_body_ptrs_) {
+      if (!b->SetUpGeometry()) return false;
+      occ.push_back(b->index());
+    }
+    m3tb_ctx* ctx = batch_->ctx();
+    if (!Check(ctx, m3tb_generate_depth_model(ctx, index_, body_ptr_->index(), occ.data(), int(occ.size()), &params_),
+               "DepthModel::GenerateModel"))
+      return false;
+    int nv = 0, np = 0;
+    if (!Check(ctx, m3tb_get_depth_model(ctx, index_, &nv, &np, nullptr, nullptr, nullptr, nullptr, nullptr),
+               "DepthModel::GenerateModel"))
+      return false;
+    std::vector<float> ori(size_t(3) * nv), area(nv), points(size_t(nv) * np * (M3TB_DEPTH_POINT_BYTES / 4));
+    if (!Check(ctx, m3tb_get_depth_model(ctx, index_, nullptr, nullptr, ori.data(), area.data(), points.data(), nullptr,
+                                         nullptr),
+               "DepthModel::GenerateModel"))
+      return false;
+    SetViews(nv, np, ori.data(), area.data(), points.data());
+    set_up_ = true;
+    return true;
+  }
+
+  // DepthModel::SaveModel (model.cpp:286-323, depth_model.cpp:265-291): the reference's .bin layout, version 9
+  bool SaveModel(const std::string& path) const {
+    if (!body_ptr_ || n_views_ == 0) {
+      std::cerr << "Depth model " << name_ << " has no body or no views" << std::endl;
+      return false;
+    }
+    std::ofstream ofs(path, std::ios::out | std::ios::binary);
+    if (!ofs.is_open()) {
+      std::cerr << "Could not open model file " << path << std::endl;
+      return false;
+    }
+    const char type = 'd';
+    const int32_t version = 9;
+    const bool use_random_seed = params_.use_random_seed != 0;
+    Write(ofs, type);
+    Write(ofs, version);
+    Write(ofs, params_.sphere_radius);
+    Write(ofs, int32_t(params_.n_divides));
+    Write(ofs, int32_t(n_points_));
+    Write(ofs, params_.max_radius_depth_offset);
+    Write(ofs, params_.stride_depth_offset);
+    Write(ofs, use_random_seed);
+    Write(ofs, int32_t(params_.image_size));
+    WriteBody(ofs, *body_ptr_);
+    Write(ofs, uint64_t(occlusion_body_ptrs_.size()));
+    for (auto& b : occlusion_body_ptrs_) WriteBody(ofs, *b);
+    Write(ofs, uint64_t(n_views_));
+    for (int v = 0; v < n_views_; ++v) {
+      ofs.write(reinterpret_cast<const char*>(points_.data() + size_t(v) * n_points_ * point_bytes_),
+                std::streamsize(n_points_) * point_bytes_);
+      ofs.write(reinterpret_cast<const char*>(&orientations_[3 * size_t(v)]), 12);
+      Write(ofs, scalars_[v]);
+    }
+    ofs.flush();
+    return bool(ofs);
+  }
+
+ private:
+  template <typename T>
+  static void Write(std::ofstream& ofs, const T& v) {
+    ofs.write(reinterpret_cast<const char*>(&v), sizeof(T));
+  }
+  // Model::SaveBodyData: path, unit, winding, culling, diameter, geometry2body as Eigen's column-major 4x4
+  static void WriteBody(std::ofstream& ofs, const Body& b) {
+    Write(ofs, uint64_t(b.geometry_path().size()));
+    ofs.write(b.geometry_path().data(), std::streamsize(b.geometry_path().size()));
+    Write(ofs, b.geometry_unit_in_meter());
+    Write(ofs, b.geometry_counterclockwise());
+    Write(ofs, b.geometry_enable_culling());
+    Write(ofs, b.maximum_body_diameter());
+    const Transform3fA& g = b.geometry2body_pose();
+    for (int c = 0; c < 4; ++c)
+      for (int r = 0; r < 4; ++r) Write(ofs, r < 3 ? g(r, c) : (c == 3 ? 1.0f : 0.0f));
+  }
+  m3tb_model_params params_{};
+  std::shared_ptr<Body> body_ptr_;
+  std::vector<std::shared_ptr<Body>> occlusion_body_ptrs_;
 };
 
 // ---- renderer_geometry.h / renderer.h / basic_depth_renderer.h / silhouette_renderer.h: device renderers (k_render) ----

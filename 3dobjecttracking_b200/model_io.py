@@ -156,3 +156,14 @@ def model_from_synthetic(model: Model, n_divides=4, sphere_radius=0.8, geometry_
     return ModelFile(kind, 10 if kind == "region" else 9, sphere_radius, n_divides, model.n_points,
                      model.max_radius_depth_offset, model.stride_depth_offset, False, 2000, body,
                      [[], [], [], []] if kind == "region" else [[]], model)
+
+
+def model_from_generated(model: Model, params, body: BodyBlock, occlusion_bodies=()) -> ModelFile:
+    """Wrap a depth model read back from the device (capi.Context.get_depth_model) with the parameters it was generated
+    with (capi.ModelParams) and the caller's body / occlusion-body blocks, so that write_model saves it in the
+    reference's format (DepthModel::SaveModel, depth_model.cpp:265-291)."""
+    if model.kind != "depth":
+        raise ValueError("only depth models are generated")
+    return ModelFile("depth", 9, params.sphere_radius, params.n_divides, model.n_points, params.max_radius_depth_offset,
+                     params.stride_depth_offset, bool(params.use_random_seed), params.image_size, body,
+                     [list(occlusion_bodies)], model)

@@ -440,6 +440,48 @@ typedef struct m3tb_launch_info {
 } m3tb_launch_info;
 int m3tb_debug_last_launch(m3tb_ctx* ctx, m3tb_launch_info* out);
 
+/* ---- depth-model generation (DepthModel::GenerateModel, depth_model.cpp:144-213) -------------------------------- */
+/* Model parameters (model.h:161-167). */
+typedef struct m3tb_model_params {
+  float sphere_radius;            /* distance of the virtual cameras from the body origin [m] */
+  int32_t n_divides;              /* icosahedron subdivisions: 10 * 4^n_divides + 2 views */
+  int32_t n_points;               /* surface points per view */
+  float max_radius_depth_offset;  /* [m] */
+  float stride_depth_offset;      /* [m]; max_radius / stride + 1 must not exceed 30 */
+  int32_t use_random_seed;        /* must be 0: the reference seeds from the clock, which no test can reproduce */
+  int32_t image_size;             /* full-frame render size [px], 21..8192 */
+} m3tb_model_params;
+/* sphere_radius 0.8, n_divides 4, n_points 200, max_radius_depth_offset 0.05, stride_depth_offset 0.002,
+ * use_random_seed 0, image_size 2000 */
+void m3tb_model_params_default(m3tb_model_params* p);
+/* Generates depth model `model_id` of body `body` from the geometry given with m3tb_set_body_geometry: the geodesic
+ * views are rendered on the device, each with the body alone (normal and depth image) and with the body in front of
+ * the `n_occlusion_bodies` occlusion bodies (silhouette), all at body2world = I; a fresh std::mt19937{7} samples the
+ * surface points of each view. The model then serves tracking exactly as if it had been uploaded with
+ * m3tb_set_depth_model. Views whose silhouette is empty get zero-filled points. Returns M3TB_ERR_UNSUPPORTED for
+ * use_random_seed != 0 and M3TB_ERR_INVALID for bad ids, a body without geometry, an offset ratio above 30 or a z_min
+ * below 0.2 * sphere_radius (Model::SetUpRenderer / AddBodiesToRenderer); a refused call leaves the model as it was.
+ * DESIGN.md §3 "k_model_raster / k_model_points" states what is computed. */
+int m3tb_generate_depth_model(m3tb_ctx* ctx, int model_id, int body, const int* occlusion_bodies, int n_occlusion_bodies,
+                              const m3tb_model_params* params);
+/* Reads back a generated depth model; every output may be NULL: *n_views, *n_points, orientations [n_views][3],
+ * surface_areas [n_views], points [n_views][n_points] x 144-B DataPoints (center_f_body[3], normal_f_body[3],
+ * depth_offsets[30]), and the stride_depth_offset / max_radius_depth_offset it was generated with (what
+ * m3tb_set_depth_model needs to rebuild the same depth-offset table). M3TB_ERR_NOT_SET_UP if the model was not
+ * generated by m3tb_generate_depth_model. */
+int m3tb_get_depth_model(m3tb_ctx* ctx, int model_id, int* n_views, int* n_points, float* orientations,
+                         float* surface_areas, void* points, float* stride_depth_offset, float* max_radius_depth_offset);
+/* Host only (no context, no GPU): the geodesic camera2body poses of a model (Model::GenerateGeodesicPoses,
+ * model.cpp:386-454) as [n][12] row-major 3x4, in the order of the model's views; the view orientation is column 2.
+ * *n_views receives the count; at most `capacity` (>= 0) poses are written (camera2body may be NULL). */
+int m3tb_model_views(const m3tb_model_params* params, float* camera2body, int capacity, int* n_views);
+/* Test aid: renders view `view` (geodesic order) of a depth-model generation with these arguments and returns its
+ * normal image (image_size^2 x 4 B, GL_BGRA order, byte 0 = x), depth image (u16) and occlusion silhouette (u8);
+ * any output may be NULL. Refusals as m3tb_generate_depth_model, plus a view index out of range. */
+int m3tb_debug_render_model_view(m3tb_ctx* ctx, int body, const int* occlusion_bodies, int n_occlusion_bodies,
+                                 const m3tb_model_params* params, int view, uint8_t* normal_bgra, uint16_t* depth,
+                                 uint8_t* silhouette);
+
 /* Test aid (host only, no context, no GPU): RegionModel/DepthModel::GetClosestView (region_model.cpp:105-130) for
  * `n_queries` orientation vectors (R^T normalize(t), 3 floats each) over `n_views` view orientations, once by the
  * reference's full scan (`out_scan`) and once by the host restatement of the pruned search the kernels use
