@@ -104,7 +104,7 @@ SYMBOLS = [
     "m3tb_debug_closest_view", "m3tb_upload_depth_rendering", "m3tb_upload_silhouette_rendering",
     "m3tb_share_color_histograms", "m3tb_debug_last_launch", "m3tb_set_body_geometry", "m3tb_set_focused_renderer",
     "m3tb_attach_renderer", "m3tb_render", "m3tb_get_rendering", "m3tb_model_params_default", "m3tb_model_views",
-    "m3tb_generate_depth_model", "m3tb_get_depth_model", "m3tb_debug_render_model_view",
+    "m3tb_generate_depth_model", "m3tb_get_depth_model", "m3tb_debug_render_model_view", "m3tb_debug_resources",
 ]
 
 KERNEL_NAMES = {0: None, 1: "k_track", 2: "k_track2", 3: "k_track_cluster"}
@@ -212,8 +212,18 @@ def lib():
     L.m3tb_generate_depth_model.argtypes = [vp, ci, ci, ip, ci, C.POINTER(ModelParams)]
     L.m3tb_get_depth_model.argtypes = [vp, ci, ip, ip, fp, fp, vp, fp, fp]
     L.m3tb_debug_render_model_view.argtypes = [vp, ci, ip, ci, C.POINTER(ModelParams), ci, vp, vp, vp]
+    L.m3tb_debug_resources.argtypes = [ci, C.POINTER(C.c_longlong)]
     _lib = L
     return L
+
+
+def debug_resources(fail_after=-1):
+    """m3tb_debug_resources: the number of CUDA resources the library holds across all contexts (device and pinned
+    allocations, streams, events). fail_after > 0 arms the n-th resource creation from now on to fail as an allocation
+    failure, 0 disarms, negative only queries."""
+    live = C.c_longlong(0)
+    lib().m3tb_debug_resources(int(fail_after), C.byref(live))
+    return int(live.value)
 
 
 def _f32(a):

@@ -11,9 +11,11 @@
 #include <array>
 #include <set>
 #include <cstring>
+#include <memory>
 #include <string>
 #include <vector>
 
+#include "m3t_b200_owned.h"
 #include "m3t_b200_model.cuh"
 #include "m3t_b200_render.cuh"
 #include "m3t_b200_structures.cuh"
@@ -39,14 +41,16 @@ using namespace m3tb;
 namespace {
 
 struct ImagePool {
-  uint8_t* base = nullptr;
+  DeviceBuffer<uint8_t> base;
   size_t frame_bytes = 0;
   unsigned pitch = 0;
   int width = 0, height = 0, capacity = 0;
   // colour pools: the bin-index images (u16 per pixel), same slot order
-  uint16_t* bins = nullptr;
+  DeviceBuffer<uint8_t> bins;
   size_t bin_frame_bytes = 0;
   unsigned bin_pitch = 0;
+
+  uint16_t* BinImage(int slot) const { return reinterpret_cast<uint16_t*>(bins.get() + bin_frame_bytes * slot); }
 };
 
 // TMA tensor maps over one pool ([camera][row][column] u16), one per tile width; cached per pool base address
@@ -66,12 +70,20 @@ struct StructureHost {
 };
 
 struct ModelAlloc {
-  float4* orientations = nullptr;
-  float* view_scalars = nullptr;
-  float4* points = nullptr;
-  float* depth_offsets = nullptr;
-  float4* cluster_info = nullptr;
-  float4* sorted_views = nullptr;
+  DeviceBuffer<float4> orientations;
+  DeviceBuffer<float> view_scalars, points, depth_offsets, cluster_info, sorted_views;
+};
+
+// Made by the first m3tb_prefetch_frames
+struct PrefetchResources {
+  Stream ingest_stream;
+  Stream table_stream;  // camera tables + counter reset of a prefetch: beside the ingest in flight, not behind it
+  PinnedBuffer<CameraDev> cam_stage[2][2];  // pinned staging [parity][colour | depth]
+  Event ev_ingest_done, ev_poses_snap, ev_tables;
+  Event ev_stage[2];  // the table copies out of cam_stage[parity] have run
+  DeviceBuffer<CameraDev> ccams_alt, dcams_alt;  // second set of camera tables / ROI records
+  DeviceBuffer<RoiRecord> roi_alt;
+  DeviceBuffer<float> poses_snap[2];  // poses at the start of the last two tracking launches (snap_parity)
 };
 
 // which device renderers one k_render launch draws
@@ -91,56 +103,51 @@ struct m3tb_ctx {
   std::vector<CameraDev> h_ccams, h_dcams;
   std::vector<ModelDev> h_rmodels, h_dmodels;
   std::vector<ModelAlloc> rmodel_alloc, dmodel_alloc;
-  std::vector<uint8_t*> private_color, private_depth;  // images that do not fit the pools
+  std::vector<DeviceBuffer<uint8_t>> private_color, private_depth;  // images that do not fit the pools
   bool bodies_dirty = true, cams_dirty = true, models_dirty = true;
 
-  BodyDev* d_bodies = nullptr;
-  CameraDev *d_ccams = nullptr, *d_dcams = nullptr;
-  ModelDev *d_rmodels = nullptr, *d_dmodels = nullptr;
-  float* d_poses = nullptr;
+  DeviceBuffer<BodyDev> d_bodies;
+  DeviceBuffer<CameraDev> d_ccams, d_dcams;
+  DeviceBuffer<ModelDev> d_rmodels, d_dmodels;
+  DeviceBuffer<float> d_poses;
   ImagePool color_pool, depth_pool;
 
-  float *d_hist_f = nullptr, *d_hist_b = nullptr, *d_mem_f = nullptr, *d_mem_b = nullptr;
-  float2* d_lut = nullptr;
+  DeviceBuffer<float> d_hist_f, d_hist_b, d_mem_f, d_mem_b;
+  DeviceBuffer<float2> d_lut;
   size_t hist_stride = 0;
 
-  float *d_rstate = nullptr, *d_dstate = nullptr;
+  DeviceBuffer<float> d_rstate, d_dstate;
   int line_cap = 0, point_cap = 0;
-  int* d_counts = nullptr;
-  float *d_gh_region = nullptr, *d_gh_depth = nullptr;
+  DeviceBuffer<int> d_counts;
+  DeviceBuffer<float> d_gh_region, d_gh_depth;
   size_t max_dyn_smem = 0;
-  RoiRecord* d_roi = nullptr;             // [max_bodies][2]
-  unsigned long long* d_ingest_bytes = nullptr;  // [2]: one counter per ingest launch in flight
+  DeviceBuffer<RoiRecord> d_roi;          // [max_bodies][2]
+  DeviceBuffer<unsigned long long> d_ingest_bytes;  // [2]: one counter per ingest launch in flight
   int ingest_bytes_slot = 0;              // the counter of the last ingest launch
   int sm_count = 132;
   bool ingest_pending = false;            // a pinned frame was handed over since the last k_ingest launch
   // frame prefetch (m3tb_prefetch_frames): second set of image pools / camera tables / ROI records, side stream
   ImagePool color_pool_alt, depth_pool_alt;
-  CameraDev *d_ccams_alt = nullptr, *d_dcams_alt = nullptr;
-  RoiRecord* d_roi_alt = nullptr;
-  float* d_poses_snap[2] = {nullptr, nullptr};  // poses at the start of the last two tracking launches; [snap_parity] is
-  int snap_parity = 0;                    //   what the next prefetch projects with, the other one may still be read by the ingest in flight
-  cudaStream_t ingest_stream = nullptr;
-  cudaStream_t table_stream = nullptr;    // camera tables + counter reset of a prefetch: beside the ingest in flight, not behind it
-  CameraDev* h_cam_stage[2][2] = {{nullptr, nullptr}, {nullptr, nullptr}};  // pinned staging [parity][colour | depth]
+  PrefetchResources pf;
+  int snap_parity = 0;  // pf.poses_snap[snap_parity] is what the next prefetch projects with, the other one may still be
+                        //   read by the ingest in flight
   int stage_parity = 0;
-  cudaEvent_t ev_ingest_done = nullptr, ev_poses_snap = nullptr, ev_tables = nullptr;
-  cudaEvent_t ev_stage[2] = {nullptr, nullptr};  // the table copies out of h_cam_stage[parity] have run
   bool prefetch_enabled = false;          // set by the first m3tb_prefetch_frames
   bool prefetched = false;                // the next consumer launch has to wait for ev_ingest_done
   bool poses_snap_valid = false;
   bool roi_ingest = true;                 // M3TB_NO_ROI_INGEST=1 forces full-frame copies
-  long long* d_phase_clock = nullptr;  // allocated when M3TB_TIMING=1
+  DeviceBuffer<long long> d_phase_clock;  // allocated when M3TB_TIMING=1
   bool use_tiles = true;  // stage ROI tiles in shared memory (M3TB_NO_TILES=1 in the environment disables it)
   bool use_track2 = true; // second-generation fused kernel where it applies (M3TB_KERNEL=1 forces k_track)
   m3tb_launch_info last_launch = {};      // variant of the last tracking launch (m3tb_debug_last_launch)
   std::vector<char> bin_stale;            // per colour camera: the bin-index image does not match the frame copy
   int bin_bitshift = -1;                  // what the bin-index images were built with
-  int* d_bin_ids = nullptr;               // staging for k_bin
-  std::vector<uint8_t*> rendering_allocs; // device copies of the renderer images (m3tb_upload_*_rendering)
+  DeviceBuffer<int> d_bin_ids;            // staging for k_bin
+  // device copies of the renderer images (m3tb_upload_*_rendering), per body and renderer slot
+  std::vector<std::array<DeviceBuffer<uint8_t>, RS_COUNT>> rendering_images;
   std::vector<PoolMaps> pool_maps;        // tensor maps of the pools seen so far (current / alternate x bins / depth)
   int tma_mode = 1;                       // M3TB_TMA: 0 legacy staging, 1 tensor maps in the kernel parameters, 2 in global memory
-  CUtensorMap* d_tmaps = nullptr;         // tma_mode 2: [2][kTileWidths]
+  DeviceBuffer<CUtensorMap> d_tmaps;      // tma_mode 2: [2][kTileWidths]
   const void* d_tmaps_bases[2] = {nullptr, nullptr};  // the pools d_tmaps currently describes
 
   // kinematic structures (empty: every body is its own rigid-body optimiser inside k_track)
@@ -148,35 +155,34 @@ struct m3tb_ctx {
   std::vector<int> hist_owner;
   std::vector<int> hist_table_uploaded;  // what d_hist_owner / d_hist_groups hold
   int n_hist_groups = 0;
-  int* d_hist_owner = nullptr;     // [max_bodies]
-  int* d_hist_groups = nullptr;    // group_owner[n] | group_first[n + 1] | members[...]
-  int hist_groups_capacity = 0;
+  DeviceBuffer<int> d_hist_owner;  // [max_bodies]
+  DeviceBuffer<int> d_hist_groups; // group_owner[n] | group_first[n + 1] | members[...]
   std::vector<StructureHost> structures;
   bool structures_dirty = false;
   int n_struct_launch = 0;                 // user structures + one implicit structure per unreferenced body
-  std::vector<int> struct_first_link;      // per launched structure
   std::vector<int> h_link_bodies;          // body index of every launched link
   bool use_clusters = false;               // M3TB_CLUSTER=1: cluster-fused structure path (see DESIGN.md: measured slower)
   std::vector<StructureDev> h_structures;
-  StructureDev* d_structures = nullptr;
-  LinkDev* d_links = nullptr;
-  LinkDev* d_links_default = nullptr;      // Link::default_body2joint_pose_ / default_joint2parent_pose_
+  DeviceBuffer<StructureDev> d_structures;
+  DeviceBuffer<LinkDev> d_links;
+  DeviceBuffer<LinkDev> d_links_default;   // Link::default_body2joint_pose_ / default_joint2parent_pose_
   int n_links_total = 0;
   bool defaults_valid = false;
   std::vector<LinkDev> h_links_default;
-  ConstraintDev* d_constraints = nullptr;
-  int cap_structures = 0, cap_links = 0, cap_constraints = 0;
-  float* d_gh_link = nullptr;
-  float* d_theta = nullptr;
-  int* d_struct_status = nullptr;
+  DeviceBuffer<ConstraintDev> d_constraints;
+  DeviceBuffer<float> d_gh_link;
+  DeviceBuffer<float> d_theta;             // [d_structures.size()][kMaxSystem]
+  DeviceBuffer<int> d_struct_status;
   size_t struct_smem = 0;
 
   // device renderers (m3tb_set_body_geometry / m3tb_set_focused_renderer / m3tb_attach_renderer, k_render)
   std::vector<GeometryDev> h_geometry;       // [max_bodies]
-  std::vector<float*> geometry_alloc;        // [max_bodies] device triangle soups
-  GeometryDev* d_geometry = nullptr;
+  std::vector<DeviceBuffer<float>> geometry_alloc;  // [max_bodies] device triangle soups
+  DeviceBuffer<GeometryDev> d_geometry;
   struct RendererHost {
-    RendererDev dev;
+    RendererDev dev;  // dev.depth / dev.silhouette view the two images below
+    DeviceBuffer<uint16_t> depth;
+    DeviceBuffer<uint8_t> silhouette;
     std::vector<int> geometry, referenced;
     bool rendered = false;  // images / records exist (m3tb_get_rendering)
   };
@@ -184,17 +190,16 @@ struct m3tb_ctx {
   std::vector<std::array<int, RS_COUNT>> attached;  // per body and renderer slot: the device renderer feeding it, or -1
   std::vector<std::array<char, RS_COUNT>> attach_uploaded;  // the slot's record went to d_bodies once (k_render owns it)
   bool render_dirty = true;                  // the renderer / geometry / attachment tables changed
-  RendererDev* d_renderers = nullptr;
-  int* d_render_lists = nullptr;             // geometry_bodies | referenced_bodies | render_list
-  int* d_visible = nullptr;
-  RenderOutDev* d_render_out = nullptr;
-  RenderAttachDev* d_attach = nullptr;
+  DeviceBuffer<RendererDev> d_renderers;
+  DeviceBuffer<int> d_render_lists;          // geometry_bodies | referenced_bodies | render_list
+  DeviceBuffer<int> d_visible;
+  DeviceBuffer<RenderOutDev> d_render_out;
+  DeviceBuffer<RenderAttachDev> d_attach;
   int n_attached = 0;                        // slots with a device renderer (0: every launch is as without renderers)
   int n_attach = 0, n_geometry_list = 0, n_referenced_list = 0;
   int render_n[kRenderLists] = {};           // renderers in each RenderList
   size_t render_smem[kRenderLists] = {};     // z-buffer bytes of the largest renderer of each list
   std::vector<int> render_list[kRenderLists];  // host copies of the lists
-  size_t render_capacity[4] = {0, 0, 0, 0};  // renderers, list ints, attachments, visible flags
 
   // host copies of the depth models made by m3tb_generate_depth_model (m3tb_get_depth_model); empty: not generated
   struct GeneratedModel {
@@ -243,27 +248,25 @@ size_t Align(size_t v, size_t a) { return (v + a - 1) / a * a; }
 int EnsureHist(m3tb_ctx* ctx, size_t stride) {
   if (stride <= ctx->hist_stride) return M3TB_OK;
   const size_t nb = size_t(ctx->max_bodies);
-  float* nf[4] = {nullptr, nullptr, nullptr, nullptr};
-  float2* nl = nullptr;
+  DeviceBuffer<float> nf[4];
+  DeviceBuffer<float2> nl;
   for (int k = 0; k < 4; ++k) {
-    CU(cudaMalloc(&nf[k], nb * stride * sizeof(float)));
+    CU(nf[k].create(nb * stride));
     CU(cudaMemsetAsync(nf[k], 0, nb * stride * sizeof(float), ctx->stream));
   }
-  CU(cudaMalloc(&nl, nb * stride * sizeof(float2)));
+  CU(nl.create(nb * stride));
   CU(cudaMemsetAsync(nl, 0, nb * stride * sizeof(float2), ctx->stream));
-  float* old[4] = {ctx->d_hist_f, ctx->d_hist_b, ctx->d_mem_f, ctx->d_mem_b};
+  DeviceBuffer<float>* old[4] = {&ctx->d_hist_f, &ctx->d_hist_b, &ctx->d_mem_f, &ctx->d_mem_b};
   if (ctx->hist_stride) {
     for (int k = 0; k < 4; ++k)
-      CU(cudaMemcpy2DAsync(nf[k], stride * sizeof(float), old[k], ctx->hist_stride * sizeof(float),
+      CU(cudaMemcpy2DAsync(nf[k], stride * sizeof(float), *old[k], ctx->hist_stride * sizeof(float),
                            ctx->hist_stride * sizeof(float), nb, cudaMemcpyDeviceToDevice, ctx->stream));
     CU(cudaMemcpy2DAsync(nl, stride * sizeof(float2), ctx->d_lut, ctx->hist_stride * sizeof(float2),
                          ctx->hist_stride * sizeof(float2), nb, cudaMemcpyDeviceToDevice, ctx->stream));
     CU(cudaStreamSynchronize(ctx->stream));
-    for (int k = 0; k < 4; ++k) cudaFree(old[k]);
-    cudaFree(ctx->d_lut);
   }
-  ctx->d_hist_f = nf[0]; ctx->d_hist_b = nf[1]; ctx->d_mem_f = nf[2]; ctx->d_mem_b = nf[3];
-  ctx->d_lut = nl;
+  for (int k = 0; k < 4; ++k) *old[k] = std::move(nf[k]);
+  ctx->d_lut = std::move(nl);
   ctx->hist_stride = stride;
   return M3TB_OK;
 }
@@ -278,19 +281,25 @@ int EnsureState(m3tb_ctx* ctx) {
   }
   lc = int(Align(size_t(std::max(lc, 1)), 32));
   pc = int(Align(size_t(std::max(pc, 1)), 32));
-  if (lc > ctx->line_cap || !ctx->d_rstate) {
-    if (ctx->d_rstate) cudaFree(ctx->d_rstate);
-    CU(cudaMalloc(&ctx->d_rstate, size_t(ctx->max_bodies) * RF_COUNT * lc * sizeof(float)));
-    CU(cudaMemsetAsync(ctx->d_rstate, 0, size_t(ctx->max_bodies) * RF_COUNT * lc * sizeof(float), ctx->stream));
-    // the stored correspondences are gone: a load-state call before the next CalculateCorrespondences sees 0 lines
-    if (ctx->d_counts) CU(cudaMemsetAsync(ctx->d_counts, 0, sizeof(int) * 4 * ctx->max_bodies, ctx->stream));
+  const bool grow_r = lc > ctx->line_cap || !ctx->d_rstate, grow_d = pc > ctx->point_cap || !ctx->d_dstate;
+  if (!grow_r && !grow_d) return M3TB_OK;
+  DeviceBuffer<float> rs, ds;
+  if (grow_r) {
+    CU(rs.create(size_t(ctx->max_bodies) * RF_COUNT * lc));
+    CU(cudaMemsetAsync(rs, 0, size_t(ctx->max_bodies) * RF_COUNT * lc * sizeof(float), ctx->stream));
+  }
+  if (grow_d) {
+    CU(ds.create(size_t(ctx->max_bodies) * DF_COUNT * pc));
+    CU(cudaMemsetAsync(ds, 0, size_t(ctx->max_bodies) * DF_COUNT * pc * sizeof(float), ctx->stream));
+  }
+  // the stored correspondences are gone: a load-state call before the next CalculateCorrespondences sees 0 lines
+  CU(cudaMemsetAsync(ctx->d_counts, 0, sizeof(int) * 4 * ctx->max_bodies, ctx->stream));
+  if (grow_r) {
+    ctx->d_rstate = std::move(rs);
     ctx->line_cap = lc;
   }
-  if (pc > ctx->point_cap || !ctx->d_dstate) {
-    if (ctx->d_dstate) cudaFree(ctx->d_dstate);
-    CU(cudaMalloc(&ctx->d_dstate, size_t(ctx->max_bodies) * DF_COUNT * pc * sizeof(float)));
-    CU(cudaMemsetAsync(ctx->d_dstate, 0, size_t(ctx->max_bodies) * DF_COUNT * pc * sizeof(float), ctx->stream));
-    if (ctx->d_counts) CU(cudaMemsetAsync(ctx->d_counts, 0, sizeof(int) * 4 * ctx->max_bodies, ctx->stream));
+  if (grow_d) {
+    ctx->d_dstate = std::move(ds);
     ctx->point_cap = pc;
   }
   return M3TB_OK;
@@ -372,7 +381,7 @@ int ValidateBodies(m3tb_ctx* ctx) {
 // Frame ingest for pinned host frames: fetch every body's ROI (k_ingest) before the first consumer of the new frame.
 int LaunchIngestIfPending(m3tb_ctx* ctx) {
   if (ctx->prefetched) {  // the frames were prefetched on the side stream: order the consumers behind that ingest
-    CU(cudaStreamWaitEvent(ctx->stream, ctx->ev_ingest_done, 0));
+    CU(cudaStreamWaitEvent(ctx->stream, ctx->pf.ev_ingest_done, 0));
     ctx->prefetched = false;
   }
   if (!ctx->ingest_pending) return M3TB_OK;
@@ -538,9 +547,9 @@ int LaunchTrack(m3tb_ctx* ctx, int iteration, int corr_begin, int corr_end, int 
     // snapshot of the launch before (it is finished before this buffer's turn comes again: the launch in between
     // waits for it).
     ctx->snap_parity ^= 1;
-    CU(cudaMemcpyAsync(ctx->d_poses_snap[ctx->snap_parity], ctx->d_poses, sizeof(float) * 12 * ctx->n_bodies,
+    CU(cudaMemcpyAsync(ctx->pf.poses_snap[ctx->snap_parity], ctx->d_poses, sizeof(float) * 12 * ctx->n_bodies,
                        cudaMemcpyDeviceToDevice, ctx->stream));
-    CU(cudaEventRecord(ctx->ev_poses_snap, ctx->stream));
+    CU(cudaEventRecord(ctx->pf.ev_poses_snap, ctx->stream));
     ctx->poses_snap_valid = true;
   }
   rc = LaunchIngestIfPending(ctx);
@@ -733,7 +742,6 @@ int SyncStructures(m3tb_ctx* ctx) {
   std::vector<ConstraintDev> cons;
   std::vector<StructureDev> sts;
   std::vector<char> used(ctx->n_bodies, 0);
-  ctx->struct_first_link.clear();
   size_t smem = 0;
   auto push = [&](const std::vector<LinkDev>& L, const std::vector<ConstraintDev>& C, float lr, float lt) {
     StructureDev d;
@@ -747,7 +755,6 @@ int SyncStructures(m3tb_ctx* ctx) {
     for (const auto& c : C) d.n_rows += c.soft ? 0 : c.n_rows;
     d.tikhonov_rotation = lr;
     d.tikhonov_translation = lt;
-    ctx->struct_first_link.push_back(d.first_link);
     links.insert(links.end(), L.begin(), L.end());
     cons.insert(cons.end(), C.begin(), C.end());
     sts.push_back(d);
@@ -781,24 +788,34 @@ int SyncStructures(m3tb_ctx* ctx) {
          ctx->h_bodies[b].tikhonov_translation);
   }
   const int ns = int(sts.size()), nl = int(links.size()), nc = int(std::max<size_t>(cons.size(), 1));
-  if (ns > ctx->cap_structures) {
-    cudaFree(ctx->d_structures); cudaFree(ctx->d_theta); cudaFree(ctx->d_struct_status);
-    CU(cudaMalloc(&ctx->d_structures, sizeof(StructureDev) * ns));
-    CU(cudaMalloc(&ctx->d_theta, sizeof(float) * kMaxSystem * ns));
-    CU(cudaMalloc(&ctx->d_struct_status, sizeof(int) * ns));
-    ctx->cap_structures = ns;
+  // grow the tables: every new one is made before any old one is replaced
+  DeviceBuffer<StructureDev> structures;
+  DeviceBuffer<float> theta;
+  DeviceBuffer<int> status;
+  DeviceBuffer<LinkDev> dlinks, dlinks_default;
+  DeviceBuffer<ConstraintDev> constraints;
+  const bool grow_s = size_t(ns) > ctx->d_structures.size(), grow_l = size_t(nl) > ctx->d_links.size(),
+             grow_c = size_t(nc) > ctx->d_constraints.size();
+  if (grow_s) {
+    CU(structures.create(ns));
+    CU(theta.create(size_t(kMaxSystem) * ns));
+    CU(status.create(ns));
   }
-  if (nl > ctx->cap_links) {
-    cudaFree(ctx->d_links); cudaFree(ctx->d_links_default);
-    CU(cudaMalloc(&ctx->d_links, sizeof(LinkDev) * nl));
-    CU(cudaMalloc(&ctx->d_links_default, sizeof(LinkDev) * nl));
-    ctx->cap_links = nl;
+  if (grow_l) {
+    CU(dlinks.create(nl));
+    CU(dlinks_default.create(nl));
   }
-  if (nc > ctx->cap_constraints) {
-    cudaFree(ctx->d_constraints);
-    CU(cudaMalloc(&ctx->d_constraints, sizeof(ConstraintDev) * nc));
-    ctx->cap_constraints = nc;
+  if (grow_c) CU(constraints.create(nc));
+  if (grow_s) {
+    ctx->d_structures = std::move(structures);
+    ctx->d_theta = std::move(theta);
+    ctx->d_struct_status = std::move(status);
   }
+  if (grow_l) {
+    ctx->d_links = std::move(dlinks);
+    ctx->d_links_default = std::move(dlinks_default);
+  }
+  if (grow_c) ctx->d_constraints = std::move(constraints);
   CU(cudaMemsetAsync(ctx->d_theta, 0, sizeof(float) * kMaxSystem * ns, ctx->stream));
   CU(cudaMemsetAsync(ctx->d_struct_status, 0, sizeof(int) * ns, ctx->stream));
   CU(cudaMemcpyAsync(ctx->d_structures, sts.data(), sizeof(StructureDev) * ns, cudaMemcpyHostToDevice, ctx->stream));
@@ -841,7 +858,7 @@ int LaunchStructure(m3tb_ctx* ctx, int mode, bool from_modalities) {
   a.links = ctx->d_links;
   a.constraints = ctx->d_constraints;
   a.poses = ctx->d_poses;
-  a.gh_link = from_modalities ? nullptr : ctx->d_gh_link;
+  a.gh_link = from_modalities ? nullptr : ctx->d_gh_link.get();
   a.gh_region = ctx->d_gh_region;
   a.gh_depth = ctx->d_gh_depth;
   a.mode = mode;
@@ -972,14 +989,14 @@ int LaunchHistogram(m3tb_ctx* ctx, int mode, int iteration) {
     std::vector<int> table(group_owner);
     table.insert(table.end(), group_first.begin(), group_first.end());
     table.insert(table.end(), members.begin(), members.end());
-    if (!ctx->d_hist_owner) CU(cudaMalloc(&ctx->d_hist_owner, sizeof(int) * ctx->max_bodies));
-    if (int(table.size()) > ctx->hist_groups_capacity) {
+    DeviceBuffer<int> owner, groups;
+    if (!ctx->d_hist_owner) CU(owner.create(ctx->max_bodies));
+    if (table.size() > ctx->d_hist_groups.size()) {
+      CU(groups.create(table.size()));
       CU(cudaStreamSynchronize(ctx->stream));
-      cudaFree(ctx->d_hist_groups);
-      ctx->d_hist_groups = nullptr;
-      CU(cudaMalloc(&ctx->d_hist_groups, sizeof(int) * table.size()));
-      ctx->hist_groups_capacity = int(table.size());
+      ctx->d_hist_groups = std::move(groups);
     }
+    if (owner) ctx->d_hist_owner = std::move(owner);
     std::vector<int> key(table);  // groups + the per-body owners of the bodies that exist now
     key.insert(key.end(), ctx->hist_owner.begin(), ctx->hist_owner.begin() + ctx->n_bodies);
     if (key != ctx->hist_table_uploaded) {
@@ -1010,15 +1027,12 @@ int LaunchHistogram(m3tb_ctx* ctx, int mode, int iteration) {
   return M3TB_OK;
 }
 
-// Grows a device table to hold `n` elements (contents are rewritten by the caller).
+// A device table of at least `n` elements: `table` itself when it is large enough, else a new one in `grown` (contents
+// are rewritten by the caller).
 template <typename T>
-int EnsureCapacity(m3tb_ctx* ctx, T*& ptr, size_t& capacity, size_t n) {
-  if (n <= capacity && ptr) return M3TB_OK;
-  CU(cudaStreamSynchronize(ctx->stream));  // a launch in flight may still read the old table
-  cudaFree(ptr);
-  ptr = nullptr;
-  capacity = std::max<size_t>(n, 16);
-  CU(cudaMalloc(&ptr, sizeof(T) * capacity));
+int GrowTable(m3tb_ctx* ctx, const DeviceBuffer<T>& table, DeviceBuffer<T>& grown, size_t n) {
+  if (n <= table.size()) return M3TB_OK;
+  CU(grown.create(std::max<size_t>(n, 16)));
   return M3TB_OK;
 }
 
@@ -1029,14 +1043,14 @@ int SyncRenderTables(m3tb_ctx* ctx) {
   std::vector<RendererDev> devs(nr);
   std::vector<int> geo, ref;
   for (int r = 0; r < nr; ++r) {
-    auto& h = ctx->renderers[r];
-    h.dev.first_geometry = int(geo.size());
-    h.dev.n_geometry = int(h.geometry.size());
-    h.dev.first_referenced = int(ref.size());
-    h.dev.n_referenced = int(h.referenced.size());
+    const auto& h = ctx->renderers[r];
+    devs[r] = h.dev;
+    devs[r].first_geometry = int(geo.size());
+    devs[r].n_geometry = int(h.geometry.size());
+    devs[r].first_referenced = int(ref.size());
+    devs[r].n_referenced = int(h.referenced.size());
     geo.insert(geo.end(), h.geometry.begin(), h.geometry.end());
     ref.insert(ref.end(), h.referenced.begin(), h.referenced.end());
-    devs[r] = h.dev;
   }
   std::vector<RenderAttachDev> att;
   for (int b = 0; b < ctx->max_bodies; ++b)
@@ -1066,20 +1080,36 @@ int SyncRenderTables(m3tb_ctx* ctx) {
       ctx->render_n[pass]++;
       ctx->render_smem[pass] = std::max(ctx->render_smem[pass], size_t(devs[r].image_size) * devs[r].image_size * sizeof(uint32_t));
     }
-  int rc = EnsureCapacity(ctx, ctx->d_renderers, ctx->render_capacity[0], size_t(std::max(nr, 1)));
-  if (!rc) rc = EnsureCapacity(ctx, ctx->d_render_lists, ctx->render_capacity[1], std::max<size_t>(lists.size(), 1));
-  if (!rc) rc = EnsureCapacity(ctx, ctx->d_attach, ctx->render_capacity[2], std::max<size_t>(att.size(), 1));
-  if (!rc) rc = EnsureCapacity(ctx, ctx->d_visible, ctx->render_capacity[3], std::max<size_t>(ref.size(), 1));
+  DeviceBuffer<RendererDev> renderers;
+  DeviceBuffer<int> render_lists, visible;
+  DeviceBuffer<RenderAttachDev> attach;
+  DeviceBuffer<RenderOutDev> render_out;
+  DeviceBuffer<GeometryDev> geometry;
+  int rc = GrowTable(ctx, ctx->d_renderers, renderers, size_t(std::max(nr, 1)));
+  if (!rc) rc = GrowTable(ctx, ctx->d_render_lists, render_lists, std::max<size_t>(lists.size(), 1));
+  if (!rc) rc = GrowTable(ctx, ctx->d_attach, attach, std::max<size_t>(att.size(), 1));
+  if (!rc) rc = GrowTable(ctx, ctx->d_visible, visible, std::max<size_t>(ref.size(), 1));
   if (rc) return rc;
-  if (!ctx->d_render_out) CU(cudaMalloc(&ctx->d_render_out, sizeof(RenderOutDev) * size_t(4 * ctx->max_bodies)));
-  if (!ctx->d_geometry) CU(cudaMalloc(&ctx->d_geometry, sizeof(GeometryDev) * ctx->max_bodies));
-  CU(cudaStreamSynchronize(ctx->stream));  // the host vectors below are temporaries (set-up path, not per step)
+  if (!ctx->d_render_out) CU(render_out.create(4 * size_t(ctx->max_bodies)));
+  if (!ctx->d_geometry) CU(geometry.create(ctx->max_bodies));
+  // the host vectors below are temporaries (set-up path, not per step), and a launch in flight may still read the
+  // tables that are replaced
+  CU(cudaStreamSynchronize(ctx->stream));
+  if (renderers) ctx->d_renderers = std::move(renderers);
+  if (render_lists) ctx->d_render_lists = std::move(render_lists);
+  if (attach) ctx->d_attach = std::move(attach);
+  if (visible) ctx->d_visible = std::move(visible);
+  if (render_out) ctx->d_render_out = std::move(render_out);
+  if (geometry) ctx->d_geometry = std::move(geometry);
   if (nr) CU(cudaMemcpy(ctx->d_renderers, devs.data(), sizeof(RendererDev) * nr, cudaMemcpyHostToDevice));
   if (!lists.empty()) CU(cudaMemcpy(ctx->d_render_lists, lists.data(), sizeof(int) * lists.size(), cudaMemcpyHostToDevice));
   if (!att.empty()) CU(cudaMemcpy(ctx->d_attach, att.data(), sizeof(RenderAttachDev) * att.size(), cudaMemcpyHostToDevice));
   CU(cudaMemcpy(ctx->d_geometry, ctx->h_geometry.data(), sizeof(GeometryDev) * ctx->max_bodies, cudaMemcpyHostToDevice));
   ctx->n_attach = int(att.size());
-  for (auto& h : ctx->renderers) h.rendered = false;  // offsets / visible flags moved: read-back waits for the next render
+  for (int r = 0; r < nr; ++r) {
+    ctx->renderers[r].dev = devs[r];
+    ctx->renderers[r].rendered = false;  // offsets / visible flags moved: read-back waits for the next render
+  }
   ctx->n_geometry_list = int(geo.size());
   ctx->n_referenced_list = int(ref.size());
   ctx->render_dirty = false;
@@ -1125,13 +1155,6 @@ int SetModel(m3tb_ctx* ctx, bool region, int model_id, int n_views, int n_points
              const float* scalars, const void* points, float stride_depth_offset, float max_radius_depth_offset) {
   if (model_id < 0 || model_id >= ctx->max_models || n_views <= 0 || n_points <= 0 || !orientations || !points)
     return Fail(ctx, M3TB_ERR_INVALID, "bad model arguments");
-  std::vector<ModelAlloc>& allocs = region ? ctx->rmodel_alloc : ctx->dmodel_alloc;
-  ModelAlloc& al = allocs[model_id];
-  if (al.orientations) {
-    cudaFree(al.orientations); cudaFree(al.view_scalars); cudaFree(al.points); cudaFree(al.depth_offsets);
-    cudaFree(al.cluster_info); cudaFree(al.sorted_views);
-    al = ModelAlloc();
-  }
   // Repack the .bin AoS DataPoints (152 B / 144 B) into the 32 B records the kernels read:
   // region (cx,cy,cz,nx)(ny,nz,fg,bg), depth (cx,cy,cz,nx)(ny,nz,0,0). One-time setup, not on the hot path.
   const int fl = region ? M3TB_REGION_POINT_BYTES / 4 : M3TB_DEPTH_POINT_BYTES / 4;
@@ -1162,10 +1185,12 @@ int SetModel(m3tb_ctx* ctx, bool region, int model_id, int n_views, int n_points
   std::vector<float> ori4(size_t(n_views) * 4, 0.0f);
   for (int v = 0; v < n_views; ++v)
     for (int c = 0; c < 3; ++c) ori4[size_t(v) * 4 + c] = orientations[3 * v + c];
-  CU(cudaMalloc(&al.orientations, sizeof(float4) * n_views));
-  CU(cudaMalloc(&al.view_scalars, sizeof(float) * n_views));
-  CU(cudaMalloc(&al.points, sizeof(float) * packed.size()));
-  CU(cudaMalloc(&al.depth_offsets, sizeof(float) * offsets.size()));
+  // the new model is complete on the device before it replaces the old one (both exist for a moment)
+  ModelAlloc al;
+  CU(al.orientations.create(n_views));
+  CU(al.view_scalars.create(n_views));
+  CU(al.points.create(packed.size()));
+  CU(al.depth_offsets.create(offsets.size()));
   CU(cudaMemcpyAsync(al.depth_offsets, offsets.data(), sizeof(float) * offsets.size(), cudaMemcpyHostToDevice, ctx->stream));
   CU(cudaMemcpyAsync(al.orientations, ori4.data(), sizeof(float4) * n_views, cudaMemcpyHostToDevice, ctx->stream));
   CU(cudaMemcpyAsync(al.view_scalars, sc.data(), sizeof(float) * n_views, cudaMemcpyHostToDevice, ctx->stream));
@@ -1173,8 +1198,8 @@ int SetModel(m3tb_ctx* ctx, bool region, int model_id, int n_views, int n_points
   // cluster tables of the pruned closest-view search (one-time, host)
   ViewClustersHost vc;
   BuildViewClusters(orientations, n_views, vc);
-  CU(cudaMalloc(&al.cluster_info, sizeof(float) * std::max<size_t>(vc.info.size(), 8)));
-  CU(cudaMalloc(&al.sorted_views, sizeof(float) * vc.sorted.size()));
+  CU(al.cluster_info.create(std::max<size_t>(vc.info.size(), 8)));
+  CU(al.sorted_views.create(vc.sorted.size()));
   CU(cudaMemcpyAsync(al.cluster_info, vc.info.data(), sizeof(float) * vc.info.size(), cudaMemcpyHostToDevice, ctx->stream));
   CU(cudaMemcpyAsync(al.sorted_views, vc.sorted.data(), sizeof(float) * vc.sorted.size(), cudaMemcpyHostToDevice, ctx->stream));
   CU(cudaStreamSynchronize(ctx->stream));  // staging vectors go out of scope
@@ -1183,16 +1208,17 @@ int SetModel(m3tb_ctx* ctx, bool region, int model_id, int n_views, int n_points
   m.n_points = n_points;
   m.orientations4 = al.orientations;
   m.view_scalars = al.view_scalars;
-  m.points = al.points;
+  m.points = reinterpret_cast<const float4*>(al.points.get());
   m.max_view_scalar = max_scalar;
   m.radius = std::sqrt(radius2);
   m.depth_offsets = al.depth_offsets;
   m.stride_depth_offset = stride_depth_offset;
   m.max_radius_depth_offset = max_radius_depth_offset;
-  m.cluster_info = al.cluster_info;
-  m.sorted_views = al.sorted_views;
+  m.cluster_info = reinterpret_cast<const float4*>(al.cluster_info.get());
+  m.sorted_views = reinterpret_cast<const float4*>(al.sorted_views.get());
   m.n_clusters = vc.n_clusters;
   m.set = 1;
+  (region ? ctx->rmodel_alloc : ctx->dmodel_alloc)[model_id] = std::move(al);  // releases the old model
   ctx->models_dirty = true;
   return M3TB_OK;
 }
@@ -1212,42 +1238,55 @@ int SetCamera(m3tb_ctx* ctx, bool color, int cam, const m3tb_intrinsics* in, con
   return M3TB_OK;
 }
 
-// Device storage of camera `cam`'s frame: a slot of the shared pool when the dimensions match the
-// pool's (so that a batch of frames is one contiguous copy), a private allocation otherwise.
-int EnsureImage(m3tb_ctx* ctx, bool color, int cam) {
-  CameraDev& c = (color ? ctx->h_ccams : ctx->h_dcams)[cam];
-  if (!c.set) return Fail(ctx, M3TB_ERR_NOT_SET_UP, "set the camera before uploading images");
-  if (c.image) return M3TB_OK;
+// Device storage of the frames of cameras [first, first + count): a slot of the shared pool when the dimensions match
+// the pool's (so that a batch of frames is one contiguous copy), a private allocation otherwise. The first frame sets
+// the pool's dimensions. The cameras change only once every allocation has succeeded.
+int EnsureImages(m3tb_ctx* ctx, bool color, int first, int count) {
+  std::vector<CameraDev>& cams = color ? ctx->h_ccams : ctx->h_dcams;
   ImagePool& pool = color ? ctx->color_pool : ctx->depth_pool;
-  const unsigned pitch = unsigned(Align(size_t(c.width) * (color ? 3 : 2), 16));
-  if (!pool.base) {
-    pool.width = c.width; pool.height = c.height; pool.pitch = pitch;
-    pool.frame_bytes = size_t(pitch) * c.height;
-    pool.capacity = ctx->max_cameras;
-    CU(cudaMalloc(&pool.base, pool.frame_bytes * pool.capacity));
-    if (color && (c.width & 3) == 0) {
-      pool.bin_pitch = unsigned(Align(size_t(c.width) * 2, 16));
-      pool.bin_frame_bytes = size_t(pool.bin_pitch) * c.height;
-      CU(cudaMalloc(&pool.bins, pool.bin_frame_bytes * pool.capacity));
+  auto pitch_of = [&](const CameraDev& c) { return unsigned(Align(size_t(c.width) * (color ? 3 : 2), 16)); };
+  ImagePool new_pool;
+  const ImagePool* p = &pool;
+  std::vector<DeviceBuffer<uint8_t>> priv(count);
+  for (int k = 0; k < count; ++k) {
+    const CameraDev& c = cams[first + k];
+    if (!c.set) return Fail(ctx, M3TB_ERR_NOT_SET_UP, "set the camera before uploading images");
+    if (c.image) continue;
+    if (!p->base) {
+      new_pool.width = c.width; new_pool.height = c.height; new_pool.pitch = pitch_of(c);
+      new_pool.frame_bytes = size_t(new_pool.pitch) * c.height;
+      new_pool.capacity = ctx->max_cameras;
+      CU(new_pool.base.create(new_pool.frame_bytes * new_pool.capacity));
+      if (color && (c.width & 3) == 0) {
+        new_pool.bin_pitch = unsigned(Align(size_t(c.width) * 2, 16));
+        new_pool.bin_frame_bytes = size_t(new_pool.bin_pitch) * c.height;
+        CU(new_pool.bins.create(new_pool.bin_frame_bytes * new_pool.capacity));
+      }
+      p = &new_pool;
     }
+    if (p->width != c.width || p->height != c.height) CU(priv[k].create(size_t(pitch_of(c)) * c.height));
   }
-  if (pool.width == c.width && pool.height == c.height) {
-    c.image = pool.base + pool.frame_bytes * cam;
-    c.pitch = pool.pitch;
-    if (color && pool.bins) {
-      c.bins = reinterpret_cast<uint16_t*>(reinterpret_cast<uint8_t*>(pool.bins) + pool.bin_frame_bytes * cam);
-      c.bin_pitch = pool.bin_pitch;
+  if (new_pool.base) pool = std::move(new_pool);
+  for (int k = 0; k < count; ++k) {
+    const int cam = first + k;
+    CameraDev& c = cams[cam];
+    if (c.image) continue;
+    if (!priv[k]) {
+      c.image = pool.base + pool.frame_bytes * cam;
+      c.pitch = pool.pitch;
+      if (color && pool.bins) {
+        c.bins = pool.BinImage(cam);
+        c.bin_pitch = pool.bin_pitch;
+      }
+    } else {
+      c.bins = nullptr;
+      c.bin_pitch = 0;
+      c.image = priv[k];
+      c.pitch = pitch_of(c);
+      (color ? ctx->private_color : ctx->private_depth)[cam] = std::move(priv[k]);
     }
-  } else {
-    c.bins = nullptr;
-    c.bin_pitch = 0;
-    uint8_t*& priv = (color ? ctx->private_color : ctx->private_depth)[cam];
-    if (priv) cudaFree(priv);
-    CU(cudaMalloc(&priv, size_t(pitch) * c.height));
-    c.image = priv;
-    c.pitch = pitch;
+    ctx->cams_dirty = true;
   }
-  ctx->cams_dirty = true;
   return M3TB_OK;
 }
 
@@ -1267,7 +1306,7 @@ const uint8_t* PinnedAlias(m3tb_ctx* ctx, const void* host) {
 int Upload(m3tb_ctx* ctx, bool color, int cam, const void* src, size_t pitch, cudaMemcpyKind kind,
            const uint8_t* pinned_alias) {
   if (cam < 0 || cam >= ctx->max_cameras || !src) return Fail(ctx, M3TB_ERR_INVALID, "bad upload arguments");
-  int rc = EnsureImage(ctx, color, cam);
+  int rc = EnsureImages(ctx, color, cam, 1);
   if (rc) return rc;
   CameraDev& c = (color ? ctx->h_ccams : ctx->h_dcams)[cam];
   const size_t row = size_t(c.width) * (color ? 3 : 2);
@@ -1292,10 +1331,10 @@ int UploadBatch(m3tb_ctx* ctx, bool color, int first, int count, const void* src
   if (first < 0 || count <= 0 || first + count > ctx->max_cameras || !src)
     return Fail(ctx, M3TB_ERR_INVALID, "bad batch upload arguments");
   ImagePool& pool = color ? ctx->color_pool : ctx->depth_pool;
+  int rc = EnsureImages(ctx, color, first, count);
+  if (rc) return rc;
   bool pooled = true;
   for (int k = 0; k < count; ++k) {
-    int rc = EnsureImage(ctx, color, first + k);
-    if (rc) return rc;
     const CameraDev& c = (color ? ctx->h_ccams : ctx->h_dcams)[first + k];
     pooled = pooled && pool.base && c.image == pool.base + pool.frame_bytes * (first + k);
   }
@@ -1513,18 +1552,13 @@ int PrepareModel(m3tb_ctx* ctx, int body, const int* occlusion_bodies, int n_occ
   return M3TB_OK;
 }
 
-// Device buffers of one generation call, freed when it returns
+// Device buffers of one generation call, released when it returns
 struct ModelBuffers {
-  uint64_t* zbuf = nullptr;
-  float *M = nullptr, *rot = nullptr, *camera2body = nullptr, *face_normals = nullptr, *points = nullptr,
-        *surface_area = nullptr;
-  int* coords = nullptr;
-  ModelBodyDev* bodies = nullptr;
+  DeviceBuffer<uint64_t> zbuf;
+  DeviceBuffer<float> M, rot, camera2body, face_normals, points, surface_area;
+  DeviceBuffer<int> coords;
+  DeviceBuffer<ModelBodyDev> bodies;
   int batch = 0;
-  ~ModelBuffers() {
-    cudaFree(zbuf); cudaFree(M); cudaFree(rot); cudaFree(camera2body); cudaFree(face_normals); cudaFree(points);
-    cudaFree(surface_area); cudaFree(coords); cudaFree(bodies);
-  }
 };
 
 // Allocates the buffers for views [first, first + n_views) of `st` (points only when n_points > 0) and uploads their
@@ -1533,21 +1567,21 @@ int AllocModel(m3tb_ctx* ctx, const ModelSetup& st, int first, int n_views, int 
   const size_t view_bytes = size_t(st.n_renderers) * st.S * st.S * sizeof(uint64_t);
   b.batch = int(std::max<size_t>(1, std::min<size_t>({size_t(n_views), kModelScratchBytes / view_bytes, 65535})));
   const size_t nm = size_t(n_views) * st.n_slots * 16, nr = size_t(n_views) * 9, nc = size_t(n_views) * 12;
-  CU(cudaMalloc(&b.zbuf, view_bytes * b.batch));
-  CU(cudaMalloc(&b.M, sizeof(float) * nm));
-  CU(cudaMalloc(&b.rot, sizeof(float) * nr));
-  CU(cudaMalloc(&b.camera2body, sizeof(float) * nc));
-  CU(cudaMalloc(&b.face_normals, sizeof(float) * st.face_normals.size()));
-  CU(cudaMalloc(&b.bodies, sizeof(ModelBodyDev) * st.bodies.size()));
+  CU(b.zbuf.create(view_bytes / sizeof(uint64_t) * b.batch));
+  CU(b.M.create(nm));
+  CU(b.rot.create(nr));
+  CU(b.camera2body.create(nc));
+  CU(b.face_normals.create(st.face_normals.size()));
+  CU(b.bodies.create(st.bodies.size()));
   CU(cudaMemcpy(b.M, st.M.data() + size_t(first) * st.n_slots * 16, sizeof(float) * nm, cudaMemcpyHostToDevice));
   CU(cudaMemcpy(b.rot, st.rot.data() + size_t(first) * 9, sizeof(float) * nr, cudaMemcpyHostToDevice));
   CU(cudaMemcpy(b.camera2body, st.camera2body.data() + size_t(first) * 12, sizeof(float) * nc, cudaMemcpyHostToDevice));
   CU(cudaMemcpy(b.face_normals, st.face_normals.data(), sizeof(float) * st.face_normals.size(), cudaMemcpyHostToDevice));
   CU(cudaMemcpy(b.bodies, st.bodies.data(), sizeof(ModelBodyDev) * st.bodies.size(), cudaMemcpyHostToDevice));
   if (n_points > 0) {
-    CU(cudaMalloc(&b.coords, sizeof(int) * size_t(b.batch) * n_points));
-    CU(cudaMalloc(&b.points, sizeof(float) * 36 * size_t(n_views) * n_points));
-    CU(cudaMalloc(&b.surface_area, sizeof(float) * n_views));
+    CU(b.coords.create(size_t(b.batch) * n_points));
+    CU(b.points.create(36 * size_t(n_views) * n_points));
+    CU(b.surface_area.create(n_views));
   }
   return M3TB_OK;
 }
@@ -1652,6 +1686,38 @@ void m3tb_optimizer_params_default(m3tb_optimizer_params* p) {
   p->tikhonov_parameter_translation = 30000.0f;
 }
 
+// The device tables every context has; m3tb_create's context owns them from here on.
+static int CreateTables(m3tb_ctx* ctx, bool want_timing) {
+  const size_t nb = size_t(ctx->max_bodies), nc = size_t(ctx->max_cameras), nm = size_t(ctx->max_models);
+  CU(cudaSetDevice(ctx->device));
+  CU(ctx->d_bodies.create(nb));
+  CU(ctx->d_ccams.create(nc));
+  CU(ctx->d_dcams.create(nc));
+  CU(ctx->d_rmodels.create(nm));
+  CU(ctx->d_dmodels.create(nm));
+  CU(ctx->d_poses.create(12 * nb));
+  CU(ctx->d_counts.create(4 * nb));
+  CU(ctx->d_gh_region.create(27 * nb));
+  CU(ctx->d_gh_depth.create(27 * nb));
+  CU(cudaMemset(ctx->d_poses, 0, sizeof(float) * 12 * nb));
+  CU(cudaMemset(ctx->d_counts, 0, sizeof(int) * 4 * nb));
+  CU(cudaMemset(ctx->d_gh_region, 0, sizeof(float) * 27 * nb));
+  CU(cudaMemset(ctx->d_gh_depth, 0, sizeof(float) * 27 * nb));
+  CU(ctx->d_gh_link.create(27 * nb));
+  CU(cudaMemset(ctx->d_gh_link, 0, sizeof(float) * 27 * nb));
+  CU(ctx->d_roi.create(2 * nb));
+  CU(cudaMemset(ctx->d_roi, 0xff, sizeof(RoiRecord) * 2 * nb));  // generation -1: nothing ingested yet
+  CU(ctx->d_bin_ids.create(nc));
+  CU(ctx->d_tmaps.create(2 * kTileWidths));
+  CU(ctx->d_ingest_bytes.create(2));
+  CU(cudaMemset(ctx->d_ingest_bytes, 0, 2 * sizeof(unsigned long long)));
+  if (want_timing) {
+    CU(ctx->d_phase_clock.create(kPhaseSlots * nb));
+    CU(cudaMemset(ctx->d_phase_clock, 0, sizeof(long long) * kPhaseSlots * nb));
+  }
+  return M3TB_OK;
+}
+
 int m3tb_create(int device, int max_bodies, int max_cameras, int max_models, m3tb_ctx** out) {
   if (!out || max_bodies <= 0 || max_cameras <= 0 || max_models <= 0) return M3TB_ERR_INVALID;
   *out = nullptr;
@@ -1660,7 +1726,7 @@ int m3tb_create(int device, int max_bodies, int max_cameras, int max_models, m3t
   cudaDeviceProp prop;
   if (cudaGetDeviceProperties(&prop, device) != cudaSuccess) return M3TB_ERR_CUDA;
   if (prop.major != 9 || prop.minor != 0) return M3TB_ERR_CUDA;  // sm_90a cubin only: no other architecture can run it
-  m3tb_ctx* ctx = new m3tb_ctx();
+  std::unique_ptr<m3tb_ctx> ctx(new m3tb_ctx());
   ctx->device = device;
   ctx->sm_count = prop.multiProcessorCount;
   ctx->max_bodies = max_bodies;
@@ -1676,14 +1742,15 @@ int m3tb_create(int device, int max_bodies, int max_cameras, int max_models, m3t
   ctx->h_dmodels.assign(max_models, ModelDev());
   std::memset(ctx->h_rmodels.data(), 0, sizeof(ModelDev) * max_models);
   std::memset(ctx->h_dmodels.data(), 0, sizeof(ModelDev) * max_models);
-  ctx->rmodel_alloc.assign(max_models, ModelAlloc());
-  ctx->dmodel_alloc.assign(max_models, ModelAlloc());
-  ctx->private_color.assign(max_cameras, nullptr);
-  ctx->private_depth.assign(max_cameras, nullptr);
+  ctx->rmodel_alloc.resize(max_models);
+  ctx->dmodel_alloc.resize(max_models);
+  ctx->private_color.resize(max_cameras);
+  ctx->private_depth.resize(max_cameras);
   ctx->bin_stale.assign(max_cameras, 1);
   ctx->h_geometry.assign(max_bodies, GeometryDev());
   std::memset(ctx->h_geometry.data(), 0, sizeof(GeometryDev) * max_bodies);
-  ctx->geometry_alloc.assign(max_bodies, nullptr);
+  ctx->geometry_alloc.resize(max_bodies);
+  ctx->rendering_images.resize(max_bodies);
   ctx->attached.assign(max_bodies, std::array<int, RS_COUNT>{-1, -1, -1, -1});
   ctx->attach_uploaded.assign(max_bodies, std::array<char, RS_COUNT>{0, 0, 0, 0});
   if (const char* e = std::getenv("M3TB_NO_TILES")) ctx->use_tiles = !(e[0] == '1');
@@ -1692,81 +1759,21 @@ int m3tb_create(int device, int max_bodies, int max_cameras, int max_models, m3t
   if (const char* e = std::getenv("M3TB_KERNEL")) ctx->use_track2 = !(e[0] == '1');
   if (const char* e = std::getenv("M3TB_TMA")) ctx->tma_mode = (e[0] >= '0' && e[0] <= '2') ? e[0] - '0' : 1;
   const char* timing_env = std::getenv("M3TB_TIMING");
-  const bool want_timing = timing_env && timing_env[0] == '1';
-  auto alloc = [&]() -> int {
-    CU(cudaSetDevice(device));
-    CU(cudaMalloc(&ctx->d_bodies, sizeof(BodyDev) * max_bodies));
-    CU(cudaMalloc(&ctx->d_ccams, sizeof(CameraDev) * max_cameras));
-    CU(cudaMalloc(&ctx->d_dcams, sizeof(CameraDev) * max_cameras));
-    CU(cudaMalloc(&ctx->d_rmodels, sizeof(ModelDev) * max_models));
-    CU(cudaMalloc(&ctx->d_dmodels, sizeof(ModelDev) * max_models));
-    CU(cudaMalloc(&ctx->d_poses, sizeof(float) * 12 * max_bodies));
-    CU(cudaMalloc(&ctx->d_counts, sizeof(int) * 4 * max_bodies));
-    CU(cudaMalloc(&ctx->d_gh_region, sizeof(float) * 27 * max_bodies));
-    CU(cudaMalloc(&ctx->d_gh_depth, sizeof(float) * 27 * max_bodies));
-    CU(cudaMemset(ctx->d_poses, 0, sizeof(float) * 12 * max_bodies));
-    CU(cudaMemset(ctx->d_counts, 0, sizeof(int) * 4 * max_bodies));
-    CU(cudaMemset(ctx->d_gh_region, 0, sizeof(float) * 27 * max_bodies));
-    CU(cudaMemset(ctx->d_gh_depth, 0, sizeof(float) * 27 * max_bodies));
-    CU(cudaMalloc(&ctx->d_gh_link, sizeof(float) * 27 * max_bodies));
-    CU(cudaMemset(ctx->d_gh_link, 0, sizeof(float) * 27 * max_bodies));
-    CU(cudaMalloc(&ctx->d_roi, sizeof(RoiRecord) * 2 * max_bodies));
-    CU(cudaMemset(ctx->d_roi, 0xff, sizeof(RoiRecord) * 2 * max_bodies));  // generation -1: nothing ingested yet
-    CU(cudaMalloc(&ctx->d_bin_ids, sizeof(int) * max_cameras));
-    CU(cudaMalloc(&ctx->d_tmaps, sizeof(CUtensorMap) * 2 * kTileWidths));
-    CU(cudaMalloc(&ctx->d_ingest_bytes, 2 * sizeof(unsigned long long)));
-    CU(cudaMemset(ctx->d_ingest_bytes, 0, 2 * sizeof(unsigned long long)));
-    if (want_timing) {
-      CU(cudaMalloc(&ctx->d_phase_clock, sizeof(long long) * kPhaseSlots * max_bodies));
-      CU(cudaMemset(ctx->d_phase_clock, 0, sizeof(long long) * kPhaseSlots * max_bodies));
-    }
-    return M3TB_OK;
-  };
-  int rc = alloc();
+  const int rc = CreateTables(ctx.get(), timing_env && timing_env[0] == '1');
   if (rc != M3TB_OK) {
     std::fprintf(stderr, "m3tb_create: %s\n", ctx->err.c_str());
-    m3tb_destroy(ctx);
     return rc;
   }
-  *out = ctx;
+  *out = ctx.release();
   return M3TB_OK;
 }
 
 int m3tb_destroy(m3tb_ctx* ctx) {
   if (!ctx) return M3TB_ERR_INVALID;
   cudaSetDevice(ctx->device);
-  cudaStreamSynchronize(ctx->stream);
-  for (auto* al : {&ctx->rmodel_alloc, &ctx->dmodel_alloc})
-    for (auto& a : *al) {
-      cudaFree(a.orientations); cudaFree(a.view_scalars); cudaFree(a.points); cudaFree(a.depth_offsets);
-      cudaFree(a.cluster_info); cudaFree(a.sorted_views);
-    }
-  for (auto p : ctx->rendering_allocs) cudaFree(p);
-  for (auto p : ctx->private_color) cudaFree(p);
-  for (auto p : ctx->private_depth) cudaFree(p);
-  cudaFree(ctx->color_pool.base); cudaFree(ctx->depth_pool.base);
-  cudaFree(ctx->color_pool.bins); cudaFree(ctx->color_pool_alt.bins); cudaFree(ctx->d_bin_ids); cudaFree(ctx->d_tmaps);
-  cudaFree(ctx->d_bodies); cudaFree(ctx->d_ccams); cudaFree(ctx->d_dcams); cudaFree(ctx->d_rmodels);
-  cudaFree(ctx->d_dmodels); cudaFree(ctx->d_poses); cudaFree(ctx->d_counts); cudaFree(ctx->d_gh_region);
-  cudaFree(ctx->d_gh_depth); cudaFree(ctx->d_hist_f); cudaFree(ctx->d_hist_b); cudaFree(ctx->d_mem_f);
-  cudaFree(ctx->d_mem_b); cudaFree(ctx->d_lut); cudaFree(ctx->d_rstate); cudaFree(ctx->d_dstate);
-  cudaFree(ctx->d_phase_clock); cudaFree(ctx->d_roi); cudaFree(ctx->d_ingest_bytes);
-  cudaFree(ctx->color_pool_alt.base); cudaFree(ctx->depth_pool_alt.base); cudaFree(ctx->d_ccams_alt);
-  cudaFree(ctx->d_dcams_alt); cudaFree(ctx->d_roi_alt); cudaFree(ctx->d_poses_snap[0]); cudaFree(ctx->d_poses_snap[1]);
-  if (ctx->table_stream) { cudaStreamSynchronize(ctx->table_stream); cudaStreamDestroy(ctx->table_stream); }
-  if (ctx->ingest_stream) { cudaStreamSynchronize(ctx->ingest_stream); cudaStreamDestroy(ctx->ingest_stream); }
-  for (int q = 0; q < 4; ++q) cudaFreeHost(ctx->h_cam_stage[q >> 1][q & 1]);
-  if (ctx->ev_ingest_done) cudaEventDestroy(ctx->ev_ingest_done);
-  if (ctx->ev_poses_snap) cudaEventDestroy(ctx->ev_poses_snap);
-  if (ctx->ev_tables) cudaEventDestroy(ctx->ev_tables);
-  for (int q = 0; q < 2; ++q) if (ctx->ev_stage[q]) cudaEventDestroy(ctx->ev_stage[q]);
-  cudaFree(ctx->d_structures); cudaFree(ctx->d_links); cudaFree(ctx->d_links_default); cudaFree(ctx->d_constraints);
-  cudaFree(ctx->d_gh_link);
-  cudaFree(ctx->d_theta); cudaFree(ctx->d_struct_status); cudaFree(ctx->d_hist_owner); cudaFree(ctx->d_hist_groups);
-  for (auto p : ctx->geometry_alloc) cudaFree(p);
-  for (auto& r : ctx->renderers) { cudaFree(r.dev.depth); cudaFree(r.dev.silhouette); }
-  cudaFree(ctx->d_geometry); cudaFree(ctx->d_renderers); cudaFree(ctx->d_render_lists); cudaFree(ctx->d_visible);
-  cudaFree(ctx->d_render_out); cudaFree(ctx->d_attach);
+  cudaStreamSynchronize(ctx->stream);  // not owned: the caller's stream of m3tb_set_stream, or the default stream
+  if (ctx->pf.table_stream) cudaStreamSynchronize(ctx->pf.table_stream);
+  if (ctx->pf.ingest_stream) cudaStreamSynchronize(ctx->pf.ingest_stream);
   delete ctx;
   return M3TB_OK;
 }
@@ -1780,7 +1787,7 @@ int m3tb_set_stream(m3tb_ctx* ctx, void* cuda_stream) {
 
 int m3tb_synchronize(m3tb_ctx* ctx) {
   CHECK_CTX();
-  if (ctx->ingest_stream) CU(cudaStreamSynchronize(ctx->ingest_stream));
+  if (ctx->pf.ingest_stream) CU(cudaStreamSynchronize(ctx->pf.ingest_stream));
   CU(cudaStreamSynchronize(ctx->stream));
   return M3TB_OK;
 }
@@ -2400,73 +2407,82 @@ int m3tb_prefetch_frames(m3tb_ctx* ctx) {
       if (!c.host_src || !pool.base || c.image != pool.base + pool.frame_bytes * i) return M3TB_OK;
     }
   }
-  if (!ctx->ingest_stream) {
-    CU(cudaStreamCreateWithFlags(&ctx->ingest_stream, cudaStreamNonBlocking));
-    CU(cudaStreamCreateWithFlags(&ctx->table_stream, cudaStreamNonBlocking));
-    CU(cudaEventCreateWithFlags(&ctx->ev_ingest_done, cudaEventDisableTiming));
-    CU(cudaEventCreateWithFlags(&ctx->ev_poses_snap, cudaEventDisableTiming));
-    CU(cudaEventCreateWithFlags(&ctx->ev_tables, cudaEventDisableTiming));
-    for (int q = 0; q < 2; ++q) CU(cudaEventCreateWithFlags(&ctx->ev_stage[q], cudaEventDisableTiming));
-    for (int q = 0; q < 4; ++q) CU(cudaMallocHost(&ctx->h_cam_stage[q >> 1][q & 1], sizeof(CameraDev) * ctx->max_cameras));
-    CU(cudaMalloc(&ctx->d_ccams_alt, sizeof(CameraDev) * ctx->max_cameras));
-    CU(cudaMalloc(&ctx->d_dcams_alt, sizeof(CameraDev) * ctx->max_cameras));
-    CU(cudaMalloc(&ctx->d_roi_alt, sizeof(RoiRecord) * 2 * ctx->max_bodies));
-    CU(cudaMemset(ctx->d_roi_alt, 0xff, sizeof(RoiRecord) * 2 * ctx->max_bodies));
-    for (int q = 0; q < 2; ++q) CU(cudaMalloc(&ctx->d_poses_snap[q], sizeof(float) * 12 * ctx->max_bodies));
+  // Everything this call creates is made first and moved into the context once all of it exists.
+  PrefetchResources pf;
+  if (!ctx->pf.ingest_stream) {
+    CU(pf.ingest_stream.create());
+    CU(pf.table_stream.create());
+    CU(pf.ev_ingest_done.create());
+    CU(pf.ev_poses_snap.create());
+    CU(pf.ev_tables.create());
+    for (int q = 0; q < 2; ++q) CU(pf.ev_stage[q].create());
+    for (int q = 0; q < 4; ++q) CU(pf.cam_stage[q >> 1][q & 1].create(ctx->max_cameras));
+    CU(pf.ccams_alt.create(ctx->max_cameras));
+    CU(pf.dcams_alt.create(ctx->max_cameras));
+    CU(pf.roi_alt.create(2 * size_t(ctx->max_bodies)));
+    CU(cudaMemset(pf.roi_alt, 0xff, sizeof(RoiRecord) * 2 * ctx->max_bodies));
+    for (int q = 0; q < 2; ++q) CU(pf.poses_snap[q].create(12 * size_t(ctx->max_bodies)));
   }
+  ImagePool new_alt[2];
+  for (int k = 0; k < 2; ++k) {
+    const ImagePool& pool = k == 0 ? ctx->color_pool : ctx->depth_pool;
+    const ImagePool& alt = k == 0 ? ctx->color_pool_alt : ctx->depth_pool_alt;
+    if (pool.base && !alt.base) {
+      ImagePool& n = new_alt[k];
+      n.frame_bytes = pool.frame_bytes; n.pitch = pool.pitch;
+      n.width = pool.width; n.height = pool.height; n.capacity = pool.capacity;
+      n.bin_frame_bytes = pool.bin_frame_bytes; n.bin_pitch = pool.bin_pitch;
+      CU(n.base.create(n.frame_bytes * n.capacity));
+      if (pool.bins) CU(n.bins.create(n.bin_frame_bytes * n.capacity));
+    }
+  }
+  if (pf.ingest_stream) ctx->pf = std::move(pf);
   for (int k = 0; k < 2; ++k) {
     ImagePool& pool = k == 0 ? ctx->color_pool : ctx->depth_pool;
     ImagePool& alt = k == 0 ? ctx->color_pool_alt : ctx->depth_pool_alt;
-    if (pool.base && !alt.base) {
-      alt = pool;
-      alt.base = nullptr;
-      alt.bins = nullptr;
-      CU(cudaMalloc(&alt.base, alt.frame_bytes * alt.capacity));
-      if (pool.bins) CU(cudaMalloc(&alt.bins, alt.bin_frame_bytes * alt.capacity));
-    }
+    if (new_alt[k].base) alt = std::move(new_alt[k]);
     std::swap(pool, alt);
     std::vector<CameraDev>& cams = k == 0 ? ctx->h_ccams : ctx->h_dcams;
     for (int i = 0; i < ctx->max_cameras; ++i)
       if (cams[i].set && cams[i].image) {
         cams[i].image = pool.base + pool.frame_bytes * i;
-        if (k == 0 && pool.bins)
-          cams[i].bins = reinterpret_cast<uint16_t*>(reinterpret_cast<uint8_t*>(pool.bins) + pool.bin_frame_bytes * i);
+        if (k == 0 && pool.bins) cams[i].bins = pool.BinImage(i);
       }
   }
   ctx->cams_dirty = false;   // the camera tables go to the alternate device copies below, on the side stream
   int rc = SyncTables(ctx);  // bodies / models only (main stream, small)
   if (rc) return rc;
-  std::swap(ctx->d_ccams, ctx->d_ccams_alt);
-  std::swap(ctx->d_dcams, ctx->d_dcams_alt);
-  std::swap(ctx->d_roi, ctx->d_roi_alt);
+  std::swap(ctx->d_ccams, ctx->pf.ccams_alt);
+  std::swap(ctx->d_dcams, ctx->pf.dcams_alt);
+  std::swap(ctx->d_roi, ctx->pf.roi_alt);
   // Stream plan. The ingest stream runs the ingests back to back: anything queued on it in front of k_ingest would sit
   // between two PCIe-bound kernels (two pageable table copies, a memset and the wait for the pose snapshot would
   // lengthen every end-to-end step). So the set-up goes to a third stream, beside the ingest in flight: wait for the pose
   // snapshot of the last tracking launch (which also orders it behind every reader of the buffers swapped in above: they
   // precede that launch on the main stream), camera tables from pinned staging, counter reset; the ingest stream then
   // waits for one event that is normally long past.
-  cudaStream_t is = ctx->ingest_stream, ts = ctx->table_stream;
+  cudaStream_t is = ctx->pf.ingest_stream, ts = ctx->pf.table_stream;
   const float* poses = ctx->d_poses;
   if (ctx->poses_snap_valid) {
-    CU(cudaStreamWaitEvent(ts, ctx->ev_poses_snap, 0));
-    poses = ctx->d_poses_snap[ctx->snap_parity];
+    CU(cudaStreamWaitEvent(ts, ctx->pf.ev_poses_snap, 0));
+    poses = ctx->pf.poses_snap[ctx->snap_parity];
   } else {
     CU(cudaStreamSynchronize(ctx->stream));  // first frame: nothing in flight that could be writing the poses
   }
   ctx->stage_parity ^= 1;  // the staging of the prefetch before this one may still be in flight; the one before that
-  CU(cudaEventSynchronize(ctx->ev_stage[ctx->stage_parity]));  // normally is not (a host that never waits could be ahead)
-  CameraDev* stage_c = ctx->h_cam_stage[ctx->stage_parity][0];
-  CameraDev* stage_d = ctx->h_cam_stage[ctx->stage_parity][1];
+  CU(cudaEventSynchronize(ctx->pf.ev_stage[ctx->stage_parity]));  // normally is not (a host that never waits could be ahead)
+  CameraDev* stage_c = ctx->pf.cam_stage[ctx->stage_parity][0];
+  CameraDev* stage_d = ctx->pf.cam_stage[ctx->stage_parity][1];
   std::memcpy(stage_c, ctx->h_ccams.data(), sizeof(CameraDev) * ctx->max_cameras);
   std::memcpy(stage_d, ctx->h_dcams.data(), sizeof(CameraDev) * ctx->max_cameras);
   CU(cudaMemcpyAsync(ctx->d_ccams, stage_c, sizeof(CameraDev) * ctx->max_cameras, cudaMemcpyHostToDevice, ts));
   CU(cudaMemcpyAsync(ctx->d_dcams, stage_d, sizeof(CameraDev) * ctx->max_cameras, cudaMemcpyHostToDevice, ts));
-  CU(cudaEventRecord(ctx->ev_stage[ctx->stage_parity], ts));
+  CU(cudaEventRecord(ctx->pf.ev_stage[ctx->stage_parity], ts));
   ctx->cams_dirty = false;
   ctx->ingest_bytes_slot ^= 1;
   CU(cudaMemsetAsync(ctx->d_ingest_bytes + ctx->ingest_bytes_slot, 0, sizeof(unsigned long long), ts));
-  CU(cudaEventRecord(ctx->ev_tables, ts));
-  CU(cudaStreamWaitEvent(is, ctx->ev_tables, 0));
+  CU(cudaEventRecord(ctx->pf.ev_tables, ts));
+  CU(cudaStreamWaitEvent(is, ctx->pf.ev_tables, 0));
   IngestArgs a;
   a.bodies = ctx->d_bodies;
   a.poses = poses;
@@ -2488,7 +2504,7 @@ int m3tb_prefetch_frames(m3tb_ctx* ctx) {
   ingest_ctas = std::min(ingest_ctas, ctx->n_bodies);
   k_ingest<<<ingest_ctas, kBlockThreads, 0, is>>>(a);
   CU(cudaGetLastError());
-  CU(cudaEventRecord(ctx->ev_ingest_done, is));
+  CU(cudaEventRecord(ctx->pf.ev_ingest_done, is));
   ctx->launches++;
   ctx->ingest_pending = false;
   ctx->prefetched = true;
@@ -2505,18 +2521,12 @@ static int UploadRendering(m3tb_ctx* ctx, int body, int slot, const m3tb_renderi
   RenderingDev& d = ctx->h_bodies[body].rend[slot];
   const unsigned pitch = unsigned(Align(size_t(r->image_size) * bytes_per_pixel, 16));
   if (!d.image || d.image_size != r->image_size) {
-    if (d.image) {
-      CU(cudaStreamSynchronize(ctx->stream));
-      uint8_t* old = const_cast<uint8_t*>(d.image);
-      for (auto& q : ctx->rendering_allocs)
-        if (q == old) q = nullptr;
-      cudaFree(old);
-      d.image = nullptr;
-    }
-    uint8_t* p = nullptr;
-    CU(cudaMalloc(&p, size_t(pitch) * r->image_size));
-    ctx->rendering_allocs.push_back(p);
-    d.image = p;
+    DeviceBuffer<uint8_t> image;
+    CU(image.create(size_t(pitch) * r->image_size));
+    if (d.image) CU(cudaStreamSynchronize(ctx->stream));
+    ctx->rendering_images[body][slot] = std::move(image);
+    d.image = ctx->rendering_images[body][slot];
+    ctx->bodies_dirty = true;  // the device copy of the record must not keep the released image
   }
   CU(cudaMemcpy2DAsync(const_cast<uint8_t*>(d.image), pitch, r->image, r->pitch, size_t(r->image_size) * bytes_per_pixel,
                        r->image_size, cudaMemcpyDefault, ctx->stream));
@@ -2554,17 +2564,18 @@ int m3tb_set_body_geometry(m3tb_ctx* ctx, int body, const float* triangles, int 
   if (body_id < 0 || body_id > 255 || region_id < 0 || region_id > 255)
     return Fail(ctx, M3TB_ERR_INVALID, "body_id / region_id must be uint8 values");
   GeometryDev& G = ctx->h_geometry[body];
-  if (ctx->geometry_alloc[body] && G.n_triangles != n_triangles) {
-    CU(cudaStreamSynchronize(ctx->stream));  // a render in flight may still read the old soup
-    cudaFree(ctx->geometry_alloc[body]);
-    ctx->geometry_alloc[body] = nullptr;
+  DeviceBuffer<float>& soup = ctx->geometry_alloc[body];
+  if (soup.size() != 9 * size_t(n_triangles)) {
+    DeviceBuffer<float> s;
+    CU(s.create(9 * size_t(n_triangles)));
+    if (soup) CU(cudaStreamSynchronize(ctx->stream));  // a render in flight may still read the old soup
+    soup = std::move(s);
+    G.triangles = soup;
+    G.n_triangles = n_triangles;
   }
-  if (!ctx->geometry_alloc[body]) CU(cudaMalloc(&ctx->geometry_alloc[body], sizeof(float) * 9 * size_t(n_triangles)));
-  CU(cudaMemcpyAsync(ctx->geometry_alloc[body], triangles, sizeof(float) * 9 * size_t(n_triangles), cudaMemcpyHostToDevice,
+  CU(cudaMemcpyAsync(soup, triangles, sizeof(float) * 9 * size_t(n_triangles), cudaMemcpyHostToDevice,
                      ctx->stream));
   CU(cudaStreamSynchronize(ctx->stream));  // the caller's triangles are free again
-  G.triangles = ctx->geometry_alloc[body];
-  G.n_triangles = n_triangles;
   std::memcpy(G.geometry2body, geometry2body, sizeof(G.geometry2body));
   G.radius = 0.5f * maximum_body_diameter;  // FocusedRenderer::CalculateProjectionMatrix (renderer.cpp:356)
   G.enable_culling = enable_culling ? 1 : 0;
@@ -2606,25 +2617,31 @@ int m3tb_set_focused_renderer(m3tb_ctx* ctx, int renderer, int camera_kind, int 
     for (const auto& at : ctx->attached)
       for (int r : at)
         if (r == renderer) return Fail(ctx, M3TB_ERR_INVALID, "renderer is attached to a modality: detach it first");
-  if (renderer == int(ctx->renderers.size())) {
-    m3tb_ctx::RendererHost h;
-    std::memset(&h.dev, 0, sizeof(h.dev));
-    ctx->renderers.push_back(h);
+  const bool is_new = renderer == int(ctx->renderers.size());
+  const unsigned depth_pitch = unsigned(Align(size_t(image_size) * 2, 16));
+  const unsigned silhouette_pitch = unsigned(Align(size_t(image_size), 16));
+  DeviceBuffer<uint16_t> depth;
+  DeviceBuffer<uint8_t> silhouette;
+  if (is_new || ctx->renderers[renderer].dev.image_size != image_size) {
+    CU(depth.create(size_t(depth_pitch) / 2 * image_size));
+    CU(silhouette.create(size_t(silhouette_pitch) * image_size));
+    CU(cudaStreamSynchronize(ctx->stream));  // a render in flight may still write the old images
+    CU(cudaMemsetAsync(depth, 0xff, size_t(depth_pitch) * image_size, ctx->stream));  // cleared: depth 1.0
+    CU(cudaMemsetAsync(silhouette, 0, size_t(silhouette_pitch) * image_size, ctx->stream));
+  }
+  if (is_new) {
+    ctx->renderers.emplace_back();
+    std::memset(&ctx->renderers.back().dev, 0, sizeof(RendererDev));
   }
   auto& h = ctx->renderers[renderer];
   RendererDev& R = h.dev;
-  if (R.image_size != image_size) {
-    CU(cudaStreamSynchronize(ctx->stream));
-    cudaFree(R.depth);
-    cudaFree(R.silhouette);
-    R.depth = nullptr;
-    R.silhouette = nullptr;
-    R.depth_pitch = unsigned(Align(size_t(image_size) * 2, 16));
-    R.silhouette_pitch = unsigned(Align(size_t(image_size), 16));
-    CU(cudaMalloc(&R.depth, size_t(R.depth_pitch) * image_size));
-    CU(cudaMalloc(&R.silhouette, size_t(R.silhouette_pitch) * image_size));
-    CU(cudaMemsetAsync(R.depth, 0xff, size_t(R.depth_pitch) * image_size, ctx->stream));  // cleared: depth 1.0
-    CU(cudaMemsetAsync(R.silhouette, 0, size_t(R.silhouette_pitch) * image_size, ctx->stream));
+  if (depth) {
+    h.depth = std::move(depth);
+    h.silhouette = std::move(silhouette);
+    R.depth = h.depth;
+    R.silhouette = h.silhouette;
+    R.depth_pitch = depth_pitch;
+    R.silhouette_pitch = silhouette_pitch;
   }
   R.camera_kind = camera_kind;
   R.camera = camera;
@@ -2718,7 +2735,7 @@ int m3tb_get_rendering(m3tb_ctx* ctx, int renderer, void* depth_u16, void* silho
 
 int m3tb_detach_frames(m3tb_ctx* ctx) {
   CHECK_CTX();
-  if (ctx->ingest_stream) CU(cudaStreamSynchronize(ctx->ingest_stream));  // a prefetch may still be reading the frames
+  if (ctx->pf.ingest_stream) CU(cudaStreamSynchronize(ctx->pf.ingest_stream));  // a prefetch may still be reading the frames
   bool any = false;
   for (int k = 0; k < 2; ++k) {
     std::vector<CameraDev>& cams = k == 0 ? ctx->h_ccams : ctx->h_dcams;
@@ -2894,27 +2911,26 @@ int m3tb_debug_render_model_view(m3tb_ctx* ctx, int body, const int* occlusion_b
   if (!rc) rc = RenderModelViews(ctx, st, b, 0, 1);
   if (rc) return rc;
   const size_t n_pix = size_t(st.S) * st.S;
-  uint8_t *d_normal = nullptr, *d_sil = nullptr;
-  uint16_t* d_depth = nullptr;
-  auto run = [&]() -> int {
-    CU(cudaMalloc(&d_normal, 4 * n_pix));
-    CU(cudaMalloc(&d_depth, 2 * n_pix));
-    CU(cudaMalloc(&d_sil, n_pix));
-    k_model_images<<<unsigned((n_pix + 255) / 256), 256, 0, ctx->stream>>>(PointArgs(st, b, params, 0), 0, d_normal,
-                                                                            d_depth, d_sil);
-    CU(cudaGetLastError());
-    ctx->launches++;
-    if (normal_bgra) CU(cudaMemcpyAsync(normal_bgra, d_normal, 4 * n_pix, cudaMemcpyDeviceToHost, ctx->stream));
-    if (depth) CU(cudaMemcpyAsync(depth, d_depth, 2 * n_pix, cudaMemcpyDeviceToHost, ctx->stream));
-    if (silhouette) CU(cudaMemcpyAsync(silhouette, d_sil, n_pix, cudaMemcpyDeviceToHost, ctx->stream));
-    CU(cudaStreamSynchronize(ctx->stream));
-    return M3TB_OK;
-  };
-  rc = run();
-  cudaFree(d_normal);
-  cudaFree(d_depth);
-  cudaFree(d_sil);
-  return rc;
+  DeviceBuffer<uint8_t> d_normal, d_sil;
+  DeviceBuffer<uint16_t> d_depth;
+  CU(d_normal.create(4 * n_pix));
+  CU(d_depth.create(n_pix));
+  CU(d_sil.create(n_pix));
+  k_model_images<<<unsigned((n_pix + 255) / 256), 256, 0, ctx->stream>>>(PointArgs(st, b, params, 0), 0, d_normal,
+                                                                          d_depth, d_sil);
+  CU(cudaGetLastError());
+  ctx->launches++;
+  if (normal_bgra) CU(cudaMemcpyAsync(normal_bgra, d_normal, 4 * n_pix, cudaMemcpyDeviceToHost, ctx->stream));
+  if (depth) CU(cudaMemcpyAsync(depth, d_depth, 2 * n_pix, cudaMemcpyDeviceToHost, ctx->stream));
+  if (silhouette) CU(cudaMemcpyAsync(silhouette, d_sil, n_pix, cudaMemcpyDeviceToHost, ctx->stream));
+  CU(cudaStreamSynchronize(ctx->stream));
+  return M3TB_OK;
+}
+
+int m3tb_debug_resources(int fail_after, long long* live) {
+  if (fail_after >= 0) g_fail_after.store(fail_after);
+  if (live) *live = g_live_resources.load();
+  return M3TB_OK;
 }
 
 }  // extern "C"

@@ -23,6 +23,13 @@
  *    tracker.cpp:251-255). Contexts are independent.
  *  - there is NO CPU fallback: every compute entry point fails with M3TB_ERR_CUDA when no
  *    sm_90 (H100-class) device is usable.
+ *  - a call that fails with M3TB_ERR_CUDA because a device / pinned allocation, stream or event could
+ *    not be created leaves the context exactly as it was before the call: the same objects of the same
+ *    sizes, the same host tables and the same renderer ids. Objects that are replaced (a model, a
+ *    renderer's images, a grown table) are released only after their replacement exists. Calls that
+ *    launch work (tracking, rendering, histogram updates) grow the device tables they need lazily, one
+ *    set after another (structures, per-body state, renderer tables, shared-histogram groups): each set
+ *    is replaced all or nothing, and a failure keeps the sets that were completed before it.
  */
 #ifndef M3T_B200_H_
 #define M3T_B200_H_
@@ -439,6 +446,12 @@ typedef struct m3tb_launch_info {
   int32_t tma_mode;          /* k_track2: 0 legacy staging, 1 tensor maps as parameters, 2 in global memory; k_track: -1 */
 } m3tb_launch_info;
 int m3tb_debug_last_launch(m3tb_ctx* ctx, m3tb_launch_info* out);
+
+/* Host only, meant for tests. *live (if not null) receives the number of CUDA resources the library holds across all
+ * contexts: device allocations, pinned host allocations, streams and events. fail_after > 0 makes the fail_after-th
+ * resource creation from now on fail as an allocation failure (cudaErrorMemoryAllocation) without calling CUDA;
+ * 0 disarms that, a negative value only queries. */
+int m3tb_debug_resources(int fail_after, long long* live);
 
 /* ---- depth-model generation (DepthModel::GenerateModel, depth_model.cpp:144-213) -------------------------------- */
 /* Model parameters (model.h:161-167). */
