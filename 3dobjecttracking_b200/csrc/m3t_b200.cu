@@ -53,6 +53,10 @@ struct ImagePool {
   uint16_t* BinImage(int slot) const { return reinterpret_cast<uint16_t*>(bins.get() + bin_frame_bytes * slot); }
 };
 
+// what a colour camera's bin-index image holds besides a bit shift (m3tb_ctx::bin_shift)
+constexpr int kBinsNone = -1;      // nothing that matches the frame copy
+constexpr int kBinsAtIngest = -2;  // a pinned frame whose bin indices the next k_ingest writes
+
 // TMA tensor maps over one pool ([camera][row][column] u16), one per tile width; cached per pool base address
 struct PoolMaps {
   const void* base = nullptr;
@@ -140,8 +144,9 @@ struct m3tb_ctx {
   bool use_tiles = true;  // stage ROI tiles in shared memory (M3TB_NO_TILES=1 in the environment disables it)
   bool use_track2 = true; // second-generation fused kernel where it applies (M3TB_KERNEL=1 forces k_track)
   m3tb_launch_info last_launch = {};      // variant of the last tracking launch (m3tb_debug_last_launch)
-  std::vector<char> bin_stale;            // per colour camera: the bin-index image does not match the frame copy
-  int bin_bitshift = -1;                  // what the bin-index images were built with
+  // per colour camera: the histogram bit shift its bin-index image was written with, kBinsNone when it holds none that
+  // matches the frame copy, kBinsAtIngest while a pinned frame waits for the k_ingest that writes them (NoteIngestBins)
+  std::vector<int> bin_shift;
   DeviceBuffer<int> d_bin_ids;            // staging for k_bin
   // device copies of the renderer images (m3tb_upload_*_rendering), per body and renderer slot
   std::vector<std::array<DeviceBuffer<uint8_t>, RS_COUNT>> rendering_images;
@@ -378,6 +383,26 @@ int ValidateBodies(m3tb_ctx* ctx) {
   return M3TB_OK;
 }
 
+// k_ingest writes the bin indices of the colour rectangles it fetches with the bit shift of the body that fetches them,
+// and none for bodies above 32 bins. Records, for every colour camera it is about to fetch from, the bit shift its
+// bin-index image will hold (kBinsNone where its region bodies disagree or write none). Called before each k_ingest.
+void NoteIngestBins(m3tb_ctx* ctx) {
+  for (int i = 0; i < ctx->max_cameras; ++i) {
+    if (ctx->bin_shift[i] != kBinsAtIngest) continue;
+    int shift = kBinsNone;
+    bool first = true;
+    for (int b = 0; b < ctx->n_bodies; ++b) {
+      const BodyDev& B = ctx->h_bodies[b];
+      if (!B.set || !B.has_region || B.color_camera != i) continue;
+      const int s = B.rp.n_bins <= 32 ? B.rp.bitshift : kBinsNone;
+      if (first) shift = s;
+      else if (s != shift) shift = kBinsNone;
+      first = false;
+    }
+    ctx->bin_shift[i] = shift;
+  }
+}
+
 // Frame ingest for pinned host frames: fetch every body's ROI (k_ingest) before the first consumer of the new frame.
 int LaunchIngestIfPending(m3tb_ctx* ctx) {
   if (ctx->prefetched) {  // the frames were prefetched on the side stream: order the consumers behind that ingest
@@ -397,6 +422,7 @@ int LaunchIngestIfPending(m3tb_ctx* ctx) {
   a.bytes = ctx->d_ingest_bytes + ctx->ingest_bytes_slot;
   a.n_bodies = ctx->n_bodies;
   CU(cudaMemsetAsync(a.bytes, 0, sizeof(unsigned long long), ctx->stream));
+  NoteIngestBins(ctx);
   k_ingest<<<ctx->n_bodies, kBlockThreads, 0, ctx->stream>>>(a);
   CU(cudaGetLastError());
   ctx->launches++;
@@ -449,7 +475,9 @@ const PoolMaps* GetPoolMaps(m3tb_ctx* ctx, void* base, int width, int height, un
 
 // Can k_track2 stage its tiles with TMA for this batch? Every camera in use sits in its pool, the region bodies share one
 // histogram resolution (<= 32 bins: the index fits 16 bits); refreshes the bin-index images of frames that were copied in
-// full (k_bin) and fills the tensor maps of `a`.
+// full (k_bin) and fills the tensor maps of `a`. A pinned frame's device copy is valid only inside the ROIs k_ingest
+// fetched, so its bin indices cannot be rebuilt: when they were written with another bit shift (the resolution changed
+// since the ingest) or none, the launch uses the legacy staging, which bins from the frame itself.
 int PrepareTensorTiles(m3tb_ctx* ctx, TrackArgs& a, bool& usable) {
   a.tma_mode = ctx->tma_mode;
   a.tma_max_w = 256;
@@ -484,16 +512,19 @@ int PrepareTensorTiles(m3tb_ctx* ctx, TrackArgs& a, bool& usable) {
     const PoolMaps* m = GetPoolMaps(ctx, p.bins, p.width, p.height, p.bin_pitch, p.bin_frame_bytes, p.capacity);
     if (!m) return M3TB_OK;
     std::memcpy(a.bin_maps, m->maps, sizeof(a.bin_maps));
-    // frames that arrived by full copy: (re)build their bin-index images
-    if (ctx->bin_bitshift != bitshift) {
-      for (int i = 0; i < ctx->max_cameras; ++i)
-        if (!ctx->h_ccams[i].host_src) ctx->bin_stale[i] = 1;
-      ctx->bin_bitshift = bitshift;
+    for (int b = 0; b < ctx->n_bodies; ++b) {
+      const BodyDev& B = ctx->h_bodies[b];
+      if (B.has_region && ctx->h_ccams[B.color_camera].host_src && ctx->bin_shift[B.color_camera] != bitshift) {
+        a.tma_mode = 0;
+        usable = true;
+        return M3TB_OK;
+      }
     }
+    // frames that arrived by full copy: (re)build their bin-index images
     std::vector<int> ids;
     for (int i = 0; i < ctx->max_cameras; ++i) {
       const CameraDev& c = ctx->h_ccams[i];
-      if (c.set && c.image && c.bins && !c.host_src && ctx->bin_stale[i]) ids.push_back(i);
+      if (c.set && c.image && c.bins && !c.host_src && ctx->bin_shift[i] != bitshift) ids.push_back(i);
     }
     if (!ids.empty()) {
       CU(cudaMemcpyAsync(ctx->d_bin_ids, ids.data(), sizeof(int) * ids.size(), cudaMemcpyHostToDevice, ctx->stream));
@@ -506,7 +537,7 @@ int PrepareTensorTiles(m3tb_ctx* ctx, TrackArgs& a, bool& usable) {
       k_bin<<<dim3(unsigned(std::min(p.height, 120)), unsigned(ids.size())), kBlockThreads, 0, ctx->stream>>>(ba);
       CU(cudaGetLastError());
       ctx->launches++;
-      for (int i : ids) ctx->bin_stale[i] = 0;
+      for (int i : ids) ctx->bin_shift[i] = bitshift;
     }
   }
   if (any_depth) {
@@ -609,12 +640,13 @@ int LaunchTrack(m3tb_ctx* ctx, int iteration, int corr_begin, int corr_end, int 
     occ = occ || (B.has_region && (B.rp.model_occlusions || B.rp.use_region_checking)) ||
           (B.has_depth && (B.dp.model_occlusions || B.dp.use_silhouette_checking));
   }
-  // ---- k_track2: rigid bodies, <= 512 items per modality, no measured occlusion handling, correspondence / fused phases,
-  //      one function lookup for the whole batch (m3t_b200_track2.cuh) --------------------------------------------------
+  // ---- k_track2: rigid bodies, <= 512 items per modality, <= 32 histogram bins (its colour tile holds 16-bit bin indices
+  //      under every staging mode), no measured occlusion handling, correspondence / fused phases, one function lookup
+  //      for the whole batch (m3t_b200_track2.cuh) --------------------------------------------------------------------
   {
     const unsigned k2_phases = PH_REGION_CORR | PH_DEPTH_CORR | PH_REGION_GH | PH_DEPTH_GH | PH_SOLVE | PH_STORE_REGION |
                                PH_STORE_DEPTH;
-    bool ok = ctx->use_track2 && cluster == 0 && !occ && items <= kGroup && (phases & ~k2_phases) == 0 &&
+    bool ok = ctx->use_track2 && bins_fit_u16 && cluster == 0 && !occ && items <= kGroup && (phases & ~k2_phases) == 0 &&
               (n_update == 0 || (phases & PH_SOLVE));
     bool both = false, have_lookup = false;
     for (int b = 0; b < ctx->n_bodies && ok; ++b) {
@@ -1317,12 +1349,12 @@ int Upload(m3tb_ctx* ctx, bool color, int cam, const void* src, size_t pitch, cu
     c.host_src = pinned_alias;
     c.host_pitch = unsigned(pitch);
     ctx->ingest_pending = true;
-    if (color) ctx->bin_stale[cam] = 0;  // k_ingest writes the bin indices of every rectangle it fetches
+    if (color) ctx->bin_shift[cam] = kBinsAtIngest;  // k_ingest writes the bin indices of every rectangle it fetches
     return M3TB_OK;
   }
   c.host_src = nullptr;
   c.host_pitch = 0;
-  if (color) ctx->bin_stale[cam] = 1;
+  if (color) ctx->bin_shift[cam] = kBinsNone;
   CU(cudaMemcpy2DAsync(const_cast<uint8_t*>(c.image), c.pitch, src, pitch, row, c.height, kind, ctx->stream));
   return M3TB_OK;
 }
@@ -1349,7 +1381,7 @@ int UploadBatch(m3tb_ctx* ctx, bool color, int first, int count, const void* src
   for (int k = 0; k < count; ++k) {
     CameraDev& c = (color ? ctx->h_ccams : ctx->h_dcams)[first + k];
     c.host_src = nullptr; c.host_pitch = 0; c.generation = (c.generation + 1) & 0x3fffffff;
-    if (color) ctx->bin_stale[first + k] = 1;
+    if (color) ctx->bin_shift[first + k] = kBinsNone;
   }
   ctx->cams_dirty = true;
   if (pooled && frame_stride == pitch * size_t(pool.height)) {
@@ -1746,7 +1778,7 @@ int m3tb_create(int device, int max_bodies, int max_cameras, int max_models, m3t
   ctx->dmodel_alloc.resize(max_models);
   ctx->private_color.resize(max_cameras);
   ctx->private_depth.resize(max_cameras);
-  ctx->bin_stale.assign(max_cameras, 1);
+  ctx->bin_shift.assign(max_cameras, kBinsNone);
   ctx->h_geometry.assign(max_bodies, GeometryDev());
   std::memset(ctx->h_geometry.data(), 0, sizeof(GeometryDev) * max_bodies);
   ctx->geometry_alloc.resize(max_bodies);
@@ -2502,6 +2534,7 @@ int m3tb_prefetch_frames(m3tb_ctx* ctx) {
   int ingest_ctas = std::max(16, ctx->sm_count / 4);
   if (forced_ctas > 0) ingest_ctas = forced_ctas;
   ingest_ctas = std::min(ingest_ctas, ctx->n_bodies);
+  NoteIngestBins(ctx);
   k_ingest<<<ingest_ctas, kBlockThreads, 0, is>>>(a);
   CU(cudaGetLastError());
   CU(cudaEventRecord(ctx->pf.ev_ingest_done, is));
@@ -2746,7 +2779,7 @@ int m3tb_detach_frames(m3tb_ctx* ctx) {
                            cudaMemcpyHostToDevice, ctx->stream));
       c.host_src = nullptr;  // FrameView: the whole device copy is valid from now on
       c.host_pitch = 0;
-      if (k == 0) ctx->bin_stale[size_t(&c - cams.data())] = 1;
+      if (k == 0) ctx->bin_shift[size_t(&c - cams.data())] = kBinsNone;
       any = true;
     }
   }

@@ -188,11 +188,14 @@ def _staged_run(capi, wl, monkeypatch, env, upload):
     return out, launch
 
 
-@pytest.mark.parametrize("which", ["border", "border_region32", "642x481", "1280x720", "644x480"])
+@pytest.mark.parametrize("which", ["border", "border_region8", "border_region32", "border_region64", "642x481",
+                                   "1280x720", "644x480"])
 def test_staging_paths_are_bit_identical(capi, synth, monkeypatch, which):
-    if which in ("border", "border_region32"):
-        wl = synth.make_edge_workload("border", "region32" if which == "border_region32" else "region+depth",
-                                      n_divides=2, seed=7)
+    if which == "border":
+        wl = synth.make_edge_workload("border", "region+depth", n_divides=2, seed=7)
+    elif which.startswith("border_region"):
+        wl = synth.make_edge_workload("border", "region16", n_divides=2, seed=7)
+        wl.region.n_histogram_bins = int(which[len("border_region"):])
     else:
         _, ci, di, _ = next(s for s in _sizes(synth) if s[0].startswith(which))
         wl = synth.make_edge_workload("border", "region+depth", n_divides=2, seed=7, color_intrinsics=ci,
@@ -217,6 +220,9 @@ def test_staging_paths_are_bit_identical(capi, synth, monkeypatch, which):
     # 642 wide: no bin-index image, so the TMA modes fall back to k_track; legacy staging (mode 0) needs none
     if which == "642x481":
         assert launches["tma1_full"]["kernel"] == "k_track" and launches["tma0_full"]["kernel"] == "k_track2", launches
+    elif which == "border_region64":
+        # 64-bin indices do not fit the u16 colour tile of either kernel: k_track without tiles on every staging path
+        assert all(l["kernel"] == "k_track" and l["tiles"] == 0 for l in launches.values()), launches
     else:
         assert all(l["kernel"] == "k_track2" for l in launches.values()), launches
 
@@ -225,13 +231,16 @@ def test_staging_paths_are_bit_identical(capi, synth, monkeypatch, which):
 def _mixed(synth, variant):
     """Bodies 3k: region only, 3k+1: depth only, 3k+2: both, all in one context. variant "one_set": one region
     parameter set; "two_sets": the region-only bodies use another function amplitude (another function lookup);
-    "bins": the region-only bodies use 32 histogram bins, the two-modality bodies 16."""
+    "bins": the region-only bodies use 32 histogram bins, the two-modality bodies 16; "bins8": the region-only bodies
+    use 8 bins, so both table sizes sit in shared memory."""
     wl = synth.make_workload("c2", n_bodies=9, n_divides=2, seed=13, margin_px=60.0, z_range=(0.45, 0.8))
     region_only = dataclasses.replace(wl.region)
     if variant == "two_sets":
         region_only.function_amplitude = 0.36
     elif variant == "bins":
         region_only.n_histogram_bins = 32
+    elif variant == "bins8":
+        region_only.n_histogram_bins = 8
     kinds = [("region", "depth", "both")[b % 3] for b in range(wl.n_bodies)]
     copies = {"region": dataclasses.replace(wl, region=region_only, depth=None),
               "depth": dataclasses.replace(wl, region=None),
@@ -239,7 +248,8 @@ def _mixed(synth, variant):
     return wl, kinds, copies
 
 
-@pytest.mark.parametrize("variant,kernel", [("one_set", "k_track2"), ("two_sets", "k_track"), ("bins", "k_track")])
+@pytest.mark.parametrize("variant,kernel", [("one_set", "k_track2"), ("two_sets", "k_track"), ("bins", "k_track"),
+                                            ("bins8", "k_track")])
 def test_mixed_batch(capi, oracle, synth, variant, kernel):
     wl, kinds, copies = _mixed(synth, variant)
     nb = wl.n_bodies
@@ -320,6 +330,8 @@ def test_mixed_batch(capi, oracle, synth, variant, kernel):
     assert launch["kernel"] == kernel, launch
     if kernel == "k_track2":
         assert launch["threads"] == 1024, launch
+    if variant == "bins8":
+        assert launch["lut_smem"] == 1, launch
     assert valid_lines > 0.3 * wl.lines_per_body * (2 * nb // 3) * wl.n_corr_iterations, valid_lines
     assert valid_points > 0.3 * wl.points_per_body * (2 * nb // 3) * wl.n_corr_iterations, valid_points
     assert mode_splits <= max(1, 0.05 * nb * wl.n_corr_iterations), mode_splits

@@ -14,12 +14,18 @@ def _bits(a):
     return np.ascontiguousarray(a, np.float32).view(np.uint32)
 
 
-@pytest.mark.parametrize("bins", [16, 32])
+def _workload(synth, n, bins):
+    """c3 (region only, 32 bins) for 32 bins; c2 (200 lines + 200 points) at the given resolution otherwise."""
+    wl = synth.make_workload("c2" if bins != 32 else "c3", n_bodies=n, n_lines=200, n_points=200 if bins != 32 else 0,
+                             n_divides=3, seed=9)
+    wl.region.n_histogram_bins = bins
+    return wl
+
+
+@pytest.mark.parametrize("bins", [2, 8, 16, 32, 64])
 def test_shared_histograms_bit_exact(capi, oracle, synth, bins):
     n = 5
-    wl = synth.make_workload("c2" if bins == 16 else "c3", n_bodies=n, n_lines=200, n_points=200 if bins == 16 else 0,
-                             n_divides=3, seed=9)
-    assert wl.region.n_histogram_bins == bins
+    wl = _workload(synth, n, bins)
     wl.histogram_owner = np.array([0, 0, 2, 2, -1], np.int32)
     ctx = capi.context_from_workload(wl)
     orc = oracle.OracleTracker(wl, rotation_mode=oracle.ROTATION_LINEAR, exp_mode=oracle.EXP_RODRIGUES)
@@ -37,8 +43,7 @@ def test_shared_histograms_bit_exact(capi, oracle, synth, bins):
 
     check("start")
     # the shared object differs from what the owner would have had alone
-    alone = synth.make_workload("c2" if bins == 16 else "c3", n_bodies=n, n_lines=200, n_points=200 if bins == 16 else 0,
-                                n_divides=3, seed=9)
+    alone = _workload(synth, n, bins)
     o2 = oracle.OracleTracker(alone, rotation_mode=oracle.ROTATION_LINEAR, exp_mode=oracle.EXP_RODRIGUES)
     o2.start_modalities(0)
     assert np.abs(o2.hist_f[0] - orc.hist_f[0]).max() > 1e-6
@@ -47,6 +52,8 @@ def test_shared_histograms_bit_exact(capi, oracle, synth, bins):
         # the lookup tables the tracking kernels read are the shared ones: same poses as the oracle after a step
         orc.tracking_step(frame)
         ctx.tracking_step(frame, wl.n_corr_iterations, wl.n_update_iterations)
+        # 64-bin indices do not fit k_track2's u16 colour tile
+        assert ctx.last_launch()["kernel"] == ("k_track" if bins > 32 else "k_track2"), ctx.last_launch()
         dt, dr = pose_error(ctx.get_poses(), orc.get_poses())
         assert np.median(dt) < 1e-5 and dt.max() < 5e-3, (frame, dt, dr)   # free-running (discrete events, DESIGN §5)
         ctx.set_poses(orc.get_poses())
