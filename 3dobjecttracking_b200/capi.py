@@ -105,6 +105,7 @@ SYMBOLS = [
     "m3tb_share_color_histograms", "m3tb_debug_last_launch", "m3tb_set_body_geometry", "m3tb_set_focused_renderer",
     "m3tb_attach_renderer", "m3tb_render", "m3tb_get_rendering", "m3tb_model_params_default", "m3tb_model_views",
     "m3tb_generate_depth_model", "m3tb_get_depth_model", "m3tb_debug_render_model_view", "m3tb_debug_resources",
+    "m3tb_generate_region_model", "m3tb_get_region_model", "m3tb_debug_region_model_view",
 ]
 
 KERNEL_NAMES = {0: None, 1: "k_track", 2: "k_track2", 3: "k_track_cluster"}
@@ -212,6 +213,10 @@ def lib():
     L.m3tb_generate_depth_model.argtypes = [vp, ci, ci, ip, ci, C.POINTER(ModelParams)]
     L.m3tb_get_depth_model.argtypes = [vp, ci, ip, ip, fp, fp, vp, fp, fp]
     L.m3tb_debug_render_model_view.argtypes = [vp, ci, ip, ci, C.POINTER(ModelParams), ci, vp, vp, vp]
+    L.m3tb_generate_region_model.argtypes = [vp, ci, ci, vp, ci, C.POINTER(ModelParams)]
+    L.m3tb_get_region_model.argtypes = [vp, ci, ip, ip, fp, fp, vp, fp, fp]
+    L.m3tb_debug_region_model_view.argtypes = [vp, ci, vp, ci, C.POINTER(ModelParams), ci, vp, ip, vp, vp, vp, ci, ip,
+                                               ip]
     L.m3tb_debug_resources.argtypes = [ci, C.POINTER(C.c_longlong)]
     _lib = L
     return L
@@ -244,6 +249,12 @@ def model_params(**kw) -> ModelParams:
             raise TypeError(f"unknown model parameter {k}")
         setattr(p, k, v)
     return p
+
+
+def associated_bodies(associated):
+    """m3tb_associated_body records [n, 3] int32 (body, movable, same_region) of a list of triples."""
+    a = np.ascontiguousarray(np.asarray(associated, np.int32).reshape(-1, 3))
+    return a
 
 
 def model_views(params=None):
@@ -491,6 +502,50 @@ class Context:
                                                      C.byref(p), view, normal.ctypes.data, depth.ctypes.data,
                                                      sil.ctypes.data))
         return dict(normal=normal, depth=depth, silhouette=sil)
+
+    def generate_region_model(self, model_id, body, associated=(), params=None):
+        """RegionModel::GenerateModel on the device. associated: (body, movable, same_region) triples in
+        RegionModel::AddAssociatedBody order (params: ModelParams, default model_params())."""
+        p = params if params is not None else model_params()
+        a = associated_bodies(associated)
+        self._ck(self.L.m3tb_generate_region_model(self.h, model_id, body, a.ctypes.data, len(a), C.byref(p)))
+
+    def get_region_model(self, model_id):
+        """A generated region model as synth.Model (orientations, contour lengths, [nv, np, 38] DataPoints, and the
+        stride_depth_offset / max_radius_depth_offset it was generated with)."""
+        from .synth import Model
+        nv, npt = C.c_int(0), C.c_int(0)
+        stride, radius = C.c_float(0.0), C.c_float(0.0)
+        ip = C.POINTER(C.c_int)
+        self._ck(self.L.m3tb_get_region_model(self.h, model_id, C.cast(C.byref(nv), ip), C.cast(C.byref(npt), ip),
+                                              None, None, None, C.byref(stride), C.byref(radius)))
+        ori = np.zeros((nv.value, 3), np.float32)
+        length = np.zeros(nv.value, np.float32)
+        pts = np.zeros((nv.value, npt.value, 38), np.float32)
+        self._ck(self.L.m3tb_get_region_model(self.h, model_id, None, None, _p(ori), _p(length), pts.ctypes.data, None,
+                                              None))
+        return Model("region", ori, length, pts, stride_depth_offset=float(np.float32(stride.value)),
+                     max_radius_depth_offset=float(np.float32(radius.value)))
+
+    def debug_region_model_view(self, body, view, associated=(), params=None):
+        """dict(silhouettes [n_renderers,S,S] u8 (main, same-region, occlusion, foreground, background, as used),
+        depth [S,S] u16, contours: list of [n,2] int32 (x, y)) of one region-generation view."""
+        p = params if params is not None else model_params()
+        S = p.image_size
+        a = associated_bodies(associated)
+        ip = C.POINTER(C.c_int)
+        n_sil, n_pts, n_c = C.c_int(0), C.c_int(0), C.c_int(0)
+        args = (self.h, body, a.ctypes.data, len(a), C.byref(p), view)
+        self._ck(self.L.m3tb_debug_region_model_view(*args, None, C.cast(C.byref(n_sil), ip), None, None, None, 0,
+                                                     C.cast(C.byref(n_pts), ip), C.cast(C.byref(n_c), ip)))
+        sil = np.zeros((n_sil.value, S, S), np.uint8)
+        depth = np.zeros((S, S), np.uint16)
+        pts = np.zeros((max(n_pts.value, 1), 2), np.int32)
+        offs = np.zeros(max(n_pts.value, 1) + 1, np.int32)
+        self._ck(self.L.m3tb_debug_region_model_view(*args, sil.ctypes.data, None, depth.ctypes.data, pts.ctypes.data,
+                                                     offs.ctypes.data, max(n_pts.value, 1), None, None))
+        contours = [pts[offs[k]:offs[k + 1]].copy() for k in range(n_c.value)]
+        return dict(silhouettes=sil, depth=depth, contours=contours)
 
     def set_body(self, body, region, depth, optimizer, region_model=0, depth_model=0, color_camera=0, depth_camera=0):
         self._ck(self.L.m3tb_set_body(self.h, body, C.byref(region) if region is not None else None,

@@ -495,6 +495,49 @@ int m3tb_debug_render_model_view(m3tb_ctx* ctx, int body, const int* occlusion_b
                                  const m3tb_model_params* params, int view, uint8_t* normal_bgra, uint16_t* depth,
                                  uint8_t* silhouette);
 
+/* ---- region-model generation (RegionModel::GenerateModel, region_model.cpp:187-257) ------------------------------ */
+/* RegionModel::AddAssociatedBody(body, movable, same_region), region_model.cpp:61-82: a fixed body (movable 0) is
+ * drawn into the main silhouette with id 120 and its contour points are tested against its depth; a movable body
+ * hides contour points it covers; a same-region body invalidates contour points next to it and extends the region
+ * the line distances walk through. */
+typedef struct m3tb_associated_body {
+  int32_t body;
+  int32_t movable;
+  int32_t same_region;
+} m3tb_associated_body;
+/* Generates region model `model_id` of body `body` from the geometry given with m3tb_set_body_geometry, with the
+ * `n_associated` associated bodies in insertion order (each of the four groups fixed, fixed same-region, movable,
+ * movable same-region keeps that order, which is the draw order of the renderers). Every view is rendered on the
+ * device with the renderers of the reference; the contours of the main silhouette are traced as
+ * cv::findContours(RETR_LIST, CHAIN_APPROX_NONE) does, contours shorter than 15 points dropped, and a fresh
+ * std::mt19937{7} samples the valid contour points. The model then serves tracking exactly as if it had been uploaded
+ * with m3tb_set_region_model. Views without a valid contour point, and views whose sampling gives up after 101
+ * consecutive rejections, get contour_length 0; points never produced are zero-filled. Refusals, which leave the model
+ * as it was: M3TB_ERR_UNSUPPORTED for use_random_seed != 0 and for a view whose contours exceed 64 * image_size points;
+ * M3TB_ERR_INVALID for bad ids, a body without geometry, the body listed as associated, a body listed twice, an
+ * offset ratio above 30, any renderer's z_min below 0.2 * sphere_radius, or an image_size at which one view's z-buffers
+ * (8 B per pixel and renderer) and contour scratch exceed the 1 GiB scratch bound (e.g. 5 renderers at 8192 px). DESIGN.md §3 "k_region_contours /
+ * k_region_points" states what is computed. */
+int m3tb_generate_region_model(m3tb_ctx* ctx, int model_id, int body, const m3tb_associated_body* associated,
+                               int n_associated, const m3tb_model_params* params);
+/* Reads back a generated region model like m3tb_get_depth_model; every output may be NULL: orientations [n_views][3],
+ * contour_lengths [n_views], points [n_views][n_points] x 152-B DataPoints (center_f_body[3], normal_f_body[3],
+ * foreground_distance, background_distance, depth_offsets[30]), stride / max radius of the depth offsets.
+ * M3TB_ERR_NOT_SET_UP if the model was not generated by m3tb_generate_region_model. */
+int m3tb_get_region_model(m3tb_ctx* ctx, int model_id, int* n_views, int* n_points, float* orientations,
+                          float* contour_lengths, void* points, float* stride_depth_offset,
+                          float* max_radius_depth_offset);
+/* Test aid: renders view `view` of a region-model generation with these arguments and returns the silhouette image
+ * (image_size^2 u8 each) of every renderer it uses, main first, then same-region, occlusion, foreground, background
+ * (each only if used; *n_silhouettes receives the count), the main renderer's depth image (u16), and the contour list
+ * as GenerateValidContours leaves it: *n_contour_points points as (x, y) int32 pairs in order, and *n_contours + 1
+ * offsets into them. At most `capacity` points and capacity + 1 offsets are written; any output may be NULL.
+ * Refusals as m3tb_generate_region_model, plus a view index out of range. */
+int m3tb_debug_region_model_view(m3tb_ctx* ctx, int body, const m3tb_associated_body* associated, int n_associated,
+                                 const m3tb_model_params* params, int view, uint8_t* silhouettes, int* n_silhouettes,
+                                 uint16_t* depth, int32_t* contour_points, int32_t* contour_offsets, int capacity,
+                                 int* n_contour_points, int* n_contours);
+
 /* Test aid (host only, no context, no GPU): RegionModel/DepthModel::GetClosestView (region_model.cpp:105-130) for
  * `n_queries` orientation vectors (R^T normalize(t), 3 floats each) over `n_views` view orientations, once by the
  * reference's full scan (`out_scan`) and once by the host restatement of the pruned search the kernels use

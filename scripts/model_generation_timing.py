@@ -1,9 +1,11 @@
-"""Depth-model generation at the reference's defaults: schauma (20950 triangles), 2562 views x 200 points at 2000 px
-(m3tb_model_params_default). Host clock around each synchronous m3tb_generate_depth_model call (it ends with a device
+"""Depth-model (default) or, with --region, region-model generation at the reference's defaults: schauma (20950
+triangles), 2562 views x 200 points at 2000 px (m3tb_model_params_default). Host clock around each synchronous
+m3tb_generate_depth_model / m3tb_generate_region_model call (it ends with a device
 synchronise), 3 runs after one warm-up. Peak scratch is measured: a second thread samples the device's free memory
 (cudaMemGetInfo through torch) while each call runs, and the drop from before the call to the lowest sample is what the
 call held at most (device-wide, so other work on the card would show up in it too). Prints one JSON line with the card's
-name and power limit read in the same call."""
+name and power limit read in the same call; with --region also the device time of each kernel of one more call
+(torch.profiler), to show which stage dominates."""
 import importlib
 import json
 import os
@@ -28,7 +30,18 @@ tri = mesh["vertices"][mesh["faces"]]
 p = capi.model_params()
 ctx = capi.Context(0, max_bodies=1, max_cameras=1, max_models=1)
 ctx.set_body_geometry(0, tri, mf.body.geometry2body[:3], mf.body.maximum_body_diameter, True)
-ctx.generate_depth_model(0, 0, (), p)  # warm-up: module load
+REGION = "--region" in sys.argv
+args = [a for a in sys.argv[1:] if a != "--region"]
+
+
+def generate():
+    if REGION:
+        ctx.generate_region_model(0, 0, (), p)
+    else:
+        ctx.generate_depth_model(0, 0, (), p)
+
+
+generate()  # warm-up: module load
 torch.cuda.init()
 
 
@@ -45,19 +58,27 @@ def generate_watched():
     w = threading.Thread(target=watch)
     w.start()
     t0 = time.perf_counter()
-    ctx.generate_depth_model(0, 0, (), p)  # ctypes releases the GIL for the call
+    generate()  # ctypes releases the GIL for the call
     dt = time.perf_counter() - t0
     done.set()
     w.join()
     return dt, free0 - low[0]
 
 
-runs = [generate_watched() for _ in range(int(sys.argv[1]) if len(sys.argv) > 1 else 3)]
+runs = [generate_watched() for _ in range(int(args[0]) if args else 3)]
 times = [r[0] for r in runs]
-m = ctx.get_depth_model(0)
+stages = {}
+if REGION:
+    from torch.profiler import ProfilerActivity, profile
+    with profile(activities=[ProfilerActivity.CUDA]) as prof:
+        generate()
+    for e in prof.key_averages():
+        if e.key.startswith(("void m3tb::k_", "m3tb::k_")) or "k_model" in e.key or "k_region" in e.key:
+            stages[e.key.split("(")[0]] = round(getattr(e, "device_time_total", getattr(e, "cuda_time_total", 0)) / 1e6, 4)
+m = ctx.get_region_model(0) if REGION else ctx.get_depth_model(0)
 ctx.close()
 gpu = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True,
                      text=True).stdout.strip()
-print(json.dumps(dict(body="schauma", triangles=int(tri.shape[0]), views=m.n_views, points=m.n_points, image_size=p.image_size,
+print(json.dumps(dict(kind="region" if REGION else "depth", stage_seconds=stages, body="schauma", triangles=int(tri.shape[0]), views=m.n_views, points=m.n_points, image_size=p.image_size,
                       seconds_per_model=times, seconds_median=float(np.median(times)),
                       peak_scratch_bytes_measured=[int(r[1]) for r in runs], gpu=gpu)))
