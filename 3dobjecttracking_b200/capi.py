@@ -105,7 +105,8 @@ SYMBOLS = [
     "m3tb_share_color_histograms", "m3tb_debug_last_launch", "m3tb_set_body_geometry", "m3tb_set_focused_renderer",
     "m3tb_attach_renderer", "m3tb_render", "m3tb_get_rendering", "m3tb_model_params_default", "m3tb_model_views",
     "m3tb_generate_depth_model", "m3tb_get_depth_model", "m3tb_debug_render_model_view", "m3tb_debug_resources",
-    "m3tb_generate_region_model", "m3tb_get_region_model", "m3tb_debug_region_model_view",
+    "m3tb_generate_region_model", "m3tb_get_region_model", "m3tb_debug_region_model_view", "m3tb_set_viewer",
+    "m3tb_update_viewers", "m3tb_get_viewer_image",
 ]
 
 KERNEL_NAMES = {0: None, 1: "k_track", 2: "k_track2", 3: "k_track_cluster"}
@@ -218,6 +219,9 @@ def lib():
     L.m3tb_debug_region_model_view.argtypes = [vp, ci, vp, ci, C.POINTER(ModelParams), ci, vp, ip, vp, vp, vp, ci, ip,
                                                ip]
     L.m3tb_debug_resources.argtypes = [ci, C.POINTER(C.c_longlong)]
+    L.m3tb_set_viewer.argtypes = [vp, ci, ci, ci, ip, ci, C.c_float, C.c_float, C.c_float]
+    L.m3tb_update_viewers.argtypes = [vp]
+    L.m3tb_get_viewer_image.argtypes = [vp, ci, vp, C.c_size_t, vp, C.c_size_t]
     _lib = L
     return L
 
@@ -464,6 +468,26 @@ class Context:
                        (np.float32(x.value) for x in f)))
         out.update(depth=depth, silhouette=sil, visible=vis)
         return out
+
+    def set_viewer(self, viewer, kind, camera, geometry_bodies, opacity=0.5, min_depth=0.0, max_depth=1.0):
+        """NormalColorViewer (kind "color" / 0) or NormalDepthViewer ("depth" / 1) of camera `camera` drawing
+        `geometry_bodies` in that order. The image size is the camera's at the next update."""
+        k = {"color": 0, "depth": 1}.get(kind, kind)
+        g = np.ascontiguousarray(geometry_bodies, np.int32)
+        self._ck(self.L.m3tb_set_viewer(self.h, viewer, int(k), camera, g.ctypes.data_as(C.POINTER(C.c_int)), g.size,
+                                        opacity, min_depth, max_depth))
+
+    def update_viewers(self):
+        """Tracker::UpdateViewers: every viewer from the current poses and camera frames."""
+        self._ck(self.L.m3tb_update_viewers(self.h))
+
+    def get_viewer_image(self, viewer, width, height):
+        """(blended BGR8 image [H,W,3], normal image [H,W,4] in GL_BGRA order) of the viewer's last update."""
+        bgr = np.zeros((height, width, 3), np.uint8)
+        normal = np.zeros((height, width, 4), np.uint8)
+        self._ck(self.L.m3tb_get_viewer_image(self.h, viewer, bgr.ctypes.data, bgr.strides[0], normal.ctypes.data,
+                                              normal.strides[0]))
+        return bgr, normal
 
     def generate_depth_model(self, model_id, body, occlusion_bodies=(), params=None):
         """DepthModel::GenerateModel on the device from the geometry of m3tb_set_body_geometry (params: ModelParams,

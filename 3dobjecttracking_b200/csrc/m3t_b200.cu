@@ -21,6 +21,7 @@
 #include "m3t_b200_structures.cuh"
 #include "m3t_b200_kernels.cuh"
 #include "m3t_b200_views.cuh"
+#include "m3t_b200_view.cuh"
 
 #include "m3t_b200_track_variants.h"
 #include "m3t_b200_track2.cuh"
@@ -214,6 +215,27 @@ struct m3tb_ctx {
     std::vector<float> orientations, view_scalars, points;
   };
   std::vector<GeneratedModel> dmodel_generated, rmodel_generated;
+
+  // viewers (m3tb_set_viewer / m3tb_update_viewers, k_view_*): dense ids
+  struct ViewerHost {
+    int kind = 0, camera = 0;
+    float opacity = 0.0f, min_depth = 0.0f, max_depth = 0.0f;
+    std::vector<int> geometry;
+    int width = 0, height = 0;           // of the images below (the camera's size when they were made)
+    DeviceBuffer<uint64_t> zbuf;          // cleared; k_view_resolve clears it again after each update
+    DeviceBuffer<uint8_t> normal, image;
+    bool updated = false;                 // the images hold an update (m3tb_get_viewer_image)
+  };
+  std::vector<ViewerHost> viewers;
+  // tables of one update, grown lazily, each set all or nothing
+  std::vector<ViewerDev> h_view_viewers;
+  std::vector<ViewDrawDev> h_view_draws;
+  DeviceBuffer<ViewerDev> d_view_viewers;
+  DeviceBuffer<ViewDrawDev> d_view_draws;
+  DeviceBuffer<float> d_view_rot;
+  DeviceBuffer<ViewFanDev> d_view_fans;
+  DeviceBuffer<uint64_t> d_view_fan_tile;
+  DeviceBuffer<unsigned long long> d_view_counter;  // 0 between updates
 };
 
 namespace {
@@ -1413,6 +1435,7 @@ constexpr int kRegionBackgroundID = 0, kRegionDifferentBodyID = 120, kRegionMain
 constexpr int kModelMaxImageSize = 8192;        // two 8192^2 z-buffers of 8 B are the whole scratch bound of a depth
                                                 // view; region generation refuses views that need more
 constexpr int kModelMaxDivides = 8;
+constexpr float kViewerZMin = 0.02f, kViewerZMax = 10.0f;  // FullNormalRenderer defaults (normal_renderer.h:84-93)
 
 using Vec3 = std::array<float, 3>;
 
@@ -3280,6 +3303,233 @@ int m3tb_debug_region_model_view(m3tb_ctx* ctx, int body, const m3tb_associated_
     }
   if (contour_offsets)
     for (int k = 0; k <= std::min(capacity, counts[0]); ++k) contour_offsets[k] = starts[k];
+  return M3TB_OK;
+}
+
+// ---- viewers (NormalColorViewer / NormalDepthViewer, normal_viewer.cpp) -------------------------------------------
+
+struct ViewerImages {
+  DeviceBuffer<uint64_t> zbuf;
+  DeviceBuffer<uint8_t> normal, image;
+};
+
+// Images of a W x H viewer; the z-buffer is cleared (k_view_resolve clears it again after every update)
+static int MakeViewerImages(m3tb_ctx* ctx, int width, int height, ViewerImages& im) {
+  const size_t n = size_t(width) * height;
+  CU(im.zbuf.create(n));
+  CU(im.normal.create(4 * n));
+  CU(im.image.create(3 * n));
+  CU(cudaMemsetAsync(im.zbuf, 0xff, n * sizeof(uint64_t), ctx->stream));
+  return M3TB_OK;
+}
+
+static const CameraDev& ViewerCamera(const m3tb_ctx* ctx, const m3tb_ctx::ViewerHost& h) {
+  return (h.kind == VK_COLOR ? ctx->h_ccams : ctx->h_dcams)[h.camera];
+}
+
+int m3tb_set_viewer(m3tb_ctx* ctx, int viewer, int kind, int camera, const int* geometry_bodies, int n_geometry,
+                    float opacity, float min_depth, float max_depth) {
+  CHECK_CTX();
+  if (viewer < 0 || viewer > int(ctx->viewers.size()))
+    return Fail(ctx, M3TB_ERR_INVALID, "viewer ids must be dense (0..n)");
+  if (kind != VK_COLOR && kind != VK_DEPTH)
+    return Fail(ctx, M3TB_ERR_INVALID, "kind must be 0 (NormalColorViewer) or 1 (NormalDepthViewer)");
+  if (camera < 0 || camera >= ctx->max_cameras || !(kind == VK_COLOR ? ctx->h_ccams : ctx->h_dcams)[camera].set)
+    return Fail(ctx, M3TB_ERR_INVALID, "camera not set");
+  if (n_geometry < 0 || n_geometry > 65535 || (n_geometry > 0 && !geometry_bodies))
+    return Fail(ctx, M3TB_ERR_INVALID, "bad geometry body list");
+  for (int k = 0; k < n_geometry; ++k) {
+    const int b = geometry_bodies[k];
+    if (b < 0 || b >= ctx->max_bodies || !ctx->h_geometry[b].set)
+      return Fail(ctx, M3TB_ERR_INVALID, "body " + std::to_string(b) + " has no geometry (m3tb_set_body_geometry)");
+    for (int q = 0; q < k; ++q)
+      if (geometry_bodies[q] == b) return Fail(ctx, M3TB_ERR_INVALID, "body listed twice");
+  }
+  m3tb_ctx::ViewerHost nv;
+  nv.kind = kind;
+  nv.camera = camera;
+  nv.opacity = opacity;
+  nv.min_depth = min_depth;
+  nv.max_depth = max_depth;
+  nv.geometry.assign(geometry_bodies, geometry_bodies + n_geometry);
+  const CameraDev& c = ViewerCamera(ctx, nv);
+  const bool is_new = viewer == int(ctx->viewers.size());
+  m3tb_ctx::ViewerHost* old = is_new ? nullptr : &ctx->viewers[viewer];
+  ViewerImages im;
+  if (!old || old->width != c.width || old->height != c.height) {
+    int rc = MakeViewerImages(ctx, c.width, c.height, im);
+    if (rc) return rc;
+    if (old) CU(cudaStreamSynchronize(ctx->stream));  // an update in flight may still use the old images
+  } else {
+    im.zbuf = std::move(old->zbuf);
+    im.normal = std::move(old->normal);
+    im.image = std::move(old->image);
+  }
+  nv.width = c.width;
+  nv.height = c.height;
+  nv.zbuf = std::move(im.zbuf);
+  nv.normal = std::move(im.normal);
+  nv.image = std::move(im.image);
+  if (is_new) ctx->viewers.push_back(std::move(nv));
+  else ctx->viewers[viewer] = std::move(nv);
+  return M3TB_OK;
+}
+
+int m3tb_update_viewers(m3tb_ctx* ctx) {
+  CHECK_CTX();
+  const int nv = int(ctx->viewers.size());
+  if (nv == 0) return M3TB_OK;
+  for (const auto& h : ctx->viewers)
+    if (!ViewerCamera(ctx, h).image)
+      return Fail(ctx, M3TB_ERR_NOT_SET_UP, "a viewer's camera has not received an image");
+  // images of viewers whose camera changed size since they were made (m3tb_set_*_camera), all or nothing
+  std::vector<ViewerImages> remade(nv);
+  bool any_remade = false;
+  for (int v = 0; v < nv; ++v) {
+    const auto& h = ctx->viewers[v];
+    const CameraDev& c = ViewerCamera(ctx, h);
+    if (h.width == c.width && h.height == c.height) continue;
+    int rc = MakeViewerImages(ctx, c.width, c.height, remade[v]);
+    if (rc) return rc;
+    any_remade = true;
+  }
+  if (any_remade) {
+    CU(cudaStreamSynchronize(ctx->stream));  // an update in flight may still use the images that are replaced
+    for (int v = 0; v < nv; ++v) {
+      if (!remade[v].zbuf) continue;
+      auto& h = ctx->viewers[v];
+      const CameraDev& c = ViewerCamera(ctx, h);
+      h.width = c.width;
+      h.height = c.height;
+      h.zbuf = std::move(remade[v].zbuf);
+      h.normal = std::move(remade[v].normal);
+      h.image = std::move(remade[v].image);
+      h.updated = false;
+    }
+  }
+  // the update's tables: viewers (projection, frame, images) and draws (RendererGeometry::render_data_bodies)
+  std::vector<ViewerDev>& V = ctx->h_view_viewers;
+  std::vector<ViewDrawDev>& D = ctx->h_view_draws;
+  V.assign(nv, ViewerDev{});
+  D.clear();
+  size_t n_triangles = 0;
+  int max_triangles = 0, max_pixels = 0;
+  for (int v = 0; v < nv; ++v) {
+    const auto& h = ctx->viewers[v];
+    const CameraDev& c = ViewerCamera(ctx, h);
+    ViewerDev& d = V[v];
+    d.width = c.width;
+    d.height = c.height;
+    d.kind = h.kind;
+    // FullRenderer::CalculateProjectionMatrix (renderer.cpp:257-264) with the viewer renderer's z range
+    const float z_min = kViewerZMin, z_max = kViewerZMax;
+    d.P00 = 2.0f * c.fu / float(c.width);
+    d.P02 = 2.0f * (c.ppu + 0.5f) / float(c.width) - 1.0f;
+    d.P11 = 2.0f * c.fv / float(c.height);
+    d.P12 = 2.0f * (c.ppv + 0.5f) / float(c.height) - 1.0f;
+    d.P22 = (z_max + z_min) / (z_max - z_min);
+    d.P23 = -2.0f * z_max * z_min / (z_max - z_min);
+    std::memcpy(d.w2c, c.w2c, sizeof(d.w2c));
+    // Camera::image(): a pinned frame's device copy is valid only inside the ROIs, the frame itself is read in place
+    d.frame = c.host_src ? c.host_src : c.image;
+    d.frame_pitch = c.host_src ? c.host_pitch : c.pitch;
+    d.opacity = h.opacity;
+    // DepthCamera::NormalizedDepthImage (camera.cpp:108-115)
+    d.depth_alpha = 255.0f / ((h.max_depth - h.min_depth) / c.depth_scale);
+    d.depth_beta = -(h.min_depth / c.depth_scale) * d.depth_alpha;
+    d.zbuf = h.zbuf;
+    d.normal = h.normal;
+    d.image = h.image;
+    d.first_draw = int(D.size());
+    d.n_draws = int(h.geometry.size());
+    for (int g = 0; g < d.n_draws; ++g) {
+      const int b = h.geometry[g];
+      const GeometryDev& G = ctx->h_geometry[b];
+      ViewDrawDev dd;
+      dd.triangles = G.triangles;
+      dd.n_triangles = G.n_triangles;
+      dd.enable_culling = G.enable_culling;
+      dd.viewer = v;
+      dd.draw = g;
+      dd.body = b;
+      std::memcpy(dd.geometry2body, G.geometry2body, sizeof(dd.geometry2body));
+      D.push_back(dd);
+      n_triangles += size_t(G.n_triangles);
+      max_triangles = std::max(max_triangles, G.n_triangles);
+    }
+    max_pixels = std::max(max_pixels, c.width * c.height);
+  }
+  const int n_draws = int(D.size());
+  const size_t fan_cap = 2 * n_triangles;
+  if (fan_cap > size_t(INT32_MAX)) return Fail(ctx, M3TB_ERR_INVALID, "too many triangles for one update");
+  // device tables, all or nothing
+  DeviceBuffer<ViewerDev> viewers;
+  DeviceBuffer<ViewDrawDev> draws;
+  DeviceBuffer<float> rot;
+  DeviceBuffer<ViewFanDev> fans;
+  DeviceBuffer<uint64_t> fan_tile;
+  DeviceBuffer<unsigned long long> counter;
+  int rc = GrowTable(ctx, ctx->d_view_viewers, viewers, size_t(nv));
+  if (!rc) rc = GrowTable(ctx, ctx->d_view_draws, draws, std::max<size_t>(n_draws, 1));
+  if (!rc) rc = GrowTable(ctx, ctx->d_view_rot, rot, 9 * std::max<size_t>(n_draws, 1));
+  if (!rc) rc = GrowTable(ctx, ctx->d_view_fans, fans, std::max<size_t>(fan_cap, 1));
+  if (!rc) rc = GrowTable(ctx, ctx->d_view_fan_tile, fan_tile, std::max<size_t>(fan_cap, 1));
+  if (rc) return rc;
+  if (!ctx->d_view_counter) {
+    CU(counter.create(1));
+    CU(cudaMemsetAsync(counter, 0, sizeof(unsigned long long), ctx->stream));
+  }
+  if (viewers || draws || rot || fans || fan_tile || counter) {
+    CU(cudaStreamSynchronize(ctx->stream));  // an update in flight may still read the tables that are replaced
+    if (viewers) ctx->d_view_viewers = std::move(viewers);
+    if (draws) ctx->d_view_draws = std::move(draws);
+    if (rot) ctx->d_view_rot = std::move(rot);
+    if (fans) ctx->d_view_fans = std::move(fans);
+    if (fan_tile) ctx->d_view_fan_tile = std::move(fan_tile);
+    if (counter) ctx->d_view_counter = std::move(counter);
+  }
+  CU(cudaMemcpyAsync(ctx->d_view_viewers, V.data(), sizeof(ViewerDev) * nv, cudaMemcpyHostToDevice, ctx->stream));
+  if (n_draws)
+    CU(cudaMemcpyAsync(ctx->d_view_draws, D.data(), sizeof(ViewDrawDev) * n_draws, cudaMemcpyHostToDevice, ctx->stream));
+  ViewArgs a;
+  a.viewers = ctx->d_view_viewers;
+  a.n_viewers = nv;
+  a.draws = ctx->d_view_draws;
+  a.n_draws = n_draws;
+  a.poses = ctx->d_poses;
+  a.rot = ctx->d_view_rot;
+  a.fans = ctx->d_view_fans;
+  a.fan_tile = ctx->d_view_fan_tile;
+  a.fan_cap = int(fan_cap);
+  a.counter = ctx->d_view_counter;
+  // the three launches always run (a grid dimension of 0 is not launchable, so empty ones get one idle block)
+  const dim3 setup_grid(unsigned(std::max(1, (max_triangles + kViewThreads - 1) / kViewThreads)),
+                        unsigned(std::max(1, n_draws)));
+  k_view_setup<<<setup_grid, kViewThreads, 0, ctx->stream>>>(a);
+  CU(cudaGetLastError());
+  k_view_raster<<<unsigned(ctx->sm_count * (2048 / kViewThreads)), kViewThreads, 0, ctx->stream>>>(a);
+  CU(cudaGetLastError());
+  k_view_resolve<<<dim3(unsigned((max_pixels + kViewThreads - 1) / kViewThreads), unsigned(nv)), kViewThreads, 0,
+                   ctx->stream>>>(a);
+  CU(cudaGetLastError());
+  ctx->launches += 3;
+  for (auto& h : ctx->viewers) h.updated = true;
+  return M3TB_OK;
+}
+
+int m3tb_get_viewer_image(m3tb_ctx* ctx, int viewer, uint8_t* bgr, size_t pitch, uint8_t* normal_bgra,
+                          size_t normal_pitch) {
+  CHECK_CTX();
+  if (viewer < 0 || viewer >= int(ctx->viewers.size())) return Fail(ctx, M3TB_ERR_INVALID, "viewer not set");
+  const auto& h = ctx->viewers[viewer];
+  if (!h.updated) return Fail(ctx, M3TB_ERR_NOT_SET_UP, "viewer has not been updated since it was set");
+  const size_t W = size_t(h.width), H = size_t(h.height);
+  if ((bgr && pitch < 3 * W) || (normal_bgra && normal_pitch < 4 * W))
+    return Fail(ctx, M3TB_ERR_INVALID, "pitch smaller than a row");
+  if (bgr) CU(cudaMemcpy2DAsync(bgr, pitch, h.image, 3 * W, 3 * W, H, cudaMemcpyDeviceToHost, ctx->stream));
+  if (normal_bgra)
+    CU(cudaMemcpy2DAsync(normal_bgra, normal_pitch, h.normal, 4 * W, 4 * W, H, cudaMemcpyDeviceToHost, ctx->stream));
+  CU(cudaStreamSynchronize(ctx->stream));
   return M3TB_OK;
 }
 

@@ -105,7 +105,7 @@ __global__ void __launch_bounds__(kRenderThreads) k_render(const __grid_constant
       const unsigned draw_index = unsigned(g);
       auto frag = [&](int i, int j, unsigned d16) { atomicMin(zbuf + j * S + i, (d16 << 16) | draw_index); };
       for (int t = warp; t < G.n_triangles; t += n_warps)
-        DrawTriangle(M, G.triangles + 9 * t, G.enable_culling, S, half, frag, lane);
+        DrawTriangle(M, G.triangles + 9 * t, G.enable_culling, S, S, half, half, frag, lane);
       __syncthreads();  // sM is rewritten for the next body
     }
   }

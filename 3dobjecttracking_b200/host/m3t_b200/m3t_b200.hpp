@@ -95,6 +95,10 @@ class Batch {
   int NextRegionModel() { return n_rmodels_++; }
   int NextDepthModel() { return n_dmodels_++; }
   int NextStructure() { return n_structures_++; }
+  int NextViewer() { return n_viewers_++; }
+  // every m3tb_update_viewers renders all viewers of the batch: read-backs older than the last update are stale
+  void ViewersUpdated() { ++viewer_version_; }
+  long viewer_version() const { return viewer_version_; }
   int n_bodies() const { return n_bodies_; }
 
   std::vector<float> region_g, region_h, depth_g, depth_h;  // last batched gradients / Hessians (all bodies)
@@ -102,6 +106,8 @@ class Batch {
  private:
   m3tb_ctx* ctx_ = nullptr;
   int max_bodies_ = 0, n_bodies_ = 0, n_renderers_ = 0, n_color_ = 0, n_depth_ = 0, n_rmodels_ = 0, n_dmodels_ = 0, n_structures_ = 0;
+  int n_viewers_ = 0;
+  long viewer_version_ = 0;
   long pose_version_ = 0;
   Key done_[kNPhases];
 };
@@ -689,6 +695,152 @@ class FocusedSilhouetteRenderer : public FocusedDepthRenderer {
       : FocusedDepthRenderer(name, batch, renderer_geometry_ptr, camera_ptr, id_type, image_size, z_min, z_max) {}
   bool FetchSilhouetteImage() { return Fetch(); }
   const std::vector<uint8_t>& focused_silhouette_image() { Fetch(); return silhouette_; }
+};
+
+// ---- normal_renderer.h / normal_viewer.h ---------------------------------------------------------------------------
+// FullNormalRenderer (normal_renderer.h:84-93) over the whole image of its camera. On the device it is the renderer of
+// one viewer slot (m3tb_set_viewer); StartRendering renders every viewer of the batch in one m3tb_update_viewers call.
+// Only the viewers' z range 0.02 .. 10 is built.
+class FullNormalRenderer {
+ public:
+  FullNormalRenderer(const std::string& name, const std::shared_ptr<Batch>& batch,
+                     const std::shared_ptr<RendererGeometry>& renderer_geometry_ptr, const std::shared_ptr<Camera>& camera_ptr,
+                     float z_min = 0.02f, float z_max = 10.0f)
+      : name_(name), batch_(batch), renderer_geometry_ptr_(renderer_geometry_ptr), camera_ptr_(camera_ptr), z_min_(z_min),
+        z_max_(z_max) {
+    index_ = batch->NextViewer();
+  }
+  bool SetUp() { return SetUpViewer(0.0f, 0.0f, 1.0f); }
+  bool StartRendering() {
+    if (!set_up_) {
+      std::cerr << "Set up renderer " << name_ << " first" << std::endl;
+      return false;
+    }
+    batch_->ViewersUpdated();
+    return Check(batch_->ctx(), m3tb_update_viewers(batch_->ctx()), "FullNormalRenderer::StartRendering");
+  }
+  bool FetchNormalImage() { return Fetch(); }
+  // BGRA8, width x height, GL_BGRA order (byte 0 encodes x)
+  const std::vector<uint8_t>& normal_image() { Fetch(); return normal_; }
+  const std::vector<uint8_t>& blended_image() { Fetch(); return image_; }
+  int index() const { return index_; }
+  bool set_up() const { return set_up_; }
+  const std::shared_ptr<Camera>& camera_ptr() const { return camera_ptr_; }
+
+  // the viewer slot behind the renderer: kind 0 colour / 1 depth camera, the viewer's blend parameters
+  bool SetUpViewer(float opacity, float min_depth, float max_depth) {
+    set_up_ = false;
+    if (z_min_ != 0.02f || z_max_ != 10.0f) {
+      std::cerr << "FullNormalRenderer " << name_ << ": only the z range 0.02 .. 10 is built" << std::endl;
+      return false;
+    }
+    std::vector<int> geo;
+    for (auto& b : renderer_geometry_ptr_->body_ptrs()) geo.push_back(b->index());
+    const int kind = std::dynamic_pointer_cast<ColorCamera>(camera_ptr_) ? 0 : 1;
+    if (!Check(batch_->ctx(),
+               m3tb_set_viewer(batch_->ctx(), index_, kind, camera_ptr_->index(), geo.data(), int(geo.size()), opacity,
+                               min_depth, max_depth),
+               "FullNormalRenderer::SetUp"))
+      return false;
+    set_up_ = true;
+    fetched_ = -1;
+    return true;
+  }
+
+ private:
+  bool Fetch() {
+    if (fetched_ == batch_->viewer_version()) return true;
+    const Intrinsics& in = camera_ptr_->intrinsics();
+    normal_.resize(size_t(in.width) * in.height * 4);
+    image_.resize(size_t(in.width) * in.height * 3);
+    if (!Check(batch_->ctx(),
+               m3tb_get_viewer_image(batch_->ctx(), index_, image_.data(), size_t(in.width) * 3, normal_.data(),
+                                     size_t(in.width) * 4),
+               "FullNormalRenderer::FetchNormalImage"))
+      return false;
+    fetched_ = batch_->viewer_version();
+    return true;
+  }
+  std::string name_;
+  std::shared_ptr<Batch> batch_;
+  std::shared_ptr<RendererGeometry> renderer_geometry_ptr_;
+  std::shared_ptr<Camera> camera_ptr_;
+  float z_min_, z_max_;
+  int index_ = 0;
+  bool set_up_ = false;
+  long fetched_ = -1;  // the batch's viewer version the images below were read at
+  std::vector<uint8_t> normal_, image_;
+};
+
+// Viewer (viewer.h): UpdateViewer renders and blends; the blended BGR8 image is read back by image() instead of being
+// displayed or saved
+class Viewer {
+ public:
+  virtual ~Viewer() = default;
+  virtual bool SetUp() = 0;
+  // UpdateViewer(save_index): one m3tb_update_viewers for every viewer of the batch
+  bool UpdateViewer(int /*save_index*/) {
+    if (!set_up_) {
+      std::cerr << "Set up viewer " << name_ << " first" << std::endl;
+      return false;
+    }
+    if (dirty_ && !SetUp()) return false;
+    return renderer_.StartRendering();
+  }
+  // the image CalculateAlphaBlend returned at the last update: width x height BGR8
+  const std::vector<uint8_t>& image() { return renderer_.blended_image(); }
+  FullNormalRenderer& renderer() { return renderer_; }
+  void set_opacity(float opacity) { opacity_ = opacity; dirty_ = true; }
+  float opacity() const { return opacity_; }
+  const std::string& name() const { return name_; }
+  bool set_up() const { return set_up_; }
+  bool dirty() const { return dirty_; }
+
+ protected:
+  Viewer(const std::string& name, const std::shared_ptr<Batch>& batch,
+         const std::shared_ptr<RendererGeometry>& renderer_geometry_ptr, const std::shared_ptr<Camera>& camera_ptr,
+         float opacity)
+      : name_(name), renderer_("renderer", batch, renderer_geometry_ptr, camera_ptr), opacity_(opacity) {}
+  bool SetUpWith(float min_depth, float max_depth) {
+    set_up_ = false;
+    if (!renderer_.camera_ptr()->set_up()) {
+      std::cerr << "Camera " << renderer_.camera_ptr()->name() << " was not set up" << std::endl;
+      return false;
+    }
+    if (!renderer_.SetUpViewer(opacity_, min_depth, max_depth)) return false;
+    set_up_ = true;
+    dirty_ = false;
+    return true;
+  }
+  std::string name_;
+  FullNormalRenderer renderer_;
+  float opacity_;
+  bool set_up_ = false, dirty_ = false;
+};
+
+class NormalColorViewer : public Viewer {
+ public:
+  NormalColorViewer(const std::string& name, const std::shared_ptr<Batch>& batch,
+                    const std::shared_ptr<ColorCamera>& color_camera_ptr,
+                    const std::shared_ptr<RendererGeometry>& renderer_geometry_ptr, float opacity = 0.5f)
+      : Viewer(name, batch, renderer_geometry_ptr, color_camera_ptr, opacity) {}
+  bool SetUp() override { return SetUpWith(0.0f, 1.0f); }
+};
+
+class NormalDepthViewer : public Viewer {
+ public:
+  NormalDepthViewer(const std::string& name, const std::shared_ptr<Batch>& batch,
+                    const std::shared_ptr<DepthCamera>& depth_camera_ptr,
+                    const std::shared_ptr<RendererGeometry>& renderer_geometry_ptr, float min_depth = 0.0f,
+                    float max_depth = 1.0f, float opacity = 0.5f)
+      : Viewer(name, batch, renderer_geometry_ptr, depth_camera_ptr, opacity), min_depth_(min_depth),
+        max_depth_(max_depth) {}
+  bool SetUp() override { return SetUpWith(min_depth_, max_depth_); }
+  void set_min_depth(float v) { min_depth_ = v; dirty_ = true; }
+  void set_max_depth(float v) { max_depth_ = v; dirty_ = true; }
+
+ private:
+  float min_depth_, max_depth_;
 };
 
 // ---- modality.h ----------------------------------------------------------------------------------------------------
@@ -1363,6 +1515,25 @@ class Tracker {
       for (auto& m : l->modality_ptrs()) modality_ptrs_.push_back(m);
     return true;
   }
+  // Tracker::AddViewer (tracker.cpp): viewers are set up with the tracker and updated by UpdateViewers
+  bool AddViewer(const std::shared_ptr<Viewer>& v) {
+    for (auto& p : viewer_ptrs_)
+      if (p->name() == v->name()) {
+        std::cerr << "Viewer " << v->name() << " already exists" << std::endl;
+        return false;
+      }
+    viewer_ptrs_.push_back(v);
+    return true;
+  }
+  // Tracker::UpdateViewers (tracker.cpp:373): one m3tb_update_viewers for all viewers, from the current poses and frames
+  bool UpdateViewers(int /*iteration*/) {
+    if (viewer_ptrs_.empty()) return true;
+    for (auto& v : viewer_ptrs_)
+      if (v->dirty() && !v->SetUp()) return false;
+    batch_->ViewersUpdated();
+    return Check(batch_->ctx(), m3tb_update_viewers(batch_->ctx()), "Tracker::UpdateViewers");
+  }
+  const std::vector<std::shared_ptr<Viewer>>& viewer_ptrs() const { return viewer_ptrs_; }
   void set_n_corr_iterations(int v) { n_corr_iterations_ = v; }
   void set_n_update_iterations(int v) { n_update_iterations_ = v; }
   int n_corr_iterations() const { return n_corr_iterations_; }
@@ -1380,6 +1551,8 @@ class Tracker {
         if (!c->SetUp()) return false;
       if (!o->SetUp()) return false;
     }
+    for (auto& v : viewer_ptrs_)
+      if (!v->SetUp()) return false;
     set_up_ = true;
     return true;
   }
@@ -1429,6 +1602,7 @@ class Tracker {
   int n_corr_iterations_, n_update_iterations_;
   std::vector<std::shared_ptr<Optimizer>> optimizer_ptrs_;
   std::vector<std::shared_ptr<Modality>> modality_ptrs_;
+  std::vector<std::shared_ptr<Viewer>> viewer_ptrs_;
   bool set_up_ = false;
 };
 

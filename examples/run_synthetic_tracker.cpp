@@ -4,7 +4,10 @@
 // object through the Modality / Optimizer methods; prints both pose sets as JSON for tests/test_gpu_host_mirror.py.
 //
 //   usage: run_synthetic_tracker [n_bodies=3] [n_lines=200] [n_points=200] [n_divides=2] [seed=1] [links_per_structure=1]
-//                                [renderers=0]
+//                                [renderers=0] [viewer_dir]
+// With viewer_dir a NormalColorViewer and a NormalDepthViewer on camera 0 draw every body; after the tracking step
+// Tracker::UpdateViewers renders them and the overlays are written as viewer_dir/color_viewer.ppm and depth_viewer.ppm
+// (binary PPM); the same viewers through the plain C ABI must give the same bytes ("viewers_equal_c_abi").
 // With renderers = 1 every body's modalities model occlusions and check regions / silhouettes with device renderers
 // (one FocusedSilhouetteRenderer per camera over all bodies of one RendererGeometry), and the same scene is also run
 // through the plain C ABI ("c_abi" poses), which the fused Tracker path must reproduce bit for bit.
@@ -12,9 +15,11 @@
 // link a revolute-x child at Tx(0.01) of the previous one, as in the reference's examples/optimization_time.cpp) that
 // are tracked by one Optimizer each; the children's start poses come from Optimizer::CalculateConsistentPoses.
 #include <cmath>
+#include <cstdio>
 #include <cstdlib>
 #include <iostream>
 #include <memory>
+#include <string>
 #include <vector>
 
 #include "m3t_b200/m3t_b200.hpp"
@@ -78,7 +83,24 @@ struct Scene {
   std::vector<std::shared_ptr<DepthCamera>> depth_cameras;
   std::vector<std::shared_ptr<Optimizer>> optimizers;
   std::shared_ptr<Tracker> tracker;
+  std::shared_ptr<NormalColorViewer> color_viewer;
+  std::shared_ptr<NormalDepthViewer> depth_viewer;
 };
+
+// binary PPM (P6) of a BGR8 image, the viewer image a display would show
+bool WritePpm(const std::string& path, const std::vector<uint8_t>& bgr, int width, int height) {
+  std::FILE* f = std::fopen(path.c_str(), "wb");
+  if (!f) return false;
+  std::fprintf(f, "P6\n%d %d\n255\n", width, height);
+  std::vector<uint8_t> rgb(bgr.size());
+  for (size_t k = 0; k + 2 < bgr.size(); k += 3) {
+    rgb[k] = bgr[k + 2];
+    rgb[k + 1] = bgr[k + 1];
+    rgb[k + 2] = bgr[k];
+  }
+  const bool ok = std::fwrite(rgb.data(), 1, rgb.size(), f) == rgb.size();
+  return std::fclose(f) == 0 && ok;
+}
 
 void PrintPoses(const char* key, Scene& s) {
   std::printf("\"%s\": [", key);
@@ -101,6 +123,10 @@ int main(int argc, char** argv) {
   const uint64_t seed = argc > 5 ? std::strtoull(argv[5], nullptr, 10) : 1;
   const int chain = argc > 6 ? std::max(1, std::atoi(argv[6])) : 1;
   const bool with_renderers = argc > 7 && std::atoi(argv[7]) != 0;
+  // viewer mode: a NormalColorViewer and a NormalDepthViewer on camera 0 draw every body; after the tracking step the
+  // two overlays are written as binary PPM files into this directory
+  const std::string viewer_dir = argc > 8 ? argv[8] : "";
+  const bool with_viewers = !viewer_dir.empty();
   float prism_diameter = 0.0f;
   const std::vector<float> prism = PrismTriangles(&prism_diameter);
   if (n_bodies % chain != 0) {
@@ -168,7 +194,7 @@ int main(int argc, char** argv) {
       all_bodies.back()->set_maximum_body_diameter(prism_diameter);
       all_bodies.back()->set_body_id(uint8_t(b + 1));
       all_bodies.back()->set_region_id(7);
-      if (with_renderers && !geometry->AddBody(all_bodies.back())) return false;
+      if ((with_renderers || with_viewers) && !geometry->AddBody(all_bodies.back())) return false;
     }
     if (!geometry->SetUp()) return false;
     for (int b = 0; b < n_bodies; ++b) {
@@ -212,6 +238,12 @@ int main(int argc, char** argv) {
       s.bodies.push_back(body);
       s.color_cameras.push_back(cc);
       s.depth_cameras.push_back(dc);
+    }
+    if (with_viewers) {
+      s.color_viewer = std::make_shared<NormalColorViewer>("color_viewer", s.batch, s.color_cameras[0], geometry);
+      s.depth_viewer = std::make_shared<NormalDepthViewer>("depth_viewer", s.batch, s.depth_cameras[0], geometry, 0.0f, 1.0f);
+      s.color_viewer->set_opacity(0.6f);
+      if (!s.tracker->AddViewer(s.color_viewer) || !s.tracker->AddViewer(s.depth_viewer)) return false;
     }
     if (!s.tracker->SetUp()) return false;
     for (int b = 0; b < n_bodies; ++b) {
@@ -276,6 +308,40 @@ int main(int argc, char** argv) {
   const bool refused = !not_set_up.ExecuteTrackingStep(0);
 
   if (!fused.tracker->ExecuteTrackingStep(0)) return 3;
+  bool viewers_equal = true;
+  if (with_viewers) {  // the overlays of the tracked poses, and the same viewers through the plain C ABI
+    if (!fused.tracker->UpdateViewers(0)) return 7;
+    const std::vector<uint8_t>& cimg = fused.color_viewer->image();
+    const std::vector<uint8_t>& dimg = fused.depth_viewer->image();
+    if (!WritePpm(viewer_dir + "/color_viewer.ppm", cimg, ci.width, ci.height) ||
+        !WritePpm(viewer_dir + "/depth_viewer.ppm", dimg, di.width, di.height))
+      return 8;
+    std::vector<float> poses(size_t(12) * n_bodies);
+    m3tb_ctx* raw = nullptr;
+    bool ok = m3tb_create(0, n_bodies, 1, 1, &raw) == M3TB_OK &&
+              m3tb_get_poses(fused.batch->ctx(), 0, n_bodies, poses.data()) == 0 &&
+              m3tb_set_poses(raw, 0, n_bodies, poses.data()) == 0 &&
+              m3tb_set_color_camera(raw, 0, &ci, color_w2c.data()) == 0 &&
+              m3tb_set_depth_camera(raw, 0, &di, depth_w2c.data(), 0.001f) == 0 &&
+              m3tb_upload_color(raw, 0, color[0].data(), cpitch) == 0 && m3tb_upload_depth(raw, 0, depth[0].data(), dpitch) == 0;
+    const Transform3fA identity;
+    std::vector<int> all(n_bodies);
+    for (int b = 0; b < n_bodies && ok; ++b) {
+      all[b] = b;
+      ok = m3tb_set_body_geometry(raw, b, prism.data(), int(prism.size() / 9), identity.data(), prism_diameter, 1, b + 1, 7) == 0;
+    }
+    std::vector<uint8_t> c2(cimg.size()), d2(dimg.size());
+    ok = ok && m3tb_set_viewer(raw, 0, 0, 0, all.data(), n_bodies, 0.6f, 0.0f, 1.0f) == 0 &&
+         m3tb_set_viewer(raw, 1, 1, 0, all.data(), n_bodies, 0.5f, 0.0f, 1.0f) == 0 && m3tb_update_viewers(raw) == 0 &&
+         m3tb_get_viewer_image(raw, 0, c2.data(), size_t(ci.width) * 3, nullptr, 0) == 0 &&
+         m3tb_get_viewer_image(raw, 1, d2.data(), size_t(di.width) * 3, nullptr, 0) == 0;
+    if (!ok) {
+      std::cerr << "C ABI viewer run failed: " << (raw ? m3tb_last_error(raw) : "no context") << std::endl;
+      return 9;
+    }
+    m3tb_destroy(raw);
+    viewers_equal = c2 == cimg && d2 == dimg;
+  }
   if (!object_wise.tracker->ExecuteTrackingStepObjectWise(0)) return 4;
   bool joints_ok = true;
   if (chain > 1) {  // the children still hang on their parents at Tx(0.01), rotated about x only
@@ -293,6 +359,7 @@ int main(int argc, char** argv) {
   std::printf("\"n_bodies\": %d, \"refused_without_setup\": %s, \"launches_fused\": %lld, \"launches_object_wise\": %lld, ",
               n_bodies, refused ? "true" : "false", (long long)m3tb_launch_count(fused.batch->ctx()),
               (long long)m3tb_launch_count(object_wise.batch->ctx()));
+  if (with_viewers) std::printf("\"viewers_equal_c_abi\": %s, ", viewers_equal ? "true" : "false");
   if (with_renderers) {
     bool visible = true;
     for (int b = 0; b < n_bodies; ++b)

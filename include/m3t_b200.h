@@ -307,6 +307,34 @@ int m3tb_render(m3tb_ctx* ctx);
 int m3tb_get_rendering(m3tb_ctx* ctx, int renderer, void* depth_u16, void* silhouette_u8, float* corner_u, float* corner_v,
                        float* scale, float* projection_term_a, float* projection_term_b, int* visible_flags);
 
+/* ---- viewers (NormalColorViewer / NormalDepthViewer, normal_viewer.cpp; FullNormalRenderer, normal_renderer.cpp) ---
+ * A viewer renders its geometry bodies over the whole camera image (width x height) with a full normal renderer
+ * (FullRenderer::CalculateProjectionMatrix from the camera intrinsics, z range 0.02 .. 10, the defaults of the viewers'
+ * renderers, normal_viewer.h:59,104) and alpha-blends the normal image over the camera frame (CalculateAlphaBlend).
+ * DESIGN.md §3 "k_view_setup / k_view_raster / k_view_resolve" states what is computed. */
+/* NormalColorViewer (kind 0, colour camera `camera`) or NormalDepthViewer (kind 1, depth camera `camera`) +
+ * SetUp (normal_viewer.cpp:46-87,141-182): `geometry_bodies` are the RendererGeometry's bodies in draw order
+ * (render_data_bodies), each with the geometry given by m3tb_set_body_geometry and its own culling flag; `opacity` is
+ * set_opacity (reference default 0.5); min_depth / max_depth are the NormalDepthViewer's (defaults 0 and 1; ignored
+ * for kind 0). Viewer ids are dense (0..n); setting an existing id replaces it. M3TB_ERR_INVALID for bad ids or kind,
+ * an unset camera, a geometry body without geometry or a body listed twice. */
+int m3tb_set_viewer(m3tb_ctx* ctx, int viewer, int kind, int camera, const int* geometry_bodies, int n_geometry,
+                    float opacity, float min_depth, float max_depth);
+/* Tracker::UpdateViewers (tracker.cpp:373) = UpdateViewer of every viewer (normal_viewer.cpp:97-113,192-211), from the
+ * current poses, in stream order after any tracking launch: FullNormalRenderer::StartRendering + FetchNormalImage and
+ * the alpha blend over the frame the camera holds (Camera::image(): the last upload; a pinned frame is read in place).
+ * After m3tb_prefetch_frames the cameras already hold the next frames, so a caller who wants each frame paired with the
+ * poses tracked on it updates the viewers before handing the next frames over. Three kernel launches for all viewers
+ * together. m3tb_tracking_step never updates viewers. M3TB_ERR_NOT_SET_UP when a viewer's camera has never received a
+ * frame; no viewer: nothing is launched. */
+int m3tb_update_viewers(m3tb_ctx* ctx);
+/* Read-back of viewer `viewer`'s last update: the blended BGR8 image (width x height, rows `pitch` bytes apart) and the
+ * renderer's normal_image() (FullNormalRenderer::FetchNormalImage: BGRA8, GL_BGRA order with byte 0 = x, cleared to
+ * 0, rows `normal_pitch` bytes apart). Either pointer may be NULL. M3TB_ERR_NOT_SET_UP before the first update since
+ * the viewer was set or its camera changed size. */
+int m3tb_get_viewer_image(m3tb_ctx* ctx, int viewer, uint8_t* bgr, size_t pitch, uint8_t* normal_bgra,
+                          size_t normal_pitch);
+
 /* Loader-style batch ingest: `count` frames for cameras [first_cam, first_cam+count), frame k at
  * base + k*frame_stride bytes. Cameras of equal size share one device pool, so this is a single
  * host->device copy when the host frames are contiguous (frame_stride == height*pitch). */
