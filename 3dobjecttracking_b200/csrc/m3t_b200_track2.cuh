@@ -12,8 +12,9 @@
 //     multiplication order, for lines walked in either direction. The 12 entries go to shared memory (24 KB); the
 //     local-mode gradient reads its two entries from there by index.
 //   * GetClosestView is the exact pruned search of m3t_b200_views.cuh (~200 instead of 2 x 2562 dot products per
-//     iteration), done by the last warp of each group while the other warps wait at the group's named barrier
-//     (every warp searching redundantly would spend the issue slots of the whole group on the same search).
+//     iteration), split over the 16 warps of each group (ClosestViewPrunedGroup): each warp bounds its share of the
+//     clusters and evaluates its candidates (usually one), one group barrier combines the 16 maxima. A single warp
+//     needed ~5 dependent trips to memory while the other 15 waited at the barrier.
 //   * CalculateOptimization (6 x 6) runs thread-serially in registers on warp 0 (every lane the same work, no
 //     shuffles in the dependent chain): pivot order from the original diagonal, gather of the permuted matrix,
 //     unrolled left-looking LDL^T, substitutions, Rodrigues, pose products; shorter than the lane-parallel form.
@@ -50,7 +51,7 @@ struct Shared2 {
   unsigned long long depth_bar, lut_bar, ctile_bar;
   float red[32][32];         // per-warp partial sums g[6] + H lower[21] (+5 pad)
   float a[36], b[6], x[6];   // normal equations
-  int views[2][2];           // [corr parity][region | depth] closest views, published by the group leaders
+  uint2 view_slots[2][2][kGroup / 32];  // [corr parity][region | depth] per-warp maxima of the closest-view searches
   FrameView cframe, dframe;  // how the body sees its colour / depth frame (read on the rare out-of-tile paths)
   int stamp_n[2];            // profiling aid: slots filled so far by the solver warp / the point group's leader warp
   // Per-body parameters, cameras and model headers are read all over the iteration loops. With 225 KB of the SM's
@@ -578,27 +579,29 @@ struct Track2Ready {
   bool lut, ctile, depth;
 };
 
-// Line role, one correspondence iteration: closest view of the region model (group leader), then RegionLine2. With one
-// warp group (POINTS: T = 512) another warp searches the depth model meanwhile, behind the same barrier.
+// Closest view of model m (0: region, searched by the line group; 1: depth, by the point group, or by the only group of
+// the 512-thread kernel), by all threads of the group. The lower bound starts from the previous iteration's answer,
+// re-read from that search's slots in shared memory: a register copy kept across the loop nest sits in local memory in
+// the 1024-thread kernel, one more L2 round trip ahead of the search. The first iteration starts from `view`.
+template <int T>
+__device__ __forceinline__ int GroupClosestView(const TrackArgs& args, Shared2& sh, int corr, int m, int view) {
+  const ModelDev& model = sh.models[m];
+  const int prev = corr > args.corr_begin ? ClosestViewOfSlots<kGroup>(sh.view_slots[(corr - 1) & 1][m]) : view;
+  return ClosestViewPrunedGroup<kGroup>(sh.info[m], model.sorted_views, model.n_clusters, model.orientations4,
+                                        model.n_views, sh.view_o[m], prev, sh.view_slots[corr & 1][m],
+                                        [m] { GroupBarrier<T>(m); });
+}
+
+// Line role, one correspondence iteration: closest view of the region model (the whole group), then RegionLine2. With
+// one warp group (POINTS: T = 512) the group searches the depth model right after.
 template <int T, bool LUT_SMEM, bool POINTS>
-__device__ __forceinline__ void LineCorrespondence(const TrackArgs& args, Shared2& sh, int corr, int& view_r, int view_d,
+__device__ __forceinline__ void LineCorrespondence(const TrackArgs& args, Shared2& sh, int corr, int& view_r, int& view_d,
                                                    int& n_lines, LineRegs& L, Track2Ready& ready) {
-  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, item = tid & (kGroup - 1);
+  const int tid = threadIdx.x, item = tid & (kGroup - 1);
   const BodyDev& body = sh.body;
   const ModelDev* rmodel = &sh.models[0];
-  if (item >= kGroup - 32) {
-    const int v = ClosestViewPrunedWarp(sh.info[0], rmodel->sorted_views, rmodel->n_clusters, rmodel->orientations4,
-                                        rmodel->n_views, sh.view_o[0], view_r);
-    if (lane == 0) sh.views[corr & 1][0] = v;
-  }
-  if (POINTS && DoPhase(sh, args, false, PH_DEPTH_CORR) && warp == T / 32 - 2) {
-    const ModelDev* dmodel = &sh.models[1];
-    const int v = ClosestViewPrunedWarp(sh.info[1], dmodel->sorted_views, dmodel->n_clusters, dmodel->orientations4,
-                                        dmodel->n_views, sh.view_o[1], view_d);
-    if (lane == 0) sh.views[corr & 1][1] = v;
-  }
-  GroupBarrier<T>(0);
-  view_r = sh.views[corr & 1][0];
+  view_r = GroupClosestView<T>(args, sh, corr, 0, view_r);
+  if (POINTS && DoPhase(sh, args, false, PH_DEPTH_CORR)) view_d = GroupClosestView<T>(args, sh, corr, 1, view_d);
   Stamp2<T>(args, sh);  // closest view (region)
   RegionIter rit;
   MakeRegionIter(body.rp, sh.cams[0], sh.rb2c, corr, rit);
@@ -627,23 +630,15 @@ __device__ __forceinline__ void LineCorrespondence(const TrackArgs& args, Shared
   Stamp2<T>(args, sh);  // region lines
 }
 
-// Point role, one correspondence iteration: closest view of the depth model (group leader; with one warp group and
+// Point role, one correspondence iteration: closest view of the depth model (the whole group; with one warp group and
 // lines it was searched in LineCorrespondence), then DepthPoint.
 template <int T, bool LINES>
 __device__ __forceinline__ void PointCorrespondence(const TrackArgs& args, Shared2& sh, int corr, int& view_d, int& n_points,
                                                     PointState& P, Track2Ready& ready) {
-  const int tid = threadIdx.x, lane = tid & 31, item = tid & (kGroup - 1);
+  const int tid = threadIdx.x, item = tid & (kGroup - 1);
   const BodyDev& body = sh.body;
   const ModelDev* dmodel = &sh.models[1];
-  if (!LINES || !DoPhase(sh, args, true, PH_REGION_CORR)) {
-    if (item >= kGroup - 32) {
-      const int v = ClosestViewPrunedWarp(sh.info[1], dmodel->sorted_views, dmodel->n_clusters, dmodel->orientations4,
-                                          dmodel->n_views, sh.view_o[1], view_d);
-      if (lane == 0) sh.views[corr & 1][1] = v;
-    }
-    GroupBarrier<T>(1);
-  }
-  view_d = sh.views[corr & 1][1];
+  if (!LINES || !DoPhase(sh, args, true, PH_REGION_CORR)) view_d = GroupClosestView<T>(args, sh, corr, 1, view_d);
   Stamp2<T>(args, sh);  // closest view (depth)
   DepthIter dit;
   MakeDepthIter(body.dp, sh.cams[1], sh.db2c, sh.dc2b, corr, dit);

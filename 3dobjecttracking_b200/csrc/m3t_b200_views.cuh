@@ -176,6 +176,59 @@ inline int ClosestViewPrunedHost(const ViewClustersHost& vc, const float* ori, i
 }
 
 #ifdef __CUDACC__
+// Evaluates the candidate clusters of one warp's bound pass: bit j of `m` (warp-uniform) marks the cluster whose packed
+// (first | count << 24) word lane j holds. B clusters at a time, so that their loads are in flight together; lane k
+// takes member k (a cluster has <= 32 members) and keeps its running maximum in best / idx (ties: smaller view index).
+template <int B>
+__device__ __forceinline__ void EvaluateViewCandidates(unsigned m, unsigned packed, const float4* __restrict__ sorted,
+                                                       float o0, float o1, float o2, float& best, int& idx) {
+  constexpr unsigned kFull = 0xffffffffu;
+  const int lane = threadIdx.x & 31;
+  while (m) {  // warp-uniform
+    unsigned pk[B];
+#pragma unroll
+    for (int u = 0; u < B; ++u) {
+      const int j = m ? __ffs(m) - 1 : 0;
+      const unsigned v = __shfl_sync(kFull, packed, j);
+      pk[u] = m ? v : 0u;
+      m &= m - 1u;  // 0 stays 0
+    }
+    float4 q[B];
+#pragma unroll
+    for (int u = 0; u < B; ++u) {
+      const int first = int(pk[u] & 0xffffffu), cnt = int(pk[u] >> 24);
+      q[u] = lane < cnt ? __ldg(sorted + first + lane) : make_float4(0.0f, 0.0f, 0.0f, 0.0f);
+    }
+#pragma unroll
+    for (int u = 0; u < B; ++u) {
+      const int cnt = int(pk[u] >> 24);
+      const float dot = o0 * q[u].x + o1 * q[u].y + o2 * q[u].z;
+      const int vi = __float_as_int(q[u].w);
+      if (lane < cnt && (dot > best || (dot == best && vi < idx))) { best = dot; idx = vi; }
+    }
+  }
+}
+
+// Order-preserving unsigned key of a dot product. -0.0 is folded to +0.0 first: the float comparison of the full scan
+// treats the two as equal (the smaller view index wins), and so must the key when the two sit in different lanes.
+__device__ __forceinline__ unsigned ViewKey(float v) {
+  const unsigned k = __float_as_uint(v == 0.0f ? 0.0f : v);
+  return (k & 0x80000000u) ? ~k : (k | 0x80000000u);
+}
+
+// Warp arg-max over (key, idx): largest key, then smallest index. Every lane receives both.
+__device__ __forceinline__ void WarpViewArgMax(unsigned& key, int& idx) {
+  constexpr unsigned kFull = 0xffffffffu;
+  const unsigned kmax = __reduce_max_sync(kFull, key);
+  idx = int(__reduce_min_sync(kFull, key == kmax ? unsigned(idx) : 0x7fffffffu));
+  key = kmax;
+}
+
+// The reference's result from the arg-max: views_[0] unless some dot product exceeded its start value -1.
+__device__ __forceinline__ int ClosestViewResult(unsigned kmax, int ri) {
+  return (ri == 0x7fffffff || kmax <= ViewKey(-1.0f)) ? 0 : ri;
+}
+
 // Device search, executed by ONE WARP (all 32 lanes call it with identical arguments; every lane returns the result).
 //   info / sorted / n_clusters: the cluster tables of the model; ori4: the model's views in original order (for the
 //   lower bound); vo: query (o0, o1, o2, nonzero flag) as the pose-product step leaves it; prev: any view index.
@@ -212,41 +265,72 @@ __device__ __forceinline__ int ClosestViewPrunedWarp(const float4* info, const f
         const float ub = ViewClusterBound(ia[h].x, ia[h].y, ia[h].z, ia[h].w, ib[h].x, ib[h].y, ib[h].z, o0, o1, o2, on2, onorm);
         cand = !(ub < lb);  // NaN-safe: a NaN bound keeps the cluster
       }
-      const unsigned packed = __float_as_uint(ib[h].w);
-      unsigned m = __ballot_sync(kFull, cand);
-      while (m) {  // warp-uniform
-        unsigned pk[4];
-#pragma unroll
-        for (int u = 0; u < 4; ++u) {
-          const int j = m ? __ffs(m) - 1 : 0;
-          const unsigned v = __shfl_sync(kFull, packed, j);
-          pk[u] = m ? v : 0u;
-          m &= m - 1u;  // 0 stays 0
-        }
-        float4 q[4];
-#pragma unroll
-        for (int u = 0; u < 4; ++u) {
-          const int first = int(pk[u] & 0xffffffu), cnt = int(pk[u] >> 24);
-          q[u] = lane < cnt ? __ldg(sorted + first + lane) : make_float4(0.0f, 0.0f, 0.0f, 0.0f);
-        }
-#pragma unroll
-        for (int u = 0; u < 4; ++u) {
-          const int cnt = int(pk[u] >> 24);
-          const float dot = o0 * q[u].x + o1 * q[u].y + o2 * q[u].z;
-          const int vi = __float_as_int(q[u].w);
-          if (lane < cnt && (dot > best || (dot == best && vi < idx))) { best = dot; idx = vi; }
-        }
-      }
+      EvaluateViewCandidates<4>(__ballot_sync(kFull, cand), __float_as_uint(ib[h].w), sorted, o0, o1, o2, best, idx);
     }
   }
-  // warp arg-max, first maximum (smallest view index) wins
-  unsigned key = __float_as_uint(best);
-  key = (key & 0x80000000u) ? ~key : (key | 0x80000000u);
-  const unsigned kmax = __reduce_max_sync(kFull, key);
-  const unsigned candi = key == kmax ? unsigned(idx) : 0x7fffffffu;
-  const int ri = int(__reduce_min_sync(kFull, candi));
-  const unsigned minus_one = ~__float_as_uint(-1.0f);  // the sortable key of -1.0f
-  return (ri == 0x7fffffff || kmax <= minus_one) ? 0 : ri;
+  unsigned key = ViewKey(best);
+  WarpViewArgMax(key, idx);
+  return ClosestViewResult(key, idx);
+}
+
+// The view that a group search published in `slots`: every thread may call this once the search's barrier has passed,
+// until the second search after it starts writing the same slots.
+template <int G>
+__device__ __forceinline__ int ClosestViewOfSlots(const uint2* slots) {
+  const int lane = threadIdx.x & 31;
+  const uint2 s = lane < G / 32 ? slots[lane] : make_uint2(0u, 0x7fffffffu);
+  unsigned key = s.x;
+  int idx = int(s.y);
+  WarpViewArgMax(key, idx);
+  return ClosestViewResult(key, idx);
+}
+
+// The same search, executed by a warp group of G threads (G / 32 warps; all threads call it with identical arguments
+// and every thread returns the result). Shorter dependent chain than the one-warp form: every thread bounds one cluster
+// of a round of G (the tables and the lower bound's view in one trip), each warp evaluates its own candidates, and one
+// group barrier (`barrier()`) publishes the per-warp maxima. Clusters are dealt to the warps round-robin
+// (c = c0 + lane * G/32 + warp): neighbouring clusters, the likely candidates of one query, land in different warps, so
+// a warp rarely holds more than one candidate and evaluates them one at a time (a batch of two costs the 1024-thread
+// k_track2 more spill traffic than it saves). The result does not depend on how the views are split: largest dot
+// product, smallest view index on ties.
+//   slots: G / 32 entries of scratch in shared memory, written on every call (also when there is nothing to search).
+//   Callers alternate two sets between consecutive searches, so that the next search's writes cannot overtake a slow
+//   warp's reads of this one, and ClosestViewOfSlots can re-read this result up to the start of the next-but-one search.
+template <int G, class Barrier>
+__device__ __forceinline__ int ClosestViewPrunedGroup(const float4* info, const float4* __restrict__ sorted,
+                                                      int n_clusters, const float4* __restrict__ ori4, int n_views,
+                                                      const float* vo, int prev, uint2* slots, Barrier barrier) {
+  constexpr unsigned kFull = 0xffffffffu;
+  constexpr int kWarps = G / 32;
+  static_assert(kWarps <= 32 && (G & (G - 1)) == 0, "one slot per warp, read by one warp");
+  const int lane = threadIdx.x & 31, warp = (threadIdx.x & (G - 1)) >> 5;
+  const bool search = vo[3] != 0.0f && n_views > 0;  // group-uniform; else (|t| = 0) the reference returns views_[0]
+  prev = min(max(prev, 0), n_views - 1);
+  // the lower bound's view and the first round's cluster tables are requested together (one trip, not two)
+  const float4 qp = search ? __ldg(ori4 + prev) : make_float4(0.0f, 0.0f, 0.0f, 0.0f);
+  int c = lane * kWarps + warp;
+  float4 ia = make_float4(0.0f, 0.0f, 0.0f, 0.0f), ib = ia;
+  if (search && c < n_clusters) { ia = info[2 * c]; ib = info[2 * c + 1]; }
+  const float o0 = vo[0], o1 = vo[1], o2 = vo[2];
+  const float on2 = o0 * o0 + o1 * o1 + o2 * o2;
+  const float onorm = sqrtf(on2);
+  float best = -1.0f;
+  int idx = 0x7fffffff;
+  for (int c0 = 0; search && c0 < n_clusters; c0 += G, c += G) {
+    bool cand = false;
+    if (c < n_clusters) {
+      const float ub = ViewClusterBound(ia.x, ia.y, ia.z, ia.w, ib.x, ib.y, ib.z, o0, o1, o2, on2, onorm);
+      const float lb = o0 * qp.x + o1 * qp.y + o2 * qp.z;
+      cand = !(ub < lb);  // NaN-safe: a NaN bound keeps the cluster
+    }
+    EvaluateViewCandidates<1>(__ballot_sync(kFull, cand), __float_as_uint(ib.w), sorted, o0, o1, o2, best, idx);
+    if (c + G < n_clusters) { ia = info[2 * (c + G)]; ib = info[2 * (c + G) + 1]; }  // next round (> G clusters)
+  }
+  unsigned key = ViewKey(best);
+  WarpViewArgMax(key, idx);
+  if (lane == 0) slots[warp] = make_uint2(key, unsigned(idx));
+  barrier();
+  return ClosestViewOfSlots<G>(slots);
 }
 #endif  // __CUDACC__
 
