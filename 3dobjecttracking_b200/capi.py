@@ -106,7 +106,8 @@ SYMBOLS = [
     "m3tb_attach_renderer", "m3tb_render", "m3tb_get_rendering", "m3tb_model_params_default", "m3tb_model_views",
     "m3tb_generate_depth_model", "m3tb_get_depth_model", "m3tb_debug_render_model_view", "m3tb_debug_resources",
     "m3tb_generate_region_model", "m3tb_get_region_model", "m3tb_debug_region_model_view", "m3tb_set_viewer",
-    "m3tb_update_viewers", "m3tb_get_viewer_image",
+    "m3tb_update_viewers", "m3tb_get_viewer_image", "m3tb_set_full_renderer", "m3tb_render_full",
+    "m3tb_get_full_rendering",
 ]
 
 KERNEL_NAMES = {0: None, 1: "k_track", 2: "k_track2", 3: "k_track_cluster"}
@@ -222,6 +223,9 @@ def lib():
     L.m3tb_set_viewer.argtypes = [vp, ci, ci, ci, ip, ci, C.c_float, C.c_float, C.c_float]
     L.m3tb_update_viewers.argtypes = [vp]
     L.m3tb_get_viewer_image.argtypes = [vp, ci, vp, C.c_size_t, vp, C.c_size_t]
+    L.m3tb_set_full_renderer.argtypes = [vp, ci, ci, ci, C.c_float, C.c_float, ci, ip, ci]
+    L.m3tb_render_full.argtypes = [vp]
+    L.m3tb_get_full_rendering.argtypes = [vp, ci, vp, C.c_size_t, vp, C.c_size_t, vp, C.c_size_t, fp, fp]
     _lib = L
     return L
 
@@ -488,6 +492,41 @@ class Context:
         self._ck(self.L.m3tb_get_viewer_image(self.h, viewer, bgr.ctypes.data, bgr.strides[0], normal.ctypes.data,
                                               normal.strides[0]))
         return bgr, normal
+
+    def set_full_renderer(self, renderer, camera_kind, camera, geometry_bodies, z_min=0.02, z_max=10.0,
+                          id_type="body"):
+        """FullBasicDepthRenderer / FullSilhouetteRenderer / FullNormalRenderer of camera `camera` (camera_kind
+        "color" | "depth", or 0 | 1) drawing `geometry_bodies` in that order; id_type "body" | "region" (or 0 | 1). The
+        image size is the camera's at the next render_full."""
+        kind = {"color": 0, "depth": 1}.get(camera_kind, camera_kind)
+        idt = {"body": 0, "region": 1}.get(id_type, id_type)
+        g = np.ascontiguousarray(geometry_bodies, np.int32)
+        self._ck(self.L.m3tb_set_full_renderer(self.h, renderer, int(kind), camera, z_min, z_max, int(idt),
+                                               g.ctypes.data_as(C.POINTER(C.c_int)), g.size))
+
+    def render_full(self):
+        """FullRenderer::StartRendering of every full renderer from the current poses."""
+        self._ck(self.L.m3tb_render_full(self.h))
+
+    def get_full_rendering(self, renderer, width, height):
+        """dict(depth [H,W] u16, silhouette [H,W] u8, normal [H,W,4] u8 in GL_BGRA order, projection_term_a / b
+        (float32)) of the renderer's last render."""
+        depth = np.zeros((height, width), np.uint16)
+        sil = np.zeros((height, width), np.uint8)
+        normal = np.zeros((height, width, 4), np.uint8)
+        out = self.get_full_rendering_to(renderer, depth.ctypes.data, depth.strides[0], sil.ctypes.data,
+                                          sil.strides[0], normal.ctypes.data, normal.strides[0])
+        out.update(depth=depth, silhouette=sil, normal=normal)
+        return out
+
+    def get_full_rendering_to(self, renderer, depth_ptr=None, depth_pitch=0, silhouette_ptr=None,
+                              silhouette_pitch=0, normal_ptr=None, normal_pitch=0):
+        """The images into caller memory, host or device (e.g. torch tensors' data_ptr(), pitch in bytes); a None
+        pointer skips that image. Returns dict(projection_term_a, projection_term_b)."""
+        a, b = C.c_float(0.0), C.c_float(0.0)
+        self._ck(self.L.m3tb_get_full_rendering(self.h, renderer, depth_ptr, depth_pitch, silhouette_ptr,
+                                                silhouette_pitch, normal_ptr, normal_pitch, C.byref(a), C.byref(b)))
+        return dict(projection_term_a=np.float32(a.value), projection_term_b=np.float32(b.value))
 
     def generate_depth_model(self, model_id, body, occlusion_bodies=(), params=None):
         """DepthModel::GenerateModel on the device from the geometry of m3tb_set_body_geometry (params: ModelParams,

@@ -1,7 +1,9 @@
 // m3t_b200_view.cu — the viewers' full normal renderers and the overlay they are blended into (NormalColorViewer /
-// NormalDepthViewer::UpdateViewer, normal_viewer.cpp; FullNormalRenderer, normal_renderer.cpp). Three launches for all
-// viewers of a context: k_view_setup clips and sets up every triangle, k_view_raster walks (triangle, screen tile)
-// pairs so that a large triangle is shared by many warps, k_view_resolve writes the normal and viewer images. Float32,
+// NormalDepthViewer::UpdateViewer, normal_viewer.cpp; FullNormalRenderer, normal_renderer.cpp), and the full renderers
+// (FullBasicDepthRenderer / FullSilhouetteRenderer / FullNormalRenderer, m3tb_render_full). Three launches for all
+// viewers (or all full renderers) of a context: k_view_setup clips and sets up every triangle, k_view_raster walks
+// (triangle, screen tile) pairs so that a large triangle is shared by many warps, k_view_resolve writes the normal and
+// viewer images (the depth, silhouette and normal images of a full renderer). Float32,
 // one rounding per operation in the order written (-fmad=false); DESIGN.md §3 "k_view_setup / k_view_raster /
 // k_view_resolve" states the contract, tests/viewer_reference.py restates it.
 #include "m3t_b200_view.cuh"
@@ -142,14 +144,20 @@ __global__ void __launch_bounds__(kViewThreads) k_view_resolve(const __grid_cons
   const uint64_t key = V.zbuf[p];
   V.zbuf[p] = kViewClear;  // glClear of the next update
   unsigned nb[4] = {0u, 0u, 0u, 0u};  // glClearColor(0, 0, 0, 0)
+  const int d = V.first_draw + int((key >> 32) & 0xffffu);
   if (key != kViewClear) {
-    const int d = V.first_draw + int((key >> 32) & 0xffffu);
     float n[3];
     FaceNormal(a.draws[d].triangles + 9 * size_t(key & 0xffffffffu), n);
     EncodeNormal(a.rot + 9 * size_t(d), n, nb);
   }
 #pragma unroll
   for (int k = 0; k < 4; ++k) V.normal[4 * size_t(p) + k] = uint8_t(nb[k]);
+  if (V.kind == VK_FULL) {
+    // glReadPixels of GL_DEPTH_COMPONENT16 (the cleared key reads 65535) and of the silhouette id attachment
+    V.depth[p] = uint16_t(key >> 48);
+    V.silhouette[p] = key != kViewClear ? uint8_t(a.draws[d].silhouette_id) : uint8_t(0);
+    return;
+  }
   unsigned cam[3];
   const uint8_t* row = V.frame + size_t(j) * V.frame_pitch;
   if (V.kind == VK_COLOR) {

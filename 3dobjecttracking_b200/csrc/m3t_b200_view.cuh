@@ -16,9 +16,11 @@ constexpr uint64_t kViewClear = ~uint64_t(0);  // glClear: depth 1.0, no triangl
 constexpr int kViewFanShift = 40;              // allocation counter of k_view_setup: triangles << 40 | tiles
 constexpr uint64_t kViewTileMask = (uint64_t(1) << kViewFanShift) - 1;
 
-enum ViewerKind { VK_COLOR = 0, VK_DEPTH = 1 };
+// VK_FULL: a full renderer (m3tb_set_full_renderer: FullBasicDepthRenderer / FullSilhouetteRenderer /
+// FullNormalRenderer), whose resolve writes depth, silhouette and normal images and blends nothing
+enum ViewerKind { VK_COLOR = 0, VK_DEPTH = 1, VK_FULL = 2 };
 
-// One viewer of an update: its renderer's projection, the camera frame it blends over and its images
+// One viewer (or full renderer) of an update: its renderer's projection, the camera frame it blends over and its images
 struct ViewerDev {
   int width, height;
   int kind;                    // ViewerKind
@@ -31,6 +33,8 @@ struct ViewerDev {
   uint64_t* zbuf;              // [H][W] depth16 << 48 | draw << 32 | triangle; kViewClear between updates
   uint8_t* normal;             // [H][W][4] FullNormalRenderer::normal_image() (GL_BGRA read-back order)
   uint8_t* image;              // [H][W][3] the blended BGR8 viewer image
+  uint16_t* depth;             // VK_FULL: [H][W] FullDepthRenderer::depth_image() (DEPTH_COMPONENT16, 65535 = clear)
+  uint8_t* silhouette;         // VK_FULL: [H][W] FullSilhouetteRenderer::silhouette_image() (0 = background)
   int first_draw, n_draws;     // the viewer's bodies in ViewArgs::draws, in draw order
 };
 
@@ -42,6 +46,7 @@ struct ViewDrawDev {
   int viewer;
   int draw;                    // index among the viewer's draws (the z-buffer key's draw field)
   int body;                    // index of the body2world pose
+  int silhouette_id;           // VK_FULL: Body::body_id() or region_id() by the renderer's id type
   float geometry2body[12];
 };
 
@@ -73,8 +78,8 @@ __global__ void k_view_setup(const __grid_constant__ ViewArgs a);
 // persistent warps over the work items of k_view_setup: the covered pixels of one tile of one triangle, atomicMin
 // into the viewer's z-buffer
 __global__ void k_view_raster(const __grid_constant__ ViewArgs a);
-// grid (pixel blocks, viewers): normal image, frame pixel (or normalised depth), alpha blend; clears the z-buffer and
-// the counter for the next update
+// grid (pixel blocks, viewers): normal image, frame pixel (or normalised depth), alpha blend; for VK_FULL the depth,
+// silhouette and normal images instead. Clears the z-buffer and the counter for the next update.
 __global__ void k_view_resolve(const __grid_constant__ ViewArgs a);
 
 }  // namespace m3tb

@@ -335,6 +335,35 @@ int m3tb_update_viewers(m3tb_ctx* ctx);
 int m3tb_get_viewer_image(m3tb_ctx* ctx, int viewer, uint8_t* bgr, size_t pitch, uint8_t* normal_bgra,
                           size_t normal_pitch);
 
+/* ---- full renderers (FullBasicDepthRenderer / FullSilhouetteRenderer / FullNormalRenderer, renderer.cpp,
+ * basic_depth_renderer.cpp, silhouette_renderer.cpp, normal_renderer.cpp) ---------------------------------------------
+ * A full renderer draws its geometry bodies over the whole image of its camera (width x height, projection
+ * FullRenderer::CalculateProjectionMatrix from the camera intrinsics and the renderer's own z range, world2camera from the
+ * camera) with the viewers' rasteriser (DESIGN.md §3 "Full renderers"). Every full renderer produces all three images:
+ * the depth image, the silhouette image and the normal image. */
+/* FullBasicDepthRenderer / FullSilhouetteRenderer / FullNormalRenderer + SetUp of the colour (camera_kind 0) or depth
+ * (1) camera `camera`: `geometry_bodies` are drawn in that order (RendererGeometry::render_data_bodies), each with the
+ * geometry given by m3tb_set_body_geometry and its own culling flag. id_type: 0 = IDType::BODY, 1 = IDType::REGION (the
+ * silhouette value). Full-renderer ids are dense (0..n) and separate from the focused renderers' and the viewers'; setting
+ * an existing id replaces it. M3TB_ERR_INVALID for bad ids, kind, z range or id type, an unset camera, a geometry body
+ * without geometry or a body listed twice. */
+int m3tb_set_full_renderer(m3tb_ctx* ctx, int renderer, int camera_kind, int camera, float z_min, float z_max,
+                           int id_type, const int* geometry_bodies, int n_geometry);
+/* FullRenderer::StartRendering of every full renderer from the current poses, in stream order after any tracking
+ * launch. Three kernel launches for all full renderers together, whatever their cameras and sizes. Never called by
+ * m3tb_tracking_step or m3tb_update_viewers; no full renderer: nothing is launched. */
+int m3tb_render_full(m3tb_ctx* ctx);
+/* Read-back of full renderer `renderer`'s last render (width x height of its camera): FetchDepthImage (u16,
+ * GL_DEPTH_COMPONENT16 as glReadPixels gives it, 65535 where nothing was drawn, row v = image row v), FetchSilhouetteImage
+ * (u8, the drawn body's body_id or region_id, 0 for background) and FetchNormalImage (BGRA8 as m3tb_get_viewer_image),
+ * rows `*_pitch` bytes apart, and FullDepthRenderer's projection terms (depth = a / (b - value), renderer.cpp:476-477).
+ * Any pointer may be NULL. The images may go to host or device memory; the call waits for the copies only when one of
+ * them goes to host memory. M3TB_ERR_NOT_SET_UP before the first render since the renderer was set or its camera
+ * changed size. */
+int m3tb_get_full_rendering(m3tb_ctx* ctx, int renderer, void* depth_u16, size_t depth_pitch, void* silhouette_u8,
+                            size_t silhouette_pitch, void* normal_bgra, size_t normal_pitch, float* projection_term_a,
+                            float* projection_term_b);
+
 /* Loader-style batch ingest: `count` frames for cameras [first_cam, first_cam+count), frame k at
  * base + k*frame_stride bytes. Cameras of equal size share one device pool, so this is a single
  * host->device copy when the host frames are contiguous (frame_stride == height*pitch). */
