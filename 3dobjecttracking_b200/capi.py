@@ -107,7 +107,7 @@ SYMBOLS = [
     "m3tb_generate_depth_model", "m3tb_get_depth_model", "m3tb_debug_render_model_view", "m3tb_debug_resources",
     "m3tb_generate_region_model", "m3tb_get_region_model", "m3tb_debug_region_model_view", "m3tb_set_viewer",
     "m3tb_update_viewers", "m3tb_get_viewer_image", "m3tb_set_full_renderer", "m3tb_render_full",
-    "m3tb_get_full_rendering",
+    "m3tb_get_full_rendering", "m3tb_undistortion_map", "m3tb_set_camera_undistortion", "m3tb_get_camera_image",
 ]
 
 KERNEL_NAMES = {0: None, 1: "k_track", 2: "k_track2", 3: "k_track_cluster"}
@@ -226,6 +226,9 @@ def lib():
     L.m3tb_set_full_renderer.argtypes = [vp, ci, ci, ci, C.c_float, C.c_float, ci, ip, ci]
     L.m3tb_render_full.argtypes = [vp]
     L.m3tb_get_full_rendering.argtypes = [vp, ci, vp, C.c_size_t, vp, C.c_size_t, vp, C.c_size_t, fp, fp]
+    L.m3tb_undistortion_map.argtypes = [C.POINTER(Intrinsics), fp, C.POINTER(Intrinsics), vp, C.c_size_t]
+    L.m3tb_set_camera_undistortion.argtypes = [vp, ci, ci, vp, C.c_size_t, ci, C.c_int32]
+    L.m3tb_get_camera_image.argtypes = [vp, ci, ci, vp, C.c_size_t]
     _lib = L
     return L
 
@@ -276,6 +279,20 @@ def model_views(params=None):
     out = np.zeros((n.value, 3, 4), np.float32)
     lib().m3tb_model_views(C.byref(p), _p(out), n.value, C.cast(C.byref(n), ip))
     return out
+
+
+def undistortion_map(raw, coefficients, rectified):
+    """m3tb_undistortion_map (host only): the (H, W, 2) int16 map of cv::initUndistortRectifyMap(CV_32FC1) +
+    cv::convertMaps(CV_16SC2, nninterpolation=True) for camera matrix `raw`, coefficients k1, k2, p1, p2, k3, k4, k5, k6
+    and new camera matrix `rectified` (both Intrinsics of the same size)."""
+    k = _f32(coefficients).reshape(8)
+    out = np.zeros((rectified.height, rectified.width, 2), np.int16)
+    if lib().m3tb_undistortion_map(C.byref(raw), _p(k), C.byref(rectified), out.ctypes.data, out.strides[0]) != 0:
+        raise M3TBError("m3tb_undistortion_map: bad arguments")
+    return out
+
+
+_KINDS = {"color": 0, "depth": 1}
 
 
 def region_params(settings=None) -> RegionParams:
@@ -404,6 +421,31 @@ class Context:
     def upload_batch_ptr(self, color, first, count, ptr, frame_stride, pitch):
         f = self.L.m3tb_upload_color_batch if color else self.L.m3tb_upload_depth_batch
         self._ck(f(self.h, first, count, C.c_void_p(ptr), frame_stride, pitch))
+
+    def set_camera_undistortion(self, camera_kind, cam, map_xy, channels, depth_value_offset=0):
+        """Every later upload to camera `cam` (camera_kind "color" | "depth", or 0 | 1) takes the raw frame (`channels`
+        bytes per colour pixel: 4 BGRA or 3 BGR; 1 for depth) and rectifies it through map_xy ([H, W, 2] int16, e.g.
+        undistortion_map()); depth_value_offset is added to every depth pixel with saturation. map_xy None removes it."""
+        kind = _KINDS.get(camera_kind, camera_kind)
+        if map_xy is None:
+            self._ck(self.L.m3tb_set_camera_undistortion(self.h, int(kind), cam, None, 0, int(channels), 0))
+            return
+        m = np.ascontiguousarray(map_xy, np.int16)
+        self._ck(self.L.m3tb_set_camera_undistortion(self.h, int(kind), cam, m.ctypes.data, m.strides[0], int(channels),
+                                                     int(depth_value_offset)))
+
+    def get_camera_image(self, camera_kind, cam, width, height):
+        """Camera::image(): the frame camera `cam` holds, [H, W, 3] u8 BGR (colour) or [H, W] u16 (depth)."""
+        kind = _KINDS.get(camera_kind, camera_kind)
+        out = np.zeros((height, width, 3), np.uint8) if kind == 0 else np.zeros((height, width), np.uint16)
+        self.get_camera_image_to(kind, cam, out.ctypes.data, out.strides[0])
+        return out
+
+    def get_camera_image_to(self, camera_kind, cam, ptr, pitch):
+        """The frame camera `cam` holds into caller memory, host or device (e.g. a torch tensor's data_ptr()), rows
+        `pitch` bytes apart."""
+        kind = _KINDS.get(camera_kind, camera_kind)
+        self._ck(self.L.m3tb_get_camera_image(self.h, int(kind), cam, C.c_void_p(ptr), pitch))
 
     def prefetch_frames(self):
         self._ck(self.L.m3tb_prefetch_frames(self.h))

@@ -23,6 +23,7 @@
 #include "m3t_b200_kernels.cuh"
 #include "m3t_b200_views.cuh"
 #include "m3t_b200_view.cuh"
+#include "m3t_b200_undistort.cuh"
 
 #include "m3t_b200_track_variants.h"
 #include "m3t_b200_track2.cuh"
@@ -249,6 +250,16 @@ struct m3tb_ctx {
   DeviceBuffer<ViewFanDev> d_view_fans;
   DeviceBuffer<uint64_t> d_view_fan_tile;
   DeviceBuffer<unsigned long long> d_view_counter;  // 0 between updates
+
+  // undistortion of raw frames as they are uploaded (m3tb_set_camera_undistortion, k_undistort)
+  struct UndistortHost {
+    DeviceBuffer<int16_t> map;  // [height][map_pitch / 2] (x, y) pairs; empty: frames are uploaded as they are
+    unsigned map_pitch = 0;     // bytes, a multiple of 16
+    int channels = 0;           // bytes per raw colour pixel (3 or 4); 1 for depth
+    int offset = 0;             // depth only
+  };
+  std::vector<UndistortHost> undistort[2];  // [colour | depth][max_cameras]
+  DeviceBuffer<uint8_t> undistort_staging;  // the raw host frames of one upload call, grown lazily
 };
 
 namespace {
@@ -1300,7 +1311,10 @@ int SetCamera(m3tb_ctx* ctx, bool color, int cam, const m3tb_intrinsics* in, con
   c.width = in->width; c.height = in->height;
   std::memcpy(c.w2c, w2c, sizeof(float) * 12);
   c.depth_scale = depth_scale;
-  if (dims_changed) c.image = nullptr;
+  if (dims_changed) {
+    c.image = nullptr;
+    ctx->undistort[color ? 0 : 1][cam] = {};  // the map was made for the old size
+  }
   c.set = 1;
   ctx->cams_dirty = true;
   return M3TB_OK;
@@ -1371,9 +1385,14 @@ const uint8_t* PinnedAlias(m3tb_ctx* ctx, const void* host) {
 // the next consumer launch first runs k_ingest, which fetches only each body's ROI. The caller keeps the frame
 // unchanged until the work that uses it has completed (m3tb_synchronize / m3tb_get_poses), exactly as for any
 // asynchronous copy from pinned memory. Pageable frames and device frames are copied in full.
+int UploadUndistorted(m3tb_ctx* ctx, bool color, const int* cams, const void* const* srcs, int n, size_t pitch,
+                      bool on_device);
+
 int Upload(m3tb_ctx* ctx, bool color, int cam, const void* src, size_t pitch, cudaMemcpyKind kind,
            const uint8_t* pinned_alias) {
   if (cam < 0 || cam >= ctx->max_cameras || !src) return Fail(ctx, M3TB_ERR_INVALID, "bad upload arguments");
+  if (ctx->undistort[color ? 0 : 1][cam].map)
+    return UploadUndistorted(ctx, color, &cam, &src, 1, pitch, kind == cudaMemcpyDeviceToDevice);
   int rc = EnsureImages(ctx, color, cam, 1);
   if (rc) return rc;
   CameraDev& c = (color ? ctx->h_ccams : ctx->h_dcams)[cam];
@@ -1398,6 +1417,27 @@ int Upload(m3tb_ctx* ctx, bool color, int cam, const void* src, size_t pitch, cu
 int UploadBatch(m3tb_ctx* ctx, bool color, int first, int count, const void* src, size_t frame_stride, size_t pitch) {
   if (first < 0 || count <= 0 || first + count > ctx->max_cameras || !src)
     return Fail(ctx, M3TB_ERR_INVALID, "bad batch upload arguments");
+  const uint8_t* s = static_cast<const uint8_t*>(src);
+  {  // cameras with an undistortion: all of them in one k_undistort launch; the others as single uploads
+    std::vector<int> und;
+    std::vector<const void*> und_src;
+    for (int k = 0; k < count; ++k)
+      if (ctx->undistort[color ? 0 : 1][first + k].map) {
+        und.push_back(first + k);
+        und_src.push_back(s + frame_stride * k);
+      }
+    if (!und.empty()) {
+      int rc = UploadUndistorted(ctx, color, und.data(), und_src.data(), int(und.size()), pitch, false);
+      if (rc) return rc;
+      for (int k = 0; k < count; ++k) {
+        if (ctx->undistort[color ? 0 : 1][first + k].map) continue;
+        const uint8_t* f = s + frame_stride * k;
+        rc = Upload(ctx, color, first + k, f, pitch, cudaMemcpyHostToDevice, PinnedAlias(ctx, f));
+        if (rc) return rc;
+      }
+      return M3TB_OK;
+    }
+  }
   ImagePool& pool = color ? ctx->color_pool : ctx->depth_pool;
   int rc = EnsureImages(ctx, color, first, count);
   if (rc) return rc;
@@ -1406,7 +1446,6 @@ int UploadBatch(m3tb_ctx* ctx, bool color, int first, int count, const void* src
     const CameraDev& c = (color ? ctx->h_ccams : ctx->h_dcams)[first + k];
     pooled = pooled && pool.base && c.image == pool.base + pool.frame_bytes * (first + k);
   }
-  const uint8_t* s = static_cast<const uint8_t*>(src);
   if (const uint8_t* alias = PinnedAlias(ctx, src)) {
     for (int k = 0; k < count; ++k) {
       int rc = Upload(ctx, color, first + k, s + frame_stride * k, pitch, cudaMemcpyHostToDevice, alias + frame_stride * k);
@@ -1435,6 +1474,84 @@ int UploadBatch(m3tb_ctx* ctx, bool color, int first, int count, const void* src
     int rc = Upload(ctx, color, first + k, s + frame_stride * k, pitch, cudaMemcpyHostToDevice, nullptr);
     if (rc) return rc;
   }
+  return M3TB_OK;
+}
+
+// Camera::UpdateImage of an AzureKinect camera: the raw frames of cameras cams[0..n) (srcs[k], `pitch` bytes per row)
+// are rectified into the cameras' device copies by one k_undistort launch (one per kUndistortMaxJobs frames). Device
+// frames are read where they are. Host frames, pageable or pinned, first go to a staging buffer by DMA: k_undistort's
+// gather would otherwise cross PCIe in small scattered reads (scripts/undistortion_timing.py measures both). Afterwards
+// the cameras refer to no host memory, as after a pageable copy.
+int UploadUndistorted(m3tb_ctx* ctx, bool color, const int* cams, const void* const* srcs, int n, size_t pitch,
+                      bool on_device) {
+  auto& U = ctx->undistort[color ? 0 : 1];
+  std::vector<CameraDev>& C = color ? ctx->h_ccams : ctx->h_dcams;
+  std::vector<size_t> offset(n, 0);
+  size_t staging = 0;
+  for (int k = 0; k < n; ++k) {
+    const CameraDev& c = C[cams[k]];
+    const size_t row = size_t(c.width) * (color ? U[cams[k]].channels : 2);
+    if (pitch < row) return Fail(ctx, M3TB_ERR_INVALID, "pitch smaller than a raw row");
+    if (!color && ((reinterpret_cast<uintptr_t>(srcs[k]) | pitch) & 1))
+      return Fail(ctx, M3TB_ERR_INVALID, "depth frame not aligned to 2 bytes");
+    offset[k] = staging;
+    if (!on_device) staging += Align(row, 16) * size_t(c.height);
+  }
+  // staging first: a failed allocation leaves the cameras as they were
+  if (staging > ctx->undistort_staging.size()) CU(ctx->undistort_staging.create(staging));
+  for (int k = 0; k < n; ++k) {
+    int rc = EnsureImages(ctx, color, cams[k], 1);
+    if (rc) return rc;
+  }
+  // a prefetched ingest may still write the device copies
+  if (ctx->prefetched) CU(cudaStreamWaitEvent(ctx->stream, ctx->pf.ev_ingest_done, 0));
+  UndistortArgs a;
+  a.n_jobs = 0;
+  unsigned blocks = 0;
+  auto launch = [&]() -> int {
+    k_undistort<<<dim3(blocks, unsigned(a.n_jobs)), kUndistortThreads, 0, ctx->stream>>>(a);
+    CU(cudaGetLastError());
+    ctx->launches++;
+    a.n_jobs = 0;
+    blocks = 0;
+    return M3TB_OK;
+  };
+  for (int k = 0; k < n; ++k) {
+    const int cam = cams[k];
+    CameraDev& c = C[cam];
+    const auto& u = U[cam];
+    UndistortJob& j = a.jobs[a.n_jobs++];
+    j.map = u.map;
+    j.map_pitch = u.map_pitch;
+    j.width = c.width;
+    j.height = c.height;
+    j.channels = u.channels;
+    j.offset = u.offset;
+    j.dst = const_cast<uint8_t*>(c.image);
+    j.dst_pitch = c.pitch;
+    if (on_device) {
+      j.src = static_cast<const uint8_t*>(srcs[k]);
+      j.src_pitch = unsigned(pitch);
+    } else {
+      const size_t row = size_t(c.width) * (color ? u.channels : 2);
+      j.src = ctx->undistort_staging + offset[k];
+      j.src_pitch = unsigned(Align(row, 16));
+      CU(cudaMemcpy2DAsync(const_cast<uint8_t*>(j.src), j.src_pitch, srcs[k], pitch, row, c.height,
+                           cudaMemcpyHostToDevice, ctx->stream));
+    }
+    const size_t threads = size_t((c.width + kUndistortPixels - 1) / kUndistortPixels) * size_t(c.height);
+    blocks = std::max(blocks, unsigned((threads + kUndistortThreads - 1) / kUndistortThreads));
+    c.host_src = nullptr;
+    c.host_pitch = 0;
+    c.generation = (c.generation + 1) & 0x3fffffff;
+    if (color) ctx->bin_shift[cam] = kBinsNone;  // k_bin rebuilds the bin indices, as after a pageable copy
+    if (a.n_jobs == kUndistortMaxJobs) {
+      int rc = launch();
+      if (rc) return rc;
+    }
+  }
+  ctx->cams_dirty = true;
+  if (a.n_jobs) return launch();
   return M3TB_OK;
 }
 
@@ -2017,6 +2134,8 @@ int m3tb_create(int device, int max_bodies, int max_cameras, int max_models, m3t
   ctx->private_color.resize(max_cameras);
   ctx->private_depth.resize(max_cameras);
   ctx->bin_shift.assign(max_cameras, kBinsNone);
+  ctx->undistort[0].resize(max_cameras);
+  ctx->undistort[1].resize(max_cameras);
   ctx->h_geometry.assign(max_bodies, GeometryDev());
   std::memset(ctx->h_geometry.data(), 0, sizeof(GeometryDev) * max_bodies);
   ctx->geometry_alloc.resize(max_bodies);
@@ -3752,6 +3871,53 @@ int m3tb_get_full_rendering(m3tb_ctx* ctx, int renderer, void* depth_u16, size_t
   if (projection_term_a) *projection_term_a = h.z_max * h.z_min * float(USHRT_MAX) / (h.z_max - h.z_min);
   if (projection_term_b) *projection_term_b = h.z_max * float(USHRT_MAX) / (h.z_max - h.z_min);
   if (to_host) CU(cudaStreamSynchronize(ctx->stream));
+  return M3TB_OK;
+}
+
+int m3tb_set_camera_undistortion(m3tb_ctx* ctx, int camera_kind, int cam, const int16_t* map_xy, size_t map_pitch,
+                                 int channels, int32_t depth_value_offset) {
+  CHECK_CTX();
+  if ((camera_kind != 0 && camera_kind != 1) || cam < 0 || cam >= ctx->max_cameras)
+    return Fail(ctx, M3TB_ERR_INVALID, "bad camera kind / index");
+  const bool color = camera_kind == 0;
+  const CameraDev& c = (color ? ctx->h_ccams : ctx->h_dcams)[cam];
+  if (!c.set) return Fail(ctx, M3TB_ERR_NOT_SET_UP, "set the camera before its undistortion");
+  auto& slot = ctx->undistort[camera_kind][cam];
+  if (!map_xy) {
+    slot = {};
+    return M3TB_OK;
+  }
+  if (color ? (channels != 3 && channels != 4) : channels != 1)
+    return Fail(ctx, M3TB_ERR_INVALID, "channels must be 3 or 4 (colour) or 1 (depth)");
+  if (depth_value_offset < SHRT_MIN || depth_value_offset > SHRT_MAX || (color && depth_value_offset != 0))
+    return Fail(ctx, M3TB_ERR_INVALID, "the depth value offset is a short, and 0 for colour cameras");
+  const size_t row = 4 * size_t(c.width);
+  if (map_pitch < row) return Fail(ctx, M3TB_ERR_INVALID, "map pitch smaller than a row");
+  m3tb_ctx::UndistortHost h;
+  h.map_pitch = unsigned(Align(row, 16));
+  h.channels = channels;
+  h.offset = depth_value_offset;
+  CU(h.map.create(size_t(h.map_pitch / 2) * c.height));
+  CU(cudaMemcpy2DAsync(h.map, h.map_pitch, map_xy, map_pitch, row, c.height, cudaMemcpyDefault, ctx->stream));
+  CU(cudaStreamSynchronize(ctx->stream));  // the caller's map may be released on return
+  slot = std::move(h);
+  return M3TB_OK;
+}
+
+int m3tb_get_camera_image(m3tb_ctx* ctx, int camera_kind, int cam, void* dst, size_t pitch) {
+  CHECK_CTX();
+  if ((camera_kind != 0 && camera_kind != 1) || cam < 0 || cam >= ctx->max_cameras || !dst)
+    return Fail(ctx, M3TB_ERR_INVALID, "bad camera image arguments");
+  const CameraDev& c = (camera_kind == 0 ? ctx->h_ccams : ctx->h_dcams)[cam];
+  if (!c.set || !c.image) return Fail(ctx, M3TB_ERR_NOT_SET_UP, "camera not set / no image uploaded");
+  const size_t row = size_t(c.width) * (camera_kind == 0 ? 3 : 2);
+  if (pitch < row) return Fail(ctx, M3TB_ERR_INVALID, "pitch smaller than a row");
+  if (ctx->prefetched) CU(cudaStreamWaitEvent(ctx->stream, ctx->pf.ev_ingest_done, 0));
+  // a pinned frame's device copy is valid only inside the fetched rectangles: the frame itself is read
+  const uint8_t* src = c.host_src ? c.host_src : c.image;
+  const size_t src_pitch = c.host_src ? c.host_pitch : c.pitch;
+  CU(cudaMemcpy2DAsync(dst, pitch, src, src_pitch, row, c.height, cudaMemcpyDefault, ctx->stream));
+  if (!IsDevicePointer(dst)) CU(cudaStreamSynchronize(ctx->stream));
   return M3TB_OK;
 }
 

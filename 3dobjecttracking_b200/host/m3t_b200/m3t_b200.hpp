@@ -253,6 +253,125 @@ class DepthCamera : public Camera {
   float depth_scale_;
 };
 
+// ---- azure_kinect_camera.h, without the SDK -------------------------------------------------------------------------
+// The calibration k4a::device::get_calibration reports for one camera (k4a_calibration_intrinsic_parameters_t::_param
+// and the resolution). The caller reads it from the SDK (or a file) and hands it over.
+struct AzureKinectCalibration {
+  float fx = 0, fy = 0, cx = 0, cy = 0;
+  float k1 = 0, k2 = 0, k3 = 0, k4 = 0, k5 = 0, k6 = 0, p1 = 0, p2 = 0;
+  int width = 0, height = 0;
+};
+
+// GetIntrinsicsAndDistortionMap (azure_kinect_camera.cpp:234-265, 387-419): fu / fv scaled by image_scale, ppu / ppv
+// kept; the map of cv::initUndistortRectifyMap + convertMaps(CV_16SC2) from camera matrix (fx, fy, cx, cy) to that
+// camera, coefficients in OpenCV order.
+inline bool AzureKinectIntrinsicsAndDistortionMap(const AzureKinectCalibration& c, float image_scale, Intrinsics* intrinsics,
+                                                  std::vector<int16_t>* map) {
+  Intrinsics raw{c.fx, c.fy, c.cx, c.cy, c.width, c.height};
+  *intrinsics = raw;
+  intrinsics->fu *= image_scale;
+  intrinsics->fv *= image_scale;
+  const float coefficients[8] = {c.k1, c.k2, c.p1, c.p2, c.k3, c.k4, c.k5, c.k6};
+  if (c.width <= 0 || c.height <= 0) return false;
+  map->assign(size_t(c.width) * size_t(c.height) * 2, 0);
+  return m3tb_undistortion_map(&raw, coefficients, intrinsics, map->data(), size_t(c.width) * 4) == M3TB_OK;
+}
+
+// AzureKinectColorCamera: UpdateImage takes the SDK's BGRA32 colour buffer (get_color_image().get_buffer()) and leaves
+// the rectified BGR frame on the device (cvtColor(RGBA2RGB) + remap, azure_kinect_camera.cpp:175-195).
+class AzureKinectColorCamera : public ColorCamera {
+ public:
+  AzureKinectColorCamera(const std::string& name, const std::shared_ptr<Batch>& batch,
+                         const AzureKinectCalibration& calibration, float image_scale = 1.05f,
+                         const Transform3fA& world2camera_pose = Transform3fA())
+      : ColorCamera(name, batch, Intrinsics{}, world2camera_pose), calibration_(calibration), image_scale_(image_scale) {}
+  float image_scale() const { return image_scale_; }
+  bool SetUp() {
+    set_up_ = false;
+    if (!AzureKinectIntrinsicsAndDistortionMap(calibration_, image_scale_, &intrinsics_, &distortion_map_)) {
+      std::cerr << "Azure Kinect color camera " << name_ << ": invalid calibration" << std::endl;
+      return false;
+    }
+    if (!ColorCamera::SetUp()) return false;
+    set_up_ = Check(batch_->ctx(),
+                    m3tb_set_camera_undistortion(batch_->ctx(), 0, index_, distortion_map_.data(),
+                                                 size_t(intrinsics_.width) * 4, 4, 0),
+                    "AzureKinectColorCamera::SetUp");
+    return set_up_;
+  }
+  // `buffer`: the BGRA32 image, `pitch` bytes per row (k4a::image::get_stride_bytes)
+  bool UpdateImage(const uint8_t* buffer, size_t pitch) {
+    if (!set_up_) {
+      std::cerr << "Set up azure kinect color camera " << name_ << " first" << std::endl;
+      return false;
+    }
+    return Check(batch_->ctx(), m3tb_upload_color(batch_->ctx(), index_, buffer, pitch),
+                 "AzureKinectColorCamera::UpdateImage");
+  }
+  const std::vector<int16_t>& distortion_map() const { return distortion_map_; }
+
+ private:
+  AzureKinectCalibration calibration_;
+  float image_scale_;
+  std::vector<int16_t> distortion_map_;
+};
+
+// AzureKinectDepthCamera: UpdateImage takes the SDK's u16 depth buffer and leaves the rectified frame, plus
+// short(depth_offset / depth_scale) with saturation, on the device (azure_kinect_camera.cpp:321-345).
+class AzureKinectDepthCamera : public DepthCamera {
+ public:
+  AzureKinectDepthCamera(const std::string& name, const std::shared_ptr<Batch>& batch,
+                         const AzureKinectCalibration& calibration, float image_scale = 1.0f, float depth_offset = 0.0f,
+                         float depth_scale = 0.001f, const Transform3fA& world2camera_pose = Transform3fA())
+      : DepthCamera(name, batch, Intrinsics{}, world2camera_pose, depth_scale),
+        calibration_(calibration),
+        image_scale_(image_scale),
+        depth_offset_(depth_offset) {}
+  float image_scale() const { return image_scale_; }
+  float depth_offset() const { return depth_offset_; }
+  // short depth_value_offset = depth_offset_ / depth_scale_ (C++ truncation); false outside the range of short
+  bool depth_value_offset(int* out) const {
+    const float q = depth_offset_ / depth_scale();
+    if (!(q > -32769.0f && q < 32768.0f)) return false;
+    *out = int(short(q));
+    return true;
+  }
+  bool SetUp() {
+    set_up_ = false;
+    int offset = 0;
+    if (!depth_value_offset(&offset)) {
+      std::cerr << "Azure Kinect depth camera " << name_ << ": depth offset outside the range of short" << std::endl;
+      return false;
+    }
+    if (!AzureKinectIntrinsicsAndDistortionMap(calibration_, image_scale_, &intrinsics_, &distortion_map_)) {
+      std::cerr << "Azure Kinect depth camera " << name_ << ": invalid calibration" << std::endl;
+      return false;
+    }
+    if (!DepthCamera::SetUp()) return false;
+    set_up_ = Check(batch_->ctx(),
+                    m3tb_set_camera_undistortion(batch_->ctx(), 1, index_, distortion_map_.data(),
+                                                 size_t(intrinsics_.width) * 4, 1, depth_offset_ ? offset : 0),
+                    "AzureKinectDepthCamera::SetUp");
+    return set_up_;
+  }
+  // `buffer`: the u16 depth image as bytes, `pitch` bytes per row
+  bool UpdateImage(const uint8_t* buffer, size_t pitch) {
+    if (!set_up_) {
+      std::cerr << "Set up azure kinect depth camera " << name_ << " first" << std::endl;
+      return false;
+    }
+    return Check(batch_->ctx(),
+                 m3tb_upload_depth(batch_->ctx(), index_, reinterpret_cast<const uint16_t*>(buffer), pitch),
+                 "AzureKinectDepthCamera::UpdateImage");
+  }
+  const std::vector<int16_t>& distortion_map() const { return distortion_map_; }
+
+ private:
+  AzureKinectCalibration calibration_;
+  float image_scale_, depth_offset_;
+  std::vector<int16_t> distortion_map_;
+};
+
 // ---- region_model.h / depth_model.h: views in the reference's DataPoint layout ---------------------------------------
 class Model {
  public:

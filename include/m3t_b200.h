@@ -372,6 +372,44 @@ int m3tb_upload_color_batch(m3tb_ctx* ctx, int first_cam, int count, const uint8
 int m3tb_upload_depth_batch(m3tb_ctx* ctx, int first_cam, int count, const uint16_t* depth,
                             size_t frame_stride, size_t pitch);
 
+/* ---- undistortion of raw frames as they are uploaded (AzureKinectColorCamera / AzureKinectDepthCamera::UpdateImage,
+ * azure_kinect_camera.cpp:175-195, 321-345; k_undistort, DESIGN.md §3) --------------------------------------------- */
+/* Host only (no context, no GPU), like m3tb_model_views: the map GetIntrinsicsAndDistortionMap builds
+ * (azure_kinect_camera.cpp:234-265, 387-419): cv::initUndistortRectifyMap(CV_32FC1) with camera matrix `raw`, the
+ * 8-coefficient rational model `distortion` in OpenCV order (k1, k2, p1, p2, k3, k4, k5, k6), R = I and new camera matrix
+ * `rectified`, followed by cv::convertMaps(CV_16SC2, nninterpolation = true). `map_xy` receives height rows of width
+ * (x, y) int16 pairs, `map_pitch` bytes apart. Every entry that lies inside the raw frame equals OpenCV's; entries far
+ * outside it (|value| beyond the int16 range) may saturate differently and select the border value either way.
+ * M3TB_ERR_INVALID for null pointers, raw and rectified sizes that differ or are not positive, non-finite intrinsics,
+ * fu / fv <= 0, ppu / ppv < 0, non-finite coefficients or map_pitch < 4 * width. */
+int m3tb_undistortion_map(const m3tb_intrinsics* raw, const float distortion[8], const m3tb_intrinsics* rectified,
+                          int16_t* map_xy, size_t map_pitch);
+/* Gives colour (camera_kind 0) or depth (1) camera `cam`, which must be set, a map (CV_16SC2 layout as above, the
+ * camera's width x height, host or device memory, copied) that all its later uploads go through: the m3tb_upload_*
+ * entry points then take the RAW frame, `channels` bytes per pixel for colour (4: the SDK's BGRA32, 3: BGR; the fourth
+ * byte is dropped as COLOR_RGBA2RGB does) and u16 for depth (channels 1), pitch >= width * bytes per pixel, and leave
+ * the rectified frame (cv::remap INTER_NEAREST, BORDER_CONSTANT: map entries outside the raw frame give 0) where an
+ * upload always leaves it. Depth only: depth_value_offset (-32768 .. 32767, the reference's short(depth_offset /
+ * depth_scale)) is added to every rectified pixel, border pixels included, with saturation to 0 .. 65535
+ * (image_ += short); 0 adds nothing. A null map removes the undistortion (the camera keeps its last frame).
+ * m3tb_set_*_camera with another width / height drops the undistortion; with the same size it is kept.
+ * Each upload call to cameras with an undistortion adds one kernel launch (a batch: one for all of them); cameras
+ * without one are uploaded exactly as before.
+ *  - device frames are read in place; host frames, pageable or pinned, are copied whole into a staging buffer (grown
+ *    lazily) and rectified from there, so the rectified camera refers to no host memory: m3tb_detach_frames has
+ *    nothing to do for it, and m3tb_prefetch_frames, which needs pinned frames on every camera in use, does not
+ *    prefetch while such a camera is in use;
+ *  - LIFETIME of a pinned raw frame: it must stay unchanged until the stream has passed the upload (m3tb_synchronize,
+ *    or any call that returns data to host memory).
+ * A failed allocation leaves the context as it was. */
+int m3tb_set_camera_undistortion(m3tb_ctx* ctx, int camera_kind, int cam, const int16_t* map_xy, size_t map_pitch,
+                                 int channels, int32_t depth_value_offset);
+/* Camera::image(): copies the frame camera `cam` (kind 0 colour BGR8, 1 depth u16) holds into `dst`, host or device
+ * memory, rows `pitch` bytes apart (waits for the copy only when `dst` is host memory). A camera that still refers to a
+ * pinned frame (ROI ingest) is read from that frame, so the result never depends on which rectangles were fetched.
+ * M3TB_ERR_NOT_SET_UP before the camera's first upload. */
+int m3tb_get_camera_image(m3tb_ctx* ctx, int camera_kind, int cam, void* dst, size_t pitch);
+
 /* ---- bodies: one rigid body = Body + RegionModality and/or DepthModality + root Link + Optimizer.
  * region == NULL / depth == NULL leaves that modality out (model / camera id then ignored).
  * Equivalent of constructing the objects and calling their SetUp() (region_modality.cpp:37-77,
@@ -473,7 +511,8 @@ int m3tb_get_closest_views(m3tb_ctx* ctx, int body, int* region_view, int* depth
  * running: the ROI ingest of those frames runs on a side stream into a second set of device buffers (the ROIs are
  * projected with the poses the last tracking launch started from), and the next tracking / histogram launch waits for
  * it. Results do not change (pixels outside a ROI are read from the pinned frame). It only takes effect when every
- * camera in use got a new pinned frame; otherwise, and for pageable frames, nothing happens and the frames are
+ * camera in use got a new pinned frame; otherwise (a camera with an undistortion holds no pinned frame), and for
+ * pageable frames, nothing happens and the frames are
  * ingested at the next launch as usual. The frames must stay unchanged until that next launch has completed. */
 int m3tb_prefetch_frames(m3tb_ctx* ctx);
 /* Bytes the last frame ingest (pinned-frame ROI fetch) moved host -> device; 0 if frames were copied in full. */
