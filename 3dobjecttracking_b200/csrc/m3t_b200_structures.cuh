@@ -512,6 +512,9 @@ static __device__ __noinline__ bool StructureSolveBlock(const StructureDev& st, 
         if (ob > best || (ob == best && oi < bi)) { best = ob; bi = oi; }
       }
       if (tid == 0) {
+        // Eigen's maxCoeff starts from the first entry of the tail and only takes strictly greater ones: a NaN there
+        // is kept (and a NaN further down never wins). Without this a tail of NaNs left bi = n, out of range.
+        if (!(s.absdiag[k] == s.absdiag[k])) bi = k;
         s.trans[k] = bi;
         const float tmp = s.absdiag[k];
         s.absdiag[k] = s.absdiag[bi];
