@@ -98,6 +98,21 @@ __device__ __forceinline__ void Stamp2(const TrackArgs& args, Shared2& sh) {
     if (args.phase_clock && (cond)) args.phase_clock[size_t(body_id) * kPhaseSlots + (slot)] = clock64(); \
   } while (0)
 
+// dynamic shared memory: [LUT when staged] [line distributions] [cluster tables] [tiles]
+__device__ __forceinline__ unsigned char* DynSmem() {
+  extern __shared__ __align__(128) unsigned char dyn[];
+  return dyn;
+}
+template <bool LUT_SMEM>
+constexpr unsigned kLutBytes = LUT_SMEM ? unsigned(16 * 16 * 16 * sizeof(float2)) : 0u;  // the LUT opens dynamic smem
+// This thread's column of the line distributions. The thread index is read where the address is needed (volatile: not
+// hoisted out of the loop nest, where the address would occupy a register, or a stack slot, all the way through).
+template <bool LUT_SMEM>
+__device__ __forceinline__ float* DistCol() {
+  unsigned tid;
+  asm volatile("mov.u32 %0, %%tid.x;" : "=r"(tid));
+  return reinterpret_cast<float*>(DynSmem() + kLutBytes<LUT_SMEM>) + (tid & (kGroup - 1));
+}
 // ---------------------------------------------------------------------------------------------
 // One correspondence line, streaming form. Walks the 19 segments of the line in pixel order; after segment w >= 7 the
 // distribution entry that has just become computable is finished from the 8-segment window:
@@ -105,14 +120,22 @@ __device__ __forceinline__ void Stamp2(const TrackArgs& args, Shared2& sh) {
 //   line walked back to front: segment index = 18 - walk index (region_modality.cpp:1470-1484), so entry d = 18 - w
 //   uses the segments walked at w, w-1, .. w-7, in that order.
 // Either way the factors are multiplied for k = 0..7 exactly as CalculateDistribution does.
+// The loop over the segments is rolled: unrolled 19 times for each compile-time scale, the walk was almost half of the
+// kernel's code, far more than the SM's instruction caches hold, and the 16 line warps streamed it in again every
+// correspondence iteration. The S samples of a segment stay unrolled. The window is a register shift (slot 7 = the
+// segment just walked, slot 0 = the one 7 steps earlier), so every index into it is a compile-time constant and it
+// stays in registers; the entry's address is formed from the thread index at the store, so the walk carries no pointer
+// to this thread's distribution column.
 // ---------------------------------------------------------------------------------------------
 template <bool LUT_SMEM, int S>
 __device__ __forceinline__ void WalkFast(int scale, int base, float minor_f, float step, int stride_major, int stride_minor,
                                          const uint16_t* tile_px, const float2* __restrict__ lut_g, const float2* lut_s,
-                                         const float* __restrict__ lf, const float* __restrict__ lb, bool rev,
-                                         float* dist_col) {
+                                         const float* __restrict__ lf, const float* __restrict__ lb, bool rev) {
   float wf[8], wb[8];
 #pragma unroll
+  for (int k = 0; k < 8; ++k) wf[k] = wb[k] = 0.0f;
+  // two segments per trip: with one, the loop's bookkeeping made the 512-thread kernel slower than the unrolled walk
+#pragma unroll 2
   for (int w = 0; w < kLineSegments; ++w) {
     float pf = 1.0f, pb = 1.0f;
     if (S > 0) {
@@ -150,17 +173,22 @@ __device__ __forceinline__ void WalkFast(int scale, int base, float minor_f, flo
         pb = 0.5f;
       }
     }
-    wf[w & 7] = pf;
-    wb[w & 7] = pb;
+#pragma unroll
+    for (int k = 0; k < 7; ++k) {
+      wf[k] = wf[k + 1];
+      wb[k] = wb[k + 1];
+    }
+    wf[7] = pf;
+    wb[7] = pb;
     if (w >= 7) {
       float val = 1.0f;
 #pragma unroll
       for (int k = 0; k < kFunctionLength; ++k) {
-        const float f = rev ? wf[(w - k) & 7] : wf[(w + 1 + k) & 7];
-        const float b = rev ? wb[(w - k) & 7] : wb[(w + 1 + k) & 7];
+        const float f = rev ? wf[7 - k] : wf[k];
+        const float b = rev ? wb[7 - k] : wb[k];
         val *= f * lf[k] + b * lb[k];
       }
-      dist_col[(rev ? kLineSegments - 1 - w : w - 7) * kGroup] = val;
+      DistCol<LUT_SMEM>()[(rev ? kLineSegments - 1 - w : w - 7) * kGroup] = val;
     }
   }
 }
@@ -229,8 +257,7 @@ template <bool LUT_SMEM>
 __device__ __forceinline__ void RegionLine2(const RegionIter& it, const RegionParamsDev& rp, const float4 p0, const float4 p1,
                                             const FrameView& frame, const Tile& tile, const uint16_t* tile_px,
                                             const BinImage& bins, const float2* __restrict__ lut_g, const float2* lut_s,
-                                            const float* __restrict__ lf, const float* __restrict__ lb,
-                                            float* dist_col, LineRegs& L) {
+                                            const float* __restrict__ lf, const float* __restrict__ lb, LineRegs& L) {
   L.valid = false;
   // CalculateBasicLineData (:1231-1250)
   float x, y, z;
@@ -280,20 +307,21 @@ __device__ __forceinline__ void RegionLine2(const RegionIter& it, const RegionPa
       const int stride_minor = horizontal ? tile.pitch : 1;
       const int base = horizontal ? (major - tile.x0) - tile.y0 * tile.pitch : (major - tile.y0) * tile.pitch - tile.x0;
       switch (it.scale) {
-        case 1: WalkFast<LUT_SMEM, 1>(1, base, minor_f, step, stride_major, stride_minor, tile_px, lut_g, lut_s, lf, lb, rev, dist_col); break;
-        case 2: WalkFast<LUT_SMEM, 2>(2, base, minor_f, step, stride_major, stride_minor, tile_px, lut_g, lut_s, lf, lb, rev, dist_col); break;
-        case 4: WalkFast<LUT_SMEM, 4>(4, base, minor_f, step, stride_major, stride_minor, tile_px, lut_g, lut_s, lf, lb, rev, dist_col); break;
-        case 6: WalkFast<LUT_SMEM, 6>(6, base, minor_f, step, stride_major, stride_minor, tile_px, lut_g, lut_s, lf, lb, rev, dist_col); break;
-        default: WalkFast<LUT_SMEM, 0>(it.scale, base, minor_f, step, stride_major, stride_minor, tile_px, lut_g, lut_s, lf, lb, rev, dist_col); break;
+        case 1: WalkFast<LUT_SMEM, 1>(1, base, minor_f, step, stride_major, stride_minor, tile_px, lut_g, lut_s, lf, lb, rev); break;
+        case 2: WalkFast<LUT_SMEM, 2>(2, base, minor_f, step, stride_major, stride_minor, tile_px, lut_g, lut_s, lf, lb, rev); break;
+        case 4: WalkFast<LUT_SMEM, 4>(4, base, minor_f, step, stride_major, stride_minor, tile_px, lut_g, lut_s, lf, lb, rev); break;
+        case 6: WalkFast<LUT_SMEM, 6>(6, base, minor_f, step, stride_major, stride_minor, tile_px, lut_g, lut_s, lf, lb, rev); break;
+        default: WalkFast<LUT_SMEM, 0>(it.scale, base, minor_f, step, stride_major, stride_minor, tile_px, lut_g, lut_s, lf, lb, rev); break;
       }
     } else {
       WalkSlow<LUT_SMEM>(it.scale, rp.bitshift, rp.n_bins, horizontal, major, minor_f, step, frame, tile, tile_px, bins,
-                         lut_g, lut_s, lf, lb, rev, dist_col);
+                         lut_g, lut_s, lf, lb, rev, DistCol<LUT_SMEM>());
     }
   }
   L.ncts = fabsf(n_major) / it.fscale;
   L.dr = (roundf(c_major - it.ll_m1_half) + it.ll_m1_half - c_major) / n_major;
   // CalculateDistribution, normalisation (:1630-1636) and CalculateDistributionMoments (:1639-1658)
+  float* dist_col = DistCol<LUT_SMEM>();
   float dist[kDistributionLength];
   float area = 0.0f;
 #pragma unroll
@@ -556,20 +584,6 @@ __device__ __forceinline__ bool SolveAndUpdateSerial(Shared2& sh, bool has_color
 // ---------------------------------------------------------------------------------------------
 // The loop nest reaches what the prologue settled (per-body copies, tiles, lookups) through `sh`, the kernel parameters and
 // threadIdx where it uses it, so that no pointer or flag is carried in registers through the loop nest.
-__device__ __forceinline__ unsigned char* DynSmem() {
-  extern __shared__ __align__(128) unsigned char dyn[];
-  return dyn;
-}
-template <bool LUT_SMEM>
-constexpr unsigned kLutBytes = LUT_SMEM ? unsigned(16 * 16 * 16 * sizeof(float2)) : 0u;  // the LUT opens dynamic smem
-// This thread's column of the line distributions. The thread index is read where the address is needed (volatile: not
-// hoisted out of the loop nest, where the address would occupy a register, or a stack slot, all the way through).
-template <bool LUT_SMEM>
-__device__ __forceinline__ float* DistCol() {
-  unsigned tid;
-  asm volatile("mov.u32 %0, %%tid.x;" : "=r"(tid));
-  return reinterpret_cast<float*>(DynSmem() + kLutBytes<LUT_SMEM>) + (tid & (kGroup - 1));
-}
 __device__ __forceinline__ bool DoPhase(const Shared2& sh, const TrackArgs& args, bool region, unsigned phase) {
   return (region ? sh.body.has_region : sh.body.has_depth) && (args.phases & phase);
 }
@@ -625,7 +639,7 @@ __device__ __forceinline__ void LineCorrespondence(const TrackArgs& args, Shared
     const float2* lut_s = reinterpret_cast<const float2*>(DynSmem());
     // function lookups (identical for every body of the launch, checked by the host): kernel-parameter constants
     RegionLine2<LUT_SMEM>(rit, body.rp, p0, p1, sh.cframe, sh.ctile, tile_px, sh.bins, lut_g, lut_s, args.lookup_f,
-                          args.lookup_b, DistCol<LUT_SMEM>(), L);
+                          args.lookup_b, L);
   }
   Stamp2<T>(args, sh);  // region lines
 }
