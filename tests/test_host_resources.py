@@ -140,6 +140,11 @@ class Scene:
             ("prefetch_frames", pinned_frames, lambda c: c.prefetch_frames()),
             ("upload_pageable_outside_pool", camera2, lambda c: c.upload_color(2, self.small_frame)),
             ("upload_pinned_outside_pool", camera2, lambda c: c.upload_color(2, self.pinned[0].numpy())),
+            ("set_viewer_new", None, lambda c: c.set_viewer(0, "color", 0, [0, 1])),
+            ("update_viewers_tables", lambda c: c.set_viewer(0, "color", 0, [0, 1]), lambda c: c.update_viewers()),
+            ("set_full_renderer_new", None, lambda c: c.set_full_renderer(0, "color", 0, [0, 1])),
+            ("render_full_tables", lambda c: c.set_full_renderer(0, "color", 0, [0, 1]), lambda c: c.render_full()),
+            ("generate_region_model", None, lambda c: c.generate_region_model(1, 0, (), self.gen)),
         ]
 
     def readbacks(self, ctx):
