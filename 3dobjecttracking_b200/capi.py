@@ -80,6 +80,26 @@ class Constraint(C.Structure):
                 ("standard_deviation_rotation", C.c_float), ("standard_deviation_translation", C.c_float)]
 
 
+def texture_params_default():
+    p = TextureParams()
+    lib().m3tb_texture_params_default(C.byref(p))
+    return p
+
+
+class TextureParams(C.Structure):
+    """m3tb_texture_params (m3t::TextureModality, texture_modality.h:400-436)."""
+    _fields_ = [("descriptor_type", C.c_int32), ("focused_image_size", C.c_int32),
+                ("descriptor_distance_threshold", C.c_float), ("tukey_norm_constant", C.c_float),
+                ("n_standard_deviations", C.c_int32), ("standard_deviations", C.c_float * 8),
+                ("max_keyframe_rotation_difference", C.c_float), ("max_keyframe_age", C.c_int32),
+                ("n_keyframes", C.c_int32), ("measure_occlusions", C.c_int32), ("measured_occlusion_radius", C.c_float),
+                ("measured_occlusion_threshold", C.c_float), ("model_occlusions", C.c_int32),
+                ("modeled_occlusion_radius", C.c_float), ("modeled_occlusion_threshold", C.c_float)]
+
+
+DESCRIPTOR_ORB = 4
+TEXTURE_POINT_DTYPE = np.dtype([("center_f_body", "<f4", 3), ("correspondence_center", "<f4", 2), ("center", "<f4", 2)])
+
 REGION_LINE_DTYPE = np.dtype([("model_index", "<i4"), ("valid", "<i4"), ("center_f_body", "<f4", 3),
                               ("center_u", "<f4"), ("center_v", "<f4"), ("normal_u", "<f4"), ("normal_v", "<f4"),
                               ("delta_r", "<f4"), ("normal_component_to_scale", "<f4"), ("distribution", "<f4", 12),
@@ -108,6 +128,9 @@ SYMBOLS = [
     "m3tb_generate_region_model", "m3tb_get_region_model", "m3tb_debug_region_model_view", "m3tb_set_viewer",
     "m3tb_update_viewers", "m3tb_get_viewer_image", "m3tb_set_full_renderer", "m3tb_render_full",
     "m3tb_get_full_rendering", "m3tb_undistortion_map", "m3tb_set_camera_undistortion", "m3tb_get_camera_image",
+    "m3tb_texture_params_default", "m3tb_set_texture_modality", "m3tb_get_texture_focus", "m3tb_upload_texture_features",
+    "m3tb_texture_correspondences", "m3tb_texture_gradient_hessian", "m3tb_get_texture_points",
+    "m3tb_get_texture_keyframes",
 ]
 
 KERNEL_NAMES = {0: None, 1: "k_track", 2: "k_track2", 3: "k_track_cluster"}
@@ -225,6 +248,14 @@ def lib():
     L.m3tb_get_viewer_image.argtypes = [vp, ci, vp, C.c_size_t, vp, C.c_size_t]
     L.m3tb_set_full_renderer.argtypes = [vp, ci, ci, ci, C.c_float, C.c_float, ci, ip, ci]
     L.m3tb_render_full.argtypes = [vp]
+    L.m3tb_texture_params_default.argtypes = [C.POINTER(TextureParams)]
+    L.m3tb_set_texture_modality.argtypes = [vp, ci, C.POINTER(TextureParams), ci]
+    L.m3tb_get_texture_focus.argtypes = [vp, ci, ci, ip, fp, ip]
+    L.m3tb_upload_texture_features.argtypes = [vp, ci, fp, vp, ci, ci, ci, C.c_float]
+    L.m3tb_texture_correspondences.argtypes = [vp, ci, ci]
+    L.m3tb_texture_gradient_hessian.argtypes = [vp, ci, ci, ci, fp, fp]
+    L.m3tb_get_texture_points.argtypes = [vp, ci, vp, ci, C.POINTER(ci)]
+    L.m3tb_get_texture_keyframes.argtypes = [vp, ci, C.POINTER(ci), ip, fp, vp, ci, C.POINTER(ci), fp]
     L.m3tb_get_full_rendering.argtypes = [vp, ci, vp, C.c_size_t, vp, C.c_size_t, vp, C.c_size_t, fp, fp]
     L.m3tb_undistortion_map.argtypes = [C.POINTER(Intrinsics), fp, C.POINTER(Intrinsics), vp, C.c_size_t]
     L.m3tb_set_camera_undistortion.argtypes = [vp, ci, ci, vp, C.c_size_t, ci, C.c_int32]
@@ -492,8 +523,9 @@ class Context:
         self._renderer_refs[renderer] = (image_size, r.size)
 
     def attach_renderer(self, body, key, renderer):
-        """key: "region_depth" | "region_silhouette" | "depth_depth" | "depth_silhouette"; renderer -1 detaches."""
-        modality = 0 if key.startswith("region") else 1
+        """key: "region_depth" | "region_silhouette" | "depth_depth" | "depth_silhouette" | "texture_depth" |
+        "texture_silhouette"; renderer -1 detaches."""
+        modality = 0 if key.startswith("region") else 2 if key.startswith("texture") else 1
         kind = 0 if key.endswith("depth") else 1
         self._ck(self.L.m3tb_attach_renderer(self.h, body, modality, kind, renderer))
 
@@ -753,6 +785,7 @@ class Context:
         self._ck(self.L.m3tb_set_structure(self.h, index, links, nl, cons, nc, C.byref(op)))
 
     def set_gradient_hessian(self, modality, g, H):
+        """modality: 0 region, 1 depth, 2 texture."""
         g = np.ascontiguousarray(g, np.float32)
         H = np.ascontiguousarray(H, np.float32)
         self._ck(self.L.m3tb_set_gradient_hessian(self.h, modality, _p(g), _p(H)))
@@ -786,6 +819,59 @@ class Context:
         n = C.c_int(0)
         self._ck(self.L.m3tb_get_region_lines(self.h, body, out.ctypes.data_as(C.c_void_p), capacity, C.byref(n)))
         return out[:min(n.value, capacity)]
+
+    # ---- texture modality (TextureModality) --------------------------------------------------------------------------
+    def set_texture_modality(self, body, params, color_camera=0):
+        """params: TextureParams (None removes the modality)."""
+        self._ck(self.L.m3tb_set_texture_modality(self.h, body, C.byref(params) if params is not None else None,
+                                                  color_camera))
+
+    def get_texture_focus(self, first=0, count=None):
+        """(roi [count, 4] int32 x, y, width, height; scale [count] float32; valid [count] bool)."""
+        count = self.n_bodies - first if count is None else count
+        roi = np.zeros((max(count, 1), 4), np.int32)
+        scale = np.zeros(max(count, 1), np.float32)
+        valid = np.zeros(max(count, 1), np.int32)
+        ip = C.POINTER(C.c_int)
+        self._ck(self.L.m3tb_get_texture_focus(self.h, first, count, roi.ctypes.data_as(ip), _p(scale),
+                                               valid.ctypes.data_as(ip)))
+        return roi[:count], scale[:count], valid[:count].astype(bool)
+
+    def upload_texture_features(self, body, keypoints_xy, descriptors, roi_x, roi_y, scale):
+        """keypoints_xy [n, 2] float32 in crop coordinates, descriptors [n, 32] uint8."""
+        xy = np.ascontiguousarray(np.asarray(keypoints_xy, np.float32).reshape(-1, 2))
+        d = np.ascontiguousarray(np.asarray(descriptors, np.uint8).reshape(-1, 32))
+        self._ck(self.L.m3tb_upload_texture_features(self.h, body, _p(xy), d.ctypes.data_as(C.c_void_p), xy.shape[0],
+                                                     int(roi_x), int(roi_y), float(scale)))
+
+    def texture_correspondences(self, iteration, corr_iteration):
+        self._ck(self.L.m3tb_texture_correspondences(self.h, iteration, corr_iteration))
+
+    def texture_gradient_hessian(self, iteration, corr_iteration, opt_iteration):
+        g = np.zeros((self.n_bodies, 6), np.float32)
+        H = np.zeros((self.n_bodies, 6, 6), np.float32)
+        self._ck(self.L.m3tb_texture_gradient_hessian(self.h, iteration, corr_iteration, opt_iteration, _p(g), _p(H)))
+        return g, H
+
+    def get_texture_points(self, body, capacity=4096):
+        out = np.zeros(capacity, TEXTURE_POINT_DTYPE)
+        n = C.c_int(0)
+        self._ck(self.L.m3tb_get_texture_points(self.h, body, out.ctypes.data_as(C.c_void_p), capacity, C.byref(n)))
+        return out[:min(n.value, capacity)]
+
+    def get_texture_keyframes(self, body, capacity=4096):
+        """dict(sizes [n_keyframes], points [total, 3] float32, descriptors [total, 32] uint8, age, orientation [3])."""
+        nk, age = C.c_int(0), C.c_int(0)
+        sizes = np.zeros(8, np.int32)
+        pts = np.zeros((capacity, 3), np.float32)
+        desc = np.zeros((capacity, 32), np.uint8)
+        o = np.zeros(3, np.float32)
+        self._ck(self.L.m3tb_get_texture_keyframes(self.h, body, C.byref(nk), sizes.ctypes.data_as(C.POINTER(C.c_int)),
+                                                   _p(pts), desc.ctypes.data_as(C.c_void_p), capacity, C.byref(age),
+                                                   _p(o)))
+        sizes = sizes[:nk.value]
+        total = min(int(sizes.sum()), capacity)
+        return dict(sizes=sizes, points=pts[:total], descriptors=desc[:total], age=age.value, orientation=o)
 
     def get_depth_points(self, body, capacity):
         out = np.zeros(capacity, DEPTH_POINT_DTYPE)

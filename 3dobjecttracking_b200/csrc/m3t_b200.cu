@@ -24,6 +24,7 @@
 #include "m3t_b200_views.cuh"
 #include "m3t_b200_view.cuh"
 #include "m3t_b200_undistort.cuh"
+#include "m3t_b200_texture.cuh"
 
 #include "m3t_b200_track_variants.h"
 #include "m3t_b200_track2.cuh"
@@ -258,6 +259,16 @@ struct m3tb_ctx {
   };
   std::vector<UndistortHost> undistort[2];  // [colour | depth][max_cameras]
   DeviceBuffer<uint8_t> undistort_staging;  // the raw host frames of one upload call, grown lazily
+
+  // texture modality (m3tb_set_texture_modality, k_texture_keyframe / k_texture_match): tables for max_bodies, made by
+  // the first m3tb_set_texture_modality (TextureArgs for the layouts)
+  int n_texture = 0;                    // bodies with a texture modality
+  std::vector<int> tex_feat_gen;        // per body: colour-frame generation its features belong to, -1: none
+  DeviceBuffer<float2> d_tex_xy;
+  DeviceBuffer<uint32_t> d_tex_desc, d_tex_kf_desc;
+  DeviceBuffer<int> d_tex_nfeat, d_tex_kf_n, d_tex_counts;
+  DeviceBuffer<float> d_tex_kf_points, d_tex_points, d_tex_pose, d_gh_texture;
+  DeviceBuffer<TexKeyframeState> d_tex_kf_state;
 };
 
 namespace {
@@ -499,6 +510,8 @@ int LaunchIngestIfPending(m3tb_ctx* ctx) {
 
 int SyncStructures(m3tb_ctx* ctx);
 int LaunchRender(m3tb_ctx* ctx, int which);
+int LaunchTexture(m3tb_ctx* ctx, bool keyframe, int mode);
+int ValidateTexture(m3tb_ctx* ctx);
 
 // cuTensorMapEncodeTiled through the runtime (libcuda is not linked: the library must load on machines without a driver)
 PFN_cuTensorMapEncodeTiled_v12000 TensorMapEncoder() {
@@ -633,6 +646,7 @@ int PrepareTensorTiles(m3tb_ctx* ctx, TrackArgs& a, bool& usable) {
 int LaunchTrack(m3tb_ctx* ctx, int iteration, int corr_begin, int corr_end, int n_update, int opt_base,
                 unsigned phases, int cluster = 0) {
   int rc = ValidateBodies(ctx);
+  if (!rc && (phases & PH_TEXTURE_GH)) rc = ValidateTexture(ctx);
   if (rc) return rc;
   rc = EnsureState(ctx);
   if (rc) return rc;
@@ -669,6 +683,10 @@ int LaunchTrack(m3tb_ctx* ctx, int iteration, int corr_begin, int corr_end, int 
   a.gh_region = ctx->d_gh_region;
   a.gh_depth = ctx->d_gh_depth;
   a.gh_link = ctx->d_gh_link;
+  a.tex_points = ctx->d_tex_points;
+  a.tex_counts = ctx->d_tex_counts;
+  a.tex_pose = ctx->d_tex_pose;
+  a.gh_texture = ctx->d_gh_texture;
   a.iteration = iteration;
   a.corr_begin = corr_begin;
   a.corr_end = corr_end;
@@ -1172,7 +1190,11 @@ int SyncRenderTables(m3tb_ctx* ctx) {
     for (int r = 0; r < nr; ++r) {
       bool use = pass == kRenderAll;
       for (const auto& x : att)
-        use = use || (x.renderer == r && (pass == kRenderAttached || x.slot == RS_REGION_DEPTH || x.slot == RS_REGION_SILHOUETTE));
+        // the texture modality has no correspondence renderers (TextureModality::correspondence_renderer_ptrs is empty):
+        // its renderers draw only for StartModality and CalculateResults
+        use = use || (x.renderer == r && ((pass == kRenderAttached && x.slot < RS_TEXTURE_SILHOUETTE) ||
+                                          x.slot == RS_REGION_DEPTH || x.slot == RS_REGION_SILHOUETTE ||
+                                          x.slot >= RS_TEXTURE_SILHOUETTE));
       if (!use) continue;
       lists.push_back(r);
       ctx->render_list[pass].push_back(r);
@@ -2160,8 +2182,11 @@ int m3tb_create(int device, int max_bodies, int max_cameras, int max_models, m3t
   std::memset(ctx->h_geometry.data(), 0, sizeof(GeometryDev) * max_bodies);
   ctx->geometry_alloc.resize(max_bodies);
   ctx->rendering_images.resize(max_bodies);
-  ctx->attached.assign(max_bodies, std::array<int, RS_COUNT>{-1, -1, -1, -1});
-  ctx->attach_uploaded.assign(max_bodies, std::array<char, RS_COUNT>{0, 0, 0, 0});
+  std::array<int, RS_COUNT> detached;
+  detached.fill(-1);
+  ctx->attached.assign(max_bodies, detached);
+  ctx->attach_uploaded.assign(max_bodies, std::array<char, RS_COUNT>{});
+  ctx->tex_feat_gen.assign(max_bodies, -1);
   if (const char* e = std::getenv("M3TB_NO_TILES")) ctx->use_tiles = !(e[0] == '1');
   if (const char* e = std::getenv("M3TB_NO_ROI_INGEST")) ctx->roi_ingest = !(e[0] == '1');
   if (const char* e = std::getenv("M3TB_CLUSTER")) ctx->use_clusters = e[0] == '1';
@@ -2274,6 +2299,10 @@ int m3tb_set_body(m3tb_ctx* ctx, int body, const m3tb_region_params* region, con
   std::memset(&B, 0, sizeof(B));
   B.first_iteration = ctx->h_bodies[body].first_iteration;
   std::memcpy(B.rend, ctx->h_bodies[body].rend, sizeof(B.rend));  // uploaded renderer images stay with the body
+  // so does a texture modality (m3tb_set_texture_modality): its keyframes, renderers and parameters are its own
+  B.has_texture = ctx->h_bodies[body].has_texture;
+  B.texture_camera = ctx->h_bodies[body].texture_camera;
+  B.tp = ctx->h_bodies[body].tp;
   m3tb_optimizer_params op;
   m3tb_optimizer_params_default(&op);
   if (optimizer) op = *optimizer;
@@ -2478,13 +2507,17 @@ int m3tb_get_histograms(m3tb_ctx* ctx, int body, float* histogram_f, float* hist
 int m3tb_tracking_step(m3tb_ctx* ctx, int iteration, int n_corr_iterations, int n_update_iterations) {
   CHECK_CTX();
   if (n_corr_iterations < 0 || n_update_iterations < 0) return Fail(ctx, M3TB_ERR_INVALID, "negative iteration count");
-  if (HasStructures(ctx)) return StructureStep(ctx, iteration, 0, n_corr_iterations, n_update_iterations);
+  if (HasStructures(ctx)) {
+    if (ctx->n_texture > 0) return Fail(ctx, M3TB_ERR_UNSUPPORTED, "texture modalities in kinematic structures");
+    return StructureStep(ctx, iteration, 0, n_corr_iterations, n_update_iterations);
+  }
   const unsigned phases = PH_REGION_CORR | PH_DEPTH_CORR | PH_REGION_GH | PH_DEPTH_GH | PH_SOLVE | PH_STORE_REGION |
-                          PH_STORE_DEPTH;
+                          PH_STORE_DEPTH | (ctx->n_texture > 0 ? unsigned(PH_TEXTURE_GH) : 0u);
   if (ctx->n_attached == 0) return LaunchTrack(ctx, iteration, 0, n_corr_iterations, n_update_iterations, 0, phases);
   // device renderers: Tracker::CalculateCorrespondences renders before every correspondence iteration (tracker.cpp:447-456)
   for (int corr = 0; corr < n_corr_iterations; ++corr) {
     int rc = LaunchRender(ctx, kRenderAttached);
+    if (!rc && corr == 0) rc = LaunchTexture(ctx, false, 1);  // texture matches of this frame (no-op without texture)
     if (!rc) rc = LaunchTrack(ctx, iteration, corr, corr + 1, n_update_iterations, 0, phases);
     if (rc) return rc;
   }
@@ -2494,14 +2527,18 @@ int m3tb_tracking_step(m3tb_ctx* ctx, int iteration, int n_corr_iterations, int 
 int m3tb_corr_iteration(m3tb_ctx* ctx, int iteration, int corr_iteration, int n_update_iterations) {
   CHECK_CTX();
   if (corr_iteration < 0 || n_update_iterations < 0) return Fail(ctx, M3TB_ERR_INVALID, "negative iteration count");
-  if (HasStructures(ctx)) return StructureStep(ctx, iteration, corr_iteration, corr_iteration + 1, n_update_iterations);
+  if (HasStructures(ctx)) {
+    if (ctx->n_texture > 0) return Fail(ctx, M3TB_ERR_UNSUPPORTED, "texture modalities in kinematic structures");
+    return StructureStep(ctx, iteration, corr_iteration, corr_iteration + 1, n_update_iterations);
+  }
   if (ctx->n_attached > 0) {
     int rc = LaunchRender(ctx, kRenderAttached);
+    if (!rc && corr_iteration == 0) rc = LaunchTexture(ctx, false, 1);
     if (rc) return rc;
   }
   return LaunchTrack(ctx, iteration, corr_iteration, corr_iteration + 1, n_update_iterations, 0,
                      PH_REGION_CORR | PH_DEPTH_CORR | PH_REGION_GH | PH_DEPTH_GH | PH_SOLVE | PH_STORE_REGION |
-                         PH_STORE_DEPTH);
+                         PH_STORE_DEPTH | (ctx->n_texture > 0 ? unsigned(PH_TEXTURE_GH) : 0u));
 }
 
 int m3tb_start_modalities(m3tb_ctx* ctx, int iteration) {
@@ -2512,7 +2549,9 @@ int m3tb_start_modalities(m3tb_ctx* ctx, int iteration) {
     int rc = LaunchRender(ctx, kRenderRegion);
     if (rc) return rc;
   }
-  return LaunchHistogram(ctx, 0, iteration);
+  int rc = LaunchHistogram(ctx, 0, iteration);
+  if (!rc) rc = LaunchTexture(ctx, true, 0);  // TextureModality::StartModality (no-op without texture)
+  return rc;
 }
 
 int m3tb_calculate_results(m3tb_ctx* ctx, int iteration) {
@@ -2521,7 +2560,9 @@ int m3tb_calculate_results(m3tb_ctx* ctx, int iteration) {
     int rc = LaunchRender(ctx, kRenderRegion);
     if (rc) return rc;
   }
-  return LaunchHistogram(ctx, 1, iteration);
+  int rc = LaunchHistogram(ctx, 1, iteration);
+  if (!rc) rc = LaunchTexture(ctx, true, 1);  // TextureModality::CalculateResults (no-op without texture)
+  return rc;
 }
 
 int m3tb_region_correspondences(m3tb_ctx* ctx, int iteration, int corr_iteration) {
@@ -2657,15 +2698,16 @@ int m3tb_set_structure(m3tb_ctx* ctx, int structure, const m3tb_link* links, int
 
 int m3tb_set_gradient_hessian(m3tb_ctx* ctx, int modality, const float* gradients, const float* hessians) {
   CHECK_CTX();
-  if ((modality != 0 && modality != 1) || !gradients || !hessians || ctx->n_bodies == 0)
+  if ((modality != 0 && modality != 1 && modality != 2) || !gradients || !hessians || ctx->n_bodies == 0)
     return Fail(ctx, M3TB_ERR_INVALID, "bad gradient / hessian arguments");
+  if (modality == 2 && !ctx->d_gh_texture) return Fail(ctx, M3TB_ERR_INVALID, "no texture modality set");
   std::vector<float> h(size_t(27) * ctx->n_bodies);
   for (int b = 0; b < ctx->n_bodies; ++b) {
     for (int i = 0; i < 6; ++i) h[27 * b + i] = gradients[6 * b + i];
     for (int i = 0; i < 6; ++i)
       for (int j = 0; j <= i; ++j) h[27 * b + 6 + Tri(i, j)] = hessians[36 * b + 6 * i + j];
   }
-  CU(cudaMemcpyAsync(modality == 0 ? ctx->d_gh_region : ctx->d_gh_depth, h.data(), h.size() * sizeof(float),
+  CU(cudaMemcpyAsync(modality == 0 ? ctx->d_gh_region : modality == 1 ? ctx->d_gh_depth : ctx->d_gh_texture, h.data(), h.size() * sizeof(float),
                      cudaMemcpyHostToDevice, ctx->stream));
   CU(cudaStreamSynchronize(ctx->stream));
   return M3TB_OK;
@@ -3062,11 +3104,55 @@ int m3tb_set_focused_renderer(m3tb_ctx* ctx, int renderer, int camera_kind, int 
   return M3TB_OK;
 }
 
+// TextureModality's silhouette renderer (kind 1, IDType::BODY; it feeds the silhouette and the depth slot) and depth
+// renderer (kind 0, model_occlusions), texture_modality.cpp:517-524
+static int AttachTextureRenderer(m3tb_ctx* ctx, int body, int kind, int renderer) {
+  BodyDev& B = ctx->h_bodies[body];
+  if (!B.has_texture) return Fail(ctx, M3TB_ERR_INVALID, "body has no such modality");
+  const int slots[2] = {kind == 1 ? RS_TEXTURE_SILHOUETTE : RS_TEXTURE_DEPTH, kind == 1 ? RS_TEXTURE_SILHOUETTE_DEPTH : -1};
+  if (renderer != -1) {
+    if (renderer < 0 || renderer >= int(ctx->renderers.size())) return Fail(ctx, M3TB_ERR_INVALID, "renderer not set");
+    const auto& h = ctx->renderers[renderer];
+    if (h.dev.camera_kind != 0 || h.dev.camera != B.texture_camera)
+      return Fail(ctx, M3TB_ERR_INVALID, "the renderer does not render the modality's camera");
+    if (std::find(h.referenced.begin(), h.referenced.end(), body) == h.referenced.end())
+      return Fail(ctx, M3TB_ERR_INVALID, "the renderer does not reference the body");
+    if (kind == 1 && h.dev.id_type != RID_BODY)
+      return Fail(ctx, M3TB_ERR_INVALID, "the texture modality needs a silhouette renderer of id_type BODY");
+  }
+  for (int slot : slots) {
+    if (slot < 0) continue;
+    int& cur = ctx->attached[body][slot];
+    RenderingDev& d = B.rend[slot];
+    if (renderer == -1) {
+      if (cur < 0) continue;
+      std::memset(&d, 0, sizeof(d));
+      cur = -1;
+      ctx->n_attached--;
+    } else {
+      const RendererDev& R = ctx->renderers[renderer].dev;
+      const bool sil = slot == RS_TEXTURE_SILHOUETTE;
+      std::memset(&d, 0, sizeof(d));  // visible = 0 until the first render
+      d.image = sil ? R.silhouette : reinterpret_cast<const uint8_t*>(R.depth);
+      d.image_size = R.image_size;
+      d.pitch = sil ? R.silhouette_pitch : R.depth_pitch;
+      if (cur < 0) ctx->n_attached++;
+      cur = renderer;
+      ctx->attach_uploaded[body][slot] = 0;
+    }
+    ctx->bodies_dirty = true;
+    ctx->render_dirty = true;
+  }
+  return M3TB_OK;
+}
+
 int m3tb_attach_renderer(m3tb_ctx* ctx, int body, int modality, int kind, int renderer) {
   CHECK_CTX();
   if (body < 0 || body >= ctx->n_bodies || !ctx->h_bodies[body].set) return Fail(ctx, M3TB_ERR_INVALID, "body not set");
-  if (modality != 0 && modality != 1) return Fail(ctx, M3TB_ERR_INVALID, "modality must be 0 (region) or 1 (depth)");
+  if (modality != 0 && modality != 1 && modality != 2)
+    return Fail(ctx, M3TB_ERR_INVALID, "modality must be 0 (region), 1 (depth) or 2 (texture)");
   if (kind != 0 && kind != 1) return Fail(ctx, M3TB_ERR_INVALID, "kind must be 0 (depth) or 1 (silhouette)");
+  if (modality == 2) return AttachTextureRenderer(ctx, body, kind, renderer);
   BodyDev& B = ctx->h_bodies[body];
   if (!(modality == 0 ? B.has_region : B.has_depth)) return Fail(ctx, M3TB_ERR_INVALID, "body has no such modality");
   const int slot = modality == 0 ? (kind == 0 ? RS_REGION_DEPTH : RS_REGION_SILHOUETTE)
@@ -3810,6 +3896,376 @@ int m3tb_get_camera_image(m3tb_ctx* ctx, int camera_kind, int cam, void* dst, si
   const size_t src_pitch = c.host_src ? c.host_pitch : c.pitch;
   CU(cudaMemcpy2DAsync(dst, pitch, src, src_pitch, row, c.height, cudaMemcpyDefault, ctx->stream));
   if (!IsDevicePointer(dst)) CU(cudaStreamSynchronize(ctx->stream));
+  return M3TB_OK;
+}
+
+// ---- texture modality (TextureModality, texture_modality.cpp) --------------------------------------------------------
+void m3tb_texture_params_default(m3tb_texture_params* p) {
+  if (!p) return;
+  std::memset(p, 0, sizeof(*p));
+  p->descriptor_type = M3TB_DESCRIPTOR_ORB;
+  p->focused_image_size = 200;
+  p->descriptor_distance_threshold = 0.7f;
+  p->tukey_norm_constant = 20.0f;
+  p->n_standard_deviations = 2;
+  p->standard_deviations[0] = 15.0f;
+  p->standard_deviations[1] = 5.0f;
+  p->max_keyframe_rotation_difference = 10.0f * 3.14159265358979323846f / 180.0f;  // kPi, common.h
+  p->max_keyframe_age = 100;
+  p->n_keyframes = 1;
+  p->measured_occlusion_radius = 0.01f;
+  p->measured_occlusion_threshold = 0.03f;
+  p->modeled_occlusion_radius = 0.01f;
+  p->modeled_occlusion_threshold = 0.03f;
+}
+
+}  // extern "C"
+
+namespace {
+
+// The texture tables for max_bodies, all or nothing (first m3tb_set_texture_modality)
+int EnsureTextureTables(m3tb_ctx* ctx) {
+  if (ctx->d_tex_xy) return M3TB_OK;
+  const size_t nb = size_t(ctx->max_bodies);
+  DeviceBuffer<float2> xy;
+  DeviceBuffer<uint32_t> desc, kf_desc;
+  DeviceBuffer<int> nfeat, kf_n, counts;
+  DeviceBuffer<float> kf_points, points, pose, gh;
+  DeviceBuffer<TexKeyframeState> state;
+  CU(xy.create(nb * kTexMaxFeatures));
+  CU(desc.create(nb * kTexMaxFeatures * kTexDescWords));
+  CU(kf_desc.create(nb * kTexMaxKeyframes * kTexMaxFeatures * kTexDescWords));
+  CU(nfeat.create(nb));
+  CU(kf_n.create(nb * kTexMaxKeyframes));
+  CU(counts.create(nb));
+  CU(kf_points.create(nb * kTexMaxKeyframes * 3 * kTexMaxFeatures));
+  CU(points.create(nb * TF_COUNT * kTexPointCap));
+  CU(pose.create(nb * 12));
+  CU(gh.create(nb * 27));
+  CU(state.create(nb));
+  CU(cudaMemsetAsync(nfeat, 0, nb * sizeof(int), ctx->stream));
+  CU(cudaMemsetAsync(kf_n, 0, nb * kTexMaxKeyframes * sizeof(int), ctx->stream));
+  CU(cudaMemsetAsync(counts, 0, nb * sizeof(int), ctx->stream));
+  CU(cudaMemsetAsync(pose, 0, nb * 12 * sizeof(float), ctx->stream));
+  CU(cudaMemsetAsync(gh, 0, nb * 27 * sizeof(float), ctx->stream));
+  CU(cudaMemsetAsync(state, 0, nb * sizeof(TexKeyframeState), ctx->stream));
+  ctx->d_tex_xy = std::move(xy);
+  ctx->d_tex_desc = std::move(desc);
+  ctx->d_tex_kf_desc = std::move(kf_desc);
+  ctx->d_tex_nfeat = std::move(nfeat);
+  ctx->d_tex_kf_n = std::move(kf_n);
+  ctx->d_tex_counts = std::move(counts);
+  ctx->d_tex_kf_points = std::move(kf_points);
+  ctx->d_tex_points = std::move(points);
+  ctx->d_tex_pose = std::move(pose);
+  ctx->d_gh_texture = std::move(gh);
+  ctx->d_tex_kf_state = std::move(state);
+  return M3TB_OK;
+}
+
+// m3tb_set_body assigned the body a depth camera (its depth modality's, or its region modality's for measured occlusions)
+bool HasDepthCamera(const BodyDev& B) { return B.has_depth || (B.has_region && B.rp.measure_occlusions); }
+
+// TextureModality::SetUp's conditions, checked before every texture launch ("Set up ... first")
+int ValidateTexture(m3tb_ctx* ctx) {
+  for (int b = 0; b < ctx->n_bodies; ++b) {
+    const BodyDev& B = ctx->h_bodies[b];
+    if (!B.set || !B.has_texture) continue;
+    if (ctx->attached[b][RS_TEXTURE_SILHOUETTE] < 0)
+      return Fail(ctx, M3TB_ERR_NOT_SET_UP, "texture modality of body " + std::to_string(b) + ": no silhouette renderer attached");
+    if (B.tp.model_occlusions && ctx->attached[b][RS_TEXTURE_DEPTH] < 0)
+      return Fail(ctx, M3TB_ERR_NOT_SET_UP, "texture modality: model_occlusions needs a depth renderer attached");
+    if (B.tp.measure_occlusions) {
+      if (!HasDepthCamera(B)) return Fail(ctx, M3TB_ERR_NOT_SET_UP, "texture measure_occlusions: the body has no depth camera");
+      const CameraDev& d = ctx->h_dcams[B.depth_camera];
+      if (!d.set || !d.image) return Fail(ctx, M3TB_ERR_NOT_SET_UP, "texture measure_occlusions: depth camera not set / no image uploaded");
+    }
+  }
+  return M3TB_OK;
+}
+
+// Features belong to the colour frame they were uploaded for: a body whose camera has received a newer frame since
+// has none (the reference's detection on that frame found nothing to work with).
+int SyncTextureFeatures(m3tb_ctx* ctx) {
+  for (int b = 0; b < ctx->n_bodies; ++b) {
+    const BodyDev& B = ctx->h_bodies[b];
+    if (!B.has_texture) continue;
+    const int gen = ctx->h_ccams[B.texture_camera].generation;
+    if (ctx->tex_feat_gen[b] != gen) {
+      CU(cudaMemsetAsync(ctx->d_tex_nfeat + b, 0, sizeof(int), ctx->stream));
+      ctx->tex_feat_gen[b] = gen;
+    }
+  }
+  return M3TB_OK;
+}
+
+// k_texture_keyframe (keyframe = true) or k_texture_match over every body; mode as TextureArgs::mode
+int LaunchTexture(m3tb_ctx* ctx, bool keyframe, int mode) {
+  if (ctx->n_texture == 0) return M3TB_OK;
+  int rc = ValidateTexture(ctx);
+  if (!rc) rc = SyncTables(ctx);
+  if (!rc) rc = SyncTextureFeatures(ctx);
+  if (rc) return rc;
+  TextureArgs a;
+  a.bodies = ctx->d_bodies;
+  a.poses = ctx->d_poses;
+  a.tex_pose = ctx->d_tex_pose;
+  a.color_cams = ctx->d_ccams;
+  a.depth_cams = ctx->d_dcams;
+  a.feat_xy = ctx->d_tex_xy;
+  a.feat_desc = ctx->d_tex_desc;
+  a.feat_n = ctx->d_tex_nfeat;
+  a.kf_points = ctx->d_tex_kf_points;
+  a.kf_desc = ctx->d_tex_kf_desc;
+  a.kf_n = ctx->d_tex_kf_n;
+  a.kf_state = ctx->d_tex_kf_state;
+  a.points = ctx->d_tex_points;
+  a.counts = ctx->d_tex_counts;
+  a.mode = mode;
+  if (keyframe) k_texture_keyframe<<<ctx->n_bodies, kTexThreads, 0, ctx->stream>>>(a);
+  else k_texture_match<<<ctx->n_bodies, kTexThreads, 0, ctx->stream>>>(a);
+  CU(cudaGetLastError());
+  ctx->launches++;
+  return M3TB_OK;
+}
+
+int CheckTextureBody(m3tb_ctx* ctx, int body) {
+  if (body < 0 || body >= ctx->n_bodies || !ctx->h_bodies[body].set || !ctx->h_bodies[body].has_texture)
+    return Fail(ctx, M3TB_ERR_INVALID, "body has no texture modality");
+  return M3TB_OK;
+}
+
+}  // namespace
+
+extern "C" {
+
+int m3tb_set_texture_modality(m3tb_ctx* ctx, int body, const m3tb_texture_params* params, int color_camera) {
+  CHECK_CTX();
+  if (body < 0 || body >= ctx->n_bodies || !ctx->h_bodies[body].set) return Fail(ctx, M3TB_ERR_INVALID, "body not set");
+  BodyDev& B = ctx->h_bodies[body];
+  if (!params) {  // the body no longer has a texture modality; its renderer slots are detached
+    if (!B.has_texture) return M3TB_OK;
+    CU(cudaStreamSynchronize(ctx->stream));
+    for (int slot = RS_TEXTURE_SILHOUETTE; slot < RS_COUNT; ++slot)
+      if (ctx->attached[body][slot] >= 0) {
+        std::memset(&B.rend[slot], 0, sizeof(RenderingDev));
+        ctx->attached[body][slot] = -1;
+        ctx->n_attached--;
+        ctx->render_dirty = true;
+      }
+    B.has_texture = 0;
+    ctx->n_texture--;
+    ctx->bodies_dirty = true;
+    return M3TB_OK;
+  }
+  const m3tb_texture_params& p = *params;
+  if (p.descriptor_type != M3TB_DESCRIPTOR_ORB)
+    return Fail(ctx, M3TB_ERR_UNSUPPORTED, "only DescriptorType::ORB (32-byte descriptors, NORM_HAMMING) is implemented");
+  if (p.n_keyframes > kTexMaxKeyframes) return Fail(ctx, M3TB_ERR_UNSUPPORTED, "n_keyframes above 8");
+  if (color_camera < 0 || color_camera >= ctx->max_cameras || !ctx->h_ccams[color_camera].set)
+    return Fail(ctx, M3TB_ERR_INVALID, "color camera not set");
+  if (p.n_keyframes < 1 || p.focused_image_size < 1 || p.n_standard_deviations < 1 ||
+      p.n_standard_deviations > M3TB_MAX_SCHEDULE || !(p.tukey_norm_constant > 0.0f) || !std::isfinite(p.tukey_norm_constant) ||
+      !std::isfinite(p.descriptor_distance_threshold) || p.max_keyframe_age < 0)
+    return Fail(ctx, M3TB_ERR_INVALID, "bad texture parameters");
+  for (int k = 0; k < p.n_standard_deviations; ++k)
+    if (!(p.standard_deviations[k] > 0.0f) || !std::isfinite(p.standard_deviations[k]))
+      return Fail(ctx, M3TB_ERR_INVALID, "standard deviations must be positive");
+  if (p.measure_occlusions && !(HasDepthCamera(B) && ctx->h_dcams[B.depth_camera].set))
+    return Fail(ctx, M3TB_ERR_INVALID, "measure_occlusions needs the body's depth camera");
+  if (!ctx->h_geometry[body].set)
+    return Fail(ctx, M3TB_ERR_INVALID, "the texture modality needs the body's geometry (m3tb_set_body_geometry)");
+  int rc = EnsureTextureTables(ctx);
+  if (rc) return rc;
+  CU(cudaStreamSynchronize(ctx->stream));  // a launch in flight may still read this body's keyframes
+  CU(cudaMemsetAsync(ctx->d_tex_kf_state + body, 0, sizeof(TexKeyframeState), ctx->stream));
+  CU(cudaMemsetAsync(ctx->d_tex_counts + body, 0, sizeof(int), ctx->stream));
+  CU(cudaMemsetAsync(ctx->d_tex_nfeat + body, 0, sizeof(int), ctx->stream));
+  TextureParamsDev& t = B.tp;
+  t.focused_image_size = p.focused_image_size;
+  t.descriptor_distance_threshold = p.descriptor_distance_threshold;
+  t.tukey_norm_constant = p.tukey_norm_constant;
+  t.n_standard_deviations = p.n_standard_deviations;
+  for (int k = 0; k < kMaxSchedule; ++k) t.standard_deviations[k] = k < p.n_standard_deviations ? p.standard_deviations[k] : 0.0f;
+  t.max_keyframe_rotation_difference = p.max_keyframe_rotation_difference;
+  t.max_keyframe_age = p.max_keyframe_age;
+  t.n_keyframes = p.n_keyframes;
+  t.measure_occlusions = p.measure_occlusions ? 1 : 0;
+  t.measured_occlusion_radius = p.measured_occlusion_radius;
+  t.measured_occlusion_threshold = p.measured_occlusion_threshold;
+  t.model_occlusions = p.model_occlusions ? 1 : 0;
+  t.modeled_occlusion_radius = p.modeled_occlusion_radius;
+  t.modeled_occlusion_threshold = p.modeled_occlusion_threshold;
+  if (B.has_texture && B.texture_camera != color_camera)  // renderers of the old camera no longer fit
+    for (int slot = RS_TEXTURE_SILHOUETTE; slot < RS_COUNT; ++slot)
+      if (ctx->attached[body][slot] >= 0) {
+        std::memset(&B.rend[slot], 0, sizeof(RenderingDev));
+        ctx->attached[body][slot] = -1;
+        ctx->n_attached--;
+        ctx->render_dirty = true;
+      }
+  if (!B.has_texture) ctx->n_texture++;
+  B.has_texture = 1;
+  B.texture_camera = color_camera;
+  ctx->tex_feat_gen[body] = -1;
+  ctx->bodies_dirty = true;
+  return M3TB_OK;
+}
+
+int m3tb_get_texture_focus(m3tb_ctx* ctx, int first, int count, int32_t* roi, float* scale, int32_t* valid) {
+  CHECK_CTX();
+  if (first < 0 || count < 0 || first + count > ctx->n_bodies || (count > 0 && (!roi || !scale || !valid)))
+    return Fail(ctx, M3TB_ERR_INVALID, "bad body range / null output");
+  std::vector<float> poses(size_t(12) * count);
+  if (count > 0) {
+    CU(cudaMemcpyAsync(poses.data(), ctx->d_poses + 12 * first, poses.size() * sizeof(float), cudaMemcpyDeviceToHost,
+                       ctx->stream));
+    CU(cudaStreamSynchronize(ctx->stream));
+  }
+  for (int k = 0; k < count; ++k) {
+    const int b = first + k;
+    const BodyDev& B = ctx->h_bodies[b];
+    roi[4 * k + 0] = roi[4 * k + 1] = roi[4 * k + 2] = roi[4 * k + 3] = 0;
+    scale[k] = 0.0f;
+    valid[k] = 0;
+    if (!B.set || !B.has_texture) continue;
+    // CalculateScaleAndRegionOfInterest (texture_modality.cpp:890-931) with PrecalculatePoseVariables' body2camera
+    const CameraDev& c = ctx->h_ccams[B.texture_camera];
+    float b2c[12];
+    PoseMul(c.w2c, poses.data() + 12 * k, b2c);
+    const float r = ctx->h_geometry[b].radius;  // 0.5f * maximum_body_diameter
+    const float x = b2c[3], y = b2c[7], z = b2c[11];
+    if (z < r * 1.5f) continue;
+    const float abs_x = std::abs(x), abs_y = std::abs(y);
+    const float x2 = x * x, y2 = y * y, z2 = z * z, r2 = r * r, rz = r * z;
+    const float z2_r2 = z2 - r2, z3_zr2 = z2_r2 * z;
+    const float r_u = c.fu * (abs_x * r2 + rz * std::sqrt(z2_r2 + x2)) / z3_zr2;
+    const float r_v = c.fv * (abs_y * r2 + rz * std::sqrt(z2_r2 + y2)) / z3_zr2;
+    const float center_u = x * c.fu / z + c.ppu, center_v = y * c.fv / z + c.ppv;
+    int u_min = int(center_u - r_u - float(kTexRoiMargin) + 0.5f);
+    int u_max = int(center_u + r_u + float(kTexRoiMargin) + 0.5f);
+    int v_min = int(center_v - r_v - float(kTexRoiMargin) + 0.5f);
+    int v_max = int(center_v + r_v + float(kTexRoiMargin) + 0.5f);
+    u_min = std::max(u_min, 0);
+    u_max = std::min(u_max, c.width - 1);
+    v_min = std::max(v_min, 0);
+    v_max = std::min(v_max, c.height - 1);
+    if (u_min >= u_max || v_min >= v_max) continue;
+    roi[4 * k + 0] = u_min;
+    roi[4 * k + 1] = v_min;
+    roi[4 * k + 2] = u_max - u_min;
+    roi[4 * k + 3] = v_max - v_min;
+    scale[k] = float(B.tp.focused_image_size) / std::max(2.0f * r_u, 2.0f * r_v);
+    valid[k] = 1;
+  }
+  return M3TB_OK;
+}
+
+int m3tb_upload_texture_features(m3tb_ctx* ctx, int body, const float* keypoints_xy, const uint8_t* descriptors, int n,
+                                 int roi_x, int roi_y, float scale) {
+  CHECK_CTX();
+  int rc = CheckTextureBody(ctx, body);
+  if (rc) return rc;
+  if (n > kTexMaxFeatures) return Fail(ctx, M3TB_ERR_UNSUPPORTED, "more than 512 features per body");
+  if (n < 0 || (n > 0 && (!keypoints_xy || !descriptors)) || !(scale > 0.0f) || !std::isfinite(scale))
+    return Fail(ctx, M3TB_ERR_INVALID, "bad feature arguments");
+  // DetectAndComputeCorrKeypoints adds the focus offset (texture_modality.cpp:884-887)
+  std::vector<float2> xy(size_t(std::max(n, 1)));
+  for (int i = 0; i < n; ++i) {
+    xy[i].x = float(roi_x) + keypoints_xy[2 * i] / scale;
+    xy[i].y = float(roi_y) + keypoints_xy[2 * i + 1] / scale;
+  }
+  if (n > 0) {
+    CU(cudaMemcpyAsync(ctx->d_tex_xy + size_t(body) * kTexMaxFeatures, xy.data(), sizeof(float2) * n,
+                       cudaMemcpyHostToDevice, ctx->stream));
+    CU(cudaMemcpyAsync(ctx->d_tex_desc + size_t(body) * kTexMaxFeatures * kTexDescWords, descriptors, size_t(32) * n,
+                       cudaMemcpyHostToDevice, ctx->stream));
+  }
+  CU(cudaMemcpyAsync(ctx->d_tex_nfeat + body, &n, sizeof(int), cudaMemcpyHostToDevice, ctx->stream));
+  CU(cudaStreamSynchronize(ctx->stream));  // xy and n are on this stack frame
+  ctx->tex_feat_gen[body] = ctx->h_ccams[ctx->h_bodies[body].texture_camera].generation;
+  return M3TB_OK;
+}
+
+int m3tb_texture_correspondences(m3tb_ctx* ctx, int iteration, int corr_iteration) {
+  CHECK_CTX();
+  (void)iteration;
+  if (corr_iteration < 0) return Fail(ctx, M3TB_ERR_INVALID, "negative iteration count");
+  if (ctx->n_texture == 0) return Fail(ctx, M3TB_ERR_NOT_SET_UP, "no texture modality set");
+  return LaunchTexture(ctx, false, corr_iteration == 0 ? 1 : 0);
+}
+
+int m3tb_texture_gradient_hessian(m3tb_ctx* ctx, int iteration, int corr_iteration, int opt_iteration, float* gradients,
+                                  float* hessians) {
+  CHECK_CTX();
+  if (ctx->n_texture == 0) return Fail(ctx, M3TB_ERR_NOT_SET_UP, "no texture modality set");
+  int rc = ValidateTexture(ctx);
+  if (!rc) rc = LaunchTrack(ctx, iteration, corr_iteration, corr_iteration + 1, 1, opt_iteration, PH_TEXTURE_GH | PH_STORE_GH);
+  if (rc) return rc;
+  return ReadGH(ctx, ctx->d_gh_texture, gradients, hessians);
+}
+
+int m3tb_get_texture_points(m3tb_ctx* ctx, int body, m3tb_texture_point* points, int capacity, int* n_out) {
+  CHECK_CTX();
+  int rc = CheckTextureBody(ctx, body);
+  if (rc) return rc;
+  if (capacity < 0 || (capacity > 0 && !points)) return Fail(ctx, M3TB_ERR_INVALID, "bad output");
+  int n = 0;
+  CU(cudaMemcpyAsync(&n, ctx->d_tex_counts + body, sizeof(int), cudaMemcpyDeviceToHost, ctx->stream));
+  CU(cudaStreamSynchronize(ctx->stream));
+  if (n_out) *n_out = n;
+  const int m = std::min(n, capacity);
+  if (m <= 0) return M3TB_OK;
+  std::vector<float> f(size_t(TF_COUNT) * m);
+  const float* src = ctx->d_tex_points + size_t(body) * TF_COUNT * kTexPointCap;
+  CU(cudaMemcpy2DAsync(f.data(), sizeof(float) * m, src, sizeof(float) * kTexPointCap, sizeof(float) * m, TF_COUNT,
+                       cudaMemcpyDeviceToHost, ctx->stream));
+  CU(cudaStreamSynchronize(ctx->stream));
+  for (int i = 0; i < m; ++i) {
+    m3tb_texture_point& p = points[i];
+    p.center_f_body[0] = f[TF_CBX * m + i];
+    p.center_f_body[1] = f[TF_CBY * m + i];
+    p.center_f_body[2] = f[TF_CBZ * m + i];
+    p.correspondence_center[0] = f[TF_CU * m + i];
+    p.correspondence_center[1] = f[TF_CV * m + i];
+    p.center[0] = f[TF_PU * m + i];
+    p.center[1] = f[TF_PV * m + i];
+  }
+  return M3TB_OK;
+}
+
+int m3tb_get_texture_keyframes(m3tb_ctx* ctx, int body, int* n_keyframes, int* sizes, float* points, uint8_t* descriptors,
+                               int capacity, int* age, float* orientation) {
+  CHECK_CTX();
+  int rc = CheckTextureBody(ctx, body);
+  if (rc) return rc;
+  if (capacity < 0) return Fail(ctx, M3TB_ERR_INVALID, "bad capacity");
+  TexKeyframeState st;
+  std::vector<int> kn(kTexMaxKeyframes);
+  std::vector<float> kp(size_t(kTexMaxKeyframes) * 3 * kTexMaxFeatures);
+  std::vector<uint32_t> kd(size_t(kTexMaxKeyframes) * kTexMaxFeatures * kTexDescWords);
+  CU(cudaMemcpyAsync(&st, ctx->d_tex_kf_state + body, sizeof(st), cudaMemcpyDeviceToHost, ctx->stream));
+  CU(cudaMemcpyAsync(kn.data(), ctx->d_tex_kf_n + body * kTexMaxKeyframes, sizeof(int) * kn.size(), cudaMemcpyDeviceToHost,
+                     ctx->stream));
+  CU(cudaMemcpyAsync(kp.data(), ctx->d_tex_kf_points + size_t(body) * kp.size(), sizeof(float) * kp.size(),
+                     cudaMemcpyDeviceToHost, ctx->stream));
+  CU(cudaMemcpyAsync(kd.data(), ctx->d_tex_kf_desc + size_t(body) * kd.size(), sizeof(uint32_t) * kd.size(),
+                     cudaMemcpyDeviceToHost, ctx->stream));
+  CU(cudaStreamSynchronize(ctx->stream));
+  if (n_keyframes) *n_keyframes = st.size;
+  if (age) *age = st.age;
+  if (orientation) std::memcpy(orientation, st.orientation, sizeof(float) * 3);
+  int written = 0;
+  for (int k = 0; k < st.size; ++k) {
+    const int slot = (st.head + k) % kTexMaxKeyframes;
+    if (sizes) sizes[k] = kn[slot];
+    for (int i = 0; i < kn[slot] && written < capacity; ++i, ++written) {
+      if (points)
+        for (int c = 0; c < 3; ++c) points[3 * written + c] = kp[(size_t(slot) * 3 + c) * kTexMaxFeatures + i];
+      if (descriptors)
+        std::memcpy(descriptors + size_t(32) * written, kd.data() + (size_t(slot) * kTexMaxFeatures + i) * kTexDescWords, 32);
+    }
+  }
   return M3TB_OK;
 }
 

@@ -48,8 +48,9 @@ enum Phase : unsigned {
   PH_LOAD_REGION = 32u, PH_LOAD_DEPTH = 64u, PH_STORE_REGION = 128u, PH_STORE_DEPTH = 256u,
   PH_STORE_GH = 512u, PH_LOAD_GH = 1024u,
   PH_STORE_LINK_GH = 2048u,  // sum over the body's modalities -> gh_link (input of k_structure)
-  PH_CLUSTER_SOLVE = 4096u   // one thread-block cluster per kinematic structure: Optimizer::CalculateOptimization
+  PH_CLUSTER_SOLVE = 4096u,  // one thread-block cluster per kinematic structure: Optimizer::CalculateOptimization
                              // over distributed shared memory inside k_track (CLUSTER variants only)
+  PH_TEXTURE_GH = 8192u      // TextureModality::CalculateGradientAndHessian of the bodies with a texture modality
 };
 
 struct CameraDev {
@@ -144,12 +145,31 @@ struct RenderingDev {
   int id;
   int visible;
 };
-enum RenderingSlot { RS_REGION_DEPTH = 0, RS_REGION_SILHOUETTE, RS_DEPTH_DEPTH, RS_DEPTH_SILHOUETTE, RS_COUNT };
+// The texture modality's silhouette renderer feeds two slots: its silhouette image and the focused depth image that
+// Reconstruct3DPoint reads beside it (texture_modality.cpp:987-1006).
+enum RenderingSlot {
+  RS_REGION_DEPTH = 0, RS_REGION_SILHOUETTE, RS_DEPTH_DEPTH, RS_DEPTH_SILHOUETTE,
+  RS_TEXTURE_SILHOUETTE, RS_TEXTURE_SILHOUETTE_DEPTH, RS_TEXTURE_DEPTH, RS_COUNT
+};
 constexpr int kNRegionStride = 5;      // region_modality.h:146
 constexpr float kRegionOffset = 2.0f;  // region_modality.h:147
 
 constexpr int kDepthOffsets = 30;        // DataPoint::depth_offsets (region_model.h:97, depth_model.h:74)
 constexpr int kMaxNOcclusionStrides = 5; // region_modality.h:145, depth_modality.h:113
+
+// Parameters of m3t::TextureModality (texture_modality.h:400-436), descriptor type ORB
+struct TextureParamsDev {
+  int focused_image_size;
+  float descriptor_distance_threshold, tukey_norm_constant;
+  int n_standard_deviations;
+  float standard_deviations[kMaxSchedule];
+  float max_keyframe_rotation_difference;
+  int max_keyframe_age, n_keyframes;
+  int measure_occlusions;
+  float measured_occlusion_radius, measured_occlusion_threshold;
+  int model_occlusions;
+  float modeled_occlusion_radius, modeled_occlusion_threshold;
+};
 
 struct BodyDev {
   int has_region, has_depth;
@@ -159,6 +179,8 @@ struct BodyDev {
   int set;
   RegionParamsDev rp;
   DepthParamsDev dp;
+  int has_texture, texture_camera;  // TextureModality: its colour camera
+  TextureParamsDev tp;
   RenderingDev rend[RS_COUNT];
 };
 
@@ -200,6 +222,12 @@ struct TrackArgs {
   // k_track2: RegionModality::PrecalculateFunctionLookup tables, identical for every region body of the launch
   // (checked by the host), so that they are kernel-parameter constants instead of per-thread registers
   float lookup_f[kFunctionLength], lookup_b[kFunctionLength];
+  // texture modality (PH_TEXTURE_GH): data points [n_bodies][TF_COUNT][kTexPointCap] and their counts from
+  // k_texture_match, the pose of each gradient pass (tex_pose [n_bodies][12]) and the sums (gh_texture [n_bodies][27])
+  float* tex_points;
+  const int* tex_counts;
+  float* tex_pose;
+  float* gh_texture;
 };
 
 // ---------------------------------------------------------------------------------------------

@@ -129,7 +129,7 @@ __global__ void __launch_bounds__(kRenderThreads) k_render(const __grid_constant
     if (at.renderer == r) {
       const RenderOutDev& o = a.out[r];
       const GeometryDev& G = a.geometry[at.body];
-      const bool sil = at.slot == RS_REGION_SILHOUETTE || at.slot == RS_DEPTH_SILHOUETTE;
+      const bool sil = at.slot == RS_REGION_SILHOUETTE || at.slot == RS_DEPTH_SILHOUETTE || at.slot == RS_TEXTURE_SILHOUETTE;
       RenderingDev d;
       d.image = sil ? R.silhouette : reinterpret_cast<const uint8_t*>(R.depth);
       d.image_size = S;

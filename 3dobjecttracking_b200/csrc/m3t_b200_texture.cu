@@ -1,0 +1,276 @@
+// m3t_b200_texture.cu — k_texture_keyframe and k_texture_match (TextureModality, texture_modality.cpp).
+// One CTA of kTexThreads threads per body; bodies without a texture modality return at once.
+#include <climits>
+
+#include <cuda_runtime.h>
+
+#include "m3t_b200_texture.cuh"
+
+namespace m3tb {
+
+namespace {
+
+// Exclusive prefix of `keep` over the CTA in thread order; returns the thread's offset, *total the CTA's count.
+__device__ __forceinline__ int BlockCompact(bool keep, int* s_warp, int* total) {
+  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  const unsigned ballot = __ballot_sync(0xffffffffu, keep);
+  if (lane == 0) s_warp[warp] = __popc(ballot);
+  __syncthreads();
+  int before = 0, sum = 0;
+  for (int w = 0; w < kTexThreads / 32; ++w) {
+    if (w < warp) before += s_warp[w];
+    sum += s_warp[w];
+  }
+  __syncthreads();  // s_warp is reused by the next call
+  *total = sum;
+  return before + __popc(ballot & ((1u << lane) - 1u));
+}
+
+__device__ __forceinline__ const uint8_t* Row(const RenderingDev& r, int v) { return r.image + size_t(v) * r.pitch; }
+
+// TextureModality::IsPointUnoccludedMeasured (texture_modality.cpp:1035-1085)
+__device__ bool UnoccludedMeasured(const CameraDev& d, const float* b2d, const TextureParamsDev& tp, float bx, float by,
+                                   float bz) {
+  const float x = b2d[0] * bx + b2d[1] * by + b2d[2] * bz + b2d[3];
+  const float y = b2d[4] * bx + b2d[5] * by + b2d[6] * bz + b2d[7];
+  const float z = b2d[8] * bx + b2d[9] * by + b2d[10] * bz + b2d[11];
+  const float center_u = x * d.fu / z + d.ppu, center_v = y * d.fv / z + d.ppv;
+  const float meter_to_pixel = d.fu / z;
+  const float diameter = 2.0f * tp.measured_occlusion_radius * meter_to_pixel;
+  const int stride = int(diameter / float(kMaxNOcclusionStrides) + 1.0f);
+  const int n_strides = int(diameter / float(stride) + 0.5f);
+  const int rounded_diameter = n_strides * stride;
+  const float rounded_radius = 0.5f * float(rounded_diameter);
+  int u_min = int(center_u - rounded_radius + 0.5f), v_min = int(center_v - rounded_radius + 0.5f);
+  int u_max = u_min + rounded_diameter, v_max = v_min + rounded_diameter;
+  u_min = max(u_min, 0);
+  v_min = max(v_min, 0);
+  u_max = min(u_max, d.width - 1);
+  v_max = min(v_max, d.height - 1);
+  const unsigned short min_depth = (unsigned short)((z - tp.measured_occlusion_threshold) / d.depth_scale);
+  // a camera that refers to a pinned frame is read from it: its device copy is valid only inside the tracking ROIs
+  const uint8_t* img = d.host_src ? d.host_src : d.image;
+  const unsigned pitch = d.host_src ? d.host_pitch : d.pitch;
+  for (int v = v_min; v <= v_max; v += stride) {
+    const uint16_t* row = reinterpret_cast<const uint16_t*>(img + size_t(v) * pitch);
+    for (int u = u_min; u <= u_max; u += stride) {
+      const unsigned short depth = row[u];
+      if (depth > 0 && depth < min_depth) return false;
+    }
+  }
+  return true;
+}
+
+// TextureModality::IsPointUnoccludedModeled (texture_modality.cpp:1087-1127)
+__device__ bool UnoccludedModeled(const CameraDev& c, const RenderingDev& r, const float* b2c, const TextureParamsDev& tp,
+                                  float bx, float by, float bz) {
+  const float x = b2c[0] * bx + b2c[1] * by + b2c[2] * bz + b2c[3];
+  const float y = b2c[4] * bx + b2c[5] * by + b2c[6] * bz + b2c[7];
+  const float z = b2c[8] * bx + b2c[9] * by + b2c[10] * bz + b2c[11];
+  const float meter_to_pixel = (c.fu / z) * r.scale;
+  const float diameter = 2.0f * tp.modeled_occlusion_radius * meter_to_pixel;
+  const int stride = int(diameter / float(kMaxNOcclusionStrides) + 1.0f);
+  const int n_strides = int(diameter / float(stride) + 0.5f);
+  const int rounded_diameter = n_strides * stride;
+  const float rounded_radius = 0.5f * float(rounded_diameter);
+  const float center_u = x * c.fu / z + c.ppu, center_v = y * c.fv / z + c.ppv;
+  const float fcu = (center_u - r.corner_u) * r.scale, fcv = (center_v - r.corner_v) * r.scale;
+  int u_min = int(fcu - rounded_radius + 0.5f), v_min = int(fcv - rounded_radius + 0.5f);
+  int u_max = u_min + rounded_diameter, v_max = v_min + rounded_diameter;
+  u_min = max(u_min, 0);
+  v_min = max(v_min, 0);
+  u_max = min(u_max, r.image_size - 1);
+  v_max = min(v_max, r.image_size - 1);
+  unsigned short min_value = 65535;
+  for (int v = v_min; v <= v_max; v += stride) {
+    const uint16_t* row = reinterpret_cast<const uint16_t*>(Row(r, v));
+    for (int u = u_min; u <= u_max; u += stride) min_value = min(min_value, row[u]);
+  }
+  const float min_depth = r.projection_term_a / (r.projection_term_b - float(min_value));
+  return min_depth > z - tp.modeled_occlusion_threshold;
+}
+
+// R^T normalize(t) of a body2camera pose (orientation_last_keyframe_, texture_modality.cpp:1016-1018); like Eigen's
+// normalized(), a zero translation stays zero
+__device__ void Orientation(const float* b2c, float* o) {
+  const float n2 = b2c[3] * b2c[3] + b2c[7] * b2c[7] + b2c[11] * b2c[11];
+  float tx = b2c[3], ty = b2c[7], tz = b2c[11];
+  if (n2 > 0.0f) {
+    const float n = sqrtf(n2);
+    tx = tx / n; ty = ty / n; tz = tz / n;
+  }
+  for (int i = 0; i < 3; ++i) o[i] = b2c[i] * tx + b2c[4 + i] * ty + b2c[8 + i] * tz;
+}
+
+}  // namespace
+
+// StartModality (mode 0: PrecalculatePoseVariables from the current pose, then ComputeKeyframeData) and CalculateResults
+// (mode 1: the rotation / age rule with the pose of the last gradient pass, texture_modality.cpp:456-472).
+__global__ void __launch_bounds__(kTexThreads) k_texture_keyframe(const __grid_constant__ TextureArgs a) {
+  const int b = blockIdx.x, tid = threadIdx.x;
+  const BodyDev& body = a.bodies[b];
+  if (!body.set || !body.has_texture) return;
+  __shared__ float b2c[12], c2b[12], b2d[12];
+  __shared__ int s_fire, s_visible, s_slot;
+  __shared__ int s_warp[kTexThreads / 32];
+  const CameraDev& cam = a.color_cams[body.texture_camera];
+  const TextureParamsDev& tp = body.tp;
+  TexKeyframeState* st = a.kf_state + b;
+  if (tid == 0) {
+    float pose[12];
+    for (int k = 0; k < 12; ++k) pose[k] = a.mode == 0 ? a.poses[12 * b + k] : a.tex_pose[12 * b + k];
+    if (a.mode == 0)
+      for (int k = 0; k < 12; ++k) a.tex_pose[12 * b + k] = pose[k];
+    PoseMul(cam.w2c, pose, b2c);
+    PoseInverse(b2c, c2b);
+    if (tp.measure_occlusions) PoseMul(a.depth_cams[body.depth_camera].w2c, pose, b2d);
+    int fire = 1;
+    if (a.mode == 1) {
+      float o[3];
+      Orientation(b2c, o);
+      const float rotation_difference = acosf(o[0] * st->orientation[0] + o[1] * st->orientation[1] + o[2] * st->orientation[2]);
+      st->age += 1;
+      fire = rotation_difference > tp.max_keyframe_rotation_difference || st->age > tp.max_keyframe_age;
+    }
+    int visible = 0;
+    if (fire) {
+      if (st->size >= tp.n_keyframes) {  // pop_front, before the visibility test
+        st->head = (st->head + 1) % kTexMaxKeyframes;
+        st->size -= 1;
+      }
+      const RenderingDev& sil = body.rend[RS_TEXTURE_SILHOUETTE];
+      visible = sil.image != nullptr && sil.visible;
+    }
+    s_fire = fire;
+    s_visible = visible;
+    s_slot = (st->head + st->size) % kTexMaxKeyframes;
+  }
+  __syncthreads();
+  if (!s_fire || !s_visible) return;
+  const RenderingDev& sil = body.rend[RS_TEXTURE_SILHOUETTE];
+  const RenderingDev& sdep = body.rend[RS_TEXTURE_SILHOUETTE_DEPTH];
+  const RenderingDev& mdep = body.rend[RS_TEXTURE_DEPTH];
+  const bool modeled = tp.model_occlusions && mdep.image != nullptr && mdep.visible;
+  const int n = a.feat_n[b];
+  const float2* xy = a.feat_xy + size_t(b) * kTexMaxFeatures;
+  const uint32_t* desc = a.feat_desc + size_t(b) * kTexMaxFeatures * kTexDescWords;
+  const int slot = s_slot;
+  float* kp = a.kf_points + (size_t(b) * kTexMaxKeyframes + slot) * 3 * kTexMaxFeatures;
+  uint32_t* kd = a.kf_desc + (size_t(b) * kTexMaxKeyframes + slot) * kTexMaxFeatures * kTexDescWords;
+  int written = 0;
+  for (int i0 = 0; i0 < n; i0 += kTexThreads) {
+    const int i = i0 + tid;
+    bool keep = false;
+    float px = 0.0f, py = 0.0f, pz = 0.0f;
+    if (i < n) {  // Reconstruct3DPoint (texture_modality.cpp:987-1023) + IsPointValid
+      const float2 c = xy[i];
+      const int us = int((c.x - sil.corner_u) * sil.scale + 0.5f), vs = int((c.y - sil.corner_v) * sil.scale + 0.5f);
+      const int s1 = sil.image_size - 1;
+      if (us >= 0 && us <= s1 && vs >= 0 && vs <= s1 && Row(sil, vs)[us] == uint8_t(sil.id)) {
+        const unsigned short value = reinterpret_cast<const uint16_t*>(Row(sdep, vs))[us];
+        const float depth = sdep.projection_term_a / (sdep.projection_term_b - float(value));
+        const float cx = depth * (c.x - cam.ppu) / cam.fu, cy = depth * (c.y - cam.ppv) / cam.fv, cz = depth;
+        px = c2b[0] * cx + c2b[1] * cy + c2b[2] * cz + c2b[3];
+        py = c2b[4] * cx + c2b[5] * cy + c2b[6] * cz + c2b[7];
+        pz = c2b[8] * cx + c2b[9] * cy + c2b[10] * cz + c2b[11];
+        keep = true;
+        if (tp.measure_occlusions) keep = UnoccludedMeasured(a.depth_cams[body.depth_camera], b2d, tp, px, py, pz);
+        if (keep && modeled) keep = UnoccludedModeled(cam, mdep, b2c, tp, px, py, pz);
+      }
+    }
+    int total;
+    const int pos = written + BlockCompact(keep, s_warp, &total);
+    if (keep) {
+      kp[0 * kTexMaxFeatures + pos] = px;
+      kp[1 * kTexMaxFeatures + pos] = py;
+      kp[2 * kTexMaxFeatures + pos] = pz;
+      for (int w = 0; w < kTexDescWords; ++w) kd[size_t(pos) * kTexDescWords + w] = desc[size_t(i) * kTexDescWords + w];
+    }
+    written += total;
+  }
+  if (tid == 0) {
+    a.kf_n[b * kTexMaxKeyframes + slot] = written;
+    st->size += 1;
+    Orientation(b2c, st->orientation);
+    st->age = 0;
+  }
+}
+
+// CalculateCorrespondences (texture_modality.cpp:322-386): with mode 1 (correspondence iteration 0) every keyframe's
+// descriptors (queries) are matched against the frame's (train set) by brute-force Hamming kNN, k = 2, and the matches
+// that pass the ratio test become the data points, keyframe by keyframe in query order. Every call then projects the
+// data points with the current pose (data_point.center) and records that pose.
+__global__ void __launch_bounds__(kTexThreads) k_texture_match(const __grid_constant__ TextureArgs a) {
+  const int b = blockIdx.x, tid = threadIdx.x;
+  const BodyDev& body = a.bodies[b];
+  if (!body.set || !body.has_texture) return;
+  __shared__ uint4 s_train[kTexMaxFeatures * 2];
+  __shared__ int s_warp[kTexThreads / 32];
+  float* pts = a.points + size_t(b) * TF_COUNT * kTexPointCap;
+  const CameraDev& cam = a.color_cams[body.texture_camera];
+  if (a.mode == 1) {
+    const int n_train = a.feat_n[b];
+    const uint4* train = reinterpret_cast<const uint4*>(a.feat_desc + size_t(b) * kTexMaxFeatures * kTexDescWords);
+    for (int k = tid; k < 2 * n_train; k += kTexThreads) s_train[k] = train[k];
+    __syncthreads();
+    const float2* xy = a.feat_xy + size_t(b) * kTexMaxFeatures;
+    const TexKeyframeState st = a.kf_state[b];
+    const float thr = body.tp.descriptor_distance_threshold;
+    int written = 0;
+    for (int k = 0; k < st.size; ++k) {
+      const int slot = (st.head + k) % kTexMaxKeyframes;
+      const int nq = a.kf_n[b * kTexMaxKeyframes + slot];
+      const float* kp = a.kf_points + (size_t(b) * kTexMaxKeyframes + slot) * 3 * kTexMaxFeatures;
+      const uint4* kd = reinterpret_cast<const uint4*>(a.kf_desc + (size_t(b) * kTexMaxKeyframes + slot) * kTexMaxFeatures * kTexDescWords);
+      for (int q0 = 0; q0 < nq; q0 += kTexThreads) {
+        const int q = q0 + tid;
+        bool keep = false;
+        int i0 = -1;
+        if (q < nq && n_train >= 2) {
+          const uint4 qa = kd[2 * q], qb = kd[2 * q + 1];
+          // cv::batchDistance's K = 2 insertion: strictly smaller distances enter, ties keep the earlier train index
+          int d0 = INT_MAX, d1 = INT_MAX, i1 = -1;
+          for (int j = 0; j < n_train; ++j) {
+            const uint4 ta = s_train[2 * j], tb = s_train[2 * j + 1];
+            const int d = __popc(qa.x ^ ta.x) + __popc(qa.y ^ ta.y) + __popc(qa.z ^ ta.z) + __popc(qa.w ^ ta.w) +
+                          __popc(qb.x ^ tb.x) + __popc(qb.y ^ tb.y) + __popc(qb.z ^ tb.z) + __popc(qb.w ^ tb.w);
+            if (d < d1) {
+              if (d < d0) { d1 = d0; i1 = i0; d0 = d; i0 = j; }
+              else { d1 = d; i1 = j; }
+            }
+          }
+          // knn_match[0].distance / knn_match[1].distance >= threshold drops the match; 0 / 0 is NaN and keeps it
+          keep = i1 >= 0 && !(float(d0) / float(d1) >= thr);
+        }
+        int total;
+        const int pos = written + BlockCompact(keep, s_warp, &total);
+        if (keep) {
+          pts[TF_CBX * kTexPointCap + pos] = kp[0 * kTexMaxFeatures + q];
+          pts[TF_CBY * kTexPointCap + pos] = kp[1 * kTexMaxFeatures + q];
+          pts[TF_CBZ * kTexPointCap + pos] = kp[2 * kTexMaxFeatures + q];
+          const float2 c = xy[i0];
+          pts[TF_CU * kTexPointCap + pos] = c.x;
+          pts[TF_CV * kTexPointCap + pos] = c.y;
+        }
+        written += total;
+      }
+    }
+    if (tid == 0) a.counts[b] = written;
+    __syncthreads();
+  }
+  __shared__ float b2c[12];
+  if (tid < 12) a.tex_pose[12 * b + tid] = a.poses[12 * b + tid];
+  if (tid == 0) PoseMul(cam.w2c, a.poses + 12 * b, b2c);
+  __syncthreads();
+  const int n = a.counts[b];
+  for (int i = tid; i < n; i += kTexThreads) {
+    const float bx = pts[TF_CBX * kTexPointCap + i], by = pts[TF_CBY * kTexPointCap + i], bz = pts[TF_CBZ * kTexPointCap + i];
+    const float x = b2c[0] * bx + b2c[1] * by + b2c[2] * bz + b2c[3];
+    const float y = b2c[4] * bx + b2c[5] * by + b2c[6] * bz + b2c[7];
+    const float z = b2c[8] * bx + b2c[9] * by + b2c[10] * bz + b2c[11];
+    pts[TF_PU * kTexPointCap + i] = x * cam.fu / z + cam.ppu;
+    pts[TF_PV * kTexPointCap + i] = y * cam.fv / z + cam.ppv;
+  }
+}
+
+}  // namespace m3tb

@@ -1,0 +1,99 @@
+// m3t_b200_texture.cuh — TextureModality on the device (texture_modality.cpp): keyframe reconstruction from the device
+// silhouette renderer, brute-force Hamming kNN matching of ORB descriptors, and the Tukey-weighted reprojection
+// gradient / Hessian that k_track adds to a body's link. Feature detection stays with the caller; what it hands over
+// (keypoints in image coordinates and 32-byte descriptors) is all these kernels read of the colour frame.
+#pragma once
+
+#include "m3t_b200_device.cuh"
+
+namespace m3tb {
+
+constexpr int kTexMaxFeatures = 512;   // frame features per body (the train set is staged in shared memory)
+constexpr int kTexMaxKeyframes = 8;    // n_keyframes
+constexpr int kTexPointCap = kTexMaxFeatures * kTexMaxKeyframes;
+constexpr int kTexDescWords = 8;       // 32-byte ORB descriptors
+constexpr int kTexThreads = 256;
+constexpr int kTexRoiMargin = 10;      // kRegionOfInterestMargin, texture_modality.h:132
+
+// per-data-point fields (SoA, [field][point]): center_f_body, correspondence_center, center
+enum TextureField { TF_CBX = 0, TF_CBY, TF_CBZ, TF_CU, TF_CV, TF_PU, TF_PV, TF_COUNT };
+
+// The keyframe deque of one body (points_keyframes_ / descriptors_keyframes_ as a ring of kTexMaxKeyframes slots)
+struct TexKeyframeState {
+  int size, head, age, pad;
+  float orientation[3];  // orientation_last_keyframe_
+  float pad1;
+};
+
+struct TextureArgs {
+  const BodyDev* bodies;
+  const float* poses;           // body2world [n_bodies][12]
+  float* tex_pose;              // [n_bodies][12]: the pose of the texture modality's last PrecalculatePoseVariables
+  const CameraDev* color_cams;
+  const CameraDev* depth_cams;
+  const float2* feat_xy;        // [n_bodies][kTexMaxFeatures] keypoints_ in image coordinates
+  const uint32_t* feat_desc;    // [n_bodies][kTexMaxFeatures][8]
+  const int* feat_n;            // [n_bodies]
+  float* kf_points;             // [n_bodies][kTexMaxKeyframes][3][kTexMaxFeatures]
+  uint32_t* kf_desc;            // [n_bodies][kTexMaxKeyframes][kTexMaxFeatures][8]
+  int* kf_n;                    // [n_bodies][kTexMaxKeyframes]
+  TexKeyframeState* kf_state;   // [n_bodies]
+  float* points;                // [n_bodies][TF_COUNT][kTexPointCap]
+  int* counts;                  // [n_bodies]
+  int mode;                     // k_texture_keyframe: 0 StartModality, 1 CalculateResults; k_texture_match: 1 = match
+};
+
+__global__ void k_texture_keyframe(const __grid_constant__ TextureArgs a);
+__global__ void k_texture_match(const __grid_constant__ TextureArgs a);
+
+// TextureModality::TukeyNorm (texture_modality.cpp:1231-1237)
+__host__ __device__ __forceinline__ float TexTukeyNorm(float error, float c) {
+  if (fabsf(error) <= c) return powf(c, 2.0f) / 6.0f * (1.0f - powf(1.0f - powf(error / c, 2.0f), 3.0f));
+  return powf(c, 2.0f) / 6.0f;
+}
+
+// TextureModality::CalculateGradientAndHessian (texture_modality.cpp:397-444) over the data points i = first, first +
+// stride, ... of one body, added to acc (g[6], H lower [21], the reference's signs). Also refreshes data_point.center.
+__device__ __forceinline__ void TextureGradient(const CameraDev& cam, const float* pose, const TextureParamsDev& tp,
+                                                int corr, float* pts, int n, int first, int stride, float* acc) {
+  float b2c[12];
+  PoseMul(cam.w2c, pose, b2c);
+  const float sd = LastValid(tp.standard_deviations, tp.n_standard_deviations, corr);
+  const float variance = powf(sd, 2.0f);
+  for (int i = first; i < n; i += stride) {
+    const float bx = pts[TF_CBX * kTexPointCap + i], by = pts[TF_CBY * kTexPointCap + i], bz = pts[TF_CBZ * kTexPointCap + i];
+    const float x = b2c[0] * bx + b2c[1] * by + b2c[2] * bz + b2c[3];
+    const float y = b2c[4] * bx + b2c[5] * by + b2c[6] * bz + b2c[7];
+    const float z = b2c[8] * bx + b2c[9] * by + b2c[10] * bz + b2c[11];
+    const float cu = x * cam.fu / z + cam.ppu, cv = y * cam.fv / z + cam.ppv;
+    pts[TF_PU * kTexPointCap + i] = cu;
+    pts[TF_PV * kTexPointCap + i] = cv;
+    const float z2 = z * z;
+    const float d0 = cu - pts[TF_CU * kTexPointCap + i], d1 = cv - pts[TF_CV * kTexPointCap + i];
+    const float squared_error = d0 * d0 + d1 * d1;
+    const float error = sqrtf(squared_error);
+    float weight = 1.0f / variance;
+    if (error > 1.17549435e-38f) weight = (TexTukeyNorm(error, tp.tukey_norm_constant) / squared_error) / variance;
+    // dx_dX (2x3) * body2camera rotation -> dx_dtranslation; rotation part = center_f_body x row
+    const float a00 = cam.fu / z, a02 = -x * cam.fu / z2, a11 = cam.fv / z, a12 = -y * cam.fv / z2;
+    float t0[3], t1[3];
+#pragma unroll
+    for (int c = 0; c < 3; ++c) {
+      t0[c] = a00 * b2c[c] + a02 * b2c[8 + c];
+      t1[c] = a11 * b2c[4 + c] + a12 * b2c[8 + c];
+    }
+    const float J0[6] = {by * t0[2] - bz * t0[1], bz * t0[0] - bx * t0[2], bx * t0[1] - by * t0[0], t0[0], t0[1], t0[2]};
+    const float J1[6] = {by * t1[2] - bz * t1[1], bz * t1[0] - bx * t1[2], bx * t1[1] - by * t1[0], t1[0], t1[1], t1[2]};
+    const float wd0 = weight * d0, wd1 = weight * d1;
+#pragma unroll
+    for (int k = 0; k < 6; ++k) acc[k] -= wd0 * J0[k] + wd1 * J1[k];
+#pragma unroll
+    for (int r = 0; r < 6; ++r) {
+      const float w0 = weight * J0[r], w1 = weight * J1[r];
+#pragma unroll
+      for (int c = 0; c <= r; ++c) acc[6 + r * (r + 1) / 2 + c] -= w0 * J0[c] + w1 * J1[c];
+    }
+  }
+}
+
+}  // namespace m3tb
