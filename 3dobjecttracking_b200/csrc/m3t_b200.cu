@@ -978,6 +978,13 @@ int LaunchStructure(m3tb_ctx* ctx, int mode, bool from_modalities) {
   a.gh_link = from_modalities ? nullptr : ctx->d_gh_link.get();
   a.gh_region = ctx->d_gh_region;
   a.gh_depth = ctx->d_gh_depth;
+  // the texture sums of the fine-grained calls; the kernel reads has_texture from the device body table
+  a.gh_texture = from_modalities && ctx->n_texture > 0 ? ctx->d_gh_texture.get() : nullptr;
+  a.bodies = ctx->d_bodies;
+  if (a.gh_texture) {
+    rc = SyncTables(ctx);
+    if (rc) return rc;
+  }
   a.mode = mode;
   a.theta_out = ctx->d_theta;
   a.status = ctx->d_struct_status;
@@ -1014,12 +1021,18 @@ int ClusterLinks(m3tb_ctx* ctx) {
 }
 
 // Tracker::ExecuteTrackingStep's loop nest (tracker.cpp:344-361) when the optimisers are kinematic structures: the
-// per-body work stays in k_track (correspondences, gradient / Hessian -> gh_link), every
-// Optimizer::CalculateOptimization is one k_structure launch over all structures.
+// per-body work stays in k_track (correspondences, gradient / Hessian of region, depth and texture -> gh_link), every
+// Optimizer::CalculateOptimization is one k_structure launch over all structures. Texture matching runs once per frame,
+// at correspondence iteration 0, as in the rigid path.
 int StructureStep(m3tb_ctx* ctx, int iteration, int corr_begin, int corr_end, int n_update) {
   int rc0 = SyncStructures(ctx);
+  // TextureModality::SetUp's conditions first: a texture modality then has its silhouette renderer attached, so a
+  // textured context renders (below) and never takes the cluster-fused path, which has no texture term
+  if (!rc0 && ctx->n_texture > 0) rc0 = ValidateTexture(ctx);
   if (rc0) return rc0;
-  const bool render = ctx->n_attached > 0;  // device renderers refresh their images before every correspondence iteration
+  // device renderers refresh their images before every correspondence iteration
+  const bool render = ctx->n_attached > 0;
+  const unsigned tex = ctx->n_texture > 0 ? unsigned(PH_TEXTURE_GH) : 0u;
   if (const int nl = render ? 0 : ClusterLinks(ctx)) {
     // fused: the whole corr x update loop nest in ONE launch, one cluster per structure, CalculateOptimization over
     // distributed shared memory
@@ -1032,6 +1045,7 @@ int StructureStep(m3tb_ctx* ctx, int iteration, int corr_begin, int corr_end, in
   for (int corr = corr_begin; corr < corr_end; ++corr) {
     if (render) {
       int rc = LaunchRender(ctx, kRenderAttached);
+      if (!rc && corr == 0) rc = LaunchTexture(ctx, false, 1);  // texture matches of this frame (no-op without texture)
       if (rc) return rc;
     }
     if (n_update == 0) {
@@ -1041,13 +1055,13 @@ int StructureStep(m3tb_ctx* ctx, int iteration, int corr_begin, int corr_end, in
     }
     int rc = LaunchTrack(ctx, iteration, corr, corr + 1, 1, 0,
                          PH_REGION_CORR | PH_DEPTH_CORR | PH_REGION_GH | PH_DEPTH_GH | PH_STORE_LINK_GH | PH_STORE_REGION |
-                             PH_STORE_DEPTH);
+                             PH_STORE_DEPTH | tex);
     if (rc) return rc;
     rc = LaunchStructure(ctx, 0, false);
     if (rc) return rc;
     for (int upd = 1; upd < n_update; ++upd) {
       rc = LaunchTrack(ctx, iteration, corr, corr + 1, 1, upd,
-                       PH_LOAD_REGION | PH_LOAD_DEPTH | PH_REGION_GH | PH_DEPTH_GH | PH_STORE_LINK_GH);
+                       PH_LOAD_REGION | PH_LOAD_DEPTH | PH_REGION_GH | PH_DEPTH_GH | PH_STORE_LINK_GH | tex);
       if (rc) return rc;
       rc = LaunchStructure(ctx, 0, false);
       if (rc) return rc;
@@ -2507,10 +2521,7 @@ int m3tb_get_histograms(m3tb_ctx* ctx, int body, float* histogram_f, float* hist
 int m3tb_tracking_step(m3tb_ctx* ctx, int iteration, int n_corr_iterations, int n_update_iterations) {
   CHECK_CTX();
   if (n_corr_iterations < 0 || n_update_iterations < 0) return Fail(ctx, M3TB_ERR_INVALID, "negative iteration count");
-  if (HasStructures(ctx)) {
-    if (ctx->n_texture > 0) return Fail(ctx, M3TB_ERR_UNSUPPORTED, "texture modalities in kinematic structures");
-    return StructureStep(ctx, iteration, 0, n_corr_iterations, n_update_iterations);
-  }
+  if (HasStructures(ctx)) return StructureStep(ctx, iteration, 0, n_corr_iterations, n_update_iterations);
   const unsigned phases = PH_REGION_CORR | PH_DEPTH_CORR | PH_REGION_GH | PH_DEPTH_GH | PH_SOLVE | PH_STORE_REGION |
                           PH_STORE_DEPTH | (ctx->n_texture > 0 ? unsigned(PH_TEXTURE_GH) : 0u);
   if (ctx->n_attached == 0) return LaunchTrack(ctx, iteration, 0, n_corr_iterations, n_update_iterations, 0, phases);
@@ -2527,10 +2538,7 @@ int m3tb_tracking_step(m3tb_ctx* ctx, int iteration, int n_corr_iterations, int 
 int m3tb_corr_iteration(m3tb_ctx* ctx, int iteration, int corr_iteration, int n_update_iterations) {
   CHECK_CTX();
   if (corr_iteration < 0 || n_update_iterations < 0) return Fail(ctx, M3TB_ERR_INVALID, "negative iteration count");
-  if (HasStructures(ctx)) {
-    if (ctx->n_texture > 0) return Fail(ctx, M3TB_ERR_UNSUPPORTED, "texture modalities in kinematic structures");
-    return StructureStep(ctx, iteration, corr_iteration, corr_iteration + 1, n_update_iterations);
-  }
+  if (HasStructures(ctx)) return StructureStep(ctx, iteration, corr_iteration, corr_iteration + 1, n_update_iterations);
   if (ctx->n_attached > 0) {
     int rc = LaunchRender(ctx, kRenderAttached);
     if (!rc && corr_iteration == 0) rc = LaunchTexture(ctx, false, 1);

@@ -12,9 +12,9 @@
 //
 // Focused depth / silhouette renderers exist as device renderers (k_render), full depth / silhouette / normal
 // renderers and the normal viewers as k_view_*, model generation as DepthModel::GenerateModel (k_model_raster /
-// k_model_points) and RegionModel::GenerateModel (k_model_raster / k_region_contours / k_region_points). Everything
-// else the reference has outside this path (focused normal renderer, detectors, texture modality, YAML metafiles)
-// is out of scope here (DESIGN.md). Poses use a minimal Transform3fA (row-major 3x4).
+// k_model_points) and RegionModel::GenerateModel (k_model_raster / k_region_contours / k_region_points), the texture
+// modality as TextureModality (ORB; the caller detects the features). Everything else the reference has outside this
+// path (focused normal renderer, detectors, feature detection, YAML metafiles) is out of scope here (DESIGN.md). Poses use a minimal Transform3fA (row-major 3x4).
 #ifndef M3T_B200_HPP_
 #define M3T_B200_HPP_
 
@@ -71,7 +71,8 @@ class Batch {
   m3tb_ctx* ctx() const { return ctx_; }
   bool ok() const { return ctx_ != nullptr; }
 
-  enum PhaseKind { kRegionCorr, kDepthCorr, kRegionGH, kDepthGH, kOptimize, kStart, kResults, kRender, kNPhases };
+  enum PhaseKind { kRegionCorr, kDepthCorr, kRegionGH, kDepthGH, kOptimize, kStart, kResults, kRender, kTextureCorr,
+                   kTextureGH, kNPhases };
   struct Key {
     int iteration = -1, corr = -1, opt = -1;
     long pose_version = -1;
@@ -102,7 +103,7 @@ class Batch {
   long viewer_version() const { return viewer_version_; }
   int n_bodies() const { return n_bodies_; }
 
-  std::vector<float> region_g, region_h, depth_g, depth_h;  // last batched gradients / Hessians (all bodies)
+  std::vector<float> region_g, region_h, depth_g, depth_h, texture_g, texture_h;  // last batched gradients / Hessians (all bodies)
 
  private:
   m3tb_ctx* ctx_ = nullptr;
@@ -1137,7 +1138,7 @@ class Modality {
   const std::shared_ptr<Body>& body_ptr() const { return body_ptr_; }
   bool set_up() const { return set_up_; }
   // Modality::correspondence_renderer_ptrs (modality.h): what Tracker renders before CalculateCorrespondences
-  std::vector<std::shared_ptr<FocusedDepthRenderer>> correspondence_renderer_ptrs() const {
+  virtual std::vector<std::shared_ptr<FocusedDepthRenderer>> correspondence_renderer_ptrs() const {
     std::vector<std::shared_ptr<FocusedDepthRenderer>> out;
     if (depth_renderer_ptr_) out.push_back(depth_renderer_ptr_);
     if (silhouette_renderer_ptr_) out.push_back(silhouette_renderer_ptr_);
@@ -1394,6 +1395,155 @@ class DepthModality : public Modality {
   m3tb_depth_params params_;
   std::shared_ptr<DepthCamera> depth_camera_ptr_;
   std::shared_ptr<DepthModel> depth_model_ptr_;
+};
+
+// ---- texture_modality.h ------------------------------------------------------------------------------------------------
+// Feature detection stays with the caller (no OpenCV here): instead of DetectAndComputeCorrKeypoints the caller asks for
+// the body's focus region with CalculateFocus, detects ORB features in the cropped and scaled grey image and hands them
+// over with SetFeatures, once per frame. Only DescriptorType::ORB is implemented.
+class TextureModality : public Modality {
+ public:
+  enum class DescriptorType { BRISK = 0, DAISY = 1, FREAK = 2, SIFT = 3, ORB = 4, ORB_CUDA = 5 };  // texture_modality.h
+
+  TextureModality(const std::string& name, const std::shared_ptr<Batch>& batch, const std::shared_ptr<Body>& body_ptr,
+                  const std::shared_ptr<ColorCamera>& color_camera_ptr,
+                  const std::shared_ptr<FocusedSilhouetteRenderer>& silhouette_renderer_ptr)
+      : Modality(name, batch, body_ptr), color_camera_ptr_(color_camera_ptr) {
+    silhouette_renderer_ptr_ = silhouette_renderer_ptr;
+    m3tb_texture_params_default(&params_);
+  }
+  // setters of the reference (texture_modality.h:186-194, 218-226), same names
+  void set_descriptor_type(DescriptorType v) { descriptor_type_ = v; set_up_ = false; }
+  void set_focused_image_size(int v) { params_.focused_image_size = v; set_up_ = false; }
+  void set_descriptor_distance_threshold(float v) { params_.descriptor_distance_threshold = v; set_up_ = false; }
+  void set_tukey_norm_constant(float v) { params_.tukey_norm_constant = v; set_up_ = false; }
+  void set_standard_deviations(const std::vector<float>& v) {
+    params_.n_standard_deviations = int(v.size());
+    for (size_t i = 0; i < v.size() && i < M3TB_MAX_SCHEDULE; ++i) params_.standard_deviations[i] = v[i];
+    set_up_ = false;
+  }
+  void set_max_keyframe_rotation_difference(float v) { params_.max_keyframe_rotation_difference = v; set_up_ = false; }
+  void set_max_keyframe_age(int v) { params_.max_keyframe_age = v; set_up_ = false; }
+  void set_n_keyframes(int v) { params_.n_keyframes = v; set_up_ = false; }
+  void MeasureOcclusions(const std::shared_ptr<DepthCamera>& depth_camera_ptr) {
+    depth_camera_ptr_ = depth_camera_ptr; params_.measure_occlusions = 1; set_up_ = false;
+  }
+  void DoNotMeasureOcclusions() { depth_camera_ptr_ = nullptr; params_.measure_occlusions = 0; set_up_ = false; }
+  void ModelOcclusions(const std::shared_ptr<FocusedDepthRenderer>& depth_renderer_ptr) {
+    depth_renderer_ptr_ = depth_renderer_ptr; params_.model_occlusions = 1; set_up_ = false;
+  }
+  void DoNotModelOcclusions() { depth_renderer_ptr_ = nullptr; params_.model_occlusions = 0; set_up_ = false; }
+  void set_measured_occlusion_radius(float v) { params_.measured_occlusion_radius = v; set_up_ = false; }
+  void set_measured_occlusion_threshold(float v) { params_.measured_occlusion_threshold = v; set_up_ = false; }
+  void set_modeled_occlusion_radius(float v) { params_.modeled_occlusion_radius = v; set_up_ = false; }
+  void set_modeled_occlusion_threshold(float v) { params_.modeled_occlusion_threshold = v; set_up_ = false; }
+  DescriptorType descriptor_type() const { return descriptor_type_; }
+  const m3tb_texture_params& params() const { return params_; }
+  const std::shared_ptr<ColorCamera>& color_camera_ptr() const { return color_camera_ptr_; }
+  const std::shared_ptr<DepthCamera>& depth_camera_ptr() const { return depth_camera_ptr_; }
+  // the texture modality renders only for StartModality / CalculateResults (texture_modality.h)
+  std::vector<std::shared_ptr<FocusedDepthRenderer>> correspondence_renderer_ptrs() const override { return {}; }
+
+  // TextureModality::SetUp (texture_modality.cpp:39-88); the body's device record is written by Optimizer::SetUp
+  bool SetUp() override {
+    set_up_ = false;
+    if (descriptor_type_ != DescriptorType::ORB) {
+      std::cerr << "Modality " << name_ << ": only DescriptorType::ORB is implemented" << std::endl;
+      return false;
+    }
+    if (!silhouette_renderer_ptr_) {
+      std::cerr << "Modality " << name_ << " has no focused silhouette renderer" << std::endl;
+      return false;
+    }
+    if (!color_camera_ptr_) {
+      std::cerr << "Modality " << name_ << " has no color camera" << std::endl;
+      return false;
+    }
+    if (params_.measure_occlusions && !depth_camera_ptr_) {
+      std::cerr << "Modality " << name_ << " measures occlusions without a depth camera" << std::endl;
+      return false;
+    }
+    for (auto* r : {static_cast<FocusedDepthRenderer*>(silhouette_renderer_ptr_.get()), depth_renderer_ptr_.get()}) {
+      if (!r) continue;
+      if (!r->set_up()) {
+        std::cerr << "Focused renderer " << r->name() << " was not set up" << std::endl;
+        return false;
+      }
+      if (!r->IsBodyReferenced(body_ptr_->name())) {
+        std::cerr << "Focused renderer " << r->name() << " does not reference body " << body_ptr_->name() << std::endl;
+        return false;
+      }
+    }
+    if (silhouette_renderer_ptr_->id_type() != IDType::BODY) {
+      std::cerr << "Focused silhouette renderer " << silhouette_renderer_ptr_->name() << " does not use id_type BODY"
+                << std::endl;
+      return false;
+    }
+    set_up_ = true;
+    return true;
+  }
+
+  // The caller's detection hook. CalculateFocus: CalculateScaleAndRegionOfInterest from the current device pose,
+  // roi = (x, y, width, height) of the crop and the factor it is resized by; false when the reference skips detection.
+  bool CalculateFocus(std::array<int32_t, 4>* roi, float* scale) {
+    int32_t valid = 0;
+    if (!Check(batch_->ctx(), m3tb_get_texture_focus(batch_->ctx(), body_ptr_->index(), 1, roi->data(), scale, &valid),
+               "TextureModality::CalculateFocus"))
+      return false;
+    return valid != 0;
+  }
+  // SetFeatures: the keypoints (x, y in crop coordinates, keypoints_xy[2 n]) and 32-byte ORB descriptors
+  // (descriptors[32 n]) detected in the crop of CalculateFocus
+  bool SetFeatures(const std::vector<float>& keypoints_xy, const std::vector<uint8_t>& descriptors,
+                   const std::array<int32_t, 4>& roi, float scale) {
+    const int n = int(keypoints_xy.size() / 2);
+    if (descriptors.size() != size_t(32) * n) {
+      std::cerr << "Modality " << name_ << ": one 32-byte descriptor per keypoint" << std::endl;
+      return false;
+    }
+    return Check(batch_->ctx(),
+                 m3tb_upload_texture_features(batch_->ctx(), body_ptr_->index(), keypoints_xy.data(), descriptors.data(), n,
+                                              roi[0], roi[1], scale),
+                 "TextureModality::SetFeatures");
+  }
+
+  bool StartModality(int iteration, int corr_iteration) override {
+    if (!IsSetup()) return false;
+    (void)corr_iteration;
+    if (!batch_->Claim(Batch::kStart, iteration, 0, 0)) return true;
+    return Check(batch_->ctx(), m3tb_start_modalities(batch_->ctx(), iteration), "TextureModality::StartModality");
+  }
+  bool CalculateCorrespondences(int iteration, int corr_iteration) override {
+    if (!IsSetup()) return false;
+    if (!batch_->Claim(Batch::kTextureCorr, iteration, corr_iteration, 0)) return true;
+    return Check(batch_->ctx(), m3tb_texture_correspondences(batch_->ctx(), iteration, corr_iteration),
+                 "TextureModality::CalculateCorrespondences");
+  }
+  bool CalculateGradientAndHessian(int iteration, int corr_iteration, int opt_iteration) override {
+    if (!IsSetup()) return false;
+    if (batch_->Claim(Batch::kTextureGH, iteration, corr_iteration, opt_iteration)) {
+      batch_->texture_g.resize(size_t(6) * batch_->n_bodies());
+      batch_->texture_h.resize(size_t(36) * batch_->n_bodies());
+      if (!Check(batch_->ctx(),
+                 m3tb_texture_gradient_hessian(batch_->ctx(), iteration, corr_iteration, opt_iteration,
+                                               batch_->texture_g.data(), batch_->texture_h.data()),
+                 "TextureModality::CalculateGradientAndHessian"))
+        return false;
+    }
+    FetchGH(batch_->texture_g, batch_->texture_h);
+    return true;
+  }
+  bool CalculateResults(int iteration) override {
+    if (!IsSetup()) return false;
+    if (!batch_->Claim(Batch::kResults, iteration, 0, 0)) return true;
+    return Check(batch_->ctx(), m3tb_calculate_results(batch_->ctx(), iteration), "TextureModality::CalculateResults");
+  }
+
+ private:
+  m3tb_texture_params params_;
+  DescriptorType descriptor_type_ = DescriptorType::ORB;
+  std::shared_ptr<ColorCamera> color_camera_ptr_;
+  std::shared_ptr<DepthCamera> depth_camera_ptr_;  // MeasureOcclusions
 };
 
 // ---- link.h: one node of a kinematic tree (M3T/include/m3t/link.h) ---------------------------------------------------------
@@ -1676,6 +1826,7 @@ class Optimizer {
     const m3tb_depth_params* dp = nullptr;
     int rmodel = 0, dmodel = 0, ccam = 0, dcam = 0;
     std::shared_ptr<ColorHistograms> shared;
+    std::shared_ptr<TextureModality> texture;
     for (auto& m : link.modality_ptrs()) {
       if (!m->set_up()) {
         std::cerr << "Modality " << m->name() << " was not set up" << std::endl;
@@ -1690,14 +1841,31 @@ class Optimizer {
         dp = &d->params();
         dmodel = d->depth_model_ptr()->index();
         dcam = d->depth_camera_ptr()->index();
+      } else if (auto t = std::dynamic_pointer_cast<TextureModality>(m)) {
+        texture = t;
       }
     }
+    if (texture && texture->depth_camera_ptr() && !dp) dcam = texture->depth_camera_ptr()->index();  // MeasureOcclusions
     const int body = link.body_ptr()->index();
     if (!Check(batch_->ctx(), m3tb_set_body(batch_->ctx(), body, rp, dp, &params_, rmodel, dmodel, ccam, dcam), "Optimizer::SetUp"))
       return false;
+    // the texture modality before its renderers are attached; removed from the device when it left the link
+    auto was_textured = std::find(texture_bodies_.begin(), texture_bodies_.end(), body);
+    if (texture) {
+      if (!Check(batch_->ctx(),
+                 m3tb_set_texture_modality(batch_->ctx(), body, &texture->params(), texture->color_camera_ptr()->index()),
+                 "TextureModality::SetUp"))
+        return false;
+      if (was_textured == texture_bodies_.end()) texture_bodies_.push_back(body);
+    } else if (was_textured != texture_bodies_.end()) {
+      if (!Check(batch_->ctx(), m3tb_set_texture_modality(batch_->ctx(), body, nullptr, 0), "Link::DeleteModality"))
+        return false;
+      texture_bodies_.erase(was_textured);
+    }
     // the modalities' renderers feed the body's renderer slots (-1: none, detaches an earlier one)
     for (auto& m : link.modality_ptrs()) {
-      const int modality = std::dynamic_pointer_cast<RegionModality>(m) ? 0 : 1;
+      const int modality =
+          std::dynamic_pointer_cast<RegionModality>(m) ? 0 : std::dynamic_pointer_cast<TextureModality>(m) ? 2 : 1;
       const int dr = m->depth_renderer_ptr() ? m->depth_renderer_ptr()->index() : -1;
       const int sr = m->silhouette_renderer_ptr() ? m->silhouette_renderer_ptr()->index() : -1;
       if (!Check(batch_->ctx(), m3tb_attach_renderer(batch_->ctx(), body, modality, 0, dr), "Modality::ModelOcclusions") ||
@@ -1779,6 +1947,7 @@ class Optimizer {
   std::vector<std::shared_ptr<SoftConstraint>> soft_constraint_ptrs_;
   m3tb_optimizer_params params_{};
   std::vector<int> shared_bodies_;  // bodies whose region modality was set up with a shared ColorHistograms object
+  std::vector<int> texture_bodies_;  // bodies whose texture modality this optimizer set on the device
   int structure_index_ = -1;
   bool set_up_ = false;
 };

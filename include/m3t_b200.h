@@ -478,7 +478,8 @@ int m3tb_share_color_histograms(m3tb_ctx* ctx, int body, int owner_body);
  * device silhouette renderer with the occlusion checks, Hamming kNN matching with the ratio test, the Tukey-weighted
  * reprojection gradient / Hessian in every update (inside k_track, added to the link after region and depth) and the
  * keyframe refresh. Bodies with a texture modality are tracked by k_track; contexts without one launch what they
- * launched before. Not supported in kinematic structures (M3TB_ERR_UNSUPPORTED from the tracking calls). */
+ * launched before. A texture body may be the body of a link of a kinematic structure, or one of its extra bodies with
+ * its own texture modality on its own camera (see m3tb_set_structure for the order of the link's sum). */
 /* TextureModality + SetUp for body `body` (set with m3tb_set_body and m3tb_set_body_geometry, whose
  * maximum_body_diameter the focus region uses) on colour camera `color_camera`; NULL params remove the modality and
  * detach its renderers. Setting it again starts with an empty keyframe deque. M3TB_ERR_UNSUPPORTED for a descriptor
@@ -559,6 +560,11 @@ int m3tb_calculate_optimization(m3tb_ctx* ctx, int iteration, int corr_iteration
  * Optimizer::CalculateOptimization per structure: Link::CalculateJacobian (link.cpp:159-182), SoftConstraint::
  * AddGradientsAndHessiansToLinks (soft_constraint.cpp:113-131), Constraint::CalculateResidualAndConstraintJacobian
  * (constraint.cpp:81-103), the (DoF + nc)^2 LDLT (optimizer.cpp:144-167) and Link::UpdatePoses (link.cpp:205-241).
+ * A link's gradient / Hessian (Link::CalculateGradientAndHessian, link.cpp:184-193) is the sum over its modality sets:
+ * its body's region, depth and texture terms (texture only where the body has a texture modality), then each extra
+ * body's in the same order. An extra body is the same physical body seen by another camera set and may carry its own
+ * texture modality on its own colour camera. With texture bodies, each update is one k_track launch (region, depth and
+ * texture terms) and one k_structure launch; the texture match runs once per frame, at correspondence iteration 0.
  * Like Optimizer::SetUp, setting a structure makes the poses consistent (UpdatePoses with theta = 0). */
 int m3tb_set_structure(m3tb_ctx* ctx, int structure, const m3tb_link* links, int n_links,
                        const m3tb_constraint* constraints, int n_constraints, const m3tb_optimizer_params* optimizer);
