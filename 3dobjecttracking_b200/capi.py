@@ -80,6 +80,9 @@ class Constraint(C.Structure):
                 ("standard_deviation_rotation", C.c_float), ("standard_deviation_translation", C.c_float)]
 
 
+DESCRIPTOR_DAISY, DESCRIPTOR_SIFT, DESCRIPTOR_ORB = 1, 3, 4  # M3TB_DESCRIPTOR_*
+
+
 def texture_params_default():
     p = TextureParams()
     lib().m3tb_texture_params_default(C.byref(p))
@@ -129,6 +132,7 @@ SYMBOLS = [
     "m3tb_update_viewers", "m3tb_get_viewer_image", "m3tb_set_full_renderer", "m3tb_render_full",
     "m3tb_get_full_rendering", "m3tb_undistortion_map", "m3tb_set_camera_undistortion", "m3tb_get_camera_image",
     "m3tb_texture_params_default", "m3tb_set_texture_modality", "m3tb_get_texture_focus", "m3tb_upload_texture_features",
+    "m3tb_upload_texture_float_features",
     "m3tb_texture_correspondences", "m3tb_texture_gradient_hessian", "m3tb_get_texture_points",
     "m3tb_get_texture_keyframes",
 ]
@@ -252,6 +256,7 @@ def lib():
     L.m3tb_set_texture_modality.argtypes = [vp, ci, C.POINTER(TextureParams), ci]
     L.m3tb_get_texture_focus.argtypes = [vp, ci, ci, ip, fp, ip]
     L.m3tb_upload_texture_features.argtypes = [vp, ci, fp, vp, ci, ci, ci, C.c_float]
+    L.m3tb_upload_texture_float_features.argtypes = [vp, ci, fp, fp, ci, ci, ci, ci, C.c_float]
     L.m3tb_texture_correspondences.argtypes = [vp, ci, ci]
     L.m3tb_texture_gradient_hessian.argtypes = [vp, ci, ci, ci, fp, fp]
     L.m3tb_get_texture_points.argtypes = [vp, ci, vp, ci, C.POINTER(ci)]
@@ -388,6 +393,7 @@ class Context:
             raise M3TBError(f"m3tb_create failed with status {rc} (no usable sm_90 CUDA device?)")
         self.h = h
         self.n_bodies = 0
+        self._texture_length = {}  # SIFT / DAISY bodies: descriptor length of their uploads (0 before the first)
         if stream is not None:
             self.set_stream(stream)
 
@@ -825,6 +831,9 @@ class Context:
         """params: TextureParams (None removes the modality)."""
         self._ck(self.L.m3tb_set_texture_modality(self.h, body, C.byref(params) if params is not None else None,
                                                   color_camera))
+        self._texture_length.pop(body, None)
+        if params is not None and params.descriptor_type in (DESCRIPTOR_DAISY, DESCRIPTOR_SIFT):
+            self._texture_length[body] = 0
 
     def get_texture_focus(self, first=0, count=None):
         """(roi [count, 4] int32 x, y, width, height; scale [count] float32; valid [count] bool)."""
@@ -838,8 +847,17 @@ class Context:
         return roi[:count], scale[:count], valid[:count].astype(bool)
 
     def upload_texture_features(self, body, keypoints_xy, descriptors, roi_x, roi_y, scale):
-        """keypoints_xy [n, 2] float32 in crop coordinates, descriptors [n, 32] uint8."""
+        """keypoints_xy [n, 2] float32 in crop coordinates; descriptors [n, 32] uint8 (ORB) or [n, length] float32
+        (SIFT / DAISY, m3tb_upload_texture_float_features)."""
         xy = np.ascontiguousarray(np.asarray(keypoints_xy, np.float32).reshape(-1, 2))
+        if isinstance(descriptors, np.ndarray) and descriptors.dtype == np.float32:
+            d = np.ascontiguousarray(descriptors)
+            assert d.ndim == 2, "float descriptors are [n, length]"
+            self._ck(self.L.m3tb_upload_texture_float_features(self.h, body, _p(xy), _p(d), xy.shape[0], d.shape[1],
+                                                               int(roi_x), int(roi_y), float(scale)))
+            if self._texture_length.get(body) == 0:
+                self._texture_length[body] = d.shape[1]
+            return
         d = np.ascontiguousarray(np.asarray(descriptors, np.uint8).reshape(-1, 32))
         self._ck(self.L.m3tb_upload_texture_features(self.h, body, _p(xy), d.ctypes.data_as(C.c_void_p), xy.shape[0],
                                                      int(roi_x), int(roi_y), float(scale)))
@@ -860,11 +878,13 @@ class Context:
         return out[:min(n.value, capacity)]
 
     def get_texture_keyframes(self, body, capacity=4096):
-        """dict(sizes [n_keyframes], points [total, 3] float32, descriptors [total, 32] uint8, age, orientation [3])."""
+        """dict(sizes [n_keyframes], points [total, 3] float32, descriptors, age, orientation [3]). descriptors:
+        [total, 32] uint8 for ORB; [total, length] float32 for a SIFT / DAISY body, length that of its uploads."""
+        length = self._texture_length.get(body)
         nk, age = C.c_int(0), C.c_int(0)
         sizes = np.zeros(8, np.int32)
         pts = np.zeros((capacity, 3), np.float32)
-        desc = np.zeros((capacity, 32), np.uint8)
+        desc = np.zeros((capacity, 32), np.uint8) if length is None else np.zeros((capacity, length), np.float32)
         o = np.zeros(3, np.float32)
         self._ck(self.L.m3tb_get_texture_keyframes(self.h, body, C.byref(nk), sizes.ctypes.data_as(C.POINTER(C.c_int)),
                                                    _p(pts), desc.ctypes.data_as(C.c_void_p), capacity, C.byref(age),

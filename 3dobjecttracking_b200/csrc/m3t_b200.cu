@@ -269,6 +269,10 @@ struct m3tb_ctx {
   DeviceBuffer<int> d_tex_nfeat, d_tex_kf_n, d_tex_counts;
   DeviceBuffer<float> d_tex_kf_points, d_tex_points, d_tex_pose, d_gh_texture;
   DeviceBuffer<TexKeyframeState> d_tex_kf_state;
+  // float descriptors (SIFT / DAISY) and k_texture_knn_l2's matches: made by the first m3tb_set_texture_modality with
+  // an L2 descriptor type, never for contexts with ORB bodies only
+  DeviceBuffer<float> d_tex_fdesc, d_tex_kf_fdesc;
+  DeviceBuffer<int> d_tex_knn;
 };
 
 namespace {
@@ -3931,10 +3935,26 @@ void m3tb_texture_params_default(m3tb_texture_params* p) {
 
 namespace {
 
-// The texture tables for max_bodies, all or nothing (first m3tb_set_texture_modality)
-int EnsureTextureTables(m3tb_ctx* ctx) {
-  if (ctx->d_tex_xy) return M3TB_OK;
+// The texture tables for max_bodies, all or nothing (first m3tb_set_texture_modality); with l2 also the float
+// descriptor tables (first L2 descriptor type), in the same all-or-nothing step
+int EnsureTextureTables(m3tb_ctx* ctx, bool l2) {
   const size_t nb = size_t(ctx->max_bodies);
+  DeviceBuffer<float> fdesc, kf_fdesc;
+  DeviceBuffer<int> knn;
+  if (l2 && !ctx->d_tex_fdesc) {
+    CU(fdesc.create(nb * kTexMaxFeatures * kTexMaxFloatDesc));
+    CU(kf_fdesc.create(nb * kTexMaxKeyframes * kTexMaxFeatures * kTexMaxFloatDesc));
+    CU(knn.create(nb * kTexMaxKeyframes * kTexMaxFeatures));
+    if (!ctx->d_tex_xy) {
+      int rc = EnsureTextureTables(ctx, false);
+      if (rc) return rc;
+    }
+    ctx->d_tex_fdesc = std::move(fdesc);
+    ctx->d_tex_kf_fdesc = std::move(kf_fdesc);
+    ctx->d_tex_knn = std::move(knn);
+    return M3TB_OK;
+  }
+  if (ctx->d_tex_xy) return M3TB_OK;
   DeviceBuffer<float2> xy;
   DeviceBuffer<uint32_t> desc, kf_desc;
   DeviceBuffer<int> nfeat, kf_n, counts;
@@ -4007,7 +4027,8 @@ int SyncTextureFeatures(m3tb_ctx* ctx) {
   return M3TB_OK;
 }
 
-// k_texture_keyframe (keyframe = true) or k_texture_match over every body; mode as TextureArgs::mode
+// k_texture_keyframe (keyframe = true) or k_texture_match over every body; mode as TextureArgs::mode. Matching
+// (mode 1) first runs k_texture_knn_l2 when an L2 body has keyframe descriptors to match.
 int LaunchTexture(m3tb_ctx* ctx, bool keyframe, int mode) {
   if (ctx->n_texture == 0) return M3TB_OK;
   int rc = ValidateTexture(ctx);
@@ -4025,11 +4046,28 @@ int LaunchTexture(m3tb_ctx* ctx, bool keyframe, int mode) {
   a.feat_n = ctx->d_tex_nfeat;
   a.kf_points = ctx->d_tex_kf_points;
   a.kf_desc = ctx->d_tex_kf_desc;
+  a.feat_fdesc = ctx->d_tex_fdesc;
+  a.kf_fdesc = ctx->d_tex_kf_fdesc;
+  a.knn = ctx->d_tex_knn;
   a.kf_n = ctx->d_tex_kf_n;
   a.kf_state = ctx->d_tex_kf_state;
   a.points = ctx->d_tex_points;
   a.counts = ctx->d_tex_counts;
   a.mode = mode;
+  int l2_length = 0, l2_keyframes = 0;  // the longest descriptor and deque of the L2 bodies
+  for (int b = 0; b < ctx->n_bodies; ++b) {
+    const BodyDev& B = ctx->h_bodies[b];
+    if (!B.set || !B.has_texture || !B.tp.l2) continue;
+    l2_length = std::max(l2_length, B.tp.descriptor_length);
+    l2_keyframes = std::max(l2_keyframes, B.tp.n_keyframes);
+  }
+  if (!keyframe && mode == 1 && l2_length > 0) {  // a body without a length has no features, hence no keyframe points
+    CU(cudaFuncSetAttribute(k_texture_knn_l2, cudaFuncAttributeMaxDynamicSharedMemorySize, KnnSharedBytes(l2_length)));
+    const dim3 grid(kKnnSplits * l2_keyframes * (kTexMaxFeatures / kKnnQueries), ctx->n_bodies);
+    k_texture_knn_l2<<<grid, kKnnThreads, KnnSharedBytes(l2_length), ctx->stream>>>(a);
+    CU(cudaGetLastError());
+    ctx->launches++;
+  }
   if (keyframe) k_texture_keyframe<<<ctx->n_bodies, kTexThreads, 0, ctx->stream>>>(a);
   else k_texture_match<<<ctx->n_bodies, kTexThreads, 0, ctx->stream>>>(a);
   CU(cudaGetLastError());
@@ -4067,8 +4105,9 @@ int m3tb_set_texture_modality(m3tb_ctx* ctx, int body, const m3tb_texture_params
     return M3TB_OK;
   }
   const m3tb_texture_params& p = *params;
-  if (p.descriptor_type != M3TB_DESCRIPTOR_ORB)
-    return Fail(ctx, M3TB_ERR_UNSUPPORTED, "only DescriptorType::ORB (32-byte descriptors, NORM_HAMMING) is implemented");
+  const bool l2 = p.descriptor_type == M3TB_DESCRIPTOR_SIFT || p.descriptor_type == M3TB_DESCRIPTOR_DAISY;
+  if (p.descriptor_type != M3TB_DESCRIPTOR_ORB && !l2)
+    return Fail(ctx, M3TB_ERR_UNSUPPORTED, "only DescriptorType::ORB (NORM_HAMMING), SIFT and DAISY (NORM_L2) are implemented");
   if (p.n_keyframes > kTexMaxKeyframes) return Fail(ctx, M3TB_ERR_UNSUPPORTED, "n_keyframes above 8");
   if (color_camera < 0 || color_camera >= ctx->max_cameras || !ctx->h_ccams[color_camera].set)
     return Fail(ctx, M3TB_ERR_INVALID, "color camera not set");
@@ -4083,7 +4122,7 @@ int m3tb_set_texture_modality(m3tb_ctx* ctx, int body, const m3tb_texture_params
     return Fail(ctx, M3TB_ERR_INVALID, "measure_occlusions needs the body's depth camera");
   if (!ctx->h_geometry[body].set)
     return Fail(ctx, M3TB_ERR_INVALID, "the texture modality needs the body's geometry (m3tb_set_body_geometry)");
-  int rc = EnsureTextureTables(ctx);
+  int rc = EnsureTextureTables(ctx, l2);
   if (rc) return rc;
   CU(cudaStreamSynchronize(ctx->stream));  // a launch in flight may still read this body's keyframes
   CU(cudaMemsetAsync(ctx->d_tex_kf_state + body, 0, sizeof(TexKeyframeState), ctx->stream));
@@ -4104,6 +4143,9 @@ int m3tb_set_texture_modality(m3tb_ctx* ctx, int body, const m3tb_texture_params
   t.model_occlusions = p.model_occlusions ? 1 : 0;
   t.modeled_occlusion_radius = p.modeled_occlusion_radius;
   t.modeled_occlusion_threshold = p.modeled_occlusion_threshold;
+  t.l2 = l2 ? 1 : 0;
+  t.descriptor_type = p.descriptor_type;
+  t.descriptor_length = 0;  // the next upload fixes it
   if (B.has_texture && B.texture_camera != color_camera)  // renderers of the old camera no longer fit
     for (int slot = RS_TEXTURE_SILHOUETTE; slot < RS_COUNT; ++slot)
       if (ctx->attached[body][slot] >= 0) {
@@ -4169,14 +4211,32 @@ int m3tb_get_texture_focus(m3tb_ctx* ctx, int first, int count, int32_t* roi, fl
   return M3TB_OK;
 }
 
-int m3tb_upload_texture_features(m3tb_ctx* ctx, int body, const float* keypoints_xy, const uint8_t* descriptors, int n,
-                                 int roi_x, int roi_y, float scale) {
-  CHECK_CTX();
+}  // extern "C"
+
+namespace {
+
+// m3tb_upload_texture_features (l2 false: 32-byte rows) and m3tb_upload_texture_float_features (l2 true: rows of
+// `length` floats)
+int UploadTextureFeatures(m3tb_ctx* ctx, int body, const float* keypoints_xy, const void* descriptors, bool l2, int n,
+                          int length, int roi_x, int roi_y, float scale) {
   int rc = CheckTextureBody(ctx, body);
   if (rc) return rc;
   if (n > kTexMaxFeatures) return Fail(ctx, M3TB_ERR_UNSUPPORTED, "more than 512 features per body");
   if (n < 0 || (n > 0 && (!keypoints_xy || !descriptors)) || !(scale > 0.0f) || !std::isfinite(scale))
     return Fail(ctx, M3TB_ERR_INVALID, "bad feature arguments");
+  TextureParamsDev& tp = ctx->h_bodies[body].tp;
+  const float* float_descriptors = static_cast<const float*>(descriptors);
+  if (l2 != (tp.l2 != 0))
+    return Fail(ctx, M3TB_ERR_INVALID, tp.l2 ? "SIFT / DAISY descriptors are uploaded as floats"
+                                             : "ORB descriptors are uploaded as 32-byte rows");
+  if (l2) {
+    if (tp.descriptor_type == M3TB_DESCRIPTOR_SIFT ? length != 128 : (length < 1 || length > kTexMaxFloatDesc))
+      return Fail(ctx, M3TB_ERR_INVALID, "descriptor length: 128 for SIFT, 1 .. 256 for DAISY");
+    if (tp.descriptor_length != 0 && length != tp.descriptor_length)
+      return Fail(ctx, M3TB_ERR_INVALID, "descriptor length differs from the first upload's");
+    for (size_t k = 0; k < size_t(n) * length; ++k)
+      if (!std::isfinite(float_descriptors[k])) return Fail(ctx, M3TB_ERR_INVALID, "non-finite descriptor");
+  }
   // DetectAndComputeCorrKeypoints adds the focus offset (texture_modality.cpp:884-887)
   std::vector<float2> xy(size_t(std::max(n, 1)));
   for (int i = 0; i < n; ++i) {
@@ -4186,13 +4246,38 @@ int m3tb_upload_texture_features(m3tb_ctx* ctx, int body, const float* keypoints
   if (n > 0) {
     CU(cudaMemcpyAsync(ctx->d_tex_xy + size_t(body) * kTexMaxFeatures, xy.data(), sizeof(float2) * n,
                        cudaMemcpyHostToDevice, ctx->stream));
-    CU(cudaMemcpyAsync(ctx->d_tex_desc + size_t(body) * kTexMaxFeatures * kTexDescWords, descriptors, size_t(32) * n,
-                       cudaMemcpyHostToDevice, ctx->stream));
+    if (l2)
+      CU(cudaMemcpy2DAsync(ctx->d_tex_fdesc + size_t(body) * kTexMaxFeatures * kTexMaxFloatDesc,
+                           sizeof(float) * kTexMaxFloatDesc, float_descriptors, sizeof(float) * length,
+                           sizeof(float) * length, n, cudaMemcpyHostToDevice, ctx->stream));
+    else
+      CU(cudaMemcpyAsync(ctx->d_tex_desc + size_t(body) * kTexMaxFeatures * kTexDescWords, descriptors, size_t(32) * n,
+                         cudaMemcpyHostToDevice, ctx->stream));
   }
   CU(cudaMemcpyAsync(ctx->d_tex_nfeat + body, &n, sizeof(int), cudaMemcpyHostToDevice, ctx->stream));
   CU(cudaStreamSynchronize(ctx->stream));  // xy and n are on this stack frame
   ctx->tex_feat_gen[body] = ctx->h_ccams[ctx->h_bodies[body].texture_camera].generation;
+  if (l2 && tp.descriptor_length == 0) {
+    tp.descriptor_length = length;
+    ctx->bodies_dirty = true;
+  }
   return M3TB_OK;
+}
+
+}  // namespace
+
+extern "C" {
+
+int m3tb_upload_texture_features(m3tb_ctx* ctx, int body, const float* keypoints_xy, const uint8_t* descriptors, int n,
+                                 int roi_x, int roi_y, float scale) {
+  CHECK_CTX();
+  return UploadTextureFeatures(ctx, body, keypoints_xy, descriptors, false, n, 0, roi_x, roi_y, scale);
+}
+
+int m3tb_upload_texture_float_features(m3tb_ctx* ctx, int body, const float* keypoints_xy, const float* descriptors,
+                                       int n, int length, int roi_x, int roi_y, float scale) {
+  CHECK_CTX();
+  return UploadTextureFeatures(ctx, body, keypoints_xy, descriptors, true, n, length, roi_x, roi_y, scale);
 }
 
 int m3tb_texture_correspondences(m3tb_ctx* ctx, int iteration, int corr_iteration) {
@@ -4249,16 +4334,21 @@ int m3tb_get_texture_keyframes(m3tb_ctx* ctx, int body, int* n_keyframes, int* s
   if (rc) return rc;
   if (capacity < 0) return Fail(ctx, M3TB_ERR_INVALID, "bad capacity");
   TexKeyframeState st;
+  const TextureParamsDev& tp = ctx->h_bodies[body].tp;
+  // a descriptor is `width` bytes in rows of `stride` words: 32 of 8 for ORB, 4 * length of kTexMaxFloatDesc for L2
+  const int stride = tp.l2 ? kTexMaxFloatDesc : kTexDescWords;
+  const size_t width = tp.l2 ? sizeof(float) * tp.descriptor_length : 32;
   std::vector<int> kn(kTexMaxKeyframes);
   std::vector<float> kp(size_t(kTexMaxKeyframes) * 3 * kTexMaxFeatures);
-  std::vector<uint32_t> kd(size_t(kTexMaxKeyframes) * kTexMaxFeatures * kTexDescWords);
+  std::vector<uint32_t> kd(size_t(kTexMaxKeyframes) * kTexMaxFeatures * stride);
+  const uint32_t* kd_src = tp.l2 ? reinterpret_cast<const uint32_t*>(ctx->d_tex_kf_fdesc.get()) : ctx->d_tex_kf_desc.get();
   CU(cudaMemcpyAsync(&st, ctx->d_tex_kf_state + body, sizeof(st), cudaMemcpyDeviceToHost, ctx->stream));
   CU(cudaMemcpyAsync(kn.data(), ctx->d_tex_kf_n + body * kTexMaxKeyframes, sizeof(int) * kn.size(), cudaMemcpyDeviceToHost,
                      ctx->stream));
   CU(cudaMemcpyAsync(kp.data(), ctx->d_tex_kf_points + size_t(body) * kp.size(), sizeof(float) * kp.size(),
                      cudaMemcpyDeviceToHost, ctx->stream));
-  CU(cudaMemcpyAsync(kd.data(), ctx->d_tex_kf_desc + size_t(body) * kd.size(), sizeof(uint32_t) * kd.size(),
-                     cudaMemcpyDeviceToHost, ctx->stream));
+  CU(cudaMemcpyAsync(kd.data(), kd_src + size_t(body) * kd.size(), sizeof(uint32_t) * kd.size(), cudaMemcpyDeviceToHost,
+                     ctx->stream));
   CU(cudaStreamSynchronize(ctx->stream));
   if (n_keyframes) *n_keyframes = st.size;
   if (age) *age = st.age;
@@ -4271,7 +4361,7 @@ int m3tb_get_texture_keyframes(m3tb_ctx* ctx, int body, int* n_keyframes, int* s
       if (points)
         for (int c = 0; c < 3; ++c) points[3 * written + c] = kp[(size_t(slot) * 3 + c) * kTexMaxFeatures + i];
       if (descriptors)
-        std::memcpy(descriptors + size_t(32) * written, kd.data() + (size_t(slot) * kTexMaxFeatures + i) * kTexDescWords, 32);
+        std::memcpy(descriptors + width * written, kd.data() + (size_t(slot) * kTexMaxFeatures + i) * stride, width);
     }
   }
   return M3TB_OK;

@@ -1,7 +1,11 @@
-// m3t_b200_texture.cu — k_texture_keyframe and k_texture_match (TextureModality, texture_modality.cpp).
-// One CTA of kTexThreads threads per body; bodies without a texture modality return at once.
+// m3t_b200_texture.cu — k_texture_keyframe, k_texture_knn_l2 and k_texture_match (TextureModality,
+// texture_modality.cpp). k_texture_keyframe / k_texture_match: one CTA of kTexThreads threads per body;
+// k_texture_knn_l2: clusters over a body's queries (m3t_b200_texture.cuh). Bodies without a texture modality return
+// at once.
+#include <cfloat>
 #include <climits>
 
+#include <cooperative_groups.h>
 #include <cuda_runtime.h>
 
 #include "m3t_b200_texture.cuh"
@@ -153,10 +157,16 @@ __global__ void __launch_bounds__(kTexThreads) k_texture_keyframe(const __grid_c
   const bool modeled = tp.model_occlusions && mdep.image != nullptr && mdep.visible;
   const int n = a.feat_n[b];
   const float2* xy = a.feat_xy + size_t(b) * kTexMaxFeatures;
-  const uint32_t* desc = a.feat_desc + size_t(b) * kTexMaxFeatures * kTexDescWords;
+  // a descriptor is `words` 32-bit words in rows of `stride`: 8 of 8 for ORB, descriptor_length floats of
+  // kTexMaxFloatDesc for SIFT / DAISY
+  const bool l2 = tp.l2 != 0;
+  const int words = l2 ? tp.descriptor_length : kTexDescWords, stride = l2 ? kTexMaxFloatDesc : kTexDescWords;
+  const uint32_t* desc = l2 ? reinterpret_cast<const uint32_t*>(a.feat_fdesc) : a.feat_desc;
+  desc += size_t(b) * kTexMaxFeatures * stride;
   const int slot = s_slot;
   float* kp = a.kf_points + (size_t(b) * kTexMaxKeyframes + slot) * 3 * kTexMaxFeatures;
-  uint32_t* kd = a.kf_desc + (size_t(b) * kTexMaxKeyframes + slot) * kTexMaxFeatures * kTexDescWords;
+  uint32_t* kd = l2 ? reinterpret_cast<uint32_t*>(a.kf_fdesc) : a.kf_desc;
+  kd += (size_t(b) * kTexMaxKeyframes + slot) * kTexMaxFeatures * stride;
   int written = 0;
   for (int i0 = 0; i0 < n; i0 += kTexThreads) {
     const int i = i0 + tid;
@@ -184,7 +194,7 @@ __global__ void __launch_bounds__(kTexThreads) k_texture_keyframe(const __grid_c
       kp[0 * kTexMaxFeatures + pos] = px;
       kp[1 * kTexMaxFeatures + pos] = py;
       kp[2 * kTexMaxFeatures + pos] = pz;
-      for (int w = 0; w < kTexDescWords; ++w) kd[size_t(pos) * kTexDescWords + w] = desc[size_t(i) * kTexDescWords + w];
+      for (int w = 0; w < words; ++w) kd[size_t(pos) * stride + w] = desc[size_t(i) * stride + w];
     }
     written += total;
   }
@@ -196,10 +206,153 @@ __global__ void __launch_bounds__(kTexThreads) k_texture_keyframe(const __grid_c
   }
 }
 
+namespace {
+
+// A top-2 list under (distance, train index) order, best first; empty entries are (FLT_MAX, INT_MAX), which every
+// candidate that can enter (a finite distance below FLT_MAX) precedes.
+struct Top2 {
+  float d0, d1;
+  int i0, i1;
+};
+
+__device__ __forceinline__ bool Precedes(float da, int ia, float db, int ib) { return da < db || (da == db && ia < ib); }
+
+// cv::batchDistance's K = 2 insertion for candidates in increasing train index: a distance enters only if strictly
+// below the second (so NaN and inf never enter), and ties keep the earlier index
+__device__ __forceinline__ void Insert(Top2& t, float d, int j) {
+  if (d < t.d1) {
+    if (d < t.d0) { t.d1 = t.d0; t.i1 = t.i0; t.d0 = d; t.i0 = j; }
+    else { t.d1 = d; t.i1 = j; }
+  }
+}
+
+// The two first of the union of two lists with distinct indices: what the insertion gives over both index ranges
+__device__ __forceinline__ Top2 Merge(const Top2& a, const Top2& b) {
+  Top2 r;
+  if (Precedes(b.d0, b.i0, a.d0, a.i0)) {
+    r.d0 = b.d0; r.i0 = b.i0;
+    if (Precedes(b.d1, b.i1, a.d0, a.i0)) { r.d1 = b.d1; r.i1 = b.i1; }
+    else { r.d1 = a.d0; r.i1 = a.i0; }
+  } else {
+    r.d0 = a.d0; r.i0 = a.i0;
+    if (Precedes(b.d0, b.i0, a.d1, a.i1)) { r.d1 = b.d0; r.i1 = b.i0; }
+    else { r.d1 = a.d1; r.i1 = a.i1; }
+  }
+  return r;
+}
+
+// rows [0, n) of a [rows][kTexMaxFloatDesc] table into shared rows of `stride` floats: the first `length` floats,
+// zero up to the next multiple of 4 and in rows [n, rows)
+__device__ __forceinline__ void StageRows(const float* src, int n, int rows, int length, int stride, float* dst) {
+  const int d4 = (length + 3) / 4;
+  for (int e = threadIdx.x; e < rows * d4; e += kKnnThreads) {
+    const int r = e / d4, c = e - r * d4;
+    float4 v = make_float4(0.0f, 0.0f, 0.0f, 0.0f);
+    if (r < n) {
+      v = *reinterpret_cast<const float4*>(src + size_t(r) * kTexMaxFloatDesc + 4 * c);
+      const int k = 4 * c;
+      if (k + 1 >= length) v.y = 0.0f;
+      if (k + 2 >= length) v.z = 0.0f;
+      if (k + 3 >= length) v.w = 0.0f;
+    }
+    *reinterpret_cast<float4*>(dst + r * stride + 4 * c) = v;
+  }
+}
+
+}  // namespace
+
+// cv::BFMatcher(NORM_L2).knnMatch(keyframe descriptors, frame descriptors, k = 2) and the ratio test of
+// CalculateCorrespondences for every L2 body at correspondence iteration 0. distance = sqrt of the float sum of
+// squared float differences, summed in descriptor order. For SIFT's whole-number descriptors every partial sum is an
+// integer below 2^24, so any order gives OpenCV's distance bit for bit (DESIGN.md section 3).
+// Each thread holds a 4 x 4 block of (query, train) sums: queries ty + 16 i, train rows tx + 16 j of the CTA's split.
+__global__ void __cluster_dims__(kKnnSplits, 1, 1) __launch_bounds__(kKnnThreads)
+    k_texture_knn_l2(const __grid_constant__ TextureArgs a) {
+  namespace cg = cooperative_groups;
+  const int b = blockIdx.y, tid = threadIdx.x;
+  const BodyDev& body = a.bodies[b];
+  // every return before the first cluster barrier depends on (body, tile) alone: a cluster leaves or stays whole
+  if (!body.set || !body.has_texture || !body.tp.l2) return;
+  const int rank = blockIdx.x % kKnnSplits, tile = blockIdx.x / kKnnSplits;
+  const int k = tile / (kTexMaxFeatures / kKnnQueries), q0 = tile % (kTexMaxFeatures / kKnnQueries) * kKnnQueries;
+  const TexKeyframeState st = a.kf_state[b];
+  if (k >= st.size) return;
+  const int slot = (st.head + k) % kTexMaxKeyframes;
+  const int nq = min(kKnnQueries, a.kf_n[b * kTexMaxKeyframes + slot] - q0);
+  if (nq <= 0) return;
+  const int length = body.tp.descriptor_length, stride = KnnStride(length);
+  const int t0 = rank * kKnnTrain, nt = max(0, min(kKnnTrain, a.feat_n[b] - t0));
+  extern __shared__ float4 s_dyn[];
+  float* s_q = reinterpret_cast<float*>(s_dyn);
+  float* s_t = s_q + kKnnQueries * stride;
+  __shared__ Top2 s_part[kKnnQueries];
+  StageRows(a.kf_fdesc + ((size_t(b) * kTexMaxKeyframes + slot) * kTexMaxFeatures + q0) * kTexMaxFloatDesc, nq,
+            kKnnQueries, length, stride, s_q);
+  StageRows(a.feat_fdesc + (size_t(b) * kTexMaxFeatures + t0) * kTexMaxFloatDesc, nt, kKnnTrain, length, stride, s_t);
+  __syncthreads();
+  const int ty = tid / 16, tx = tid % 16, s4 = stride / 4, d4 = (length + 3) / 4;
+  const float4* q4 = reinterpret_cast<const float4*>(s_q);
+  const float4* t4 = reinterpret_cast<const float4*>(s_t);
+  float acc[4][4];
+#pragma unroll
+  for (int i = 0; i < 4; ++i)
+#pragma unroll
+    for (int j = 0; j < 4; ++j) acc[i][j] = 0.0f;
+  for (int c = 0; c < d4; ++c) {
+    float4 qv[4], tv[4];
+#pragma unroll
+    for (int i = 0; i < 4; ++i) qv[i] = q4[(ty + 16 * i) * s4 + c];
+#pragma unroll
+    for (int j = 0; j < 4; ++j) tv[j] = t4[(tx + 16 * j) * s4 + c];
+#pragma unroll
+    for (int i = 0; i < 4; ++i)
+#pragma unroll
+      for (int j = 0; j < 4; ++j) {
+        float d = qv[i].x - tv[j].x;
+        acc[i][j] = fmaf(d, d, acc[i][j]);
+        d = qv[i].y - tv[j].y;
+        acc[i][j] = fmaf(d, d, acc[i][j]);
+        d = qv[i].z - tv[j].z;
+        acc[i][j] = fmaf(d, d, acc[i][j]);
+        d = qv[i].w - tv[j].w;
+        acc[i][j] = fmaf(d, d, acc[i][j]);
+      }
+  }
+#pragma unroll
+  for (int i = 0; i < 4; ++i) {
+    Top2 t{FLT_MAX, FLT_MAX, INT_MAX, INT_MAX};
+#pragma unroll
+    for (int j = 0; j < 4; ++j)
+      if (tx + 16 * j < nt) Insert(t, sqrtf(acc[i][j]), t0 + tx + 16 * j);
+    // the 16 lanes of a half-warp share ty: merge their lists
+#pragma unroll
+    for (int off = 8; off >= 1; off >>= 1) {
+      Top2 o;
+      o.d0 = __shfl_xor_sync(0xffffffffu, t.d0, off);
+      o.d1 = __shfl_xor_sync(0xffffffffu, t.d1, off);
+      o.i0 = __shfl_xor_sync(0xffffffffu, t.i0, off);
+      o.i1 = __shfl_xor_sync(0xffffffffu, t.i1, off);
+      t = Merge(t, o);
+    }
+    if (tx == 0) s_part[ty + 16 * i] = t;
+  }
+  cg::cluster_group cluster = cg::this_cluster();
+  cluster.sync();
+  if (rank == 0 && tid < nq) {
+    Top2 t = s_part[tid];
+    for (int r = 1; r < kKnnSplits; ++r) t = Merge(t, cluster.map_shared_rank(s_part, r)[tid]);
+    // knn_match[0].distance / knn_match[1].distance >= threshold drops the match; 0 / 0 is NaN and keeps it
+    const bool keep = t.i1 != INT_MAX && !(t.d0 / t.d1 >= body.tp.descriptor_distance_threshold);
+    a.knn[(size_t(b) * kTexMaxKeyframes + slot) * kTexMaxFeatures + q0 + tid] = keep ? t.i0 : -1;
+  }
+  cluster.sync();  // the partial lists of ranks 1.. stay in place until rank 0 has read them
+}
+
 // CalculateCorrespondences (texture_modality.cpp:322-386): with mode 1 (correspondence iteration 0) every keyframe's
-// descriptors (queries) are matched against the frame's (train set) by brute-force Hamming kNN, k = 2, and the matches
-// that pass the ratio test become the data points, keyframe by keyframe in query order. Every call then projects the
-// data points with the current pose (data_point.center) and records that pose.
+// descriptors (queries) are matched against the frame's (train set) by brute-force Hamming kNN, k = 2 (for L2 bodies
+// k_texture_knn_l2 has matched them just before), and the matches that pass the ratio test become the data points,
+// keyframe by keyframe in query order. Every call then projects the data points with the current pose
+// (data_point.center) and records that pose.
 __global__ void __launch_bounds__(kTexThreads) k_texture_match(const __grid_constant__ TextureArgs a) {
   const int b = blockIdx.x, tid = threadIdx.x;
   const BodyDev& body = a.bodies[b];
@@ -210,8 +363,10 @@ __global__ void __launch_bounds__(kTexThreads) k_texture_match(const __grid_cons
   const CameraDev& cam = a.color_cams[body.texture_camera];
   if (a.mode == 1) {
     const int n_train = a.feat_n[b];
+    const bool l2 = body.tp.l2 != 0;
     const uint4* train = reinterpret_cast<const uint4*>(a.feat_desc + size_t(b) * kTexMaxFeatures * kTexDescWords);
-    for (int k = tid; k < 2 * n_train; k += kTexThreads) s_train[k] = train[k];
+    if (!l2)
+      for (int k = tid; k < 2 * n_train; k += kTexThreads) s_train[k] = train[k];
     __syncthreads();
     const float2* xy = a.feat_xy + size_t(b) * kTexMaxFeatures;
     const TexKeyframeState st = a.kf_state[b];
@@ -222,11 +377,15 @@ __global__ void __launch_bounds__(kTexThreads) k_texture_match(const __grid_cons
       const int nq = a.kf_n[b * kTexMaxKeyframes + slot];
       const float* kp = a.kf_points + (size_t(b) * kTexMaxKeyframes + slot) * 3 * kTexMaxFeatures;
       const uint4* kd = reinterpret_cast<const uint4*>(a.kf_desc + (size_t(b) * kTexMaxKeyframes + slot) * kTexMaxFeatures * kTexDescWords);
+      const int* knn = l2 ? a.knn + (size_t(b) * kTexMaxKeyframes + slot) * kTexMaxFeatures : nullptr;
       for (int q0 = 0; q0 < nq; q0 += kTexThreads) {
         const int q = q0 + tid;
         bool keep = false;
         int i0 = -1;
-        if (q < nq && n_train >= 2) {
+        if (q < nq && knn) {
+          i0 = knn[q];
+          keep = i0 >= 0;
+        } else if (q < nq && n_train >= 2) {
           const uint4 qa = kd[2 * q], qb = kd[2 * q + 1];
           // cv::batchDistance's K = 2 insertion: strictly smaller distances enter, ties keep the earlier train index
           int d0 = INT_MAX, d1 = INT_MAX, i1 = -1;

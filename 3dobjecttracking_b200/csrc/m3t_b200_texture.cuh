@@ -1,7 +1,8 @@
 // m3t_b200_texture.cuh — TextureModality on the device (texture_modality.cpp): keyframe reconstruction from the device
-// silhouette renderer, brute-force Hamming kNN matching of ORB descriptors, and the Tukey-weighted reprojection
-// gradient / Hessian that k_track adds to a body's link. Feature detection stays with the caller; what it hands over
-// (keypoints in image coordinates and 32-byte descriptors) is all these kernels read of the colour frame.
+// silhouette renderer, brute-force kNN matching (Hamming for ORB's 32-byte descriptors, L2 for SIFT / DAISY float
+// descriptors), and the Tukey-weighted reprojection gradient / Hessian that k_track adds to a body's link. Feature
+// detection stays with the caller; what it hands over (keypoints in image coordinates and descriptors) is all these
+// kernels read of the colour frame.
 #pragma once
 
 #include "m3t_b200_device.cuh"
@@ -12,6 +13,7 @@ constexpr int kTexMaxFeatures = 512;   // frame features per body (the train set
 constexpr int kTexMaxKeyframes = 8;    // n_keyframes
 constexpr int kTexPointCap = kTexMaxFeatures * kTexMaxKeyframes;
 constexpr int kTexDescWords = 8;       // 32-byte ORB descriptors
+constexpr int kTexMaxFloatDesc = 256;  // float descriptor cap and the stride of the float tables (SIFT 128, DAISY 104)
 constexpr int kTexThreads = 256;
 constexpr int kTexRoiMargin = 10;      // kRegionOfInterestMargin, texture_modality.h:132
 
@@ -33,9 +35,13 @@ struct TextureArgs {
   const CameraDev* depth_cams;
   const float2* feat_xy;        // [n_bodies][kTexMaxFeatures] keypoints_ in image coordinates
   const uint32_t* feat_desc;    // [n_bodies][kTexMaxFeatures][8]
+  const float* feat_fdesc;      // [n_bodies][kTexMaxFeatures][kTexMaxFloatDesc] (L2 bodies; null without any)
   const int* feat_n;            // [n_bodies]
   float* kf_points;             // [n_bodies][kTexMaxKeyframes][3][kTexMaxFeatures]
   uint32_t* kf_desc;            // [n_bodies][kTexMaxKeyframes][kTexMaxFeatures][8]
+  float* kf_fdesc;              // [n_bodies][kTexMaxKeyframes][kTexMaxFeatures][kTexMaxFloatDesc] (L2 bodies)
+  int* knn;                     // [n_bodies][kTexMaxKeyframes][kTexMaxFeatures] k_texture_knn_l2: the train index of
+                                // a query's best match that passes the ratio test, -1 otherwise (by keyframe slot)
   int* kf_n;                    // [n_bodies][kTexMaxKeyframes]
   TexKeyframeState* kf_state;   // [n_bodies]
   float* points;                // [n_bodies][TF_COUNT][kTexPointCap]
@@ -45,6 +51,19 @@ struct TextureArgs {
 
 __global__ void k_texture_keyframe(const __grid_constant__ TextureArgs a);
 __global__ void k_texture_match(const __grid_constant__ TextureArgs a);
+
+// k_texture_knn_l2: a cluster of kKnnSplits CTAs per tile of kKnnQueries queries of one keyframe; CTA r of the cluster
+// scans train rows [r * kKnnTrain, (r + 1) * kKnnTrain) and rank 0 merges the partial top-2 lists. Grid:
+// (kKnnSplits * kKnnTiles, n_bodies), dynamic shared memory KnnSharedBytes(longest descriptor of the context).
+constexpr int kKnnQueries = 64, kKnnTrain = 64, kKnnThreads = 256;
+constexpr int kKnnSplits = kTexMaxFeatures / kKnnTrain;                         // 8, the portable cluster size
+constexpr int kKnnTiles = kTexMaxKeyframes * (kTexMaxFeatures / kKnnQueries);  // query tiles of a full deque
+// shared rows are padded to a stride of 4 (mod 8) floats, so the 8 float4 reads of a quarter-warp hit distinct banks
+__host__ __device__ constexpr int KnnStride(int length) { return (length + 7) / 8 * 8 + 4; }
+__host__ __device__ constexpr int KnnSharedBytes(int length) {
+  return int(sizeof(float)) * (kKnnQueries + kKnnTrain) * KnnStride(length);
+}
+__global__ void k_texture_knn_l2(const __grid_constant__ TextureArgs a);
 
 // TextureModality::TukeyNorm (texture_modality.cpp:1231-1237)
 __host__ __device__ __forceinline__ float TexTukeyNorm(float error, float c) {

@@ -1399,8 +1399,9 @@ class DepthModality : public Modality {
 
 // ---- texture_modality.h ------------------------------------------------------------------------------------------------
 // Feature detection stays with the caller (no OpenCV here): instead of DetectAndComputeCorrKeypoints the caller asks for
-// the body's focus region with CalculateFocus, detects ORB features in the cropped and scaled grey image and hands them
-// over with SetFeatures, once per frame. Only DescriptorType::ORB is implemented.
+// the body's focus region with CalculateFocus, detects features in the cropped and scaled grey image and hands them
+// over with SetFeatures, once per frame. DescriptorType ORB (32-byte descriptors), SIFT and DAISY (float descriptors)
+// are implemented.
 class TextureModality : public Modality {
  public:
   enum class DescriptorType { BRISK = 0, DAISY = 1, FREAK = 2, SIFT = 3, ORB = 4, ORB_CUDA = 5 };  // texture_modality.h
@@ -1447,8 +1448,9 @@ class TextureModality : public Modality {
   // TextureModality::SetUp (texture_modality.cpp:39-88); the body's device record is written by Optimizer::SetUp
   bool SetUp() override {
     set_up_ = false;
-    if (descriptor_type_ != DescriptorType::ORB) {
-      std::cerr << "Modality " << name_ << ": only DescriptorType::ORB is implemented" << std::endl;
+    if (descriptor_type_ != DescriptorType::ORB && descriptor_type_ != DescriptorType::SIFT &&
+        descriptor_type_ != DescriptorType::DAISY) {
+      std::cerr << "Modality " << name_ << ": only DescriptorType::ORB, SIFT and DAISY are implemented" << std::endl;
       return false;
     }
     if (!silhouette_renderer_ptr_) {
@@ -1479,6 +1481,7 @@ class TextureModality : public Modality {
                 << std::endl;
       return false;
     }
+    params_.descriptor_type = int32_t(descriptor_type_);
     set_up_ = true;
     return true;
   }
@@ -1504,6 +1507,20 @@ class TextureModality : public Modality {
     return Check(batch_->ctx(),
                  m3tb_upload_texture_features(batch_->ctx(), body_ptr_->index(), keypoints_xy.data(), descriptors.data(), n,
                                               roi[0], roi[1], scale),
+                 "TextureModality::SetFeatures");
+  }
+  // SetFeatures for SIFT and DAISY: `length` floats per keypoint (descriptors[length n]); 128 for SIFT, 1 .. 256 for
+  // DAISY, the same length for every frame until SetUp runs again
+  bool SetFeatures(const std::vector<float>& keypoints_xy, const std::vector<float>& descriptors, int length,
+                   const std::array<int32_t, 4>& roi, float scale) {
+    const int n = int(keypoints_xy.size() / 2);
+    if (length < 1 || descriptors.size() != size_t(length) * n) {
+      std::cerr << "Modality " << name_ << ": one descriptor of `length` floats per keypoint" << std::endl;
+      return false;
+    }
+    return Check(batch_->ctx(),
+                 m3tb_upload_texture_float_features(batch_->ctx(), body_ptr_->index(), keypoints_xy.data(),
+                                                    descriptors.data(), n, length, roi[0], roi[1], scale),
                  "TextureModality::SetFeatures");
   }
 

@@ -1,12 +1,13 @@
 // texture_mirror_tracker.cpp — drives the C++ mirror's TextureModality on a seeded synthetic scene: one rigid body and
 // one 3-link chain (root with 6 DoF, revolute-x children at Tx(0.01)), every body with region, depth and texture
 // modalities on its own RGB-D pair and its own focused silhouette renderer. The features a detector would find are
-// generated here from a seed: points on the prism's mid-plane with random 32-byte descriptors, seen at the start pose
-// for StartModality and at the ground-truth pose for the tracked frame. The scene is tracked once through
-// Tracker::ExecuteTrackingStep and once through ExecuteTrackingStepObjectWise; both pose sets are printed as JSON for
-// tests/test_gpu_texture_mirror.py.
+// generated here from a seed: points on the prism's mid-plane with random 32-byte descriptors (orb) or 128
+// whole-number floats in 0 .. 255, as cv::SIFT writes them (sift), seen at the start pose for StartModality and at the
+// ground-truth pose for the tracked frame. The scene is tracked once through Tracker::ExecuteTrackingStep and once
+// through ExecuteTrackingStepObjectWise; both pose sets are printed as JSON for tests/test_gpu_texture_mirror.py and
+// tests/test_gpu_texture_l2.py.
 //
-//   usage: texture_mirror_tracker [seed=1] [n_features=300]
+//   usage: texture_mirror_tracker [seed=1] [n_features=300] [orb|sift]
 #include <algorithm>
 #include <array>
 #include <cmath>
@@ -74,12 +75,15 @@ std::vector<float> PrismTriangles(float* diameter) {
   return out;
 }
 
+constexpr int kSiftLength = 128;
+
 // a body's texture: n points on the prism's triangular mid-plane (body frame) and their descriptors
 struct Texture {
   std::vector<float> points;  // [n][3]
-  std::vector<uint8_t> descriptors;  // [n][32]
+  std::vector<uint8_t> descriptors;  // [n][32] (orb)
+  std::vector<float> float_descriptors;  // [n][kSiftLength] (sift)
 };
-Texture MakeTexture(uint64_t seed, int body, int n) {
+Texture MakeTexture(uint64_t seed, int body, int n, bool sift) {
   std::mt19937 rng(uint32_t(seed * 7919u + uint64_t(body)));
   std::uniform_real_distribution<float> u(0.0f, 1.0f);
   std::uniform_int_distribution<int> byte(0, 255);
@@ -90,7 +94,10 @@ Texture MakeTexture(uint64_t seed, int body, int n) {
     for (int k = 0; k < 2; ++k)  // vertices 0, 2, 4 span the triangle
       t.points.push_back(kPrism[0][k] + a * (kPrism[2][k] - kPrism[0][k]) + b * (kPrism[4][k] - kPrism[0][k]));
     t.points.push_back(0.0f);
-    for (int k = 0; k < 32; ++k) t.descriptors.push_back(uint8_t(byte(rng)));
+    if (sift)
+      for (int k = 0; k < kSiftLength; ++k) t.float_descriptors.push_back(float(byte(rng)));
+    else
+      for (int k = 0; k < 32; ++k) t.descriptors.push_back(uint8_t(byte(rng)));
   }
   return t;
 }
@@ -117,6 +124,7 @@ bool UploadFeatures(TextureModality& m, const Texture& t, const Transform3fA& bo
     xy.push_back((x * ci.fu / z + ci.ppu - float(roi[0])) * scale);
     xy.push_back((y * ci.fv / z + ci.ppv - float(roi[1])) * scale);
   }
+  if (!t.float_descriptors.empty()) return m.SetFeatures(xy, t.float_descriptors, kSiftLength, roi, scale);
   return m.SetFeatures(xy, t.descriptors, roi, scale);
 }
 
@@ -141,6 +149,7 @@ std::vector<Transform3fA> Poses(Scene& s) {
 int main(int argc, char** argv) {
   const uint64_t seed = argc > 1 ? std::strtoull(argv[1], nullptr, 10) : 1;
   const int n_features = argc > 2 ? std::atoi(argv[2]) : 300;
+  const bool sift = argc > 3 && std::string(argv[3]) == "sift";
   const int n_lines = 200, n_points = 200, n_divides = 2;
   float prism_diameter = 0.0f;
   const std::vector<float> prism = PrismTriangles(&prism_diameter);
@@ -181,7 +190,7 @@ int main(int argc, char** argv) {
     }
     m3ts_render_color(&sci, Mul(color_w2c, gt[b]).data(), seed * 1000003 + b, fg, bg, 10.0f, color[b].data(), cpitch);
     m3ts_render_depth(&sdi, Mul(depth_w2c, gt[b]).data(), seed * 1000003 + b, 1.0f, 0.001f, 0.01f, 0.001f, depth[b].data(), dpitch);
-    textures.push_back(MakeTexture(seed, b, n_features));
+    textures.push_back(MakeTexture(seed, b, n_features, sift));
   }
 
   std::vector<Transform3fA> start;
@@ -214,6 +223,7 @@ int main(int argc, char** argv) {
       auto dm = std::make_shared<DepthModality>("depth_modality_" + std::to_string(b), s.batch, body, dc, depth_model);
       dm->set_n_points_max(n_points);
       auto tm = std::make_shared<TextureModality>("texture_modality_" + std::to_string(b), s.batch, body, cc, silhouette);
+      if (sift) tm->set_descriptor_type(TextureModality::DescriptorType::SIFT);
       auto link = std::make_shared<Link>("link_" + std::to_string(b), body);
       link->AddModality(rm);
       link->AddModality(dm);
@@ -255,7 +265,7 @@ int main(int argc, char** argv) {
   }
   if (!fused.tracker->ExecuteTrackingStep(0)) return 3;
   if (!object_wise.tracker->ExecuteTrackingStepObjectWise(0)) return 4;
-  std::printf("{\"n_bodies\": %d, \"texture_points\": [", kBodies);
+  std::printf("{\"descriptor\": \"%s\", \"n_bodies\": %d, \"texture_points\": [", sift ? "sift" : "orb", kBodies);
   for (int b = 0; b < kBodies; ++b) {
     std::vector<m3tb_texture_point> pts(512);
     int n = 0;

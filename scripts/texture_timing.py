@@ -8,7 +8,16 @@ Reports, with the card's name and power limit, host-clock times around K calls e
   - one tracking step (2 x 2 iterations) of 32 kinematic chains of 4 links (config-5 shape, 300 lines and points per
     link) with a texture modality on every link against the same chains without texture (k_track + k_structure per
     update either way).
-Prints one JSON line."""
+Prints one JSON line.
+
+With --descriptor sift|daisy it measures the L2 matcher instead (512 features per body of 128 / 104 floats, whole
+numbers in 0 .. 255 for SIFT, unit-norm for DAISY, every query a keyframe point):
+  - k_texture_knn_l2 per launch (torch.profiler CUDA activity over K calls of m3tb_texture_correspondences at
+    correspondence iteration 0) for 1, 8 and 128 bodies and n_keyframes 1 and 4, with the FP32 rate from
+    2 * queries * train * length against the 67 TFLOP/s data sheet;
+  - one tracking step at the ORB shape above (128 bodies, 300 features) with ORB against the L2 descriptor.
+
+    python scripts/texture_timing.py [K] [--descriptor sift|daisy]"""
 import importlib
 import json
 import os
@@ -24,37 +33,72 @@ pkg = importlib.import_module("3dobjecttracking_b200")
 capi = importlib.import_module("3dobjecttracking_b200.capi")
 synth = pkg.synth
 
-K = int(sys.argv[1]) if len(sys.argv) > 1 else 100
+ARGS = [a for a in sys.argv[1:] if not a.startswith("--")]
+K = int(ARGS[0]) if ARGS else 100
+DESCRIPTOR = sys.argv[sys.argv.index("--descriptor") + 1] if "--descriptor" in sys.argv else None
+ARGS = [a for a in ARGS if a != DESCRIPTOR]
 N_FEAT = 300
+L2_LENGTH = {"sift": 128, "daisy": 104}
+L2_TYPE = {"sift": capi.DESCRIPTOR_SIFT, "daisy": capi.DESCRIPTOR_DAISY}
 
 
-def make(wl, texture):
+def descriptors(rng, kind, n):
+    if kind is None:
+        return rng.integers(0, 256, (n, 32), dtype=np.uint8)
+    if kind == "sift":
+        return rng.integers(0, 256, (n, 128)).astype(np.float32)
+    v = rng.random((n, L2_LENGTH[kind])).astype(np.float32)
+    return (v / np.linalg.norm(v, axis=1, keepdims=True)).astype(np.float32)
+
+
+def perturbed(rng, kind, desc):
+    if kind is None:
+        desc = desc.copy()
+        desc[:, ::4] ^= 1
+        return desc
+    noise = rng.integers(-3, 4, desc.shape) if kind == "sift" else rng.normal(0, 0.02, desc.shape)
+    return np.clip(desc + noise, 0, None).astype(np.float32)
+
+
+def make(wl, texture, kind=None, n_feat=N_FEAT, n_keyframes=1, central=False):
     """A context of the workload; with texture, every body gets a texture modality on its own camera, a keyframe from
-    the first frame's features and the next frame's features (the same ones, a few descriptor bits flipped)."""
+    the first frame's features and the next frame's features (the same ones, a few descriptor bits flipped).
+    kind: None (ORB) or an L2 descriptor; n_keyframes > 1 refreshes the keyframe every frame until the deque is full;
+    central puts every feature near the body's centre, so that all become keyframe points."""
     ctx = capi.context_from_workload(wl)
     tri, diam = synth.prism_triangles()
     for b in range(wl.n_bodies):
         ctx.set_body_geometry(b, tri, None, diam, True, b % 255 + 1, 7)
     if texture:
         rng = np.random.default_rng(0)
+        params = capi.texture_params_default()
+        if kind is not None:
+            params.descriptor_type = L2_TYPE[kind]
+        params.n_keyframes = n_keyframes
+        params.max_keyframe_age = 0 if n_keyframes > 1 else params.max_keyframe_age
         for b in range(wl.n_bodies):
             ctx.set_focused_renderer(b, "color", b, [b], [b], id_type="body")
-            ctx.set_texture_modality(b, capi.texture_params_default(), b)
+            ctx.set_texture_modality(b, params, b)
             ctx.attach_renderer(b, "texture_silhouette", b)
         roi, scale, valid = ctx.get_texture_focus()
         feats = []
         for b in range(wl.n_bodies):
             x, y, w, h = roi[b]
-            xy = np.stack([rng.uniform(0, w, N_FEAT), rng.uniform(0, h, N_FEAT)], 1) * scale[b]
-            desc = rng.integers(0, 256, (N_FEAT, 32), dtype=np.uint8)
+            if central:
+                xy = np.stack([rng.uniform(0.47 * w, 0.53 * w, n_feat), rng.uniform(0.47 * h, 0.53 * h, n_feat)], 1)
+            else:
+                xy = np.stack([rng.uniform(0, w, n_feat), rng.uniform(0, h, n_feat)], 1)
+            xy = xy * scale[b]
+            desc = descriptors(rng, kind, n_feat)
             feats.append((xy.astype(np.float32), desc))
             ctx.upload_texture_features(b, xy, desc, x, y, scale[b] if valid[b] else 1.0)
         ctx.start_modalities(0)
-        for b in range(wl.n_bodies):  # the next frame: the same features, a few descriptor bits flipped
+        for frame in range(1, n_keyframes):
+            ctx.calculate_results(frame)
+        for b in range(wl.n_bodies):  # the next frame: the same features, descriptors perturbed
             xy, desc = feats[b]
-            desc = desc.copy()
-            desc[:, ::4] ^= 1
-            ctx.upload_texture_features(b, xy, desc, roi[b][0], roi[b][1], scale[b] if valid[b] else 1.0)
+            ctx.upload_texture_features(b, xy, perturbed(rng, kind, desc), roi[b][0], roi[b][1],
+                                        scale[b] if valid[b] else 1.0)
     return wl, ctx
 
 
@@ -69,8 +113,64 @@ def time_calls(ctx, fn):
     return (time.perf_counter() - t0) / K * 1e3
 
 
-wl = synth.make_workload("c4", n_bodies=128, n_divides=2, seed=0)
+def gpu_name():
+    return subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True,
+                          text=True).stdout.strip()
+
+
 step = lambda c, n_corr, n_update: (lambda: c.tracking_step(0, n_corr, n_update))  # noqa: E731
+
+
+def knn_kernel_ms(ctx):
+    """k_texture_knn_l2's mean device time per launch over K calls of the match (torch.profiler CUDA activity)."""
+    import torch
+    from torch.profiler import ProfilerActivity, profile
+    for _ in range(10):
+        ctx.texture_correspondences(0, 0)
+    ctx.synchronize()
+    with profile(activities=[ProfilerActivity.CUDA]) as prof:
+        for _ in range(K):
+            ctx.texture_correspondences(0, 0)
+        ctx.synchronize()
+        torch.cuda.synchronize()
+    rows = [e for e in prof.key_averages() if "k_texture_knn_l2" in e.key]
+    assert len(rows) == 1 and rows[0].count == K, [(e.key, e.count) for e in rows]
+    return max(rows[0].self_device_time_total, rows[0].device_time_total) / K / 1e3
+
+
+def l2_main(kind):
+    import torch
+    torch.cuda.init()
+    length = L2_LENGTH[kind]
+    shapes = []
+    for n_bodies in (1, 8, 128):
+        for n_keyframes in (1, 4):
+            wl = synth.make_workload("c4", n_bodies=n_bodies, n_divides=2, seed=0)
+            wl, ctx = make(wl, True, kind, n_feat=512, n_keyframes=n_keyframes, central=True)
+            queries = sum(int(ctx.get_texture_keyframes(b)["sizes"].sum()) for b in range(n_bodies))
+            ms = knn_kernel_ms(ctx)
+            flop = 2.0 * queries * 512 * length
+            ms_call = time_calls(ctx, lambda: ctx.texture_correspondences(0, 0))
+            shapes.append(dict(bodies=n_bodies, n_keyframes=n_keyframes, queries=queries, train_per_body=512,
+                               length=length, ms_knn_l2=ms, ms_match_call=ms_call, tflops=flop / ms / 1e9,
+                               share_of_67_tflops=flop / ms / 1e9 / 67.0, datasheet_floor_ms=flop / 67e12 * 1e3))
+            ctx.close()
+    wl = synth.make_workload("c4", n_bodies=128, n_divides=2, seed=0)
+    steps = {}
+    for name, k in (("orb", None), (kind, kind)):
+        wl, ctx = make(wl, True, k)
+        steps[name] = time_calls(ctx, step(ctx, wl.n_corr_iterations, wl.n_update_iterations))
+        ctx.close()
+    print(json.dumps(dict(descriptor=kind, K=K, shapes=shapes, step_bodies=wl.n_bodies, step_features_per_body=N_FEAT,
+                          n_corr=wl.n_corr_iterations, n_update=wl.n_update_iterations,
+                          ms_step_orb=steps["orb"], **{"ms_step_" + kind: steps[kind]}, gpu=gpu_name())))
+
+
+if DESCRIPTOR is not None:
+    assert DESCRIPTOR in L2_LENGTH, DESCRIPTOR
+    l2_main(DESCRIPTOR)
+    sys.exit(0)
+wl = synth.make_workload("c4", n_bodies=128, n_divides=2, seed=0)
 wl, plain = make(wl, False)
 ms_plain = time_calls(plain, step(plain, wl.n_corr_iterations, wl.n_update_iterations))
 plain_kernel = plain.last_launch()["kernel"]
@@ -93,8 +193,7 @@ chain_points = int(np.mean([len(chain_tex.get_texture_points(b)) for b in range(
 ms_chain_tex = time_calls(chain_tex, step(chain_tex, 2, 2))
 chain_tex_kernel = chain_tex.last_launch()["kernel"]
 chain_tex.close()
-gpu = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True,
-                     text=True).stdout.strip()
+gpu = gpu_name()
 print(json.dumps(dict(bodies=wl.n_bodies, features_per_body=N_FEAT, mean_data_points_per_body=n_points,
                       n_corr=wl.n_corr_iterations, n_update=wl.n_update_iterations, ms_texture_match=ms_match,
                       ms_step_without_texture=ms_plain, kernel_without_texture=plain_kernel, ms_step_with_texture=ms_tex,
