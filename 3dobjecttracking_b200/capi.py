@@ -122,7 +122,7 @@ SYMBOLS = [
     "m3tb_region_gradient_hessian", "m3tb_depth_correspondences", "m3tb_depth_gradient_hessian",
     "m3tb_calculate_optimization", "m3tb_get_region_lines", "m3tb_get_depth_points", "m3tb_get_closest_views",
     "m3tb_debug_phase_clocks", "m3tb_last_ingest_bytes", "m3tb_set_structure", "m3tb_clear_structures",
-    "m3tb_n_structures", "m3tb_calculate_consistent_poses", "m3tb_get_link_poses", "m3tb_get_structure_theta",
+    "m3tb_n_structures", "m3tb_calculate_consistent_poses", "m3tb_refine_poses", "m3tb_get_link_poses", "m3tb_get_structure_theta",
     "m3tb_set_gradient_hessian", "m3tb_reset_joint_poses", "m3tb_prefetch_frames", "m3tb_detach_frames",
     "m3tb_debug_closest_view", "m3tb_upload_depth_rendering", "m3tb_upload_silhouette_rendering",
     "m3tb_share_color_histograms", "m3tb_debug_last_launch", "m3tb_set_body_geometry", "m3tb_set_focused_renderer",
@@ -221,6 +221,7 @@ def lib():
     L.m3tb_clear_structures.argtypes = [vp]
     L.m3tb_n_structures.argtypes = [vp]
     L.m3tb_calculate_consistent_poses.argtypes = [vp]
+    L.m3tb_refine_poses.argtypes = [vp, C.POINTER(ci), ci, C.POINTER(ci), ci, ci, ci]
     L.m3tb_reset_joint_poses.argtypes = [vp]
     L.m3tb_prefetch_frames.argtypes = [vp]
     L.m3tb_detach_frames.argtypes = [vp]
@@ -807,6 +808,15 @@ class Context:
 
     def calculate_consistent_poses(self):
         self._ck(self.L.m3tb_calculate_consistent_poses(self.h))
+
+    def refine_poses(self, bodies=(), structures=(), n_corr_iterations=7, n_update_iterations=2):
+        """Refiner::RefinePoses for the rigid bodies `bodies` and the kinematic structures `structures`; every other
+        body and structure keeps its state. Nothing is launched when both are empty."""
+        b = np.ascontiguousarray(list(bodies), dtype=np.int32)
+        s = np.ascontiguousarray(list(structures), dtype=np.int32)
+        ip = C.POINTER(C.c_int)
+        self._ck(self.L.m3tb_refine_poses(self.h, b.ctypes.data_as(ip), len(b), s.ctypes.data_as(ip), len(s),
+                                          n_corr_iterations, n_update_iterations))
 
     def get_link_poses(self, structure, n_links):
         """(body2joint, joint2parent, link2world), each [n_links, 3, 4]."""

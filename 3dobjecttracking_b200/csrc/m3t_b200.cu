@@ -4,6 +4,7 @@
 
 #include <cudaTypedefs.h>  // PFN_cuTensorMapEncodeTiled
 
+#include <algorithm>
 #include <climits>
 #include <cmath>
 #include <cstddef>
@@ -96,6 +97,23 @@ struct PrefetchResources {
 
 // which device renderers one k_render launch draws
 enum RenderList { kRenderAll = 0, kRenderAttached, kRenderRegion, kRenderLists };
+
+// What one m3tb_refine_poses launches on: lists in m3tb_ctx::d_refine and their lengths. m3tb_ctx::refine points at it
+// while the refinement runs and is null otherwise, so every other entry point launches over the whole context.
+struct RefineSelection {
+  const int* bodies = nullptr;          // k_histogram, k_ingest: the refined bodies with the bodies of the
+  int n_bodies = 0;                     //   refined structures (links and extra bodies)
+  const int* structures = nullptr;      // k_structure: the refined structures and the implicit one-link structures of
+  int n_structures = 0;                 //   the refined rigid bodies (contexts with kinematic structures only)
+  const int* renderers[kRenderLists] = {};  // k_render: the renderers attached to the refined bodies (kRenderAttached:
+  int n_renderers[kRenderLists] = {};       //   every slot that feeds correspondences, kRenderRegion: the region slots)
+  size_t render_smem[kRenderLists] = {};
+  std::vector<int> renderer_ids[kRenderLists];  // host copies
+  const int* hist_groups = nullptr;     // shared ColorHistograms objects with a refined member:
+  int n_hist_groups = 0;                //   owner[n] | first[n + 1] | summed[n] | members (refined ones first)
+  bool ingested = false;                // k_ingest ran for the refined bodies
+  std::vector<std::pair<int, int>> runs;  // k_track: (first body, count) of each run of consecutive refined bodies
+};
 
 }  // namespace
 
@@ -273,6 +291,10 @@ struct m3tb_ctx {
   // an L2 descriptor type, never for contexts with ORB bodies only
   DeviceBuffer<float> d_tex_fdesc, d_tex_kf_fdesc;
   DeviceBuffer<int> d_tex_knn;
+
+  // pose refinement (m3tb_refine_poses): the lists of RefineSelection, grown on demand; `refine` is set while it runs
+  DeviceBuffer<int> d_refine;
+  RefineSelection* refine = nullptr;
 };
 
 namespace {
@@ -492,6 +514,9 @@ int LaunchIngestIfPending(m3tb_ctx* ctx) {
     ctx->prefetched = false;
   }
   if (!ctx->ingest_pending) return M3TB_OK;
+  // a refinement fetches the ROIs of its bodies only; the others are fetched by the next launch over the whole context
+  RefineSelection* sel = ctx->refine;
+  if (sel && sel->ingested) return M3TB_OK;
   IngestArgs a;
   a.bodies = ctx->d_bodies;
   a.poses = ctx->d_poses;
@@ -502,13 +527,15 @@ int LaunchIngestIfPending(m3tb_ctx* ctx) {
   a.roi = ctx->d_roi;
   ctx->ingest_bytes_slot ^= 1;
   a.bytes = ctx->d_ingest_bytes + ctx->ingest_bytes_slot;
-  a.n_bodies = ctx->n_bodies;
+  a.n_bodies = sel ? sel->n_bodies : ctx->n_bodies;
+  a.body_list = sel ? sel->bodies : nullptr;
   CU(cudaMemsetAsync(a.bytes, 0, sizeof(unsigned long long), ctx->stream));
-  NoteIngestBins(ctx);
-  k_ingest<<<ctx->n_bodies, kBlockThreads, 0, ctx->stream>>>(a);
+  if (!sel) NoteIngestBins(ctx);  // the bin-index images are complete once every body's rectangles are fetched
+  k_ingest<<<a.n_bodies, kBlockThreads, 0, ctx->stream>>>(a);
   CU(cudaGetLastError());
   ctx->launches++;
-  ctx->ingest_pending = false;
+  if (sel) sel->ingested = true;
+  else ctx->ingest_pending = false;
   return M3TB_OK;
 }
 
@@ -646,6 +673,31 @@ int PrepareTensorTiles(m3tb_ctx* ctx, TrackArgs& a, bool& usable) {
   return M3TB_OK;
 }
 
+// The arguments of a k_track launch over bodies [first, first + gridDim.x): every per-body table starts at body `first`,
+// so that the kernel, which indexes them by blockIdx.x, runs unchanged on a run of refined bodies (m3tb_refine_poses)
+TrackArgs RunArgs(const TrackArgs& a, int first) {
+  if (first == 0) return a;
+  TrackArgs r = a;
+  const size_t f = size_t(first);
+  r.bodies += f;
+  r.poses += 12 * f;
+  r.lut += f * a.lut_stride;
+  r.region_state += f * RF_COUNT * size_t(a.line_cap);
+  r.depth_state += f * DF_COUNT * size_t(a.point_cap);
+  r.counts += 4 * f;
+  r.roi += 2 * f;
+  auto shift = [](auto* p, size_t n) { return p ? p + n : p; };  // tables a context may not have made
+  r.gh_region = shift(a.gh_region, 27 * f);
+  r.gh_depth = shift(a.gh_depth, 27 * f);
+  r.gh_link = shift(a.gh_link, 27 * f);
+  r.gh_texture = shift(a.gh_texture, 27 * f);
+  r.tex_points = shift(a.tex_points, f * TF_COUNT * kTexPointCap);
+  r.tex_counts = shift(a.tex_counts, f);
+  r.tex_pose = shift(a.tex_pose, 12 * f);
+  r.phase_clock = shift(a.phase_clock, f * kPhaseSlots);
+  return r;
+}
+
 // cluster > 0: one thread-block cluster of `cluster` CTAs per kinematic structure (PH_CLUSTER_SOLVE)
 int LaunchTrack(m3tb_ctx* ctx, int iteration, int corr_begin, int corr_end, int n_update, int opt_base,
                 unsigned phases, int cluster = 0) {
@@ -735,7 +787,7 @@ int LaunchTrack(m3tb_ctx* ctx, int iteration, int corr_begin, int corr_end, int 
   {
     const unsigned k2_phases = PH_REGION_CORR | PH_DEPTH_CORR | PH_REGION_GH | PH_DEPTH_GH | PH_SOLVE | PH_STORE_REGION |
                                PH_STORE_DEPTH;
-    bool ok = ctx->use_track2 && bins_fit_u16 && cluster == 0 && !occ && items <= kGroup && (phases & ~k2_phases) == 0 &&
+    bool ok = ctx->use_track2 && !ctx->refine && bins_fit_u16 && cluster == 0 && !occ && items <= kGroup && (phases & ~k2_phases) == 0 &&
               (n_update == 0 || (phases & PH_SOLVE));
     bool both = false, have_lookup = false;
     for (int b = 0; b < ctx->n_bodies && ok; ++b) {
@@ -777,7 +829,9 @@ int LaunchTrack(m3tb_ctx* ctx, int iteration, int corr_begin, int corr_end, int 
 #define M3TB_LAUNCH1(T_, K_, L_, O_)                                                                                   \
   do {                                                                                                                 \
     CU(cudaFuncSetAttribute(k_track<T_, K_, L_, O_, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, int(dyn)));   \
-    k_track<T_, K_, L_, O_, false><<<ctx->n_bodies, T_, dyn, ctx->stream>>>(a);                                        \
+    for (size_t r_ = 0; r_ < n_runs; ++r_)                                                                             \
+      k_track<T_, K_, L_, O_, false><<<runs_begin[r_].second, T_, dyn, ctx->stream>>>(RunArgs(a, runs_begin[r_].first)); \
+    n_launches = int(n_runs);                                                                                          \
     info = {M3TB_KERNEL_TRACK, T_, K_, L_ ? 1 : 0, O_ ? 1 : 0, tiles ? 1 : 0, -1};                                     \
   } while (0)
 #define M3TB_LAUNCH_CLUSTER(T_, K_, L_)                                                                                \
@@ -812,6 +866,11 @@ int LaunchTrack(m3tb_ctx* ctx, int iteration, int corr_begin, int corr_end, int 
     else M3TB_LAUNCH1(T_, K_, false, true);                       \
   } while (0)
   m3tb_launch_info info = {};
+  int n_launches = 1;
+  // a refinement launches k_track once per run of consecutive refined bodies (RunArgs), one CTA per body
+  const std::pair<int, int> all_bodies(0, ctx->n_bodies);
+  const std::pair<int, int>* runs_begin = ctx->refine ? ctx->refine->runs.data() : &all_bodies;
+  const size_t n_runs = ctx->refine ? ctx->refine->runs.size() : 1;
   if (cluster > 0) {
     // cluster-fused structures: 256-thread CTAs without ROI tiles, so that two CTAs share an SM and every cluster of
     // a 32-chain shard is resident at once (with 220 KB tiles at most 16 clusters of 8 fit on the 132 SMs)
@@ -827,7 +886,7 @@ int LaunchTrack(m3tb_ctx* ctx, int iteration, int corr_begin, int corr_end, int 
 #undef M3TB_LAUNCH1
 #undef M3TB_LAUNCH_CLUSTER
   CU(cudaGetLastError());
-  ctx->launches++;
+  ctx->launches += n_launches;
   ctx->last_launch = info;
   return M3TB_OK;
 }
@@ -992,9 +1051,12 @@ int LaunchStructure(m3tb_ctx* ctx, int mode, bool from_modalities) {
   a.mode = mode;
   a.theta_out = ctx->d_theta;
   a.status = ctx->d_struct_status;
+  a.list = ctx->refine ? ctx->refine->structures : nullptr;
+  const int n = ctx->refine ? ctx->refine->n_structures : ctx->n_struct_launch;
+  if (n == 0) return M3TB_OK;
   if (ctx->struct_smem > 48 * 1024)
     CU(cudaFuncSetAttribute(k_structure, cudaFuncAttributeMaxDynamicSharedMemorySize, int(ctx->struct_smem)));
-  k_structure<<<ctx->n_struct_launch, kStructThreads, ctx->struct_smem, ctx->stream>>>(a);
+  k_structure<<<n, kStructThreads, ctx->struct_smem, ctx->stream>>>(a);
   CU(cudaGetLastError());
   ctx->launches++;
   return M3TB_OK;
@@ -1098,6 +1160,8 @@ int LaunchHistogram(m3tb_ctx* ctx, int mode, int iteration) {
   a.depth_cams = ctx->d_dcams;
   a.iteration = iteration;
   a.shared_owner = nullptr;
+  const RefineSelection* sel = ctx->refine;
+  a.body_list = sel ? sel->bodies : nullptr;
   // shared ColorHistograms objects: group tables (owner first), checked against the bodies as they are now
   std::vector<int> group_owner, group_first, members;
   bool any_shared = false;
@@ -1143,10 +1207,10 @@ int LaunchHistogram(m3tb_ctx* ctx, int mode, int iteration) {
     }
     a.shared_owner = ctx->d_hist_owner;
   }
-  k_histogram<<<ctx->n_bodies, kBlockThreads, 0, ctx->stream>>>(a);
+  k_histogram<<<sel ? sel->n_bodies : ctx->n_bodies, kBlockThreads, 0, ctx->stream>>>(a);
   CU(cudaGetLastError());
   ctx->launches++;
-  if (any_shared) {
+  if (any_shared && (!sel || sel->n_hist_groups > 0)) {
     SharedHistArgs s;
     s.bodies = ctx->d_bodies;
     s.hist_f = ctx->d_hist_f; s.hist_b = ctx->d_hist_b; s.mem_f = ctx->d_mem_f; s.mem_b = ctx->d_mem_b; s.lut = ctx->d_lut;
@@ -1155,7 +1219,16 @@ int LaunchHistogram(m3tb_ctx* ctx, int mode, int iteration) {
     s.group_owner = ctx->d_hist_groups;
     s.group_first = ctx->d_hist_groups + ctx->n_hist_groups;
     s.members = ctx->d_hist_groups + 2 * ctx->n_hist_groups + 1;
-    k_histogram_shared<<<ctx->n_hist_groups, kBlockThreads, 0, ctx->stream>>>(s);
+    s.group_summed = nullptr;
+    int n_groups = ctx->n_hist_groups;
+    if (sel) {  // the objects a refined body uses, from the refined members' line pixels only (Refiner::StartModalities)
+      n_groups = sel->n_hist_groups;
+      s.group_owner = sel->hist_groups;
+      s.group_first = sel->hist_groups + n_groups;
+      s.group_summed = sel->hist_groups + 2 * n_groups + 1;
+      s.members = sel->hist_groups + 3 * n_groups + 1;
+    }
+    k_histogram_shared<<<n_groups, kBlockThreads, 0, ctx->stream>>>(s);
     CU(cudaGetLastError());
     ctx->launches++;
   }
@@ -1263,11 +1336,13 @@ int LaunchRender(m3tb_ctx* ctx, int which) {
   int rc = SyncTables(ctx);  // pending body-table uploads go first: k_render then owns the attached records
   if (!rc) rc = SyncRenderTables(ctx);
   if (rc) return rc;
-  const int n = ctx->render_n[which];
-  const size_t smem = ctx->render_smem[which];
+  const RefineSelection* sel = ctx->refine;
+  const int n = sel ? sel->n_renderers[which] : ctx->render_n[which];
+  const size_t smem = sel ? sel->render_smem[which] : ctx->render_smem[which];
   if (n == 0) return M3TB_OK;
   const int* d_list = ctx->d_render_lists + ctx->n_geometry_list + ctx->n_referenced_list;
   for (int k = 0; k < which; ++k) d_list += ctx->render_n[k];
+  if (sel) d_list = sel->renderers[which];
   RenderArgs a;
   a.renderers = ctx->d_renderers;
   a.render_list = d_list;
@@ -1286,7 +1361,7 @@ int LaunchRender(m3tb_ctx* ctx, int which) {
   k_render<<<unsigned(n), kRenderThreads, smem, ctx->stream>>>(a);
   CU(cudaGetLastError());
   ctx->launches++;
-  for (int r : ctx->render_list[which]) ctx->renderers[r].rendered = true;
+  for (int r : sel ? sel->renderer_ids[which] : ctx->render_list[which]) ctx->renderers[r].rendered = true;
   return M3TB_OK;
 }
 
@@ -2759,6 +2834,192 @@ int m3tb_calculate_consistent_poses(m3tb_ctx* ctx) {
   return LaunchStructure(ctx, 1, false);
 }
 
+// Refiner::RefinePoses (refiner.cpp:76-117) for the named optimisers: Refiner::CalculateConsistentPoses, then per
+// correspondence iteration StartModalities (render, ClearMemory, StartModality(0, corr), InitializeHistograms),
+// CalculateCorrespondences (render, CalculateCorrespondences(0, corr)) and n_update x (CalculateGradientAndHessian,
+// CalculateOptimization). The launches are the tracking step's, restricted to the refined bodies, structures and
+// renderers through RefineSelection; every other body keeps its state.
+int m3tb_refine_poses(m3tb_ctx* ctx, const int* bodies, int n_bodies, const int* structures, int n_structures,
+                      int n_corr_iterations, int n_update_iterations) {
+  CHECK_CTX();
+  if (n_bodies < 0 || n_structures < 0 || (n_bodies > 0 && !bodies) || (n_structures > 0 && !structures))
+    return Fail(ctx, M3TB_ERR_INVALID, "bad body / structure list");
+  if (n_corr_iterations < 0 || n_update_iterations < 0) return Fail(ctx, M3TB_ERR_INVALID, "negative iteration count");
+  const int n_user = int(ctx->structures.size());
+  std::vector<char> in_link(ctx->max_bodies, 0), body_named(ctx->max_bodies, 0), structure_named(n_user, 0);
+  for (const auto& st : ctx->structures)
+    for (const auto& l : st.links) {
+      if (l.body >= 0 && l.body < ctx->max_bodies) in_link[l.body] = 1;
+      for (int x = 0; x < l.n_extra; ++x) in_link[l.extra[x]] = 1;
+    }
+  for (int k = 0; k < n_bodies; ++k) {
+    const int b = bodies[k];
+    if (b < 0 || b >= ctx->n_bodies || !ctx->h_bodies[b].set)
+      return Fail(ctx, M3TB_ERR_INVALID, "body " + std::to_string(b) + " is not set");
+    if (body_named[b]) return Fail(ctx, M3TB_ERR_INVALID, "body " + std::to_string(b) + " listed twice");
+    if (in_link[b])
+      return Fail(ctx, M3TB_ERR_INVALID, "body " + std::to_string(b) + " belongs to a kinematic structure: name the structure");
+    body_named[b] = 1;
+  }
+  for (int k = 0; k < n_structures; ++k) {
+    const int s = structures[k];
+    if (s < 0 || s >= n_user || !ctx->structures[s].set)
+      return Fail(ctx, M3TB_ERR_INVALID, "structure " + std::to_string(s) + " is not set");
+    if (structure_named[s]) return Fail(ctx, M3TB_ERR_INVALID, "structure " + std::to_string(s) + " listed twice");
+    structure_named[s] = 1;
+  }
+  // the bodies whose modalities run: the named ones, then every body of the named structures
+  std::vector<int> track;
+  for (int k = 0; k < n_bodies; ++k) track.push_back(bodies[k]);
+  for (int k = 0; k < n_structures; ++k)
+    for (const auto& l : ctx->structures[structures[k]].links) {
+      if (l.body < 0) continue;
+      if (l.body >= ctx->n_bodies || !ctx->h_bodies[l.body].set)
+        return Fail(ctx, M3TB_ERR_NOT_SET_UP, "structure references a body that is not set");
+      track.push_back(l.body);
+      for (int x = 0; x < l.n_extra; ++x) {
+        if (l.extra[x] >= ctx->n_bodies || !ctx->h_bodies[l.extra[x]].set)
+          return Fail(ctx, M3TB_ERR_NOT_SET_UP, "structure references a body that is not set");
+        track.push_back(l.extra[x]);
+      }
+    }
+  // TextureModality::StartModality detects features in a pose-dependent focus region before every correspondence
+  // iteration; with detection left to the caller one call cannot serve it
+  for (int b : track)
+    if (ctx->h_bodies[b].has_texture)
+      return Fail(ctx, M3TB_ERR_UNSUPPORTED, "body " + std::to_string(b) + " has a texture modality: it cannot be refined");
+  if (track.empty()) return M3TB_OK;  // if (!optimizer_found) return true
+
+  RefineSelection sel;
+  std::vector<int> struct_list;
+  if (HasStructures(ctx)) {
+    int rc = SyncStructures(ctx);
+    if (rc) return rc;
+    for (int k = 0; k < n_structures; ++k) struct_list.push_back(structures[k]);
+    for (int k = 0; k < n_bodies; ++k)  // a rigid body is the implicit one-link structure that SyncStructures appended
+      for (int si = n_user; si < ctx->n_struct_launch; ++si)
+        if (ctx->h_link_bodies[ctx->h_structures[si].first_link] == bodies[k]) struct_list.push_back(si);
+  }
+  if (ctx->n_attached > 0) {
+    int rc = SyncTables(ctx);
+    if (!rc) rc = SyncRenderTables(ctx);
+    if (rc) return rc;
+    for (int which : {int(kRenderAttached), int(kRenderRegion)}) {
+      std::vector<char> use(ctx->renderers.size(), 0);
+      for (int b : track)
+        for (int slot = 0; slot < RS_TEXTURE_SILHOUETTE; ++slot) {
+          const int r = ctx->attached[b][slot];
+          if (r >= 0 && (which == kRenderAttached || slot == RS_REGION_DEPTH || slot == RS_REGION_SILHOUETTE)) use[r] = 1;
+        }
+      for (int r = 0; r < int(use.size()); ++r) {
+        if (!use[r]) continue;
+        const int S = ctx->renderers[r].dev.image_size;
+        sel.renderer_ids[which].push_back(r);
+        sel.render_smem[which] = std::max(sel.render_smem[which], size_t(S) * S * sizeof(uint32_t));
+      }
+    }
+  }
+  // shared ColorHistograms objects with a refined member: the refined members first, only they add line pixels
+  std::vector<int> g_owner, g_first, g_summed, g_members;
+  std::vector<char> tracked(ctx->max_bodies, 0);
+  for (int b : track) tracked[b] = 1;
+  for (int o = 0; o < ctx->n_bodies && o < int(ctx->hist_owner.size()); ++o) {
+    if (ctx->hist_owner[o] != o) continue;
+    std::vector<int> refined, rest;
+    for (int b = 0; b < ctx->n_bodies; ++b)
+      if (ctx->hist_owner[b] == o) (tracked[b] && ctx->h_bodies[b].has_region ? refined : rest).push_back(b);
+    if (refined.empty()) continue;
+    g_owner.push_back(o);
+    g_first.push_back(int(g_members.size()));
+    g_summed.push_back(int(refined.size()));
+    g_members.insert(g_members.end(), refined.begin(), refined.end());
+    g_members.insert(g_members.end(), rest.begin(), rest.end());
+  }
+  g_first.push_back(int(g_members.size()));
+
+  // one device table: bodies | structures | renderers (attached) | renderers (region) | shared-object groups
+  std::vector<int> h(track);
+  const size_t o_struct = h.size();
+  h.insert(h.end(), struct_list.begin(), struct_list.end());
+  size_t o_render[kRenderLists] = {};
+  for (int which : {int(kRenderAttached), int(kRenderRegion)}) {
+    o_render[which] = h.size();
+    h.insert(h.end(), sel.renderer_ids[which].begin(), sel.renderer_ids[which].end());
+  }
+  const size_t o_groups = h.size();
+  if (!g_owner.empty()) {
+    h.insert(h.end(), g_owner.begin(), g_owner.end());
+    h.insert(h.end(), g_first.begin(), g_first.end());
+    h.insert(h.end(), g_summed.begin(), g_summed.end());
+    h.insert(h.end(), g_members.begin(), g_members.end());
+  }
+  DeviceBuffer<int> grown;
+  int rc = GrowTable(ctx, ctx->d_refine, grown, h.size());
+  if (rc) return rc;
+  CU(cudaStreamSynchronize(ctx->stream));  // the launches of an earlier refinement may still read the old lists
+  if (grown) ctx->d_refine = std::move(grown);
+  CU(cudaMemcpyAsync(ctx->d_refine, h.data(), sizeof(int) * h.size(), cudaMemcpyHostToDevice, ctx->stream));
+  CU(cudaStreamSynchronize(ctx->stream));  // `h` is a temporary
+  const int* d = ctx->d_refine;
+  sel.bodies = d;
+  sel.n_bodies = int(track.size());
+  {
+    std::vector<int> sorted(track);
+    std::sort(sorted.begin(), sorted.end());
+    for (int b : sorted) {
+      if (!sel.runs.empty() && sel.runs.back().first + sel.runs.back().second == b) ++sel.runs.back().second;
+      else sel.runs.push_back({b, 1});
+    }
+  }
+  sel.structures = d + o_struct;
+  sel.n_structures = int(struct_list.size());
+  for (int which : {int(kRenderAttached), int(kRenderRegion)}) {
+    sel.renderers[which] = d + o_render[which];
+    sel.n_renderers[which] = int(sel.renderer_ids[which].size());
+  }
+  sel.hist_groups = d + o_groups;
+  sel.n_hist_groups = int(g_owner.size());
+
+  struct Scope {  // every launch helper sees the selection until this call returns
+    m3tb_ctx* c;
+    ~Scope() { c->refine = nullptr; }
+  } scope{ctx};
+  ctx->refine = &sel;
+  const bool structured = !struct_list.empty();
+  if (structured) {  // Refiner::CalculateConsistentPoses
+    rc = LaunchStructure(ctx, 1, false);
+    if (rc) return rc;
+  }
+  for (int b : track) ctx->h_bodies[b].first_iteration = 0;  // StartModality(0, corr)
+  ctx->bodies_dirty = true;
+  const unsigned corr_phases = PH_REGION_CORR | PH_DEPTH_CORR | PH_STORE_REGION | PH_STORE_DEPTH;
+  for (int corr = 0; corr < n_corr_iterations; ++corr) {
+    if (ctx->n_attached > 0) rc = LaunchRender(ctx, kRenderRegion);  // start_modality_renderer_ptrs
+    if (!rc) rc = LaunchHistogram(ctx, 0, 0);
+    if (!rc && ctx->n_attached > 0) rc = LaunchRender(ctx, kRenderAttached);  // correspondence_renderer_ptrs
+    if (rc) return rc;
+    if (!structured) {
+      rc = LaunchTrack(ctx, 0, corr, corr + 1, n_update_iterations, 0,
+                       corr_phases | PH_REGION_GH | PH_DEPTH_GH | PH_SOLVE);
+      if (rc) return rc;
+      continue;
+    }
+    if (n_update_iterations == 0) {
+      rc = LaunchTrack(ctx, 0, corr, corr + 1, 0, 0, corr_phases);
+      if (rc) return rc;
+      continue;
+    }
+    for (int upd = 0; upd < n_update_iterations; ++upd) {
+      rc = LaunchTrack(ctx, 0, corr, corr + 1, 1, upd,
+                       (upd == 0 ? corr_phases : unsigned(PH_LOAD_REGION | PH_LOAD_DEPTH)) | PH_REGION_GH | PH_DEPTH_GH |
+                           PH_STORE_LINK_GH);
+      if (!rc) rc = LaunchStructure(ctx, 0, false);
+      if (rc) return rc;
+    }
+  }
+  return M3TB_OK;
+}
+
 int m3tb_get_link_poses(m3tb_ctx* ctx, int structure, float* body2joint, float* joint2parent, float* link2world) {
   CHECK_CTX();
   if (structure < 0 || structure >= int(ctx->structures.size())) return Fail(ctx, M3TB_ERR_INVALID, "structure index out of range");
@@ -2958,6 +3219,7 @@ int m3tb_prefetch_frames(m3tb_ctx* ctx) {
   a.roi = ctx->d_roi;
   a.bytes = ctx->d_ingest_bytes + ctx->ingest_bytes_slot;
   a.n_bodies = ctx->n_bodies;
+  a.body_list = nullptr;
   // Grid of the prefetch ingest: a quarter of the SMs, CTAs looping over the bodies. k_track2 takes a whole SM per body
   // (1024 threads x 64 registers), so an ingest CTA that sits on an SM keeps a body waiting for as long as the ingest
   // lasts, and whichever kernel is dispatched first wins: with one CTA per body the end-to-end step time swings widely

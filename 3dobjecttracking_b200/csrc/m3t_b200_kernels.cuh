@@ -1657,6 +1657,7 @@ struct HistArgs {
   const CameraDev* depth_cams;  // measured occlusion handling
   int iteration;
   const int* shared_owner;      // per body: -1 = its own ColorHistograms, else the owner of the shared one (or null: none shared)
+  const int* body_list;         // optional: CTA i handles body body_list[i] (m3tb_refine_poses), null: body i
 };
 
 // RegionModality::UseSharedColorHistograms (region_modality.cpp:168-179): the members of a group only ADD their line
@@ -1674,6 +1675,8 @@ struct SharedHistArgs {
   const int* group_owner;   // [n_groups]
   const int* group_first;   // [n_groups + 1] into members
   const int* members;       // body indices, owner first
+  const int* group_summed;  // optional [n_groups]: only members [first, first + summed) add their counts (the refined
+                            //   ones, m3tb_refine_poses); the result still goes to every member. null: all of them
 };
 
 // ---------------------------------------------------------------------------------------------
@@ -1697,6 +1700,7 @@ struct IngestArgs {
   RoiRecord* roi;
   unsigned long long* bytes;  // total bytes fetched by this launch
   int n_bodies;               // the grid may be smaller: CTAs loop over the bodies (see m3tb_prefetch_frames)
+  const int* body_list;       // optional: the n_bodies bodies to fetch for (m3tb_refine_poses), null: bodies 0..n_bodies
 };
 
 __device__ __forceinline__ void IngestRect(const CameraDev& cam, const Tile& t, unsigned bpp, unsigned long long* bytes) {
@@ -1972,8 +1976,8 @@ __global__ void __launch_bounds__(kBlockThreads) k_ingest(IngestArgs args) {
   __shared__ int todo[2];
   __shared__ float s_red[5 * (kBlockThreads / 32)];
   __shared__ int s_view;
-  for (int body_id = blockIdx.x; body_id < args.n_bodies; body_id += gridDim.x) {
-    IngestBody(args, body_id, rect, todo, s_red, s_view);
+  for (int i = blockIdx.x; i < args.n_bodies; i += gridDim.x) {
+    IngestBody(args, args.body_list ? args.body_list[i] : i, rect, todo, s_red, s_view);
     __syncthreads();  // rect / todo belong to the next body now
   }
 }
@@ -1983,7 +1987,7 @@ __device__ __forceinline__ float sgnf_dev(float v) { return v < 0.0f ? -1.0f : (
 __global__ void __launch_bounds__(kBlockThreads) k_histogram(HistArgs args) {
   __shared__ Shared sh;
   __shared__ float s_sum[2][kWarps];
-  const int body_id = blockIdx.x;
+  const int body_id = args.body_list ? args.body_list[blockIdx.x] : int(blockIdx.x);
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   const BodyDev& body = args.bodies[body_id];
   if (!body.set || !body.has_region) return;
@@ -2164,6 +2168,7 @@ __global__ void __launch_bounds__(kBlockThreads) k_histogram_shared(SharedHistAr
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   const int owner = args.group_owner[g];
   const int first = args.group_first[g], last = args.group_first[g + 1];
+  const int summed = args.group_summed ? first + args.group_summed[g] : last;
   const RegionParamsDev& rp = args.bodies[owner].rp;
   const int nbins3 = rp.n_bins * rp.n_bins * rp.n_bins;
   float* mem_f = args.mem_f + size_t(owner) * args.stride;
@@ -2173,12 +2178,12 @@ __global__ void __launch_bounds__(kBlockThreads) k_histogram_shared(SharedHistAr
   float sf = 0.0f, sb = 0.0f;
   for (int k = tid; k < nbins3; k += kBlockThreads) {
     float mf = 0.0f, mb = 0.0f;
-    for (int q = first; q < last; ++q) {
+    for (int q = first; q < summed; ++q) {
       const size_t off = size_t(args.members[q]) * args.stride + k;
       mf += args.mem_f[off];
       mb += args.mem_b[off];
     }
-    mem_f[k] = mf;  // the owner is members[first]: its own counts were read above, by this thread
+    mem_f[k] = mf;  // the owner's own counts, if summed, were read above, by this thread
     mem_b[k] = mb;
     sf += mf;
     sb += mb;

@@ -65,6 +65,7 @@ struct StructArgs {
   int mode;                  // 0: CalculateOptimization, 1: CalculateConsistentPoses (UpdatePoses with theta = 0)
   float* theta_out;          // optional [n_structures][kMaxSystem]
   int* status;               // [n_structures]: 1 updated, 0 NaN guard
+  const int* list;           // optional: CTA i handles structure list[i] (m3tb_refine_poses), null: structure i
 };
 
 __device__ __forceinline__ void Skew3(const float* v, float* m) {
@@ -597,7 +598,8 @@ static __device__ __noinline__ bool StructureSolveBlock(const StructureDev& st, 
 #ifndef M3TB_TRACK_TU
 __global__ void __launch_bounds__(kStructThreads) k_structure(const StructArgs args) {
   extern __shared__ __align__(16) float smem_f[];
-  const StructureDev st = args.structures[blockIdx.x];
+  const int si = args.list ? args.list[blockIdx.x] : int(blockIdx.x);
+  const StructureDev st = args.structures[si];
   LinkDev* links = args.links + st.first_link;
   const ConstraintDev* cons = args.constraints + st.first_constraint;
   const int nl = st.n_links, dof = st.dof, nc = st.n_constraints, n = st.dof + st.n_rows;
@@ -642,8 +644,8 @@ __global__ void __launch_bounds__(kStructThreads) k_structure(const StructArgs a
     UpdatePosesBlock(s, links, nl, tid, T);
     __syncthreads();
   } else {
-    const bool updated = StructureSolveBlock(st, links, cons, s, args.theta_out ? args.theta_out + size_t(blockIdx.x) * kMaxSystem : nullptr, tid, T);
-    if (tid == 0) args.status[blockIdx.x] = updated ? 1 : 0;
+    const bool updated = StructureSolveBlock(st, links, cons, s, args.theta_out ? args.theta_out + size_t(si) * kMaxSystem : nullptr, tid, T);
+    if (tid == 0) args.status[si] = updated ? 1 : 0;
     if (!updated) return;
   }
   // Body::set_body2world_pose of every link that carries a body

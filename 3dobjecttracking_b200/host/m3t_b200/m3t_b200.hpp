@@ -26,6 +26,7 @@
 #include <fstream>
 #include <iostream>
 #include <memory>
+#include <set>
 #include <string>
 #include <vector>
 
@@ -1725,6 +1726,7 @@ class Optimizer {
   const std::vector<std::shared_ptr<Constraint>>& constraint_ptrs() const { return constraint_ptrs_; }
   const std::vector<std::shared_ptr<SoftConstraint>>& soft_constraint_ptrs() const { return soft_constraint_ptrs_; }
   bool set_up() const { return set_up_; }
+  const std::shared_ptr<Batch>& batch() const { return batch_; }
   int structure_index() const { return structure_index_; }
 
   // Optimizer::ReferencedLinks (optimizer.cpp:254-260): pre-order
@@ -2068,6 +2070,77 @@ class Tracker {
   std::vector<std::shared_ptr<Optimizer>> optimizer_ptrs_;
   std::vector<std::shared_ptr<Modality>> modality_ptrs_;
   std::vector<std::shared_ptr<Viewer>> viewer_ptrs_;
+  bool set_up_ = false;
+};
+
+// ---- refiner.h ------------------------------------------------------------------------------------------------------
+// Refiner (refiner.h): refines the poses of the named optimizers, e.g. after a detector, while every other body keeps
+// tracking undisturbed. RefinePoses is one m3tb_refine_poses call: a rigid optimizer is refined through its body, a
+// kinematic structure as a whole.
+class Refiner {
+ public:
+  Refiner(const std::string& name, int n_corr_iterations = 7, int n_update_iterations = 2)
+      : name_(name), n_corr_iterations_(n_corr_iterations), n_update_iterations_(n_update_iterations) {}
+  bool AddOptimizer(const std::shared_ptr<Optimizer>& o) {
+    for (auto& p : optimizer_ptrs_)
+      if (p->name() == o->name()) {
+        std::cerr << "Optimizer " << o->name() << " already exists" << std::endl;
+        return false;
+      }
+    if (!optimizer_ptrs_.empty() && optimizer_ptrs_.front()->batch() != o->batch()) {
+      std::cerr << "Optimizer " << o->name() << " belongs to another batch than refiner " << name_ << std::endl;
+      return false;
+    }
+    optimizer_ptrs_.push_back(o);
+    set_up_ = false;
+    return true;
+  }
+  // Refiner::SetUp (refiner.cpp:24-45) without set_up_all_objects: the optimizers are set up by the tracker (or
+  // their own SetUp), so that the refiner and the tracker share the device records
+  bool SetUp() {
+    set_up_ = false;
+    for (auto& o : optimizer_ptrs_)
+      if (!o->set_up()) {
+        std::cerr << "Optimizer " << o->name() << " was not set up" << std::endl;
+        return false;
+      }
+    set_up_ = true;
+    return true;
+  }
+  // Refiner::RefinePoses (refiner.cpp:76-117): names that match no optimizer are ignored
+  bool RefinePoses(const std::set<std::string>& names) {
+    if (!set_up_) {
+      std::cerr << "Set up refiner " << name_ << " first" << std::endl;
+      return false;
+    }
+    std::vector<int> bodies, structures;
+    for (auto& o : optimizer_ptrs_) {
+      if (names.find(o->name()) == names.end()) continue;
+      if (o->structure_index() >= 0) structures.push_back(o->structure_index());
+      else bodies.push_back(o->root_link_ptr()->body_ptr()->index());
+    }
+    if (bodies.empty() && structures.empty()) return true;
+    const auto& batch = optimizer_ptrs_.front()->batch();
+    const bool ok = Check(batch->ctx(),
+                          m3tb_refine_poses(batch->ctx(), bodies.data(), int(bodies.size()), structures.data(),
+                                            int(structures.size()), n_corr_iterations_, n_update_iterations_),
+                          "Refiner::RefinePoses");
+    batch->PosesChanged();
+    return ok;
+  }
+  void set_name(const std::string& name) { name_ = name; }
+  void set_n_corr_iterations(int v) { n_corr_iterations_ = v; }
+  void set_n_update_iterations(int v) { n_update_iterations_ = v; }
+  const std::string& name() const { return name_; }
+  const std::vector<std::shared_ptr<Optimizer>>& optimizer_ptrs() const { return optimizer_ptrs_; }
+  int n_corr_iterations() const { return n_corr_iterations_; }
+  int n_update_iterations() const { return n_update_iterations_; }
+  bool set_up() const { return set_up_; }
+
+ private:
+  std::string name_;
+  int n_corr_iterations_, n_update_iterations_;
+  std::vector<std::shared_ptr<Optimizer>> optimizer_ptrs_;
   bool set_up_ = false;
 };
 

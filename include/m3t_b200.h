@@ -591,6 +591,22 @@ int m3tb_n_structures(const m3tb_ctx* ctx);
 int m3tb_reset_joint_poses(m3tb_ctx* ctx);
 /* Optimizer::CalculateConsistentPoses (optimizer.cpp:133-142) for every structure. */
 int m3tb_calculate_consistent_poses(m3tb_ctx* ctx);
+/* Refiner::RefinePoses (refiner.cpp:76-117) for the rigid bodies `bodies` and the kinematic structures `structures`
+ * (the Optimizers named). Defaults: n_corr_iterations 7, n_update_iterations 2 (refiner.h:40).
+ * CalculateConsistentPoses of the named structures, then per correspondence iteration: render the start renderers of
+ * the refined bodies, StartModality(0, corr) (first_iteration = 0, ClearMemory, line pixels, InitializeHistograms),
+ * render their correspondence renderers, CalculateCorrespondences(0, corr) and n_update x (CalculateGradientAndHessian +
+ * CalculateOptimization). A shared colour-histogram object with a refined member is initialised from the line pixels
+ * of its refined members only, and every member reads the result. Every other body and structure is left exactly as
+ * it was: poses, joint poses, histograms, lookup tables, per-line / per-point state, first_iteration, texture state and
+ * the images of renderers that no refined body uses. The launches are those of the tracking step with one CTA per
+ * refined body or structure (k_track, never k_track2; k_track once per run of consecutive refined bodies).
+ * Both lists empty: M3TB_OK, nothing is launched. M3TB_ERR_INVALID: an id that is out of range or not set, an id listed
+ * twice, a negative iteration count, or a body that is a link or an extra body of a structure (name the structure).
+ * M3TB_ERR_UNSUPPORTED: a refined body, or a body of a refined structure, has a texture modality
+ * (TextureModality::StartModality detects features before every correspondence iteration, which the caller does). */
+int m3tb_refine_poses(m3tb_ctx* ctx, const int* bodies, int n_bodies, const int* structures, int n_structures,
+                      int n_corr_iterations, int n_update_iterations);
 /* Link::body2joint_pose / joint2parent_pose / link2world_pose of every link of one structure after the last update,
  * each [n_links][12]; any pointer may be NULL. */
 int m3tb_get_link_poses(m3tb_ctx* ctx, int structure, float* body2joint, float* joint2parent, float* link2world);
