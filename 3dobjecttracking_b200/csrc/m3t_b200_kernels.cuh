@@ -708,24 +708,29 @@ struct PointState {  // DepthModality::DataPoint (depth_modality.h:139-150)
   bool valid;
 };
 
-static __device__ __noinline__ void DepthSearchSlow(const DepthIter& it, int u_min, int u_max, int v_min, int v_max, int stride,
-                                             float min_depth_value, float max_depth_value, float x, float y, float z,
-                                             const FrameView& frame, const Tile& tile, const uint16_t* tile_px, float* r) {
-  float best = r[0], bx = r[1], by = r[2], bz = r[3];
+// Rare path of FindCorrespondence: the search window leaves the tile. Takes the camera scalars by value and returns
+// (best, x, y, z) by value, so that neither the caller's DepthIter nor its result has its address taken: an
+// address-taken struct lives in local memory, and k_track2 rebuilt its DepthIter there every update iteration.
+static __device__ __noinline__ float4 DepthSearchSlow(float ppu, float ppv, float fu, float fv, float depth_scale, int u_min,
+                                                      int u_max, int v_min, int v_max, int stride, float min_depth_value,
+                                                      float max_depth_value, float x, float y, float z,
+                                                      const FrameView& frame, const Tile& tile, const uint16_t* tile_px,
+                                                      float best) {
+  float bx = 0.0f, by = 0.0f, bz = 0.0f;
   for (int v = v_min; v <= v_max; v += stride) {
     for (int u = u_min; u <= u_max; u += stride) {
       float depth = float(DepthAt(tile, tile_px, frame, u, v));
       if (depth > min_depth_value && depth < max_depth_value) {
-        depth *= it.depth_scale;
-        float tx = (float(u) - it.ppu) * depth / it.fu;
-        float ty = (float(v) - it.ppv) * depth / it.fv;
+        depth *= depth_scale;
+        float tx = (float(u) - ppu) * depth / fu;
+        float ty = (float(v) - ppv) * depth / fv;
         float dx = tx - x, dy = ty - y, dz = depth - z;
         float d2 = dx * dx + dy * dy + dz * dz;
         if (d2 < best) { bx = tx; by = ty; bz = depth; best = d2; }
       }
     }
   }
-  r[0] = best; r[1] = bx; r[2] = by; r[3] = bz;
+  return make_float4(best, bx, by, bz);
 }
 
 template <bool OCC = false>
@@ -842,10 +847,9 @@ __device__ __forceinline__ void DepthPoint(const DepthIter& it, const DepthParam
       }
     }
   } else {
-    float r[4] = {best, bx, by, bz};
-    DepthSearchSlow(it, u_min, u_max, v_min, v_max, stride, min_depth_value, max_depth_value, x, y, z, frame, tile,
-                    tile_px, r);
-    best = r[0]; bx = r[1]; by = r[2]; bz = r[3];
+    const float4 r = DepthSearchSlow(it.ppu, it.ppv, it.fu, it.fv, it.depth_scale, u_min, u_max, v_min, v_max, stride,
+                                     min_depth_value, max_depth_value, x, y, z, frame, tile, tile_px, best);
+    best = r.x; bx = r.y; by = r.z; bz = r.w;
   }
   if (best == min_considered_distance_square) return;
   P.yx = bx; P.yy = by; P.yz = bz;

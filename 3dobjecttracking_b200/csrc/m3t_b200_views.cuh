@@ -181,9 +181,8 @@ inline int ClosestViewPrunedHost(const ViewClustersHost& vc, const float* ori, i
 // takes member k (a cluster has <= 32 members) and keeps its running maximum in best / idx (ties: smaller view index).
 template <int B>
 __device__ __forceinline__ void EvaluateViewCandidates(unsigned m, unsigned packed, const float4* __restrict__ sorted,
-                                                       float o0, float o1, float o2, float& best, int& idx) {
+                                                       float o0, float o1, float o2, int lane, float& best, int& idx) {
   constexpr unsigned kFull = 0xffffffffu;
-  const int lane = threadIdx.x & 31;
   while (m) {  // warp-uniform
     unsigned pk[B];
 #pragma unroll
@@ -265,7 +264,7 @@ __device__ __forceinline__ int ClosestViewPrunedWarp(const float4* info, const f
         const float ub = ViewClusterBound(ia[h].x, ia[h].y, ia[h].z, ia[h].w, ib[h].x, ib[h].y, ib[h].z, o0, o1, o2, on2, onorm);
         cand = !(ub < lb);  // NaN-safe: a NaN bound keeps the cluster
       }
-      EvaluateViewCandidates<4>(__ballot_sync(kFull, cand), __float_as_uint(ib[h].w), sorted, o0, o1, o2, best, idx);
+      EvaluateViewCandidates<4>(__ballot_sync(kFull, cand), __float_as_uint(ib[h].w), sorted, o0, o1, o2, lane, best, idx);
     }
   }
   unsigned key = ViewKey(best);
@@ -274,10 +273,11 @@ __device__ __forceinline__ int ClosestViewPrunedWarp(const float4* info, const f
 }
 
 // The view that a group search published in `slots`: every thread may call this once the search's barrier has passed,
-// until the second search after it starts writing the same slots.
+// until the second search after it starts writing the same slots. `tid` is the calling thread's index (threadIdx.x): the
+// caller decides where it is read (k_track2 reads it at the use in its 1024-thread kernel, see NestTid).
 template <int G>
-__device__ __forceinline__ int ClosestViewOfSlots(const uint2* slots) {
-  const int lane = threadIdx.x & 31;
+__device__ __forceinline__ int ClosestViewOfSlots(const uint2* slots, int tid) {
+  const int lane = tid & 31;
   const uint2 s = lane < G / 32 ? slots[lane] : make_uint2(0u, 0x7fffffffu);
   unsigned key = s.x;
   int idx = int(s.y);
@@ -294,16 +294,17 @@ __device__ __forceinline__ int ClosestViewOfSlots(const uint2* slots) {
 // k_track2 more spill traffic than it saves). The result does not depend on how the views are split: largest dot
 // product, smallest view index on ties.
 //   slots: G / 32 entries of scratch in shared memory, written on every call (also when there is nothing to search).
+//   tid: the calling thread's index, threadIdx.x (see ClosestViewOfSlots).
 //   Callers alternate two sets between consecutive searches, so that the next search's writes cannot overtake a slow
 //   warp's reads of this one, and ClosestViewOfSlots can re-read this result up to the start of the next-but-one search.
 template <int G, class Barrier>
 __device__ __forceinline__ int ClosestViewPrunedGroup(const float4* info, const float4* __restrict__ sorted,
                                                       int n_clusters, const float4* __restrict__ ori4, int n_views,
-                                                      const float* vo, int prev, uint2* slots, Barrier barrier) {
+                                                      const float* vo, int prev, uint2* slots, int tid, Barrier barrier) {
   constexpr unsigned kFull = 0xffffffffu;
   constexpr int kWarps = G / 32;
   static_assert(kWarps <= 32 && (G & (G - 1)) == 0, "one slot per warp, read by one warp");
-  const int lane = threadIdx.x & 31, warp = (threadIdx.x & (G - 1)) >> 5;
+  const int lane = tid & 31, warp = (tid & (G - 1)) >> 5;
   const bool search = vo[3] != 0.0f && n_views > 0;  // group-uniform; else (|t| = 0) the reference returns views_[0]
   prev = min(max(prev, 0), n_views - 1);
   // the lower bound's view and the first round's cluster tables are requested together (one trip, not two)
@@ -323,14 +324,14 @@ __device__ __forceinline__ int ClosestViewPrunedGroup(const float4* info, const 
       const float lb = o0 * qp.x + o1 * qp.y + o2 * qp.z;
       cand = !(ub < lb);  // NaN-safe: a NaN bound keeps the cluster
     }
-    EvaluateViewCandidates<1>(__ballot_sync(kFull, cand), __float_as_uint(ib.w), sorted, o0, o1, o2, best, idx);
+    EvaluateViewCandidates<1>(__ballot_sync(kFull, cand), __float_as_uint(ib.w), sorted, o0, o1, o2, lane, best, idx);
     if (c + G < n_clusters) { ia = info[2 * (c + G)]; ib = info[2 * (c + G) + 1]; }  // next round (> G clusters)
   }
   unsigned key = ViewKey(best);
   WarpViewArgMax(key, idx);
   if (lane == 0) slots[warp] = make_uint2(key, unsigned(idx));
   barrier();
-  return ClosestViewOfSlots<G>(slots);
+  return ClosestViewOfSlots<G>(slots, tid);
 }
 #endif  // __CUDACC__
 
