@@ -101,6 +101,14 @@ class TextureParams(C.Structure):
 
 
 DESCRIPTOR_ORB = 4
+
+
+class DeviceFeatures(C.Structure):
+    """m3tb_device_features: one body's keypoints (x[i * xy_stride], y[i * xy_stride], crop coordinates) and descriptor
+    rows (descriptor_pitch bytes apart; 32-byte ORB rows with length 0, `length` floats for SIFT / DAISY) in device
+    memory."""
+    _fields_ = [("n", C.c_int), ("length", C.c_int), ("x", C.c_void_p), ("y", C.c_void_p), ("xy_stride", C.c_int),
+                ("descriptors", C.c_void_p), ("descriptor_pitch", C.c_size_t)]
 TEXTURE_POINT_DTYPE = np.dtype([("center_f_body", "<f4", 3), ("correspondence_center", "<f4", 2), ("center", "<f4", 2)])
 
 REGION_LINE_DTYPE = np.dtype([("model_index", "<i4"), ("valid", "<i4"), ("center_f_body", "<f4", 3),
@@ -134,7 +142,8 @@ SYMBOLS = [
     "m3tb_texture_params_default", "m3tb_set_texture_modality", "m3tb_get_texture_focus", "m3tb_upload_texture_features",
     "m3tb_upload_texture_float_features",
     "m3tb_texture_correspondences", "m3tb_texture_gradient_hessian", "m3tb_get_texture_points",
-    "m3tb_get_texture_keyframes",
+    "m3tb_get_texture_keyframes", "m3tb_texture_crop", "m3tb_upload_texture_features_device",
+    "m3tb_get_texture_feature_flags",
 ]
 
 KERNEL_NAMES = {0: None, 1: "k_track", 2: "k_track2", 3: "k_track_cluster"}
@@ -262,6 +271,9 @@ def lib():
     L.m3tb_texture_gradient_hessian.argtypes = [vp, ci, ci, ci, fp, fp]
     L.m3tb_get_texture_points.argtypes = [vp, ci, vp, ci, C.POINTER(ci)]
     L.m3tb_get_texture_keyframes.argtypes = [vp, ci, C.POINTER(ci), ip, fp, vp, ci, C.POINTER(ci), fp]
+    L.m3tb_texture_crop.argtypes = [vp, ip, ci, vp, C.c_size_t, C.c_size_t, ci, ci, ip, fp, ip, ip]
+    L.m3tb_upload_texture_features_device.argtypes = [vp, ip, C.POINTER(DeviceFeatures), ci]
+    L.m3tb_get_texture_feature_flags.argtypes = [vp, ci, ci, ip]
     L.m3tb_get_full_rendering.argtypes = [vp, ci, vp, C.c_size_t, vp, C.c_size_t, vp, C.c_size_t, fp, fp]
     L.m3tb_undistortion_map.argtypes = [C.POINTER(Intrinsics), fp, C.POINTER(Intrinsics), vp, C.c_size_t]
     L.m3tb_set_camera_undistortion.argtypes = [vp, ci, ci, vp, C.c_size_t, ci, C.c_int32]
@@ -871,6 +883,39 @@ class Context:
         d = np.ascontiguousarray(np.asarray(descriptors, np.uint8).reshape(-1, 32))
         self._ck(self.L.m3tb_upload_texture_features(self.h, body, _p(xy), d.ctypes.data_as(C.c_void_p), xy.shape[0],
                                                      int(roi_x), int(roi_y), float(scale)))
+
+    def texture_crop(self, bodies, ptr, pitch, body_stride, capacity_width, capacity_height):
+        """The focused grey images of `bodies` into device memory at ptr (e.g. a torch uint8 tensor's data_ptr()):
+        body k's crop at ptr + k * body_stride, rows `pitch` bytes apart, at most capacity_width x capacity_height.
+        Returns (roi [n, 4] int32, scale [n] float32, size [n, 2] int32 width, height, valid [n] bool)."""
+        ids = np.ascontiguousarray(bodies, np.int32).reshape(-1)
+        n = len(ids)
+        roi = np.zeros((max(n, 1), 4), np.int32)
+        scale = np.zeros(max(n, 1), np.float32)
+        size = np.zeros((max(n, 1), 2), np.int32)
+        valid = np.zeros(max(n, 1), np.int32)
+        ip = C.POINTER(C.c_int)
+        self._ck(self.L.m3tb_texture_crop(self.h, ids.ctypes.data_as(ip), n, C.c_void_p(ptr), pitch, body_stride,
+                                          capacity_width, capacity_height, roi.ctypes.data_as(ip), _p(scale),
+                                          size.ctypes.data_as(ip), valid.ctypes.data_as(ip)))
+        return roi[:n], scale[:n], size[:n], valid[:n].astype(bool)
+
+    def upload_texture_features_device(self, bodies, features):
+        """features: one DeviceFeatures per body (m3tb_upload_texture_features_device); does not synchronise."""
+        ids = np.ascontiguousarray(bodies, np.int32).reshape(-1)
+        arr = (DeviceFeatures * max(len(ids), 1))(*features)
+        self._ck(self.L.m3tb_upload_texture_features_device(self.h, ids.ctypes.data_as(C.POINTER(C.c_int)), arr,
+                                                            len(ids)))
+        for b, f in zip(ids, features):
+            if f.length and self._texture_length.get(int(b)) == 0:
+                self._texture_length[int(b)] = f.length
+
+    def get_texture_feature_flags(self, first=0, count=None):
+        """[count] bool: the body's last device upload held a non-finite descriptor value and was dropped."""
+        count = self.n_bodies - first if count is None else count
+        out = np.zeros(max(count, 1), np.int32)
+        self._ck(self.L.m3tb_get_texture_feature_flags(self.h, first, count, out.ctypes.data_as(C.POINTER(C.c_int))))
+        return out[:count].astype(bool)
 
     def texture_correspondences(self, iteration, corr_iteration):
         self._ck(self.L.m3tb_texture_correspondences(self.h, iteration, corr_iteration))

@@ -432,4 +432,112 @@ __global__ void __launch_bounds__(kTexThreads) k_texture_match(const __grid_cons
   }
 }
 
+namespace {
+
+// cvtColor(BGR2GRAY) on 8-bit pixels: equal to OpenCV's result on all 2^24 triples
+// (tests/texture_crop_reference.py)
+__device__ __forceinline__ int Grey(const uint8_t* p) {
+  return (3735 * int(p[0]) + 19235 * int(p[1]) + 9798 * int(p[2]) + 16384) >> 15;
+}
+
+// cv::resize's INTER_LINEAR coefficient of output position d (resize.cpp): the two source positions and their weights
+// in 1/2048. Columns pin a position before the first or at the last source pixel to it with weights (2048, 0); rows
+// keep their weights and only clamp the two source rows. The build compiles without FMA contraction, so
+// (d + 0.5) * inv - 0.5 rounds twice in double, as on the host.
+struct Tap {
+  int s0, s1, w0, w1;
+};
+__device__ __forceinline__ Tap LinearTap(int d, double inv, int n, bool column) {
+  float f = float((double(d) + 0.5) * inv - 0.5);
+  int s = int(floorf(f));
+  f -= float(s);
+  if (column && s < 0) { s = 0; f = 0.0f; }
+  if (column && s >= n - 1) { s = n - 1; f = 0.0f; }
+  Tap t;
+  t.w0 = __float2int_rn((1.0f - f) * 2048.0f);
+  t.w1 = __float2int_rn(f * 2048.0f);
+  t.s0 = min(max(s, 0), n - 1);
+  t.s1 = min(max(s + 1, 0), n - 1);
+  return t;
+}
+
+__device__ __forceinline__ int GreyAt(const TexCropJob& j, int x, int y) {
+  return Grey(j.src + size_t(j.roi_y + y) * j.src_pitch + size_t(j.roi_x + x) * 3u);
+}
+
+// One output pixel (tests/texture_crop_reference.py states every case)
+__device__ __forceinline__ uint8_t CropPixel(const TexCropJob& j, int dx, int dy, double inv, bool area, bool copy) {
+  if (copy) return uint8_t(GreyAt(j, dx, dy));
+  if (area) {  // cv::resize's fast INTER_AREA path at exactly 2x
+    const int x0 = 2 * dx, y0 = 2 * dy;
+    const bool full_row = 2 * (dy + 1) <= j.roi_h;
+    if (full_row && x0 + 1 < j.roi_w)
+      return uint8_t((GreyAt(j, x0, y0) + GreyAt(j, x0 + 1, y0) + GreyAt(j, x0, y0 + 1) + GreyAt(j, x0 + 1, y0 + 1) + 2) >> 2);
+    int sum = 0, count = 0;
+    for (int y = y0; y < min(y0 + 2, j.roi_h); ++y)
+      for (int x = x0; x < min(x0 + 2, j.roi_w); ++x) {
+        sum += GreyAt(j, x, y);
+        ++count;
+      }
+    return uint8_t(min(__float2int_rn(float(sum) / float(count)), 255));
+  }
+  const Tap tx = LinearTap(dx, inv, j.roi_w, true), ty = LinearTap(dy, inv, j.roi_h, false);
+  const int h0 = GreyAt(j, tx.s0, ty.s0) * tx.w0 + GreyAt(j, tx.s1, ty.s0) * tx.w1;
+  const int h1 = GreyAt(j, tx.s0, ty.s1) * tx.w0 + GreyAt(j, tx.s1, ty.s1) * tx.w1;
+  // OpenCV's vectorised vertical pass: 16-bit high products of the weights and the sums shifted by 4
+  const int v = (((ty.w0 * min(h0 >> 4, 32767)) >> 16) + ((ty.w1 * min(h1 >> 4, 32767)) >> 16) + 2) >> 2;
+  return uint8_t(min(max(v, 0), 255));
+}
+
+}  // namespace
+
+// Each thread writes kTexCropPixels consecutive pixels of one output row of job blockIdx.y.
+__global__ void __launch_bounds__(kTexCropThreads) k_texture_crop(const __grid_constant__ TexCropArgs a) {
+  const TexCropJob& j = a.jobs[blockIdx.y];
+  const int groups = (j.out_w + kTexCropPixels - 1) / kTexCropPixels;
+  const int t = blockIdx.x * kTexCropThreads + threadIdx.x;
+  if (t >= groups * j.out_h) return;
+  const int dy = t / groups, dx0 = (t - dy * groups) * kTexCropPixels;
+  const bool copy = j.out_w == j.roi_w && j.out_h == j.roi_h;
+  const bool area = !copy && j.scale == 0.5f;
+  const double inv = 1.0 / double(j.scale);
+  uint8_t* row = j.dst + size_t(dy) * a.dst_pitch;
+#pragma unroll
+  for (int k = 0; k < kTexCropPixels; ++k)
+    if (dx0 + k < j.out_w) row[dx0 + k] = CropPixel(j, dx0 + k, dy, inv, area, copy);
+}
+
+// The host upload's conversion (UploadTextureFeatures): keypoint roi + pt / scale, descriptors into the frame tables.
+// Float descriptors are checked here: a body with a non-finite value gets no features and its flag is raised.
+__global__ void __launch_bounds__(kTexThreads) k_texture_features(const __grid_constant__ TexFeatArgs a) {
+  const TexFeatJob& j = a.jobs[blockIdx.x];
+  const int tid = threadIdx.x, b = j.body;
+  float2* xy = a.feat_xy + size_t(b) * kTexMaxFeatures;
+  for (int i = tid; i < j.n; i += kTexThreads) {
+    const float x = j.x[size_t(i) * j.xy_stride], y = j.y[size_t(i) * j.xy_stride];
+    xy[i] = make_float2(float(j.roi_x) + x / j.scale, float(j.roi_y) + y / j.scale);
+  }
+  int bad = 0;
+  if (j.length == 0) {
+    uint32_t* dst = a.feat_desc + size_t(b) * kTexMaxFeatures * kTexDescWords;
+    for (int e = tid; e < j.n * 32; e += kTexThreads) {  // byte by byte: the caller's rows need no alignment
+      const int i = e >> 5, c = e & 31;
+      reinterpret_cast<uint8_t*>(dst)[e] = j.desc[size_t(i) * j.desc_pitch + c];
+    }
+  } else {
+    float* dst = a.feat_fdesc + size_t(b) * kTexMaxFeatures * kTexMaxFloatDesc;
+    for (int e = tid; e < j.n * j.length; e += kTexThreads) {
+      const int i = e / j.length, c = e - i * j.length;
+      const float v = reinterpret_cast<const float*>(j.desc + size_t(i) * j.desc_pitch)[c];
+      bad |= !isfinite(v);
+      dst[size_t(i) * kTexMaxFloatDesc + c] = v;
+    }
+  }
+  bad = __syncthreads_or(bad);
+  if (tid == 0) {
+    a.feat_n[b] = bad ? 0 : j.n;
+    a.nonfinite[b] = bad;
+  }
+}
+
 }  // namespace m3tb

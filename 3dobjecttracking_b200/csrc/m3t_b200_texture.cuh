@@ -65,6 +65,56 @@ __host__ __device__ constexpr int KnnSharedBytes(int length) {
 }
 __global__ void k_texture_knn_l2(const __grid_constant__ TextureArgs a);
 
+// k_texture_crop / k_texture_features: up to kTexJobs bodies per launch; the jobs travel in the kernel parameters
+constexpr int kTexJobs = 128;
+constexpr int kTexCropThreads = 256;
+constexpr int kTexCropPixels = 4;  // output pixels per thread (one row, consecutive columns)
+
+// One body's focused grey image (DetectAndComputeCorrKeypoints, texture_modality.cpp:862-868):
+// resize(cvtColor(image, BGR2GRAY)(roi), Size(), scale, scale, INTER_LINEAR) into out_w x out_h bytes at dst.
+struct TexCropJob {
+  const uint8_t* src;  // BGR8 frame: the camera's device copy, or its pinned frame read in place
+  uint8_t* dst;        // rows dst_pitch apart (TexCropArgs)
+  unsigned src_pitch;
+  int roi_x, roi_y, roi_w, roi_h;
+  int out_w, out_h;
+  float scale;
+};
+
+struct TexCropArgs {
+  TexCropJob jobs[kTexJobs];
+  size_t dst_pitch;
+  int n_jobs;
+};
+
+// grid: (ceil(max over jobs of ceil(out_w / kTexCropPixels) * out_h / kTexCropThreads), n_jobs)
+__global__ void k_texture_crop(const __grid_constant__ TexCropArgs a);
+
+// One body's features from device memory, converted as the host upload converts them.
+struct TexFeatJob {
+  const float* x;        // keypoint i at x[i * xy_stride], y[i * xy_stride] (crop coordinates)
+  const float* y;
+  const uint8_t* desc;   // descriptor row i at desc + i * desc_pitch: 32 bytes (ORB) or `length` floats
+  size_t desc_pitch;
+  int body, n, xy_stride, length;  // length 0: ORB
+  int roi_x, roi_y;
+  float scale;
+  int pad;
+};
+
+struct TexFeatArgs {
+  TexFeatJob jobs[kTexJobs];
+  float2* feat_xy;       // TextureArgs' frame-feature tables
+  uint32_t* feat_desc;
+  float* feat_fdesc;
+  int* feat_n;
+  int* nonfinite;        // [n_bodies] 1: the body's last device upload held a non-finite descriptor value
+  int n_jobs;
+};
+
+// one CTA of kTexThreads per job
+__global__ void k_texture_features(const __grid_constant__ TexFeatArgs a);
+
 // TextureModality::TukeyNorm (texture_modality.cpp:1231-1237)
 __host__ __device__ __forceinline__ float TexTukeyNorm(float error, float c) {
   if (fabsf(error) <= c) return powf(c, 2.0f) / 6.0f * (1.0f - powf(1.0f - powf(error / c, 2.0f), 3.0f));

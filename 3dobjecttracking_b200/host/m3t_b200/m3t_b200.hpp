@@ -106,6 +106,31 @@ class Batch {
 
   std::vector<float> region_g, region_h, depth_g, depth_h, texture_g, texture_h;  // last batched gradients / Hessians (all bodies)
 
+  // Texture features uploaded from device memory (TextureModality::SetFeatures(const m3tb_device_features&)): their
+  // float descriptors are checked on the device, so whether a body's were dropped as non-finite is known once the
+  // stream has passed the upload. Every synchronising read of the mirror (Body::body2world_pose, the texture
+  // gradient / Hessian) reports it here: a message on std::cerr, and features_dropped(body) until the next upload.
+  void NoteDeviceFeatures(int body) {
+    pending_features_.push_back(body);
+    if (int(dropped_.size()) <= body) dropped_.resize(size_t(body) + 1, 0);
+    dropped_[body] = 0;
+  }
+  bool ReportDroppedFeatures() {
+    for (int b : pending_features_) {
+      int32_t nonfinite = 0;
+      if (m3tb_get_texture_feature_flags(ctx_, b, 1, &nonfinite) != M3TB_OK) {
+        std::cerr << "m3tb_get_texture_feature_flags: " << m3tb_last_error(ctx_) << std::endl;
+        return false;
+      }
+      dropped_[b] = nonfinite != 0;
+      if (nonfinite)
+        std::cerr << "Body " << b << ": non-finite texture descriptor, the frame's features were dropped" << std::endl;
+    }
+    pending_features_.clear();
+    return true;
+  }
+  bool features_dropped(int body) const { return body < int(dropped_.size()) && dropped_[body]; }
+
  private:
   m3tb_ctx* ctx_ = nullptr;
   int max_bodies_ = 0, n_bodies_ = 0, n_renderers_ = 0, n_color_ = 0, n_depth_ = 0, n_rmodels_ = 0, n_dmodels_ = 0, n_structures_ = 0;
@@ -113,6 +138,8 @@ class Batch {
   long viewer_version_ = 0;
   long pose_version_ = 0;
   Key done_[kNPhases];
+  std::vector<int> pending_features_;
+  std::vector<char> dropped_;
 };
 
 // ---- body.h --------------------------------------------------------------------------------------------------------
@@ -132,6 +159,7 @@ class Body {
   // Body::body2world_pose(): reads the pose back from the device (it is updated there by the optimizer)
   const Transform3fA& body2world_pose() {
     Check(batch_->ctx(), m3tb_get_poses(batch_->ctx(), index_, 1, body2world_pose_.data()), "Body::body2world_pose");
+    batch_->ReportDroppedFeatures();
     return body2world_pose_;
   }
   // geometry setters (body.h:57-66). The mesh is handed over as the triangle soup Body::SetUp would load from
@@ -1524,6 +1552,67 @@ class TextureModality : public Modality {
                                                     descriptors.data(), n, length, roi[0], roi[1], scale),
                  "TextureModality::SetFeatures");
   }
+  // The device crops of several texture modalities of one Batch in ONE m3tb_texture_crop call (one pose download, one
+  // stream synchronisation, one launch per 128 bodies): modality k's focused grey image of CalculateFocus's region
+  // (cvtColor BGR2GRAY, roi, resize by scale, bit-exact against OpenCV) at d_out + k * body_stride in device memory,
+  // rows `pitch` bytes apart; per modality its roi, scale, size (width, height) and whether it has a focus. Each crop
+  // also records the focus that SetFeatures(const m3tb_device_features&) uses. False on an error, e.g. a crop larger
+  // than capacity_width x capacity_height (sizes are still filled then).
+  static bool CropFocusedImages(const std::vector<std::shared_ptr<TextureModality>>& modalities, uint8_t* d_out,
+                                size_t pitch, size_t body_stride, int capacity_width, int capacity_height,
+                                std::vector<std::array<int32_t, 4>>* rois, std::vector<float>* scales,
+                                std::vector<std::array<int32_t, 2>>* sizes, std::vector<char>* valid) {
+    const size_t n = modalities.size();
+    rois->assign(n, {});
+    scales->assign(n, 0.0f);
+    sizes->assign(n, {});
+    valid->assign(n, 0);
+    if (n == 0) return true;
+    m3tb_ctx* ctx = modalities[0]->batch_->ctx();
+    std::vector<int> bodies;
+    for (auto& m : modalities) {
+      if (m->batch_->ctx() != ctx) {
+        std::cerr << "TextureModality::CropFocusedImages: the modalities belong to different batches" << std::endl;
+        return false;
+      }
+      bodies.push_back(m->body_ptr_->index());
+    }
+    std::vector<int32_t> roi(4 * n), size(2 * n), ok(n);
+    const bool done = Check(ctx, m3tb_texture_crop(ctx, bodies.data(), int(n), d_out, pitch, body_stride, capacity_width,
+                                                   capacity_height, roi.data(), scales->data(), size.data(), ok.data()),
+                            "TextureModality::CropFocusedImages");
+    for (size_t k = 0; k < n; ++k) {
+      for (int c = 0; c < 4; ++c) (*rois)[k][c] = roi[4 * k + c];
+      (*sizes)[k] = {size[2 * k], size[2 * k + 1]};
+      (*valid)[k] = ok[k] != 0;
+    }
+    return done;
+  }
+  // One modality's device crop; each call synchronises the stream, so several bodies go through CropFocusedImages
+  bool CropFocusedImage(uint8_t* d_out, size_t pitch, int capacity_width, int capacity_height,
+                        std::array<int32_t, 2>* size) {
+    std::vector<std::array<int32_t, 4>> rois;
+    std::vector<float> scales;
+    std::vector<std::array<int32_t, 2>> sizes;
+    std::vector<char> valid;
+    std::vector<std::shared_ptr<TextureModality>> self{std::shared_ptr<TextureModality>(this, [](TextureModality*) {})};
+    if (!CropFocusedImages(self, d_out, pitch, pitch * size_t(capacity_height), capacity_width, capacity_height, &rois,
+                           &scales, &sizes, &valid))
+      return false;
+    *size = sizes[0];
+    return valid[0] != 0;
+  }
+  // SetFeatures from device memory (e.g. cv::cuda::ORB's GpuMat keypoints and descriptors) in the crop of the last
+  // CropFocusedImage(s); does not synchronise. A non-finite float descriptor drops the frame's features on the device;
+  // the Batch reports it at the next synchronising read.
+  bool SetFeatures(const m3tb_device_features& features) {
+    const int body = body_ptr_->index();
+    if (!Check(batch_->ctx(), m3tb_upload_texture_features_device(batch_->ctx(), &body, &features, 1),
+               "TextureModality::SetFeatures"))
+      return false;
+    if (features.length != 0) batch_->NoteDeviceFeatures(body);
+    return true;
+  }
 
   bool StartModality(int iteration, int corr_iteration) override {
     if (!IsSetup()) return false;
@@ -1549,7 +1638,7 @@ class TextureModality : public Modality {
         return false;
     }
     FetchGH(batch_->texture_g, batch_->texture_h);
-    return true;
+    return batch_->ReportDroppedFeatures();  // the sums above synchronised the stream
   }
   bool CalculateResults(int iteration) override {
     if (!IsSetup()) return false;

@@ -514,6 +514,48 @@ int m3tb_upload_texture_features(m3tb_ctx* ctx, int body, const float* keypoints
  * length later, for a non-finite descriptor value and for an ORB body. */
 int m3tb_upload_texture_float_features(m3tb_ctx* ctx, int body, const float* keypoints_xy, const float* descriptors,
                                        int n, int length, int roi_x, int roi_y, float scale);
+/* The focused grey images of bodies[0 .. count) on the device (k_texture_crop, one launch per 128 bodies): what
+ * DetectAndComputeCorrKeypoints hands the detector (texture_modality.cpp:862-868),
+ *   cv::cvtColor(color_camera_ptr_->image(), image, cv::COLOR_BGR2GRAY);
+ *   cv::resize(image(roi), image, cv::Size(), scale, scale);   (INTER_LINEAR)
+ * bit for bit as OpenCV computes it (DESIGN.md §3 "k_texture_crop"). roi and scale are m3tb_get_texture_focus's, from
+ * the current device poses; the source is the camera's current frame wherever it is (a device copy, the rectified
+ * frame of an undistorting camera, or a pinned frame read in place, whichever ROIs were fetched). Body k's crop is
+ * size[2k] x size[2k + 1] bytes at out + k * body_stride, rows `pitch` bytes apart (device memory the caller owns),
+ * size = saturate_cast<int>(roi.w * (double)scale) x ... as cv::resize sizes it; it grows with the distance of the
+ * body. roi [count][4], scale [count], size [count][2] and valid [count] (0: no focus, nothing written) may be NULL.
+ * The crop also records the body's roi, scale and frame for m3tb_upload_texture_features_device. M3TB_ERR_INVALID,
+ * with nothing launched or recorded but the outputs filled, when a crop exceeds capacity_width x capacity_height;
+ * M3TB_ERR_INVALID for a body without a texture modality or listed twice. Synchronises the stream once (poses). */
+int m3tb_texture_crop(m3tb_ctx* ctx, const int* bodies, int count, uint8_t* out, size_t pitch, size_t body_stride,
+                      int capacity_width, int capacity_height, int32_t* roi, float* scale, int32_t* size, int32_t* valid);
+/* One body's features in device memory (cv::cuda::ORB's GpuMat keypoints and descriptors, a torch detector's
+ * tensors): keypoint i at x[i * xy_stride], y[i * xy_stride] in crop coordinates (GpuMat rows: x and y rows of the
+ * keypoint matrix, stride 1; interleaved xy: y = x + 1, stride 2); descriptor row i at descriptors + i *
+ * descriptor_pitch bytes, 32 bytes for ORB (length 0) or `length` floats for SIFT / DAISY (4-byte aligned). */
+typedef struct m3tb_device_features {
+  int n;
+  int length;
+  const float* x;
+  const float* y;
+  int xy_stride;
+  const void* descriptors;
+  size_t descriptor_pitch;
+} m3tb_device_features;
+/* m3tb_upload_texture_features / _float_features for bodies[0 .. count) from device memory, in one k_texture_features
+ * launch per 128 bodies and without synchronising: keypoints become float(roi_x) + x / scale with the roi and scale of
+ * the body's last m3tb_texture_crop. Replaces, per body and frame, the host copy of the detector's output
+ * (DetectAndComputeCorrKeypoints, texture_modality.cpp:870-887). Refusals as the host upload (M3TB_ERR_UNSUPPORTED
+ * above 512 features; M3TB_ERR_INVALID for the other descriptor kind, a bad length and a length other than the first
+ * upload's), and M3TB_ERR_INVALID for a body whose last crop is not of its camera's current frame; nothing is launched
+ * when any body is refused. Float descriptors are checked on the device: a body with a non-finite value gets no
+ * features this frame and its flag (m3tb_get_texture_feature_flags) is raised. The caller keeps the buffers unchanged
+ * until the stream has passed the upload (any synchronising call). */
+int m3tb_upload_texture_features_device(m3tb_ctx* ctx, const int* bodies, const m3tb_device_features* features,
+                                        int count);
+/* nonfinite[k] = 1 when body first + k's last m3tb_upload_texture_features_device held a non-finite descriptor
+ * value (its features were dropped). Synchronises the stream. */
+int m3tb_get_texture_feature_flags(m3tb_ctx* ctx, int first, int count, int32_t* nonfinite);
 /* TextureModality::CalculateCorrespondences (texture_modality.cpp:322-386) for every body with a texture modality:
  * matching at corr_iteration 0, the data points' projection (center) at every iteration. */
 int m3tb_texture_correspondences(m3tb_ctx* ctx, int iteration, int corr_iteration);
