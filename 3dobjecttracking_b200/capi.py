@@ -97,10 +97,12 @@ class TextureParams(C.Structure):
                 ("max_keyframe_rotation_difference", C.c_float), ("max_keyframe_age", C.c_int32),
                 ("n_keyframes", C.c_int32), ("measure_occlusions", C.c_int32), ("measured_occlusion_radius", C.c_float),
                 ("measured_occlusion_threshold", C.c_float), ("model_occlusions", C.c_int32),
-                ("modeled_occlusion_radius", C.c_float), ("modeled_occlusion_threshold", C.c_float)]
+                ("modeled_occlusion_radius", C.c_float), ("modeled_occlusion_threshold", C.c_float),
+                ("n_features_max", C.c_int32)]  # device capacity: 512 .. 4096 features per upload
 
 
 DESCRIPTOR_ORB = 4
+TEXTURE_POINT_LIMIT = 8 * 4096  # a full deque of 8 keyframes at n_features_max 4096
 
 
 class DeviceFeatures(C.Structure):
@@ -926,13 +928,13 @@ class Context:
         self._ck(self.L.m3tb_texture_gradient_hessian(self.h, iteration, corr_iteration, opt_iteration, _p(g), _p(H)))
         return g, H
 
-    def get_texture_points(self, body, capacity=4096):
+    def get_texture_points(self, body, capacity=TEXTURE_POINT_LIMIT):
         out = np.zeros(capacity, TEXTURE_POINT_DTYPE)
         n = C.c_int(0)
         self._ck(self.L.m3tb_get_texture_points(self.h, body, out.ctypes.data_as(C.c_void_p), capacity, C.byref(n)))
         return out[:min(n.value, capacity)]
 
-    def get_texture_keyframes(self, body, capacity=4096):
+    def get_texture_keyframes(self, body, capacity=TEXTURE_POINT_LIMIT):
         """dict(sizes [n_keyframes], points [total, 3] float32, descriptors, age, orientation [3]). descriptors:
         [total, 32] uint8 for ORB; [total, length] float32 for a SIFT / DAISY body, length that of its uploads."""
         length = self._texture_length.get(body)

@@ -281,14 +281,16 @@ struct m3tb_ctx {
   // texture modality (m3tb_set_texture_modality, k_texture_keyframe / k_texture_match): tables for max_bodies, made by
   // the first m3tb_set_texture_modality (TextureArgs for the layouts)
   int n_texture = 0;                    // bodies with a texture modality
+  int tex_cap = 0;                      // features per body of the tables (TextureArgs::cap); 0 before they exist
   std::vector<int> tex_feat_gen;        // per body: colour-frame generation its features belong to, -1: none
   DeviceBuffer<float2> d_tex_xy;
   DeviceBuffer<uint32_t> d_tex_desc, d_tex_kf_desc;
   DeviceBuffer<int> d_tex_nfeat, d_tex_kf_n, d_tex_counts;
   DeviceBuffer<float> d_tex_kf_points, d_tex_points, d_tex_pose, d_gh_texture;
   DeviceBuffer<TexKeyframeState> d_tex_kf_state;
-  // float descriptors (SIFT / DAISY) and k_texture_knn_l2's matches: made by the first m3tb_set_texture_modality with
-  // an L2 descriptor type, never for contexts with ORB bodies only
+  // float descriptors (SIFT / DAISY): made by the first m3tb_set_texture_modality with an L2 descriptor type; the
+  // matches of k_texture_knn_l2 / _hamming: made with them or by the first ORB body above kTexMaxFeatures. Contexts
+  // whose ORB bodies keep the default n_features_max have neither.
   DeviceBuffer<float> d_tex_fdesc, d_tex_kf_fdesc;
   DeviceBuffer<int> d_tex_knn;
   // device front end (m3tb_texture_crop / m3tb_upload_texture_features_device): per body, the focus of its last crop
@@ -700,7 +702,7 @@ TrackArgs RunArgs(const TrackArgs& a, int first) {
   r.gh_depth = shift(a.gh_depth, 27 * f);
   r.gh_link = shift(a.gh_link, 27 * f);
   r.gh_texture = shift(a.gh_texture, 27 * f);
-  r.tex_points = shift(a.tex_points, f * TF_COUNT * kTexPointCap);
+  r.tex_points = shift(a.tex_points, f * TF_COUNT * size_t(a.tex_point_cap));
   r.tex_counts = shift(a.tex_counts, f);
   r.tex_pose = shift(a.tex_pose, 12 * f);
   r.phase_clock = shift(a.phase_clock, f * kPhaseSlots);
@@ -752,6 +754,7 @@ int LaunchTrack(m3tb_ctx* ctx, int iteration, int corr_begin, int corr_end, int 
   a.tex_counts = ctx->d_tex_counts;
   a.tex_pose = ctx->d_tex_pose;
   a.gh_texture = ctx->d_gh_texture;
+  a.tex_point_cap = kTexMaxKeyframes * ctx->tex_cap;
   a.iteration = iteration;
   a.corr_begin = corr_begin;
   a.corr_end = corr_end;
@@ -4201,65 +4204,109 @@ void m3tb_texture_params_default(m3tb_texture_params* p) {
   p->measured_occlusion_threshold = 0.03f;
   p->modeled_occlusion_radius = 0.01f;
   p->modeled_occlusion_threshold = 0.03f;
+  p->n_features_max = kTexMaxFeatures;
 }
 
 }  // extern "C"
 
 namespace {
 
-// The texture tables for max_bodies, all or nothing (first m3tb_set_texture_modality); with l2 also the float
-// descriptor tables (first L2 descriptor type), in the same all-or-nothing step
-int EnsureTextureTables(m3tb_ctx* ctx, bool l2) {
-  const size_t nb = size_t(ctx->max_bodies);
-  DeviceBuffer<float> fdesc, kf_fdesc;
-  DeviceBuffer<int> knn;
-  if (l2 && !ctx->d_tex_fdesc) {
-    CU(fdesc.create(nb * kTexMaxFeatures * kTexMaxFloatDesc));
-    CU(kf_fdesc.create(nb * kTexMaxKeyframes * kTexMaxFeatures * kTexMaxFloatDesc));
-    CU(knn.create(nb * kTexMaxKeyframes * kTexMaxFeatures));
-    if (!ctx->d_tex_xy) {
-      int rc = EnsureTextureTables(ctx, false);
-      if (rc) return rc;
-    }
-    ctx->d_tex_fdesc = std::move(fdesc);
-    ctx->d_tex_kf_fdesc = std::move(kf_fdesc);
-    ctx->d_tex_knn = std::move(knn);
-    return M3TB_OK;
+// One capacity-sized texture table: `rows` rows of per_feature * cap elements. make() creates its replacement at
+// capacity `cap` (when it is wanted and missing, or the tables grow), copy() moves each row of the table it replaces to
+// the front of its new row, replace() swaps it in.
+template <typename T>
+struct TexTable {
+  DeviceBuffer<T>& cur;
+  size_t rows, per_feature;
+  DeviceBuffer<T> out;
+  cudaError_t make(bool want, bool grow, int cap) {
+    return want && (grow || !cur) ? out.create(rows * per_feature * size_t(cap)) : cudaSuccess;
   }
-  if (ctx->d_tex_xy) return M3TB_OK;
-  DeviceBuffer<float2> xy;
-  DeviceBuffer<uint32_t> desc, kf_desc;
+  cudaError_t copy(int old_cap, int cap, cudaStream_t stream) {
+    if (!out || !cur) return cudaSuccess;
+    const size_t w_old = sizeof(T) * per_feature * size_t(old_cap), w_new = sizeof(T) * per_feature * size_t(cap);
+    return cudaMemcpy2DAsync(out, w_new, cur, w_old, w_old, rows, cudaMemcpyDeviceToDevice, stream);
+  }
+  void replace() {
+    if (out) cur = std::move(out);
+  }
+};
+
+// The texture tables for max_bodies at `cap` features per body (m3tb_set_texture_modality): the base tables, with knn
+// the kNN match table, with l2 also the float descriptor tables. Whatever is missing is made, and when `cap` exceeds
+// the capacity of the existing tables every capacity-sized table is remade at `cap` with its contents kept; all of it
+// in one all-or-nothing step. A context whose bodies keep kTexMaxFeatures never grows.
+int EnsureTextureTables(m3tb_ctx* ctx, bool l2, bool knn, int cap) {
+  const size_t nb = size_t(ctx->max_bodies), K = kTexMaxKeyframes;
+  const bool base = !ctx->d_tex_xy;
+  cap = std::max(cap, base ? kTexMaxFeatures : ctx->tex_cap);
+  const bool grow = !base && cap > ctx->tex_cap;
+  l2 = l2 || ctx->d_tex_fdesc;
+  knn = knn || l2 || ctx->d_tex_knn;
+  if (!base && !grow && (!l2 || ctx->d_tex_fdesc) && (!knn || ctx->d_tex_knn)) return M3TB_OK;
+  TexTable<float> fdesc{ctx->d_tex_fdesc, nb, kTexMaxFloatDesc};
+  TexTable<float> kf_fdesc{ctx->d_tex_kf_fdesc, nb * K, kTexMaxFloatDesc};
+  TexTable<int> knn_t{ctx->d_tex_knn, nb * K, 1};
+  TexTable<float2> xy{ctx->d_tex_xy, nb, 1};
+  TexTable<uint32_t> desc{ctx->d_tex_desc, nb, kTexDescWords};
+  TexTable<uint32_t> kf_desc{ctx->d_tex_kf_desc, nb * K, kTexDescWords};
+  TexTable<float> kf_points{ctx->d_tex_kf_points, nb * K * 3, 1};
+  TexTable<float> points{ctx->d_tex_points, nb * TF_COUNT, K};
+  CU(fdesc.make(l2, grow, cap));
+  CU(kf_fdesc.make(l2, grow, cap));
+  CU(knn_t.make(knn, grow, cap));
+  CU(xy.make(true, grow, cap));
+  CU(desc.make(true, grow, cap));
+  CU(kf_desc.make(true, grow, cap));
   DeviceBuffer<int> nfeat, kf_n, counts;
-  DeviceBuffer<float> kf_points, points, pose, gh;
+  DeviceBuffer<float> pose, gh;
   DeviceBuffer<TexKeyframeState> state;
-  CU(xy.create(nb * kTexMaxFeatures));
-  CU(desc.create(nb * kTexMaxFeatures * kTexDescWords));
-  CU(kf_desc.create(nb * kTexMaxKeyframes * kTexMaxFeatures * kTexDescWords));
-  CU(nfeat.create(nb));
-  CU(kf_n.create(nb * kTexMaxKeyframes));
-  CU(counts.create(nb));
-  CU(kf_points.create(nb * kTexMaxKeyframes * 3 * kTexMaxFeatures));
-  CU(points.create(nb * TF_COUNT * kTexPointCap));
-  CU(pose.create(nb * 12));
-  CU(gh.create(nb * 27));
-  CU(state.create(nb));
-  CU(cudaMemsetAsync(nfeat, 0, nb * sizeof(int), ctx->stream));
-  CU(cudaMemsetAsync(kf_n, 0, nb * kTexMaxKeyframes * sizeof(int), ctx->stream));
-  CU(cudaMemsetAsync(counts, 0, nb * sizeof(int), ctx->stream));
-  CU(cudaMemsetAsync(pose, 0, nb * 12 * sizeof(float), ctx->stream));
-  CU(cudaMemsetAsync(gh, 0, nb * 27 * sizeof(float), ctx->stream));
-  CU(cudaMemsetAsync(state, 0, nb * sizeof(TexKeyframeState), ctx->stream));
-  ctx->d_tex_xy = std::move(xy);
-  ctx->d_tex_desc = std::move(desc);
-  ctx->d_tex_kf_desc = std::move(kf_desc);
-  ctx->d_tex_nfeat = std::move(nfeat);
-  ctx->d_tex_kf_n = std::move(kf_n);
-  ctx->d_tex_counts = std::move(counts);
-  ctx->d_tex_kf_points = std::move(kf_points);
-  ctx->d_tex_points = std::move(points);
-  ctx->d_tex_pose = std::move(pose);
-  ctx->d_gh_texture = std::move(gh);
-  ctx->d_tex_kf_state = std::move(state);
+  if (base) {
+    CU(nfeat.create(nb));
+    CU(kf_n.create(nb * K));
+    CU(counts.create(nb));
+  }
+  CU(kf_points.make(true, grow, cap));
+  CU(points.make(true, grow, cap));
+  if (base) {
+    CU(pose.create(nb * 12));
+    CU(gh.create(nb * 27));
+    CU(state.create(nb));
+    CU(cudaMemsetAsync(nfeat, 0, nb * sizeof(int), ctx->stream));
+    CU(cudaMemsetAsync(kf_n, 0, nb * K * sizeof(int), ctx->stream));
+    CU(cudaMemsetAsync(counts, 0, nb * sizeof(int), ctx->stream));
+    CU(cudaMemsetAsync(pose, 0, nb * 12 * sizeof(float), ctx->stream));
+    CU(cudaMemsetAsync(gh, 0, nb * 27 * sizeof(float), ctx->stream));
+    CU(cudaMemsetAsync(state, 0, nb * sizeof(TexKeyframeState), ctx->stream));
+  }
+  // every table exists: the ones that are remade keep their rows
+  const int old_cap = ctx->tex_cap;
+  CU(fdesc.copy(old_cap, cap, ctx->stream));
+  CU(kf_fdesc.copy(old_cap, cap, ctx->stream));
+  CU(knn_t.copy(old_cap, cap, ctx->stream));
+  CU(xy.copy(old_cap, cap, ctx->stream));
+  CU(desc.copy(old_cap, cap, ctx->stream));
+  CU(kf_desc.copy(old_cap, cap, ctx->stream));
+  CU(kf_points.copy(old_cap, cap, ctx->stream));
+  CU(points.copy(old_cap, cap, ctx->stream));
+  if (grow) CU(cudaStreamSynchronize(ctx->stream));  // the copies read the tables released below
+  fdesc.replace();
+  kf_fdesc.replace();
+  knn_t.replace();
+  xy.replace();
+  desc.replace();
+  kf_desc.replace();
+  kf_points.replace();
+  points.replace();
+  if (base) {
+    ctx->d_tex_nfeat = std::move(nfeat);
+    ctx->d_tex_kf_n = std::move(kf_n);
+    ctx->d_tex_counts = std::move(counts);
+    ctx->d_tex_pose = std::move(pose);
+    ctx->d_gh_texture = std::move(gh);
+    ctx->d_tex_kf_state = std::move(state);
+  }
+  ctx->tex_cap = cap;
   return M3TB_OK;
 }
 
@@ -4326,17 +4373,31 @@ int LaunchTexture(m3tb_ctx* ctx, bool keyframe, int mode) {
   a.points = ctx->d_tex_points;
   a.counts = ctx->d_tex_counts;
   a.mode = mode;
-  int l2_length = 0, l2_keyframes = 0;  // the longest descriptor and deque of the L2 bodies
+  a.cap = ctx->tex_cap;
+  // the longest descriptor, deque and n_features_max of the L2 bodies and of the ORB bodies matched by kNN
+  int l2_length = 0, l2_keyframes = 0, l2_features = 0, ham_keyframes = 0, ham_features = 0;
   for (int b = 0; b < ctx->n_bodies; ++b) {
     const BodyDev& B = ctx->h_bodies[b];
-    if (!B.set || !B.has_texture || !B.tp.l2) continue;
-    l2_length = std::max(l2_length, B.tp.descriptor_length);
-    l2_keyframes = std::max(l2_keyframes, B.tp.n_keyframes);
+    if (!B.set || !B.has_texture) continue;
+    if (B.tp.l2) {
+      l2_length = std::max(l2_length, B.tp.descriptor_length);
+      l2_keyframes = std::max(l2_keyframes, B.tp.n_keyframes);
+      l2_features = std::max(l2_features, B.tp.n_features_max);
+    } else if (TexHammingKnn(B.tp)) {
+      ham_keyframes = std::max(ham_keyframes, B.tp.n_keyframes);
+      ham_features = std::max(ham_features, B.tp.n_features_max);
+    }
   }
   if (!keyframe && mode == 1 && l2_length > 0) {  // a body without a length has no features, hence no keyframe points
     CU(cudaFuncSetAttribute(k_texture_knn_l2, cudaFuncAttributeMaxDynamicSharedMemorySize, KnnSharedBytes(l2_length)));
-    const dim3 grid(kKnnSplits * l2_keyframes * (kTexMaxFeatures / kKnnQueries), ctx->n_bodies);
+    const dim3 grid(kKnnSplits * l2_keyframes * KnnTilesPerKeyframe(l2_features), ctx->n_bodies);
     k_texture_knn_l2<<<grid, kKnnThreads, KnnSharedBytes(l2_length), ctx->stream>>>(a);
+    CU(cudaGetLastError());
+    ctx->launches++;
+  }
+  if (!keyframe && mode == 1 && ham_features > 0) {
+    const dim3 grid(kKnnSplits * ham_keyframes * KnnTilesPerKeyframe(ham_features), ctx->n_bodies);
+    k_texture_knn_hamming<<<grid, kKnnThreads, KnnSharedBytes(kTexDescWords), ctx->stream>>>(a);
     CU(cudaGetLastError());
     ctx->launches++;
   }
@@ -4419,6 +4480,8 @@ int m3tb_set_texture_modality(m3tb_ctx* ctx, int body, const m3tb_texture_params
   if (p.descriptor_type != M3TB_DESCRIPTOR_ORB && !l2)
     return Fail(ctx, M3TB_ERR_UNSUPPORTED, "only DescriptorType::ORB (NORM_HAMMING), SIFT and DAISY (NORM_L2) are implemented");
   if (p.n_keyframes > kTexMaxKeyframes) return Fail(ctx, M3TB_ERR_UNSUPPORTED, "n_keyframes above 8");
+  if (p.n_features_max > kTexFeatureLimit) return Fail(ctx, M3TB_ERR_UNSUPPORTED, "n_features_max above 4096");
+  if (p.n_features_max < kTexMaxFeatures) return Fail(ctx, M3TB_ERR_INVALID, "n_features_max below 512");
   if (color_camera < 0 || color_camera >= ctx->max_cameras || !ctx->h_ccams[color_camera].set)
     return Fail(ctx, M3TB_ERR_INVALID, "color camera not set");
   if (p.n_keyframes < 1 || p.focused_image_size < 1 || p.n_standard_deviations < 1 ||
@@ -4432,7 +4495,7 @@ int m3tb_set_texture_modality(m3tb_ctx* ctx, int body, const m3tb_texture_params
     return Fail(ctx, M3TB_ERR_INVALID, "measure_occlusions needs the body's depth camera");
   if (!ctx->h_geometry[body].set)
     return Fail(ctx, M3TB_ERR_INVALID, "the texture modality needs the body's geometry (m3tb_set_body_geometry)");
-  int rc = EnsureTextureTables(ctx, l2);
+  int rc = EnsureTextureTables(ctx, l2, !l2 && p.n_features_max > kTexMaxFeatures, p.n_features_max);
   if (rc) return rc;
   CU(cudaStreamSynchronize(ctx->stream));  // a launch in flight may still read this body's keyframes
   CU(cudaMemsetAsync(ctx->d_tex_kf_state + body, 0, sizeof(TexKeyframeState), ctx->stream));
@@ -4457,6 +4520,7 @@ int m3tb_set_texture_modality(m3tb_ctx* ctx, int body, const m3tb_texture_params
   t.l2 = l2 ? 1 : 0;
   t.descriptor_type = p.descriptor_type;
   t.descriptor_length = 0;  // the next upload fixes it
+  t.n_features_max = p.n_features_max;
   if (B.has_texture && B.texture_camera != color_camera)  // renderers of the old camera no longer fit
     for (int slot = RS_TEXTURE_SILHOUETTE; slot < RS_COUNT; ++slot)
       if (ctx->attached[body][slot] >= 0) {
@@ -4499,7 +4563,8 @@ int UploadTextureFeatures(m3tb_ctx* ctx, int body, const float* keypoints_xy, co
                           int length, int roi_x, int roi_y, float scale) {
   int rc = CheckTextureBody(ctx, body);
   if (rc) return rc;
-  if (n > kTexMaxFeatures) return Fail(ctx, M3TB_ERR_UNSUPPORTED, "more than 512 features per body");
+  if (n > ctx->h_bodies[body].tp.n_features_max)
+    return Fail(ctx, M3TB_ERR_UNSUPPORTED, "more than the body's n_features_max features");
   if (n < 0 || (n > 0 && (!keypoints_xy || !descriptors)) || !(scale > 0.0f) || !std::isfinite(scale))
     return Fail(ctx, M3TB_ERR_INVALID, "bad feature arguments");
   TextureParamsDev& tp = ctx->h_bodies[body].tp;
@@ -4522,14 +4587,15 @@ int UploadTextureFeatures(m3tb_ctx* ctx, int body, const float* keypoints_xy, co
     xy[i].y = float(roi_y) + keypoints_xy[2 * i + 1] / scale;
   }
   if (n > 0) {
-    CU(cudaMemcpyAsync(ctx->d_tex_xy + size_t(body) * kTexMaxFeatures, xy.data(), sizeof(float2) * n,
-                       cudaMemcpyHostToDevice, ctx->stream));
+    const size_t cap = size_t(ctx->tex_cap);
+    CU(cudaMemcpyAsync(ctx->d_tex_xy + size_t(body) * cap, xy.data(), sizeof(float2) * n, cudaMemcpyHostToDevice,
+                       ctx->stream));
     if (l2)
-      CU(cudaMemcpy2DAsync(ctx->d_tex_fdesc + size_t(body) * kTexMaxFeatures * kTexMaxFloatDesc,
+      CU(cudaMemcpy2DAsync(ctx->d_tex_fdesc + size_t(body) * cap * kTexMaxFloatDesc,
                            sizeof(float) * kTexMaxFloatDesc, float_descriptors, sizeof(float) * length,
                            sizeof(float) * length, n, cudaMemcpyHostToDevice, ctx->stream));
     else
-      CU(cudaMemcpyAsync(ctx->d_tex_desc + size_t(body) * kTexMaxFeatures * kTexDescWords, descriptors, size_t(32) * n,
+      CU(cudaMemcpyAsync(ctx->d_tex_desc + size_t(body) * cap * kTexDescWords, descriptors, size_t(32) * n,
                          cudaMemcpyHostToDevice, ctx->stream));
   }
   CU(cudaMemcpyAsync(ctx->d_tex_nfeat + body, &n, sizeof(int), cudaMemcpyHostToDevice, ctx->stream));
@@ -4642,7 +4708,8 @@ int m3tb_upload_texture_features_device(m3tb_ctx* ctx, const int* bodies, const 
     int rc = CheckTextureBody(ctx, b);
     if (rc) return rc;
     if (listed[b]++) return Fail(ctx, M3TB_ERR_INVALID, "body listed twice");
-    if (f.n > kTexMaxFeatures) return Fail(ctx, M3TB_ERR_UNSUPPORTED, "more than 512 features per body");
+    if (f.n > ctx->h_bodies[b].tp.n_features_max)
+      return Fail(ctx, M3TB_ERR_UNSUPPORTED, "more than the body's n_features_max features");
     if (f.n < 0 || (f.n > 0 && (!f.x || !f.y || !f.descriptors || f.xy_stride < 1)))
       return Fail(ctx, M3TB_ERR_INVALID, "bad feature arguments");
     const TextureParamsDev& tp = ctx->h_bodies[b].tp;
@@ -4679,6 +4746,7 @@ int m3tb_upload_texture_features_device(m3tb_ctx* ctx, const int* bodies, const 
     a.feat_fdesc = ctx->d_tex_fdesc;
     a.feat_n = ctx->d_tex_nfeat;
     a.nonfinite = ctx->d_tex_nonfinite;
+    a.cap = ctx->tex_cap;
     for (int k = 0; k < a.n_jobs; ++k) {
       const m3tb_device_features& f = features[first + k];
       const m3tb_ctx::TexCrop& c = ctx->tex_crop[bodies[first + k]];
@@ -4757,8 +4825,9 @@ int m3tb_get_texture_points(m3tb_ctx* ctx, int body, m3tb_texture_point* points,
   const int m = std::min(n, capacity);
   if (m <= 0) return M3TB_OK;
   std::vector<float> f(size_t(TF_COUNT) * m);
-  const float* src = ctx->d_tex_points + size_t(body) * TF_COUNT * kTexPointCap;
-  CU(cudaMemcpy2DAsync(f.data(), sizeof(float) * m, src, sizeof(float) * kTexPointCap, sizeof(float) * m, TF_COUNT,
+  const size_t point_cap = size_t(kTexMaxKeyframes) * ctx->tex_cap;
+  const float* src = ctx->d_tex_points + size_t(body) * TF_COUNT * point_cap;
+  CU(cudaMemcpy2DAsync(f.data(), sizeof(float) * m, src, sizeof(float) * point_cap, sizeof(float) * m, TF_COUNT,
                        cudaMemcpyDeviceToHost, ctx->stream));
   CU(cudaStreamSynchronize(ctx->stream));
   for (int i = 0; i < m; ++i) {
@@ -4785,17 +4854,25 @@ int m3tb_get_texture_keyframes(m3tb_ctx* ctx, int body, int* n_keyframes, int* s
   // a descriptor is `width` bytes in rows of `stride` words: 32 of 8 for ORB, 4 * length of kTexMaxFloatDesc for L2
   const int stride = tp.l2 ? kTexMaxFloatDesc : kTexDescWords;
   const size_t width = tp.l2 ? sizeof(float) * tp.descriptor_length : 32;
+  const size_t cap = size_t(ctx->tex_cap);
   std::vector<int> kn(kTexMaxKeyframes);
-  std::vector<float> kp(size_t(kTexMaxKeyframes) * 3 * kTexMaxFeatures);
-  std::vector<uint32_t> kd(size_t(kTexMaxKeyframes) * kTexMaxFeatures * stride);
   const uint32_t* kd_src = tp.l2 ? reinterpret_cast<const uint32_t*>(ctx->d_tex_kf_fdesc.get()) : ctx->d_tex_kf_desc.get();
   CU(cudaMemcpyAsync(&st, ctx->d_tex_kf_state + body, sizeof(st), cudaMemcpyDeviceToHost, ctx->stream));
   CU(cudaMemcpyAsync(kn.data(), ctx->d_tex_kf_n + body * kTexMaxKeyframes, sizeof(int) * kn.size(), cudaMemcpyDeviceToHost,
                      ctx->stream));
-  CU(cudaMemcpyAsync(kp.data(), ctx->d_tex_kf_points + size_t(body) * kp.size(), sizeof(float) * kp.size(),
-                     cudaMemcpyDeviceToHost, ctx->stream));
-  CU(cudaMemcpyAsync(kd.data(), kd_src + size_t(body) * kd.size(), sizeof(uint32_t) * kd.size(), cudaMemcpyDeviceToHost,
-                     ctx->stream));
+  CU(cudaStreamSynchronize(ctx->stream));
+  // the rows of the deque's keyframes only: a keyframe slot holds up to cap points
+  std::vector<float> kp(size_t(kTexMaxKeyframes) * 3 * cap);
+  std::vector<uint32_t> kd(size_t(kTexMaxKeyframes) * cap * stride);
+  for (int k = 0; k < st.size; ++k) {
+    const int slot = (st.head + k) % kTexMaxKeyframes;
+    if (kn[slot] <= 0) continue;
+    const size_t kf = size_t(body) * kTexMaxKeyframes + slot;
+    CU(cudaMemcpy2DAsync(kp.data() + size_t(slot) * 3 * cap, sizeof(float) * cap, ctx->d_tex_kf_points + kf * 3 * cap,
+                         sizeof(float) * cap, sizeof(float) * kn[slot], 3, cudaMemcpyDeviceToHost, ctx->stream));
+    CU(cudaMemcpyAsync(kd.data() + size_t(slot) * cap * stride, kd_src + kf * cap * stride,
+                       sizeof(uint32_t) * kn[slot] * stride, cudaMemcpyDeviceToHost, ctx->stream));
+  }
   CU(cudaStreamSynchronize(ctx->stream));
   if (n_keyframes) *n_keyframes = st.size;
   if (age) *age = st.age;
@@ -4806,9 +4883,8 @@ int m3tb_get_texture_keyframes(m3tb_ctx* ctx, int body, int* n_keyframes, int* s
     if (sizes) sizes[k] = kn[slot];
     for (int i = 0; i < kn[slot] && written < capacity; ++i, ++written) {
       if (points)
-        for (int c = 0; c < 3; ++c) points[3 * written + c] = kp[(size_t(slot) * 3 + c) * kTexMaxFeatures + i];
-      if (descriptors)
-        std::memcpy(descriptors + width * written, kd.data() + (size_t(slot) * kTexMaxFeatures + i) * stride, width);
+        for (int c = 0; c < 3; ++c) points[3 * written + c] = kp[(size_t(slot) * 3 + c) * cap + i];
+      if (descriptors) std::memcpy(descriptors + width * written, kd.data() + (size_t(slot) * cap + i) * stride, width);
     }
   }
   return M3TB_OK;

@@ -172,6 +172,10 @@ struct TextureParamsDev {
   // l2 0: 32-byte binary descriptors (ORB, NORM_HAMMING); 1: float descriptors (SIFT / DAISY, NORM_L2) of
   // descriptor_length floats, fixed by the first upload after m3tb_set_texture_modality (0 before it)
   int descriptor_type, l2, descriptor_length;
+  // m3tb_texture_params::n_features_max: a body above kTexMaxFeatures matches ORB descriptors with
+  // k_texture_knn_hamming instead of k_texture_match's in-CTA scan
+  int n_features_max;
+  int pad[3];  // keeps BodyDev::rend 16-byte aligned
 };
 
 struct BodyDev {
@@ -225,12 +229,13 @@ struct TrackArgs {
   // k_track2: RegionModality::PrecalculateFunctionLookup tables, identical for every region body of the launch
   // (checked by the host), so that they are kernel-parameter constants instead of per-thread registers
   float lookup_f[kFunctionLength], lookup_b[kFunctionLength];
-  // texture modality (PH_TEXTURE_GH): data points [n_bodies][TF_COUNT][kTexPointCap] and their counts from
+  // texture modality (PH_TEXTURE_GH): data points [n_bodies][TF_COUNT][tex_point_cap] and their counts from
   // k_texture_match, the pose of each gradient pass (tex_pose [n_bodies][12]) and the sums (gh_texture [n_bodies][27])
   float* tex_points;
   const int* tex_counts;
   float* tex_pose;
   float* gh_texture;
+  int tex_point_cap;            // kTexMaxKeyframes x the context's feature capacity (TextureArgs::cap)
 };
 
 // ---------------------------------------------------------------------------------------------

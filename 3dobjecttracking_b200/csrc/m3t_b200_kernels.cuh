@@ -1463,7 +1463,8 @@ __global__ void __launch_bounds__(T, 512 / T) k_track(const __grid_constant__ Tr
       const bool tex_gh = body.has_texture && (args.phases & PH_TEXTURE_GH);
       if (tex_gh) {  // the texture term after region and depth (the evaluators' AddModality order)
         TextureGradient(args.color_cams[body.texture_camera], sh.pose, body.tp, corr,
-                        args.tex_points + size_t(body_id) * TF_COUNT * kTexPointCap, args.tex_counts[body_id], tid, T, acc);
+                        args.tex_points + size_t(body_id) * TF_COUNT * args.tex_point_cap, args.tex_point_cap,
+                        args.tex_counts[body_id], tid, T, acc);
         // PrecalculatePoseVariables of this pass: CalculateResults reconstructs keyframes with it (sh.pose changes
         // only in the solve, behind the barrier below)
         if (tid < 12) args.tex_pose[12 * body_id + tid] = sh.pose[tid];

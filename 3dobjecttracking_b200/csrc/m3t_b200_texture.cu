@@ -156,17 +156,18 @@ __global__ void __launch_bounds__(kTexThreads) k_texture_keyframe(const __grid_c
   const RenderingDev& mdep = body.rend[RS_TEXTURE_DEPTH];
   const bool modeled = tp.model_occlusions && mdep.image != nullptr && mdep.visible;
   const int n = a.feat_n[b];
-  const float2* xy = a.feat_xy + size_t(b) * kTexMaxFeatures;
+  const size_t cap = size_t(a.cap);
+  const float2* xy = a.feat_xy + size_t(b) * cap;
   // a descriptor is `words` 32-bit words in rows of `stride`: 8 of 8 for ORB, descriptor_length floats of
   // kTexMaxFloatDesc for SIFT / DAISY
   const bool l2 = tp.l2 != 0;
   const int words = l2 ? tp.descriptor_length : kTexDescWords, stride = l2 ? kTexMaxFloatDesc : kTexDescWords;
   const uint32_t* desc = l2 ? reinterpret_cast<const uint32_t*>(a.feat_fdesc) : a.feat_desc;
-  desc += size_t(b) * kTexMaxFeatures * stride;
+  desc += size_t(b) * cap * stride;
   const int slot = s_slot;
-  float* kp = a.kf_points + (size_t(b) * kTexMaxKeyframes + slot) * 3 * kTexMaxFeatures;
+  float* kp = a.kf_points + (size_t(b) * kTexMaxKeyframes + slot) * 3 * cap;
   uint32_t* kd = l2 ? reinterpret_cast<uint32_t*>(a.kf_fdesc) : a.kf_desc;
-  kd += (size_t(b) * kTexMaxKeyframes + slot) * kTexMaxFeatures * stride;
+  kd += (size_t(b) * kTexMaxKeyframes + slot) * cap * stride;
   int written = 0;
   for (int i0 = 0; i0 < n; i0 += kTexThreads) {
     const int i = i0 + tid;
@@ -191,9 +192,9 @@ __global__ void __launch_bounds__(kTexThreads) k_texture_keyframe(const __grid_c
     int total;
     const int pos = written + BlockCompact(keep, s_warp, &total);
     if (keep) {
-      kp[0 * kTexMaxFeatures + pos] = px;
-      kp[1 * kTexMaxFeatures + pos] = py;
-      kp[2 * kTexMaxFeatures + pos] = pz;
+      kp[0 * cap + pos] = px;
+      kp[1 * cap + pos] = py;
+      kp[2 * cap + pos] = pz;
       for (int w = 0; w < words; ++w) kd[size_t(pos) * stride + w] = desc[size_t(i) * stride + w];
     }
     written += total;
@@ -241,89 +242,111 @@ __device__ __forceinline__ Top2 Merge(const Top2& a, const Top2& b) {
   return r;
 }
 
-// rows [0, n) of a [rows][kTexMaxFloatDesc] table into shared rows of `stride` floats: the first `length` floats,
-// zero up to the next multiple of 4 and in rows [n, rows)
-__device__ __forceinline__ void StageRows(const float* src, int n, int rows, int length, int stride, float* dst) {
+// rows [0, n) of a table of 32-bit words in rows of src_stride into shared rows of `stride` words: the first `length`
+// words, zero up to the next multiple of 4 and in rows [n, rows)
+__device__ __forceinline__ void StageRows(const uint32_t* src, size_t src_stride, int n, int rows, int length, int stride,
+                                          uint32_t* dst) {
   const int d4 = (length + 3) / 4;
   for (int e = threadIdx.x; e < rows * d4; e += kKnnThreads) {
     const int r = e / d4, c = e - r * d4;
-    float4 v = make_float4(0.0f, 0.0f, 0.0f, 0.0f);
+    uint4 v = make_uint4(0u, 0u, 0u, 0u);
     if (r < n) {
-      v = *reinterpret_cast<const float4*>(src + size_t(r) * kTexMaxFloatDesc + 4 * c);
+      v = *reinterpret_cast<const uint4*>(src + r * src_stride + 4 * c);
       const int k = 4 * c;
-      if (k + 1 >= length) v.y = 0.0f;
-      if (k + 2 >= length) v.z = 0.0f;
-      if (k + 3 >= length) v.w = 0.0f;
+      if (k + 1 >= length) v.y = 0u;
+      if (k + 2 >= length) v.z = 0u;
+      if (k + 3 >= length) v.w = 0u;
     }
-    *reinterpret_cast<float4*>(dst + r * stride + 4 * c) = v;
+    *reinterpret_cast<uint4*>(dst + r * stride + 4 * c) = v;
   }
 }
 
-}  // namespace
+// The distance sums of one (query, train) pair over four 32-bit words: L2, float descriptors: squared differences
+// in descriptor order; Hamming, 32-byte binary descriptors: bits that differ
+template <bool kHamming>
+__device__ __forceinline__ void KnnAccumulate(const uint4& q, const uint4& t, float& acc) {
+  if constexpr (kHamming) {
+    acc += float(__popc(q.x ^ t.x) + __popc(q.y ^ t.y) + __popc(q.z ^ t.z) + __popc(q.w ^ t.w));
+  } else {
+    float d = __uint_as_float(q.x) - __uint_as_float(t.x);
+    acc = fmaf(d, d, acc);
+    d = __uint_as_float(q.y) - __uint_as_float(t.y);
+    acc = fmaf(d, d, acc);
+    d = __uint_as_float(q.z) - __uint_as_float(t.z);
+    acc = fmaf(d, d, acc);
+    d = __uint_as_float(q.w) - __uint_as_float(t.w);
+    acc = fmaf(d, d, acc);
+  }
+}
 
-// cv::BFMatcher(NORM_L2).knnMatch(keyframe descriptors, frame descriptors, k = 2) and the ratio test of
-// CalculateCorrespondences for every L2 body at correspondence iteration 0. distance = sqrt of the float sum of
-// squared float differences, summed in descriptor order. For SIFT's whole-number descriptors every partial sum is an
-// integer below 2^24, so any order gives OpenCV's distance bit for bit (DESIGN.md section 3).
-// Each thread holds a 4 x 4 block of (query, train) sums: queries ty + 16 i, train rows tx + 16 j of the CTA's split.
-__global__ void __cluster_dims__(kKnnSplits, 1, 1) __launch_bounds__(kKnnThreads)
-    k_texture_knn_l2(const __grid_constant__ TextureArgs a) {
+// One cluster's tile of k_texture_knn_l2 / k_texture_knn_hamming: kKnnQueries queries of one keyframe against the
+// frame's train set. Each thread holds a 4 x 4 block of (query, train) sums, queries ty + 16 i and train rows tx + 16 j
+// of the CTA's slice of a chunk, and a running top-2 list per query over its train rows in increasing index: the
+// insertion of cv::batchDistance. The lists of the 16 lanes sharing a query and then of the cluster's CTAs are merged
+// under (distance, train index) order, which is what that insertion gives over the union.
+template <bool kHamming>
+__device__ __forceinline__ void KnnTile(const TextureArgs& a) {
   namespace cg = cooperative_groups;
   const int b = blockIdx.y, tid = threadIdx.x;
   const BodyDev& body = a.bodies[b];
   // every return before the first cluster barrier depends on (body, tile) alone: a cluster leaves or stays whole
-  if (!body.set || !body.has_texture || !body.tp.l2) return;
+  if (!body.set || !body.has_texture || (kHamming ? !TexHammingKnn(body.tp) : !body.tp.l2)) return;
   const int rank = blockIdx.x % kKnnSplits, tile = blockIdx.x / kKnnSplits;
-  const int k = tile / (kTexMaxFeatures / kKnnQueries), q0 = tile % (kTexMaxFeatures / kKnnQueries) * kKnnQueries;
+  const int tiles = KnnTilesPerKeyframe(body.tp.n_features_max);
+  const int k = tile / tiles, q0 = tile % tiles * kKnnQueries;
   const TexKeyframeState st = a.kf_state[b];
   if (k >= st.size) return;
   const int slot = (st.head + k) % kTexMaxKeyframes;
   const int nq = min(kKnnQueries, a.kf_n[b * kTexMaxKeyframes + slot] - q0);
   if (nq <= 0) return;
-  const int length = body.tp.descriptor_length, stride = KnnStride(length);
-  const int t0 = rank * kKnnTrain, nt = max(0, min(kKnnTrain, a.feat_n[b] - t0));
-  extern __shared__ float4 s_dyn[];
-  float* s_q = reinterpret_cast<float*>(s_dyn);
-  float* s_t = s_q + kKnnQueries * stride;
+  // rows of `length` words, `src_stride` words apart in the tables
+  const int length = kHamming ? kTexDescWords : body.tp.descriptor_length, stride = KnnStride(length);
+  const size_t src_stride = kHamming ? kTexDescWords : kTexMaxFloatDesc, cap = size_t(a.cap);
+  const uint32_t* kf_rows = kHamming ? a.kf_desc : reinterpret_cast<const uint32_t*>(a.kf_fdesc);
+  const uint32_t* feat_rows = kHamming ? a.feat_desc : reinterpret_cast<const uint32_t*>(a.feat_fdesc);
+  const int n_train = a.feat_n[b];
+  extern __shared__ uint4 s_dyn[];
+  uint32_t* s_q = reinterpret_cast<uint32_t*>(s_dyn);
+  uint32_t* s_t = s_q + kKnnQueries * stride;
   __shared__ Top2 s_part[kKnnQueries];
-  StageRows(a.kf_fdesc + ((size_t(b) * kTexMaxKeyframes + slot) * kTexMaxFeatures + q0) * kTexMaxFloatDesc, nq,
-            kKnnQueries, length, stride, s_q);
-  StageRows(a.feat_fdesc + (size_t(b) * kTexMaxFeatures + t0) * kTexMaxFloatDesc, nt, kKnnTrain, length, stride, s_t);
-  __syncthreads();
+  StageRows(kf_rows + ((size_t(b) * kTexMaxKeyframes + slot) * cap + q0) * src_stride, src_stride, nq, kKnnQueries,
+            length, stride, s_q);
   const int ty = tid / 16, tx = tid % 16, s4 = stride / 4, d4 = (length + 3) / 4;
-  const float4* q4 = reinterpret_cast<const float4*>(s_q);
-  const float4* t4 = reinterpret_cast<const float4*>(s_t);
-  float acc[4][4];
+  const uint4* q4 = reinterpret_cast<const uint4*>(s_q);
+  const uint4* t4 = reinterpret_cast<const uint4*>(s_t);
+  Top2 top[4];
 #pragma unroll
-  for (int i = 0; i < 4; ++i)
-#pragma unroll
-    for (int j = 0; j < 4; ++j) acc[i][j] = 0.0f;
-  for (int c = 0; c < d4; ++c) {
-    float4 qv[4], tv[4];
-#pragma unroll
-    for (int i = 0; i < 4; ++i) qv[i] = q4[(ty + 16 * i) * s4 + c];
-#pragma unroll
-    for (int j = 0; j < 4; ++j) tv[j] = t4[(tx + 16 * j) * s4 + c];
+  for (int i = 0; i < 4; ++i) top[i] = Top2{FLT_MAX, FLT_MAX, INT_MAX, INT_MAX};
+  for (int c0 = 0; c0 < n_train; c0 += kKnnChunk) {
+    const int t0 = c0 + rank * kKnnTrain, nt = max(0, min(kKnnTrain, n_train - t0));
+    if (c0 > 0) __syncthreads();  // every thread is done with the previous chunk's rows
+    StageRows(feat_rows + (size_t(b) * cap + t0) * src_stride, src_stride, nt, kKnnTrain, length, stride, s_t);
+    __syncthreads();
+    float acc[4][4];
 #pragma unroll
     for (int i = 0; i < 4; ++i)
 #pragma unroll
-      for (int j = 0; j < 4; ++j) {
-        float d = qv[i].x - tv[j].x;
-        acc[i][j] = fmaf(d, d, acc[i][j]);
-        d = qv[i].y - tv[j].y;
-        acc[i][j] = fmaf(d, d, acc[i][j]);
-        d = qv[i].z - tv[j].z;
-        acc[i][j] = fmaf(d, d, acc[i][j]);
-        d = qv[i].w - tv[j].w;
-        acc[i][j] = fmaf(d, d, acc[i][j]);
-      }
+      for (int j = 0; j < 4; ++j) acc[i][j] = 0.0f;
+    for (int c = 0; c < d4; ++c) {
+      uint4 qv[4], tv[4];
+#pragma unroll
+      for (int i = 0; i < 4; ++i) qv[i] = q4[(ty + 16 * i) * s4 + c];
+#pragma unroll
+      for (int j = 0; j < 4; ++j) tv[j] = t4[(tx + 16 * j) * s4 + c];
+#pragma unroll
+      for (int i = 0; i < 4; ++i)
+#pragma unroll
+        for (int j = 0; j < 4; ++j) KnnAccumulate<kHamming>(qv[i], tv[j], acc[i][j]);
+    }
+#pragma unroll
+    for (int i = 0; i < 4; ++i)
+#pragma unroll
+      for (int j = 0; j < 4; ++j)
+        if (tx + 16 * j < nt) Insert(top[i], kHamming ? acc[i][j] : sqrtf(acc[i][j]), t0 + tx + 16 * j);
   }
 #pragma unroll
   for (int i = 0; i < 4; ++i) {
-    Top2 t{FLT_MAX, FLT_MAX, INT_MAX, INT_MAX};
-#pragma unroll
-    for (int j = 0; j < 4; ++j)
-      if (tx + 16 * j < nt) Insert(t, sqrtf(acc[i][j]), t0 + tx + 16 * j);
+    Top2 t = top[i];
     // the 16 lanes of a half-warp share ty: merge their lists
 #pragma unroll
     for (int off = 8; off >= 1; off >>= 1) {
@@ -343,41 +366,61 @@ __global__ void __cluster_dims__(kKnnSplits, 1, 1) __launch_bounds__(kKnnThreads
     for (int r = 1; r < kKnnSplits; ++r) t = Merge(t, cluster.map_shared_rank(s_part, r)[tid]);
     // knn_match[0].distance / knn_match[1].distance >= threshold drops the match; 0 / 0 is NaN and keeps it
     const bool keep = t.i1 != INT_MAX && !(t.d0 / t.d1 >= body.tp.descriptor_distance_threshold);
-    a.knn[(size_t(b) * kTexMaxKeyframes + slot) * kTexMaxFeatures + q0 + tid] = keep ? t.i0 : -1;
+    a.knn[(size_t(b) * kTexMaxKeyframes + slot) * cap + q0 + tid] = keep ? t.i0 : -1;
   }
   cluster.sync();  // the partial lists of ranks 1.. stay in place until rank 0 has read them
 }
 
+}  // namespace
+
+// cv::BFMatcher(NORM_L2).knnMatch(keyframe descriptors, frame descriptors, k = 2) and the ratio test of
+// CalculateCorrespondences for every L2 body at correspondence iteration 0. distance = sqrt of the float sum of
+// squared float differences, summed in descriptor order. For SIFT's whole-number descriptors every partial sum is an
+// integer below 2^24, so any order gives OpenCV's distance bit for bit (DESIGN.md section 3).
+__global__ void __cluster_dims__(kKnnSplits, 1, 1) __launch_bounds__(kKnnThreads)
+    k_texture_knn_l2(const __grid_constant__ TextureArgs a) {
+  KnnTile<false>(a);
+}
+
+// cv::BFMatcher(NORM_HAMMING).knnMatch(k = 2) and the ratio test for every ORB body whose n_features_max is above
+// kTexMaxFeatures, at correspondence iteration 0. Distances are bit counts, exact as floats.
+__global__ void __cluster_dims__(kKnnSplits, 1, 1) __launch_bounds__(kKnnThreads)
+    k_texture_knn_hamming(const __grid_constant__ TextureArgs a) {
+  KnnTile<true>(a);
+}
+
 // CalculateCorrespondences (texture_modality.cpp:322-386): with mode 1 (correspondence iteration 0) every keyframe's
-// descriptors (queries) are matched against the frame's (train set) by brute-force Hamming kNN, k = 2 (for L2 bodies
-// k_texture_knn_l2 has matched them just before), and the matches that pass the ratio test become the data points,
-// keyframe by keyframe in query order. Every call then projects the data points with the current pose
-// (data_point.center) and records that pose.
+// descriptors (queries) are matched against the frame's (train set) by brute-force kNN, k = 2, and the matches that pass
+// the ratio test become the data points, keyframe by keyframe in query order. ORB bodies up to kTexMaxFeatures are
+// matched here (Hamming, the train set in shared memory); k_texture_knn_l2 / _hamming have matched the others just
+// before. Every call then projects the data points with the current pose (data_point.center) and records that pose.
 __global__ void __launch_bounds__(kTexThreads) k_texture_match(const __grid_constant__ TextureArgs a) {
   const int b = blockIdx.x, tid = threadIdx.x;
   const BodyDev& body = a.bodies[b];
   if (!body.set || !body.has_texture) return;
   __shared__ uint4 s_train[kTexMaxFeatures * 2];
   __shared__ int s_warp[kTexThreads / 32];
-  float* pts = a.points + size_t(b) * TF_COUNT * kTexPointCap;
+  const size_t cap = size_t(a.cap), point_cap = kTexMaxKeyframes * cap;
+  float* pts = a.points + size_t(b) * TF_COUNT * point_cap;
   const CameraDev& cam = a.color_cams[body.texture_camera];
   if (a.mode == 1) {
     const int n_train = a.feat_n[b];
-    const bool l2 = body.tp.l2 != 0;
-    const uint4* train = reinterpret_cast<const uint4*>(a.feat_desc + size_t(b) * kTexMaxFeatures * kTexDescWords);
-    if (!l2)
+    const bool knn_matched = body.tp.l2 != 0 || TexHammingKnn(body.tp);
+    const uint4* train = reinterpret_cast<const uint4*>(a.feat_desc + size_t(b) * cap * kTexDescWords);
+    if (!knn_matched)
       for (int k = tid; k < 2 * n_train; k += kTexThreads) s_train[k] = train[k];
     __syncthreads();
-    const float2* xy = a.feat_xy + size_t(b) * kTexMaxFeatures;
+    const float2* xy = a.feat_xy + size_t(b) * cap;
     const TexKeyframeState st = a.kf_state[b];
     const float thr = body.tp.descriptor_distance_threshold;
     int written = 0;
     for (int k = 0; k < st.size; ++k) {
       const int slot = (st.head + k) % kTexMaxKeyframes;
       const int nq = a.kf_n[b * kTexMaxKeyframes + slot];
-      const float* kp = a.kf_points + (size_t(b) * kTexMaxKeyframes + slot) * 3 * kTexMaxFeatures;
-      const uint4* kd = reinterpret_cast<const uint4*>(a.kf_desc + (size_t(b) * kTexMaxKeyframes + slot) * kTexMaxFeatures * kTexDescWords);
-      const int* knn = l2 ? a.knn + (size_t(b) * kTexMaxKeyframes + slot) * kTexMaxFeatures : nullptr;
+      const size_t kf = size_t(b) * kTexMaxKeyframes + slot;
+      const float* kp = a.kf_points + kf * 3 * cap;
+      const uint4* kd = reinterpret_cast<const uint4*>(a.kf_desc + kf * cap * kTexDescWords);
+      const int* knn = knn_matched ? a.knn + kf * cap : nullptr;
       for (int q0 = 0; q0 < nq; q0 += kTexThreads) {
         const int q = q0 + tid;
         bool keep = false;
@@ -404,12 +447,12 @@ __global__ void __launch_bounds__(kTexThreads) k_texture_match(const __grid_cons
         int total;
         const int pos = written + BlockCompact(keep, s_warp, &total);
         if (keep) {
-          pts[TF_CBX * kTexPointCap + pos] = kp[0 * kTexMaxFeatures + q];
-          pts[TF_CBY * kTexPointCap + pos] = kp[1 * kTexMaxFeatures + q];
-          pts[TF_CBZ * kTexPointCap + pos] = kp[2 * kTexMaxFeatures + q];
+          pts[TF_CBX * point_cap + pos] = kp[0 * cap + q];
+          pts[TF_CBY * point_cap + pos] = kp[1 * cap + q];
+          pts[TF_CBZ * point_cap + pos] = kp[2 * cap + q];
           const float2 c = xy[i0];
-          pts[TF_CU * kTexPointCap + pos] = c.x;
-          pts[TF_CV * kTexPointCap + pos] = c.y;
+          pts[TF_CU * point_cap + pos] = c.x;
+          pts[TF_CV * point_cap + pos] = c.y;
         }
         written += total;
       }
@@ -423,12 +466,12 @@ __global__ void __launch_bounds__(kTexThreads) k_texture_match(const __grid_cons
   __syncthreads();
   const int n = a.counts[b];
   for (int i = tid; i < n; i += kTexThreads) {
-    const float bx = pts[TF_CBX * kTexPointCap + i], by = pts[TF_CBY * kTexPointCap + i], bz = pts[TF_CBZ * kTexPointCap + i];
+    const float bx = pts[TF_CBX * point_cap + i], by = pts[TF_CBY * point_cap + i], bz = pts[TF_CBZ * point_cap + i];
     const float x = b2c[0] * bx + b2c[1] * by + b2c[2] * bz + b2c[3];
     const float y = b2c[4] * bx + b2c[5] * by + b2c[6] * bz + b2c[7];
     const float z = b2c[8] * bx + b2c[9] * by + b2c[10] * bz + b2c[11];
-    pts[TF_PU * kTexPointCap + i] = x * cam.fu / z + cam.ppu;
-    pts[TF_PV * kTexPointCap + i] = y * cam.fv / z + cam.ppv;
+    pts[TF_PU * point_cap + i] = x * cam.fu / z + cam.ppu;
+    pts[TF_PV * point_cap + i] = y * cam.fv / z + cam.ppv;
   }
 }
 
@@ -512,20 +555,21 @@ __global__ void __launch_bounds__(kTexCropThreads) k_texture_crop(const __grid_c
 __global__ void __launch_bounds__(kTexThreads) k_texture_features(const __grid_constant__ TexFeatArgs a) {
   const TexFeatJob& j = a.jobs[blockIdx.x];
   const int tid = threadIdx.x, b = j.body;
-  float2* xy = a.feat_xy + size_t(b) * kTexMaxFeatures;
+  const size_t cap = size_t(a.cap);
+  float2* xy = a.feat_xy + size_t(b) * cap;
   for (int i = tid; i < j.n; i += kTexThreads) {
     const float x = j.x[size_t(i) * j.xy_stride], y = j.y[size_t(i) * j.xy_stride];
     xy[i] = make_float2(float(j.roi_x) + x / j.scale, float(j.roi_y) + y / j.scale);
   }
   int bad = 0;
   if (j.length == 0) {
-    uint32_t* dst = a.feat_desc + size_t(b) * kTexMaxFeatures * kTexDescWords;
+    uint32_t* dst = a.feat_desc + size_t(b) * cap * kTexDescWords;
     for (int e = tid; e < j.n * 32; e += kTexThreads) {  // byte by byte: the caller's rows need no alignment
       const int i = e >> 5, c = e & 31;
       reinterpret_cast<uint8_t*>(dst)[e] = j.desc[size_t(i) * j.desc_pitch + c];
     }
   } else {
-    float* dst = a.feat_fdesc + size_t(b) * kTexMaxFeatures * kTexMaxFloatDesc;
+    float* dst = a.feat_fdesc + size_t(b) * cap * kTexMaxFloatDesc;
     for (int e = tid; e < j.n * j.length; e += kTexThreads) {
       const int i = e / j.length, c = e - i * j.length;
       const float v = reinterpret_cast<const float*>(j.desc + size_t(i) * j.desc_pitch)[c];

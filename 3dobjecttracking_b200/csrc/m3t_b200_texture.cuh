@@ -9,9 +9,13 @@
 
 namespace m3tb {
 
-constexpr int kTexMaxFeatures = 512;   // frame features per body (the train set is staged in shared memory)
+// Frame features per body: n_features_max, kTexMaxFeatures (the default) .. kTexFeatureLimit. The tables of a context
+// hold TextureArgs::cap features per body, the largest n_features_max any of its texture bodies has asked for.
+// k_texture_match stages an ORB body's train set in shared memory up to kTexMaxFeatures; ORB bodies above it and every
+// L2 body are matched by the cluster kNN kernels below.
+constexpr int kTexMaxFeatures = 512;
+constexpr int kTexFeatureLimit = 4096;
 constexpr int kTexMaxKeyframes = 8;    // n_keyframes
-constexpr int kTexPointCap = kTexMaxFeatures * kTexMaxKeyframes;
 constexpr int kTexDescWords = 8;       // 32-byte ORB descriptors
 constexpr int kTexMaxFloatDesc = 256;  // float descriptor cap and the stride of the float tables (SIFT 128, DAISY 104)
 constexpr int kTexThreads = 256;
@@ -33,37 +37,48 @@ struct TextureArgs {
   float* tex_pose;              // [n_bodies][12]: the pose of the texture modality's last PrecalculatePoseVariables
   const CameraDev* color_cams;
   const CameraDev* depth_cams;
-  const float2* feat_xy;        // [n_bodies][kTexMaxFeatures] keypoints_ in image coordinates
-  const uint32_t* feat_desc;    // [n_bodies][kTexMaxFeatures][8]
-  const float* feat_fdesc;      // [n_bodies][kTexMaxFeatures][kTexMaxFloatDesc] (L2 bodies; null without any)
+  const float2* feat_xy;        // [n_bodies][cap] keypoints_ in image coordinates
+  const uint32_t* feat_desc;    // [n_bodies][cap][8]
+  const float* feat_fdesc;      // [n_bodies][cap][kTexMaxFloatDesc] (L2 bodies; null without any)
   const int* feat_n;            // [n_bodies]
-  float* kf_points;             // [n_bodies][kTexMaxKeyframes][3][kTexMaxFeatures]
-  uint32_t* kf_desc;            // [n_bodies][kTexMaxKeyframes][kTexMaxFeatures][8]
-  float* kf_fdesc;              // [n_bodies][kTexMaxKeyframes][kTexMaxFeatures][kTexMaxFloatDesc] (L2 bodies)
-  int* knn;                     // [n_bodies][kTexMaxKeyframes][kTexMaxFeatures] k_texture_knn_l2: the train index of
+  float* kf_points;             // [n_bodies][kTexMaxKeyframes][3][cap]
+  uint32_t* kf_desc;            // [n_bodies][kTexMaxKeyframes][cap][8]
+  float* kf_fdesc;              // [n_bodies][kTexMaxKeyframes][cap][kTexMaxFloatDesc] (L2 bodies)
+  int* knn;                     // [n_bodies][kTexMaxKeyframes][cap] k_texture_knn_l2 / _hamming: the train index of
                                 // a query's best match that passes the ratio test, -1 otherwise (by keyframe slot)
   int* kf_n;                    // [n_bodies][kTexMaxKeyframes]
   TexKeyframeState* kf_state;   // [n_bodies]
-  float* points;                // [n_bodies][TF_COUNT][kTexPointCap]
+  float* points;                // [n_bodies][TF_COUNT][kTexMaxKeyframes * cap]
   int* counts;                  // [n_bodies]
   int mode;                     // k_texture_keyframe: 0 StartModality, 1 CalculateResults; k_texture_match: 1 = match
+  int cap;                      // features per body of every table above (kTexMaxFeatures .. kTexFeatureLimit)
 };
+
+// k_texture_match reads an ORB body's matches from knn (k_texture_knn_hamming) instead of scanning its train set
+__host__ __device__ __forceinline__ bool TexHammingKnn(const TextureParamsDev& tp) {
+  return !tp.l2 && tp.n_features_max > kTexMaxFeatures;
+}
 
 __global__ void k_texture_keyframe(const __grid_constant__ TextureArgs a);
 __global__ void k_texture_match(const __grid_constant__ TextureArgs a);
 
-// k_texture_knn_l2: a cluster of kKnnSplits CTAs per tile of kKnnQueries queries of one keyframe; CTA r of the cluster
-// scans train rows [r * kKnnTrain, (r + 1) * kKnnTrain) and rank 0 merges the partial top-2 lists. Grid:
-// (kKnnSplits * kKnnTiles, n_bodies), dynamic shared memory KnnSharedBytes(longest descriptor of the context).
+// k_texture_knn_l2 (SIFT / DAISY bodies) and k_texture_knn_hamming (ORB bodies above kTexMaxFeatures): a cluster of
+// kKnnSplits CTAs per tile of kKnnQueries queries of one keyframe. The train set is walked in chunks of kKnnChunk rows;
+// CTA r of the cluster scans rows [c * kKnnChunk + r * kKnnTrain, ... + kKnnTrain) of every chunk c and rank 0 merges
+// the partial top-2 lists. Grid: (kKnnSplits * keyframes * KnnTilesPerKeyframe(features), n_bodies), with the longest
+// deque and the largest n_features_max of the bodies the kernel matches; dynamic shared memory KnnSharedBytes(row
+// length in 32-bit words: the longest descriptor of the context's L2 bodies, kTexDescWords for Hamming).
 constexpr int kKnnQueries = 64, kKnnTrain = 64, kKnnThreads = 256;
-constexpr int kKnnSplits = kTexMaxFeatures / kKnnTrain;                         // 8, the portable cluster size
-constexpr int kKnnTiles = kTexMaxKeyframes * (kTexMaxFeatures / kKnnQueries);  // query tiles of a full deque
-// shared rows are padded to a stride of 4 (mod 8) floats, so the 8 float4 reads of a quarter-warp hit distinct banks
+constexpr int kKnnSplits = 8;                       // the portable cluster size
+constexpr int kKnnChunk = kKnnSplits * kKnnTrain;   // 512 train rows per chunk
+__host__ __device__ constexpr int KnnTilesPerKeyframe(int features) { return (features + kKnnQueries - 1) / kKnnQueries; }
+// shared rows are padded to a stride of 4 (mod 8) words, so the 8 16-byte reads of a quarter-warp hit distinct banks
 __host__ __device__ constexpr int KnnStride(int length) { return (length + 7) / 8 * 8 + 4; }
 __host__ __device__ constexpr int KnnSharedBytes(int length) {
   return int(sizeof(float)) * (kKnnQueries + kKnnTrain) * KnnStride(length);
 }
 __global__ void k_texture_knn_l2(const __grid_constant__ TextureArgs a);
+__global__ void k_texture_knn_hamming(const __grid_constant__ TextureArgs a);
 
 // k_texture_crop / k_texture_features: up to kTexJobs bodies per launch; the jobs travel in the kernel parameters
 constexpr int kTexJobs = 128;
@@ -104,12 +119,13 @@ struct TexFeatJob {
 
 struct TexFeatArgs {
   TexFeatJob jobs[kTexJobs];
-  float2* feat_xy;       // TextureArgs' frame-feature tables
+  float2* feat_xy;       // TextureArgs' frame-feature tables, `cap` features per body
   uint32_t* feat_desc;
   float* feat_fdesc;
   int* feat_n;
   int* nonfinite;        // [n_bodies] 1: the body's last device upload held a non-finite descriptor value
   int n_jobs;
+  int cap;
 };
 
 // one CTA of kTexThreads per job
@@ -122,23 +138,25 @@ __host__ __device__ __forceinline__ float TexTukeyNorm(float error, float c) {
 }
 
 // TextureModality::CalculateGradientAndHessian (texture_modality.cpp:397-444) over the data points i = first, first +
-// stride, ... of one body, added to acc (g[6], H lower [21], the reference's signs). Also refreshes data_point.center.
+// stride, ... of one body (fields point_cap floats apart), added to acc (g[6], H lower [21], the reference's signs). Also
+// refreshes data_point.center.
 __device__ __forceinline__ void TextureGradient(const CameraDev& cam, const float* pose, const TextureParamsDev& tp,
-                                                int corr, float* pts, int n, int first, int stride, float* acc) {
+                                                int corr, float* pts, int point_cap, int n, int first, int stride,
+                                                float* acc) {
   float b2c[12];
   PoseMul(cam.w2c, pose, b2c);
   const float sd = LastValid(tp.standard_deviations, tp.n_standard_deviations, corr);
   const float variance = powf(sd, 2.0f);
   for (int i = first; i < n; i += stride) {
-    const float bx = pts[TF_CBX * kTexPointCap + i], by = pts[TF_CBY * kTexPointCap + i], bz = pts[TF_CBZ * kTexPointCap + i];
+    const float bx = pts[TF_CBX * point_cap + i], by = pts[TF_CBY * point_cap + i], bz = pts[TF_CBZ * point_cap + i];
     const float x = b2c[0] * bx + b2c[1] * by + b2c[2] * bz + b2c[3];
     const float y = b2c[4] * bx + b2c[5] * by + b2c[6] * bz + b2c[7];
     const float z = b2c[8] * bx + b2c[9] * by + b2c[10] * bz + b2c[11];
     const float cu = x * cam.fu / z + cam.ppu, cv = y * cam.fv / z + cam.ppv;
-    pts[TF_PU * kTexPointCap + i] = cu;
-    pts[TF_PV * kTexPointCap + i] = cv;
+    pts[TF_PU * point_cap + i] = cu;
+    pts[TF_PV * point_cap + i] = cv;
     const float z2 = z * z;
-    const float d0 = cu - pts[TF_CU * kTexPointCap + i], d1 = cv - pts[TF_CV * kTexPointCap + i];
+    const float d0 = cu - pts[TF_CU * point_cap + i], d1 = cv - pts[TF_CV * point_cap + i];
     const float squared_error = d0 * d0 + d1 * d1;
     const float error = sqrtf(squared_error);
     float weight = 1.0f / variance;

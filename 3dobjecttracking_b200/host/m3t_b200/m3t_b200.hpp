@@ -1467,6 +1467,10 @@ class TextureModality : public Modality {
   void set_measured_occlusion_threshold(float v) { params_.measured_occlusion_threshold = v; set_up_ = false; }
   void set_modeled_occlusion_radius(float v) { params_.modeled_occlusion_radius = v; set_up_ = false; }
   void set_modeled_occlusion_threshold(float v) { params_.modeled_occlusion_threshold = v; set_up_ = false; }
+  // A device capacity the reference does not have: the most features SetFeatures may hand over per frame, 512 (the
+  // default) .. 4096. It sizes the context's texture tables (m3tb_texture_params::n_features_max).
+  void set_n_features_max(int v) { params_.n_features_max = v; set_up_ = false; }
+  int n_features_max() const { return params_.n_features_max; }
   DescriptorType descriptor_type() const { return descriptor_type_; }
   const m3tb_texture_params& params() const { return params_; }
   const std::shared_ptr<ColorCamera>& color_camera_ptr() const { return color_camera_ptr_; }

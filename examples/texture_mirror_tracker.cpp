@@ -5,7 +5,8 @@
 // whole-number floats in 0 .. 255, as cv::SIFT writes them (sift), seen at the start pose for StartModality and at the
 // ground-truth pose for the tracked frame. The scene is tracked once through Tracker::ExecuteTrackingStep and once
 // through ExecuteTrackingStepObjectWise; both pose sets are printed as JSON for tests/test_gpu_texture_mirror.py and
-// tests/test_gpu_texture_l2.py.
+// tests/test_gpu_texture_l2.py. Above 512 features per body (up to 4096) every texture modality raises its
+// n_features_max to n_features, so the frame's features are matched in full (k_texture_knn_hamming for orb).
 //
 //   usage: texture_mirror_tracker [seed=1] [n_features=300] [orb|sift]
 #include <algorithm>
@@ -224,6 +225,7 @@ int main(int argc, char** argv) {
       dm->set_n_points_max(n_points);
       auto tm = std::make_shared<TextureModality>("texture_modality_" + std::to_string(b), s.batch, body, cc, silhouette);
       if (sift) tm->set_descriptor_type(TextureModality::DescriptorType::SIFT);
+      tm->set_n_features_max(std::max(n_features, tm->n_features_max()));
       auto link = std::make_shared<Link>("link_" + std::to_string(b), body);
       link->AddModality(rm);
       link->AddModality(dm);
@@ -265,7 +267,8 @@ int main(int argc, char** argv) {
   }
   if (!fused.tracker->ExecuteTrackingStep(0)) return 3;
   if (!object_wise.tracker->ExecuteTrackingStepObjectWise(0)) return 4;
-  std::printf("{\"descriptor\": \"%s\", \"n_bodies\": %d, \"texture_points\": [", sift ? "sift" : "orb", kBodies);
+  std::printf("{\"descriptor\": \"%s\", \"n_bodies\": %d, \"n_features_max\": %d, \"texture_points\": [",
+              sift ? "sift" : "orb", kBodies, fused.textures[0]->n_features_max());
   for (int b = 0; b < kBodies; ++b) {
     std::vector<m3tb_texture_point> pts(512);
     int n = 0;

@@ -210,6 +210,10 @@ typedef struct m3tb_texture_params {
   int32_t model_occlusions;                /* 0  (needs a depth renderer attached with m3tb_attach_renderer) */
   float modeled_occlusion_radius;          /* 0.01 */
   float modeled_occlusion_threshold;       /* 0.03 */
+  int32_t n_features_max;                  /* 512 (512 .. 4096): a device capacity, like n_lines_max; the reference
+                                              has no counterpart and matches any number of features. The most
+                                              keypoints one upload of the body may hand over; above 4096
+                                              M3TB_ERR_UNSUPPORTED, below 512 M3TB_ERR_INVALID. */
 } m3tb_texture_params;
 
 /* TextureModality::DataPoint (texture_modality.h:136-141) - debug / parity read-back only. */
@@ -480,7 +484,8 @@ int m3tb_share_color_histograms(m3tb_ctx* ctx, int body, int owner_body);
  * BGR2GRAY, image(roi), resize by `scale` in both directions), runs cv::ORB, cv::SIFT or cv::xfeatures2d::DAISY on the
  * crop and hands the keypoints and descriptors over. Everything after detection runs on the device: keyframe
  * reconstruction from the device silhouette renderer with the occlusion checks, kNN matching with the ratio test
- * (Hamming for ORB; L2 for SIFT and DAISY, k_texture_knn_l2 at correspondence iteration 0), the Tukey-weighted
+ * (Hamming for ORB, with k_texture_knn_hamming at correspondence iteration 0 for bodies above 512 features; L2 for SIFT
+ * and DAISY, k_texture_knn_l2 at correspondence iteration 0), the Tukey-weighted
  * reprojection gradient / Hessian in every update (inside k_track, added to the link after region and depth) and the
  * keyframe refresh. Bodies with a texture modality are tracked by k_track; contexts without one launch what they
  * launched before. A texture body may be the body of a link of a kinematic structure, or one of its extra bodies with
@@ -491,21 +496,26 @@ int m3tb_share_color_histograms(m3tb_ctx* ctx, int body, int owner_body);
  * descriptor length. M3TB_ERR_UNSUPPORTED for BRISK, FREAK and ORB_CUDA and for n_keyframes above 8;
  * M3TB_ERR_INVALID for bad ids, an unset camera, a body without geometry, non-positive standard deviations or Tukey
  * constant, and measure_occlusions without the body's depth camera.
- * Device memory: the first call allocates the texture tables for max_bodies, about 0.32 MB per body slot; the first
- * call with SIFT or DAISY adds the float descriptor tables, 4.7 MB per slot (512 frame and 8 x 512 keyframe rows of
- * 256 floats, and 8 x 512 match results). Either allocation is all or nothing: on failure the context is as it
- * was. */
+ * M3TB_ERR_UNSUPPORTED for n_features_max above 4096 and M3TB_ERR_INVALID below 512.
+ * Device memory: the tables hold C features per body slot for max_bodies, C the largest n_features_max any texture
+ * body of the context has asked for (512 while every body keeps the default). The first call allocates the base
+ * tables, 616 C bytes per slot (0.32 MB at 512, 2.5 MB at 4096); the first call with SIFT or DAISY adds the float
+ * descriptor tables and the match table, 9248 C bytes per slot (C frame and 8 x C keyframe rows of 256 floats, and
+ * 8 x C match results: 4.7 MB at 512, 37.9 MB at 4096); the first ORB body above 512 adds the match table alone
+ * (32 C bytes per slot). A call that raises C remakes every table at the new C and keeps what the other bodies hold.
+ * Each of these steps is all or nothing: on failure the context is as it was. */
 int m3tb_set_texture_modality(m3tb_ctx* ctx, int body, const m3tb_texture_params* params, int color_camera);
 /* TextureModality::CalculateScaleAndRegionOfInterest (texture_modality.cpp:890-931, margin 10 px) from the current
  * device poses, for bodies [first, first + count): roi[4 * k] = x, y, width, height, scale[k] the factor the crop is
  * resized by, valid[k] = 0 when the reference returns false (z < 1.5 r, an empty region) or the body has no texture
  * modality (roi and scale are then 0). Synchronises the stream. */
 int m3tb_get_texture_focus(m3tb_ctx* ctx, int first, int count, int32_t* roi, float* scale, int32_t* valid);
-/* The keypoints_ / descriptors_ of the current colour frame of one body: `n` (0 .. 512) keypoints as (x, y) in crop
+/* The keypoints_ / descriptors_ of the current colour frame of one body: `n` (0 .. n_features_max) keypoints as (x, y) in crop
  * coordinates, which become roi + pt / scale in the image (texture_modality.cpp:884-887), and n 32-byte ORB
  * descriptors. One upload per frame serves m3tb_start_modalities, correspondence iteration 0 (both detect on the same
  * frame at the same pose) and m3tb_calculate_results. A body whose camera received a newer frame since its last upload
- * has no features, as when the reference's detection returns early. M3TB_ERR_UNSUPPORTED above 512 features;
+ * has no features, as when the reference's detection returns early. M3TB_ERR_UNSUPPORTED above the body's
+ * n_features_max features;
  * M3TB_ERR_INVALID for a SIFT / DAISY body (m3tb_upload_texture_float_features). */
 int m3tb_upload_texture_features(m3tb_ctx* ctx, int body, const float* keypoints_xy, const uint8_t* descriptors, int n,
                                  int roi_x, int roi_y, float scale);
@@ -546,7 +556,7 @@ typedef struct m3tb_device_features {
  * launch per 128 bodies and without synchronising: keypoints become float(roi_x) + x / scale with the roi and scale of
  * the body's last m3tb_texture_crop. Replaces, per body and frame, the host copy of the detector's output
  * (DetectAndComputeCorrKeypoints, texture_modality.cpp:870-887). Refusals as the host upload (M3TB_ERR_UNSUPPORTED
- * above 512 features; M3TB_ERR_INVALID for the other descriptor kind, a bad length and a length other than the first
+ * above the body's n_features_max features; M3TB_ERR_INVALID for the other descriptor kind, a bad length and a length other than the first
  * upload's), and M3TB_ERR_INVALID for a body whose last crop is not of its camera's current frame; nothing is launched
  * when any body is refused. Float descriptors are checked on the device: a body with a non-finite value gets no
  * features this frame and its flag (m3tb_get_texture_feature_flags) is raised. The caller keeps the buffers unchanged

@@ -17,7 +17,14 @@ numbers in 0 .. 255 for SIFT, unit-norm for DAISY, every query a keyframe point)
     2 * queries * train * length against the 67 TFLOP/s data sheet;
   - one tracking step at the ORB shape above (128 bodies, 300 features) with ORB against the L2 descriptor.
 
-    python scripts/texture_timing.py [K] [--descriptor sift|daisy]"""
+With --features N (512 .. 4096) it measures a context whose bodies keep N features each (n_features_max N, every
+feature near the body's centre, so all become keyframe points), for ORB and SIFT and for 1, 8 and 128 bodies:
+  - the matcher's device time per launch (torch.profiler CUDA activity over K calls of m3tb_texture_correspondences at
+    correspondence iteration 0): k_texture_knn_hamming for ORB above 512 (k_texture_match's in-CTA scan at 512) and
+    k_texture_knn_l2 for SIFT;
+  - one tracking step (n_corr x n_update of the workload).
+
+    python scripts/texture_timing.py [K] [--descriptor sift|daisy] [--features N]"""
 import importlib
 import json
 import os
@@ -34,9 +41,10 @@ capi = importlib.import_module("3dobjecttracking_b200.capi")
 synth = pkg.synth
 
 ARGS = [a for a in sys.argv[1:] if not a.startswith("--")]
-K = int(ARGS[0]) if ARGS else 100
 DESCRIPTOR = sys.argv[sys.argv.index("--descriptor") + 1] if "--descriptor" in sys.argv else None
-ARGS = [a for a in ARGS if a != DESCRIPTOR]
+FEATURES = int(sys.argv[sys.argv.index("--features") + 1]) if "--features" in sys.argv else None
+ARGS = [a for a in ARGS if a not in (DESCRIPTOR, str(FEATURES))]
+K = int(ARGS[0]) if ARGS else 100
 N_FEAT = 300
 L2_LENGTH = {"sift": 128, "daisy": 104}
 L2_TYPE = {"sift": capi.DESCRIPTOR_SIFT, "daisy": capi.DESCRIPTOR_DAISY}
@@ -75,6 +83,7 @@ def make(wl, texture, kind=None, n_feat=N_FEAT, n_keyframes=1, central=False):
         if kind is not None:
             params.descriptor_type = L2_TYPE[kind]
         params.n_keyframes = n_keyframes
+        params.n_features_max = max(params.n_features_max, n_feat)
         params.max_keyframe_age = 0 if n_keyframes > 1 else params.max_keyframe_age
         for b in range(wl.n_bodies):
             ctx.set_focused_renderer(b, "color", b, [b], [b], id_type="body")
@@ -121,8 +130,8 @@ def gpu_name():
 step = lambda c, n_corr, n_update: (lambda: c.tracking_step(0, n_corr, n_update))  # noqa: E731
 
 
-def knn_kernel_ms(ctx):
-    """k_texture_knn_l2's mean device time per launch over K calls of the match (torch.profiler CUDA activity)."""
+def knn_kernel_ms(ctx, kernel="k_texture_knn_l2"):
+    """The kernel's mean device time per launch over K calls of the match (torch.profiler CUDA activity)."""
     import torch
     from torch.profiler import ProfilerActivity, profile
     for _ in range(10):
@@ -133,7 +142,7 @@ def knn_kernel_ms(ctx):
             ctx.texture_correspondences(0, 0)
         ctx.synchronize()
         torch.cuda.synchronize()
-    rows = [e for e in prof.key_averages() if "k_texture_knn_l2" in e.key]
+    rows = [e for e in prof.key_averages() if kernel in e.key]
     assert len(rows) == 1 and rows[0].count == K, [(e.key, e.count) for e in rows]
     return max(rows[0].self_device_time_total, rows[0].device_time_total) / K / 1e3
 
@@ -166,6 +175,30 @@ def l2_main(kind):
                           ms_step_orb=steps["orb"], **{"ms_step_" + kind: steps[kind]}, gpu=gpu_name())))
 
 
+def features_main(n_feat):
+    import torch
+    torch.cuda.init()
+    shapes = []
+    for kind in ("orb", "sift"):
+        kernel = "k_texture_knn_l2" if kind == "sift" else "k_texture_knn_hamming" if n_feat > 512 else "k_texture_match"
+        for n_bodies in (1, 8, 128):
+            wl = synth.make_workload("c4", n_bodies=n_bodies, n_divides=2, seed=0)
+            wl, ctx = make(wl, True, None if kind == "orb" else kind, n_feat=n_feat, central=True)
+            queries = sum(int(ctx.get_texture_keyframes(b)["sizes"].sum()) for b in range(n_bodies))
+            ms = knn_kernel_ms(ctx, kernel)
+            ms_step = time_calls(ctx, step(ctx, wl.n_corr_iterations, wl.n_update_iterations))
+            points = int(np.mean([len(ctx.get_texture_points(b)) for b in range(n_bodies)]))
+            shapes.append(dict(descriptor=kind, bodies=n_bodies, queries=queries, train_per_body=n_feat, kernel=kernel,
+                               ms_kernel=ms, ms_step=ms_step, mean_data_points_per_body=points,
+                               n_corr=wl.n_corr_iterations, n_update=wl.n_update_iterations))
+            ctx.close()
+    print(json.dumps(dict(features=n_feat, K=K, shapes=shapes, gpu=gpu_name())))
+
+
+if FEATURES is not None:
+    assert 512 <= FEATURES <= 4096, FEATURES
+    features_main(FEATURES)
+    sys.exit(0)
 if DESCRIPTOR is not None:
     assert DESCRIPTOR in L2_LENGTH, DESCRIPTOR
     l2_main(DESCRIPTOR)
