@@ -133,7 +133,7 @@ SYMBOLS = [
     "m3tb_calculate_optimization", "m3tb_get_region_lines", "m3tb_get_depth_points", "m3tb_get_closest_views",
     "m3tb_debug_phase_clocks", "m3tb_last_ingest_bytes", "m3tb_set_structure", "m3tb_clear_structures",
     "m3tb_n_structures", "m3tb_calculate_consistent_poses", "m3tb_refine_poses", "m3tb_get_link_poses", "m3tb_get_structure_theta",
-    "m3tb_set_gradient_hessian", "m3tb_reset_joint_poses", "m3tb_prefetch_frames", "m3tb_detach_frames",
+    "m3tb_set_gradient_hessian", "m3tb_debug_rigid_solve", "m3tb_reset_joint_poses", "m3tb_prefetch_frames", "m3tb_detach_frames",
     "m3tb_debug_closest_view", "m3tb_upload_depth_rendering", "m3tb_upload_silhouette_rendering",
     "m3tb_share_color_histograms", "m3tb_debug_last_launch", "m3tb_set_body_geometry", "m3tb_set_focused_renderer",
     "m3tb_attach_renderer", "m3tb_render", "m3tb_get_rendering", "m3tb_model_params_default", "m3tb_model_views",
@@ -243,6 +243,7 @@ def lib():
     L.m3tb_get_link_poses.argtypes = [vp, ci, fp, fp, fp]
     L.m3tb_get_structure_theta.argtypes = [vp, ci, fp, ci, C.POINTER(ci), C.POINTER(ci)]
     L.m3tb_set_gradient_hessian.argtypes = [vp, ci, fp, fp]
+    L.m3tb_debug_rigid_solve.argtypes = [vp, ci, ci, fp, fp, fp, fp, C.POINTER(ci)]
     L.m3tb_debug_last_launch.argtypes = [vp, C.POINTER(LaunchInfo)]
     L.m3tb_set_body_geometry.argtypes = [vp, ci, fp, ci, fp, C.c_float, ci, ci, ci]
     L.m3tb_set_focused_renderer.argtypes = [vp, ci, ci, ci, ci, C.c_float, C.c_float, ci, ip, ci, ip, ci]
@@ -810,6 +811,19 @@ class Context:
         g = np.ascontiguousarray(g, np.float32)
         H = np.ascontiguousarray(H, np.float32)
         self._ck(self.L.m3tb_set_gradient_hessian(self.h, modality, _p(g), _p(H)))
+
+    def debug_rigid_solve(self, solve, a, b, poses):
+        """Test aid: the device rigid-body solve of k_track (solve 0) or k_track2 (solve 1) on systems a [n, 6, 6]
+        (lower triangle read), b [n, 6] from start poses [n, 3, 4]: (theta [n, 6], updated [n] bool, poses [n, 3, 4])."""
+        a = np.ascontiguousarray(a, np.float32).reshape(-1, 36)
+        n = a.shape[0]
+        b = np.ascontiguousarray(b, np.float32).reshape(n, 6)
+        p = np.array(poses, np.float32).reshape(n, 12)
+        theta = np.zeros((n, 6), np.float32)
+        upd = np.zeros(n, np.int32)
+        self._ck(self.L.m3tb_debug_rigid_solve(self.h, solve, n, _p(a), _p(b), _p(p), _p(theta),
+                                               upd.ctypes.data_as(C.POINTER(C.c_int))))
+        return theta, upd.astype(bool), p.reshape(n, 3, 4)
 
     def clear_structures(self):
         self._ck(self.L.m3tb_clear_structures(self.h))

@@ -15,6 +15,7 @@
 #include <cstring>
 #include <memory>
 #include <string>
+#include <type_traits>
 #include <vector>
 
 #include "m3t_b200_owned.h"
@@ -2164,6 +2165,38 @@ int ContourOverflow(m3tb_ctx* ctx, const RegionBuffers& rb) {
 
 }  // namespace
 
+namespace {
+// m3tb_debug_rigid_solve: one warp per system runs the rigid-body solve of k_track (SolveAndUpdateWarp) or of k_track2
+// (SolveAndUpdateSerial) itself, on the system as the kernels leave it in shared memory (sh.a full symmetric), with no
+// camera to refresh pose products for.
+template <bool SERIAL>
+__global__ void __launch_bounds__(32) k_debug_rigid_solve(const float* __restrict__ a, const float* __restrict__ b,
+                                                          float* __restrict__ poses, float* __restrict__ theta,
+                                                          int* __restrict__ updated) {
+  using Sh = typename std::conditional<SERIAL, Shared2, Shared>::type;
+  __shared__ Sh sh;
+  const int s = blockIdx.x, lane = threadIdx.x;
+  for (int e = lane; e < 36; e += 32) {
+    const int i = e / 6, j = e - 6 * (e / 6);
+    sh.a[e] = a[36 * s + (i >= j ? 6 * i + j : 6 * j + i)];  // the lower triangle, mirrored
+  }
+  if (lane < 6) sh.b[lane] = b[6 * s + lane];
+  if (lane < 12) sh.pose[lane] = poses[12 * s + lane];
+  __syncwarp();
+  bool ok;
+  if constexpr (SERIAL) {
+    ok = SolveAndUpdateSerial(sh, false, false);
+  } else {
+    int stamp_i = 0;
+    ok = SolveAndUpdateWarp(sh, nullptr, nullptr, nullptr, nullptr, stamp_i);
+  }
+  __syncwarp();
+  if (lane < 6) theta[6 * s + lane] = sh.x[lane];
+  if (lane < 12) poses[12 * s + lane] = sh.pose[lane];
+  if (lane == 0) updated[s] = ok ? 1 : 0;
+}
+}  // namespace
+
 extern "C" {
 
 void m3tb_region_params_default(m3tb_region_params* p) {
@@ -2713,6 +2746,33 @@ int m3tb_calculate_optimization(m3tb_ctx* ctx, int iteration, int corr_iteration
   CHECK_CTX();
   if (HasStructures(ctx)) return LaunchStructure(ctx, 0, true);
   return LaunchTrack(ctx, iteration, corr_iteration, corr_iteration + 1, 1, opt_iteration, PH_LOAD_GH | PH_SOLVE);
+}
+
+int m3tb_debug_rigid_solve(m3tb_ctx* ctx, int solve, int n, const float* a, const float* b, float* poses, float* theta,
+                           int* updated) {
+  CHECK_CTX();
+  if ((solve != 0 && solve != 1) || n < 0 || (n > 0 && (!a || !b || !poses || !theta || !updated)))
+    return Fail(ctx, M3TB_ERR_INVALID, "bad rigid-solve arguments");
+  if (n == 0) return M3TB_OK;
+  DeviceBuffer<float> d_a, d_b, d_pose, d_theta;
+  DeviceBuffer<int> d_upd;
+  CU(d_a.create(size_t(36) * n));
+  CU(d_b.create(size_t(6) * n));
+  CU(d_pose.create(size_t(12) * n));
+  CU(d_theta.create(size_t(6) * n));
+  CU(d_upd.create(size_t(n)));
+  CU(cudaMemcpyAsync(d_a, a, sizeof(float) * 36 * n, cudaMemcpyHostToDevice, ctx->stream));
+  CU(cudaMemcpyAsync(d_b, b, sizeof(float) * 6 * n, cudaMemcpyHostToDevice, ctx->stream));
+  CU(cudaMemcpyAsync(d_pose, poses, sizeof(float) * 12 * n, cudaMemcpyHostToDevice, ctx->stream));
+  if (solve == 0) k_debug_rigid_solve<false><<<unsigned(n), 32, 0, ctx->stream>>>(d_a, d_b, d_pose, d_theta, d_upd);
+  else k_debug_rigid_solve<true><<<unsigned(n), 32, 0, ctx->stream>>>(d_a, d_b, d_pose, d_theta, d_upd);
+  CU(cudaGetLastError());
+  ctx->launches++;
+  CU(cudaMemcpyAsync(poses, d_pose, sizeof(float) * 12 * n, cudaMemcpyDeviceToHost, ctx->stream));
+  CU(cudaMemcpyAsync(theta, d_theta, sizeof(float) * 6 * n, cudaMemcpyDeviceToHost, ctx->stream));
+  CU(cudaMemcpyAsync(updated, d_upd, sizeof(int) * n, cudaMemcpyDeviceToHost, ctx->stream));
+  CU(cudaStreamSynchronize(ctx->stream));
+  return M3TB_OK;
 }
 
 int m3tb_set_structure(m3tb_ctx* ctx, int structure, const m3tb_link* links, int n_links,

@@ -966,6 +966,8 @@ __device__ __forceinline__ void PoseProductsWarp(bool has_color, bool has_depth,
   }
 }
 
+constexpr unsigned kFloatInfBits = 0x7f800000u;  // bits of +inf: the bits of |x| are greater exactly when x is NaN
+
 // sh.a (full symmetric 6x6) and sh.b must be visible to the calling warp (all 32 lanes call this).
 // Lane r < 6 owns row r of the permuted matrix; lanes >= 6 shadow row 5 and never publish anything. The code is
 // deliberately compact (it runs on one warp while 15 others wait at the barrier, so its instruction-fetch
@@ -981,13 +983,17 @@ __device__ __forceinline__ bool SolveAndUpdateWarp(Shared& sh, const CameraDev* 
   // 1. transposition sequence from the ORIGINAL diagonal: the left-looking factorisation never touches a
   //    diagonal entry before it is chosen as pivot (Eigen LDLT.h, "Find largest diagonal element"; first max wins)
   //    |d| >= 0, so the float bit patterns order like the values: one REDUX.MAX + one ballot per step.
+  //    NaN as in maxCoeff: it is compared false, so it stays pivot when it heads the tail and never wins further down;
+  //    a NaN or zero first pivot is the zero-matrix exit, which keeps the identity transpositions.
   unsigned key = lane < n ? __float_as_uint(fabsf(sh.a[r * (n + 1)])) : 0u;
   int pm = r;
+  bool zero_exit = false;
 #pragma unroll
   for (int k = 0; k < n - 1; ++k) {
-    const bool eligible = lane >= k && lane < n;
+    const bool eligible = lane >= k && lane < n && (key <= kFloatInfBits || lane == k);
     const unsigned big = __reduce_max_sync(kFull, eligible ? key : 0u);
-    const int p = __ffs(__ballot_sync(kFull, eligible && key == big)) - 1;
+    if (k == 0) zero_exit = big - 1u >= kFloatInfBits;
+    const int p = zero_exit ? k : __ffs(__ballot_sync(kFull, eligible && key == big)) - 1;
     const unsigned key_k = __shfl_sync(kFull, key, k), key_p = __shfl_sync(kFull, key, p);
     const int pm_k = __shfl_sync(kFull, pm, k), pm_p = __shfl_sync(kFull, pm, p);
     if (lane == k) { key = key_p; pm = pm_p; }

@@ -518,8 +518,18 @@ __device__ __forceinline__ bool SolveAndUpdateSerial(Shared2& sh, bool has_color
   // 1. transposition sequence from the ORIGINAL diagonal (see SolveAndUpdateWarp)
   unsigned key[n];
   int pm[n];
+  // A NaN is pivoted only when it heads the tail and never wins below it, so it never moves: the NaN positions are
+  // those of the original diagonal, their keys are 0 and no step that a NaN heads swaps. A NaN first pivot is the
+  // zero-matrix exit (identity transpositions); with a zero first pivot every key is 0 and no step swaps either.
+  unsigned nan_steps = 0u;
 #pragma unroll
-  for (int i = 0; i < n; ++i) { key[i] = __float_as_uint(fabsf(sh.a[i * (n + 1)])); pm[i] = i; }
+  for (int i = 0; i < n; ++i) {
+    const unsigned bits = __float_as_uint(fabsf(sh.a[i * (n + 1)]));
+    nan_steps |= unsigned(bits > kFloatInfBits) << i;
+    key[i] = bits > kFloatInfBits ? 0u : bits;
+    pm[i] = i;
+  }
+  if (nan_steps & 1u) nan_steps = (1u << n) - 1u;
 #pragma unroll
   for (int k = 0; k < n - 1; ++k) {
     int p = k;
@@ -527,6 +537,7 @@ __device__ __forceinline__ bool SolveAndUpdateSerial(Shared2& sh, bool has_color
 #pragma unroll
     for (int q = k + 1; q < n; ++q)
       if (key[q] > big) { big = key[q]; p = q; }
+    if (nan_steps & (1u << k)) p = k;
 #pragma unroll
     for (int q = k + 1; q < n; ++q)
       if (p == q) {

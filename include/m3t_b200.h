@@ -670,6 +670,13 @@ int m3tb_get_structure_theta(m3tb_ctx* ctx, int structure, float* theta, int cap
  * bodies with one add it); gradients[n_bodies][6], hessians[n_bodies][36] (symmetric).
  * For adapters that compute a modality elsewhere and for the parity tests of m3tb_calculate_optimization. */
 int m3tb_set_gradient_hessian(m3tb_ctx* ctx, int modality, const float* gradients, const float* hessians);
+/* Test aid: Optimizer::CalculateOptimization + Link::UpdatePoses of n rigid bodies from given systems, through the
+ * device solve of k_track (solve 0) or of k_track2 (solve 1). a[n][36]: the normal matrix -H + diag(Tikhonov), only
+ * its lower triangle is read; b[n][6]: the gradient; poses[n][12]: body2world, replaced by the updated pose (left as
+ * it was when the NaN guard refuses the update); theta[n][6]: the solution before the guard; updated[n]: 1 if the
+ * pose was updated. */
+int m3tb_debug_rigid_solve(m3tb_ctx* ctx, int solve, int n, const float* a, const float* b, float* poses, float* theta,
+                           int* updated);
 
 /* ---- parity read-back of the per-line / per-point state (data_lines_, data_points_) ----------- */
 /* `lines` must hold n_lines_max records; *n_out receives how many model points were processed. */
