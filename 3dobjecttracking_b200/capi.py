@@ -813,8 +813,9 @@ class Context:
         self._ck(self.L.m3tb_set_gradient_hessian(self.h, modality, _p(g), _p(H)))
 
     def debug_rigid_solve(self, solve, a, b, poses):
-        """Test aid: the device rigid-body solve of k_track (solve 0) or k_track2 (solve 1) on systems a [n, 6, 6]
-        (lower triangle read), b [n, 6] from start poses [n, 3, 4]: (theta [n, 6], updated [n] bool, poses [n, 3, 4])."""
+        """Test aid: the device rigid-body solve, on the shared-memory layout of k_track (solve 0) or k_track2 (solve 1),
+        on systems a [n, 6, 6] (lower triangle read), b [n, 6] from start poses [n, 3, 4]: (theta [n, 6], updated [n]
+        bool, poses [n, 3, 4])."""
         a = np.ascontiguousarray(a, np.float32).reshape(-1, 36)
         n = a.shape[0]
         b = np.ascontiguousarray(b, np.float32).reshape(n, 6)

@@ -15,7 +15,6 @@
 #include <cstring>
 #include <memory>
 #include <string>
-#include <type_traits>
 #include <vector>
 
 #include "m3t_b200_owned.h"
@@ -2166,14 +2165,13 @@ int ContourOverflow(m3tb_ctx* ctx, const RegionBuffers& rb) {
 }  // namespace
 
 namespace {
-// m3tb_debug_rigid_solve: one warp per system runs the rigid-body solve of k_track (SolveAndUpdateWarp) or of k_track2
-// (SolveAndUpdateSerial) itself, on the system as the kernels leave it in shared memory (sh.a full symmetric), with no
-// camera to refresh pose products for.
-template <bool SERIAL>
+// m3tb_debug_rigid_solve: one warp per system runs the rigid-body solve (SolveAndUpdateSerial) itself, on k_track's
+// shared-memory layout (Shared) or k_track2's (Shared2), on the system as the kernels leave it in shared memory (sh.a
+// full symmetric), with no camera to refresh pose products for.
+template <class Sh>
 __global__ void __launch_bounds__(32) k_debug_rigid_solve(const float* __restrict__ a, const float* __restrict__ b,
                                                           float* __restrict__ poses, float* __restrict__ theta,
                                                           int* __restrict__ updated) {
-  using Sh = typename std::conditional<SERIAL, Shared2, Shared>::type;
   __shared__ Sh sh;
   const int s = blockIdx.x, lane = threadIdx.x;
   for (int e = lane; e < 36; e += 32) {
@@ -2183,13 +2181,7 @@ __global__ void __launch_bounds__(32) k_debug_rigid_solve(const float* __restric
   if (lane < 6) sh.b[lane] = b[6 * s + lane];
   if (lane < 12) sh.pose[lane] = poses[12 * s + lane];
   __syncwarp();
-  bool ok;
-  if constexpr (SERIAL) {
-    ok = SolveAndUpdateSerial(sh, false, false);
-  } else {
-    int stamp_i = 0;
-    ok = SolveAndUpdateWarp(sh, nullptr, nullptr, nullptr, nullptr, stamp_i);
-  }
+  const bool ok = SolveAndUpdateSerial(sh, false, false);
   __syncwarp();
   if (lane < 6) theta[6 * s + lane] = sh.x[lane];
   if (lane < 12) poses[12 * s + lane] = sh.pose[lane];
@@ -2764,8 +2756,8 @@ int m3tb_debug_rigid_solve(m3tb_ctx* ctx, int solve, int n, const float* a, cons
   CU(cudaMemcpyAsync(d_a, a, sizeof(float) * 36 * n, cudaMemcpyHostToDevice, ctx->stream));
   CU(cudaMemcpyAsync(d_b, b, sizeof(float) * 6 * n, cudaMemcpyHostToDevice, ctx->stream));
   CU(cudaMemcpyAsync(d_pose, poses, sizeof(float) * 12 * n, cudaMemcpyHostToDevice, ctx->stream));
-  if (solve == 0) k_debug_rigid_solve<false><<<unsigned(n), 32, 0, ctx->stream>>>(d_a, d_b, d_pose, d_theta, d_upd);
-  else k_debug_rigid_solve<true><<<unsigned(n), 32, 0, ctx->stream>>>(d_a, d_b, d_pose, d_theta, d_upd);
+  if (solve == 0) k_debug_rigid_solve<Shared><<<unsigned(n), 32, 0, ctx->stream>>>(d_a, d_b, d_pose, d_theta, d_upd);
+  else k_debug_rigid_solve<Shared2><<<unsigned(n), 32, 0, ctx->stream>>>(d_a, d_b, d_pose, d_theta, d_upd);
   CU(cudaGetLastError());
   ctx->launches++;
   CU(cudaMemcpyAsync(poses, d_pose, sizeof(float) * 12 * n, cudaMemcpyDeviceToHost, ctx->stream));

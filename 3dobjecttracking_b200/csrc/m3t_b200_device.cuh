@@ -277,6 +277,32 @@ __host__ __device__ __forceinline__ void PoseInverse(const float* p, float* o) {
   }
 }
 
+// Vector2Skewsymmetric(w).exp() in closed form (Rodrigues), row-major 3x3; the reference uses Eigen's Pade approximant
+// (link.cpp:224), the two agree to < 1e-7 for |w| <= 1 (tests/test_oracle_math.py). Rigid bodies and kinematic
+// structures share it.
+__device__ __forceinline__ void ExpSkew(const float* w, float* r) {
+  float t2 = w[0] * w[0] + w[1] * w[1] + w[2] * w[2];
+  float a, b;
+  if (t2 < 0.01f) {
+    // |w| < 0.1 rad (every realistic Gauss-Newton step): truncated series, remainder < 3e-14 relative
+    a = 1.0f + t2 * (-1.0f / 6.0f + t2 * (1.0f / 120.0f + t2 * (-1.0f / 5040.0f)));
+    b = 0.5f + t2 * (-1.0f / 24.0f + t2 * (1.0f / 720.0f + t2 * (-1.0f / 40320.0f)));
+  } else {
+    float t = sqrtf(t2);
+    float sh = sinf(0.5f * t);
+    a = sinf(t) / t;
+    b = 2.0f * sh * sh / t2;
+  }
+  float A[9] = {0.0f, -w[2], w[1], w[2], 0.0f, -w[0], -w[1], w[0], 0.0f};
+  float A2[9];
+#pragma unroll
+  for (int i = 0; i < 3; ++i)
+#pragma unroll
+    for (int j = 0; j < 3; ++j) A2[3 * i + j] = A[3 * i + 0] * A[0 + j] + A[3 * i + 1] * A[3 + j] + A[3 * i + 2] * A[6 + j];
+#pragma unroll
+  for (int k = 0; k < 9; ++k) r[k] = ((k % 4 == 0) ? 1.0f : 0.0f) + a * A[k] + b * A2[k];
+}
+
 template <typename T>
 __device__ __forceinline__ T LastValid(const T* v, int n, int idx) {  // common.h:170-176
   return idx < n ? v[idx] : v[n - 1];

@@ -246,26 +246,6 @@ __device__ inline void SoftLinkTermsDev(const ConstraintDev& c, const JointGeome
   }
 }
 
-// Vector2Skewsymmetric(w).exp(), the closed form of m3t_b200_kernels.cuh::ExpSkew (kept identical)
-__device__ inline void ExpSkewStruct(const float* w, float* r) {
-  const float t2 = w[0] * w[0] + w[1] * w[1] + w[2] * w[2];
-  float a, b;
-  if (t2 < 0.01f) {
-    a = 1.0f + t2 * (-1.0f / 6.0f + t2 * (1.0f / 120.0f + t2 * (-1.0f / 5040.0f)));
-    b = 0.5f + t2 * (-1.0f / 24.0f + t2 * (1.0f / 720.0f + t2 * (-1.0f / 40320.0f)));
-  } else {
-    const float t = sqrtf(t2);
-    const float sh = sinf(0.5f * t);
-    a = sinf(t) / t;
-    b = 2.0f * sh * sh / t2;
-  }
-  const float A[9] = {0.0f, -w[2], w[1], w[2], 0.0f, -w[0], -w[1], w[0], 0.0f};
-  float A2[9];
-  for (int i = 0; i < 3; ++i)
-    for (int j = 0; j < 3; ++j) A2[3 * i + j] = A[3 * i + 0] * A[0 + j] + A[3 * i + 1] * A[3 + j] + A[3 * i + 2] * A[6 + j];
-  for (int k = 0; k < 9; ++k) r[k] = ((k % 4 == 0) ? 1.0f : 0.0f) + a * A[k] + b * A2[k];
-}
-
 // Shared-memory carve-up of one structure (floats unless noted); sizes depend on (n_links, dof, n, n_constraints)
 struct StructSmem {
   float *l2w, *g, *H, *ad, *adj, *jac, *var, *cdata, *a, *b, *dst, *temp, *absdiag;
@@ -326,7 +306,7 @@ __device__ inline void UpdatePosesBlock(const StructSmem& s, LinkDev* links, int
     int idx = link.first_index;
     for (int d = 0; d < 6; ++d) th[d] = link.free_directions[d] ? s.dst[idx++] : 0.0f;
     float e[9];
-    ExpSkewStruct(th, e);
+    ExpSkew(th, e);
     float* var = s.var + 12 * tid;
     var[0] = e[0]; var[1] = e[1]; var[2] = e[2]; var[3] = th[3];
     var[4] = e[3]; var[5] = e[4]; var[6] = e[5]; var[7] = th[4];

@@ -671,7 +671,7 @@ int m3tb_get_structure_theta(m3tb_ctx* ctx, int structure, float* theta, int cap
  * For adapters that compute a modality elsewhere and for the parity tests of m3tb_calculate_optimization. */
 int m3tb_set_gradient_hessian(m3tb_ctx* ctx, int modality, const float* gradients, const float* hessians);
 /* Test aid: Optimizer::CalculateOptimization + Link::UpdatePoses of n rigid bodies from given systems, through the
- * device solve of k_track (solve 0) or of k_track2 (solve 1). a[n][36]: the normal matrix -H + diag(Tikhonov), only
+ * device's rigid-body solve on the shared-memory layout of k_track (solve 0) or of k_track2 (solve 1). a[n][36]: the normal matrix -H + diag(Tikhonov), only
  * its lower triangle is read; b[n][6]: the gradient; poses[n][12]: body2world, replaced by the updated pose (left as
  * it was when the NaN guard refuses the update); theta[n][6]: the solution before the guard; updated[n]: 1 if the
  * pose was updated. */

@@ -19,8 +19,8 @@ for body in (0, wl.n_bodies // 2):
     c = c[c > 0]
     d = np.diff(c)
     print(f"{name} body {body}: total {c[-1]-c[0]} cycles; prologue {d[0]}")
-    per = d[1:].reshape(-1, 3 + 2 * 9)
-    u = ["acc", "bar", "sum", "perm", "fact", "subst", "exp", "prod", "bar2"]
+    per = d[1:].reshape(-1, 3 + 2 * 5)
+    u = ["acc", "bar", "sum", "solve", "bar2"]
     labels = ["views", "region", "depth"] + [x + "0" for x in u] + [x + "1" for x in u]
     print("   " + " ".join(f"{l:>7}" for l in labels))
     for row in per:

@@ -1,13 +1,13 @@
-"""The device's rigid-body solve (SolveAndUpdateWarp of k_track, SolveAndUpdateSerial of k_track2) on the systems of
+"""The device's rigid-body solve (SolveAndUpdateSerial, shared by k_track and k_track2) on the systems of
 rigid_solve_cases, against the mirror oracle (orc_optimize_rigid, EXP_RODRIGUES) and the float64 restatement.
 
   * public C ABI: one context, one case per body, every case in one launch: m3tb_set_gradient_hessian for the region,
     depth and texture modalities, then m3tb_calculate_optimization (k_track). A refused update leaves the pose
     bit-identical; otherwise the pose equals the mirror oracle's bit for bit where ExpSkew takes its series
     (t2 < 0.01f) and within 4 ulps of the pose's largest entry where it calls sinf.
-  * test aid (m3tb_debug_rigid_solve): both device solves on every case, bit-identical to each other and theta
-    bit-identical to the mirror oracle; on finite regular systems theta also meets the float64 gate of
-    test_gpu_structure_limits.py (max(4 |theta_oracle32 - theta64|, 1e-6 |theta64|)).
+  * test aid (m3tb_debug_rigid_solve): the solve on both shared-memory layouts (k_track's and k_track2's) on every
+    case, bit-identical to each other and theta bit-identical to the mirror oracle; on finite regular systems theta
+    also meets the float64 gate of test_gpu_structure_limits.py (max(4 |theta_oracle32 - theta64|, 1e-6 |theta64|)).
   * end to end: correspondence iterations of k_track2 and of k_track (M3TB_KERNEL=1) with degenerate Tikhonov
     parameters, each started from the mirror oracle's pose: where the oracle refuses the update the device keeps the
     pose bit for bit, elsewhere the 1e-4 gate holds; and one refine_poses call with a NaN translation parameter.

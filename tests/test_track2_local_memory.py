@@ -78,7 +78,7 @@ def test_track2_hot_sections_do_not_touch_local_memory(pkg):
     kernels = os.path.join(CSRC, "m3t_b200_kernels.cuh")
     hot = {
         "warp reduction": ("m3t_b200_track2.cuh", _reduction_lines(track2)),
-        "SolveAndUpdateSerial": ("m3t_b200_track2.cuh", _function_lines(track2, "SolveAndUpdateSerial")),
+        "SolveAndUpdateSerial": ("m3t_b200_kernels.cuh", _function_lines(kernels, "SolveAndUpdateSerial")),
         "DepthGradient": ("m3t_b200_kernels.cuh", _function_lines(kernels, "DepthGradient")),
     }
     found = _local_accesses(os.path.join(CSRC, "libm3t_b200.so"))
