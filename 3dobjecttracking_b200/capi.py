@@ -111,6 +111,13 @@ class DeviceFeatures(C.Structure):
     memory."""
     _fields_ = [("n", C.c_int), ("length", C.c_int), ("x", C.c_void_p), ("y", C.c_void_p), ("xy_stride", C.c_int),
                 ("descriptors", C.c_void_p), ("descriptor_pitch", C.c_size_t)]
+
+
+class OrbParams(C.Structure):
+    """m3tb_orb_params: cv::ORB's n_features, scale_factor and n_levels (300, 1.2, 3 by default)."""
+    _fields_ = [("n_features", C.c_int32), ("scale_factor", C.c_float), ("n_levels", C.c_int32)]
+
+
 TEXTURE_POINT_DTYPE = np.dtype([("center_f_body", "<f4", 3), ("correspondence_center", "<f4", 2), ("center", "<f4", 2)])
 
 REGION_LINE_DTYPE = np.dtype([("model_index", "<i4"), ("valid", "<i4"), ("center_f_body", "<f4", 3),
@@ -145,7 +152,8 @@ SYMBOLS = [
     "m3tb_upload_texture_float_features",
     "m3tb_texture_correspondences", "m3tb_texture_gradient_hessian", "m3tb_get_texture_points",
     "m3tb_get_texture_keyframes", "m3tb_texture_crop", "m3tb_upload_texture_features_device",
-    "m3tb_get_texture_feature_flags",
+    "m3tb_get_texture_feature_flags", "m3tb_orb_params_default", "m3tb_texture_detect_orb",
+    "m3tb_get_texture_detections", "m3tb_get_texture_orb_keypoints",
 ]
 
 KERNEL_NAMES = {0: None, 1: "k_track", 2: "k_track2", 3: "k_track_cluster"}
@@ -277,6 +285,11 @@ def lib():
     L.m3tb_texture_crop.argtypes = [vp, ip, ci, vp, C.c_size_t, C.c_size_t, ci, ci, ip, fp, ip, ip]
     L.m3tb_upload_texture_features_device.argtypes = [vp, ip, C.POINTER(DeviceFeatures), ci]
     L.m3tb_get_texture_feature_flags.argtypes = [vp, ci, ci, ip]
+    L.m3tb_orb_params_default.argtypes = [C.POINTER(OrbParams)]
+    L.m3tb_orb_params_default.restype = None
+    L.m3tb_texture_detect_orb.argtypes = [vp, ip, ci, C.POINTER(OrbParams)]
+    L.m3tb_get_texture_detections.argtypes = [vp, ci, ci, ip]
+    L.m3tb_get_texture_orb_keypoints.argtypes = [vp, ci, fp, fp, fp, ip, vp, ci, C.POINTER(ci)]
     L.m3tb_get_full_rendering.argtypes = [vp, ci, vp, C.c_size_t, vp, C.c_size_t, vp, C.c_size_t, fp, fp]
     L.m3tb_undistortion_map.argtypes = [C.POINTER(Intrinsics), fp, C.POINTER(Intrinsics), vp, C.c_size_t]
     L.m3tb_set_camera_undistortion.argtypes = [vp, ci, ci, vp, C.c_size_t, ci, C.c_int32]
@@ -933,6 +946,42 @@ class Context:
         out = np.zeros(max(count, 1), np.int32)
         self._ck(self.L.m3tb_get_texture_feature_flags(self.h, first, count, out.ctypes.data_as(C.POINTER(C.c_int))))
         return out[:count].astype(bool)
+
+    def texture_detect_orb(self, bodies, params=None):
+        """cv::ORB detect + compute on the device for the ORB bodies `bodies` (m3tb_texture_detect_orb): the focused
+        crop of each body's current frame, its keypoints and descriptors stored in the body's feature slot. params:
+        None (defaults), one (n_features, scale_factor, n_levels) tuple / OrbParams for all, or one per body."""
+        ids = np.ascontiguousarray(bodies, np.int32).reshape(-1)
+        arr = None
+        if params is not None:
+            if isinstance(params, (OrbParams, tuple)):
+                params = [params] * len(ids)
+            arr = (OrbParams * max(len(ids), 1))(*[p if isinstance(p, OrbParams) else OrbParams(int(p[0]), float(p[1]), int(p[2]))
+                                                   for p in params])
+        self._ck(self.L.m3tb_texture_detect_orb(self.h, ids.ctypes.data_as(C.POINTER(C.c_int)), len(ids), arr))
+
+    def get_texture_detections(self, first=0, count=None):
+        """[count] int32: the keypoints cv::ORB kept at each body's last device detection (m3tb_get_texture_detections)."""
+        count = self.n_bodies - first if count is None else count
+        out = np.zeros(max(count, 1), np.int32)
+        self._ck(self.L.m3tb_get_texture_detections(self.h, first, count, out.ctypes.data_as(C.POINTER(C.c_int))))
+        return out[:count]
+
+    def get_texture_orb_keypoints(self, body, capacity=4096):
+        """The body's last device detection in canonical order (m3tb_get_texture_orb_keypoints): a dict of xy [n, 2]
+        (crop coordinates), angle, response (float32), octave (int32) and descriptors [n, 32] (uint8)."""
+        xy = np.zeros((capacity, 2), np.float32)
+        angle = np.zeros(capacity, np.float32)
+        response = np.zeros(capacity, np.float32)
+        octave = np.zeros(capacity, np.int32)
+        desc = np.zeros((capacity, 32), np.uint8)
+        n = C.c_int(0)
+        self._ck(self.L.m3tb_get_texture_orb_keypoints(self.h, body, _p(xy), _p(angle), _p(response),
+                                                        octave.ctypes.data_as(C.POINTER(C.c_int)),
+                                                        desc.ctypes.data_as(C.c_void_p), capacity, C.byref(n)))
+        k = n.value
+        return {"xy": xy[:k], "angle": angle[:k], "response": response[:k], "octave": octave[:k],
+                "descriptors": desc[:k]}
 
     def texture_correspondences(self, iteration, corr_iteration):
         self._ck(self.L.m3tb_texture_correspondences(self.h, iteration, corr_iteration))

@@ -302,6 +302,17 @@ struct m3tb_ctx {
   };
   std::vector<TexCrop> tex_crop;
   DeviceBuffer<int> d_tex_nonfinite;
+  // device ORB (m3tb_texture_detect_orb, k_texture_orb): scratch for up to kTexJobs bodies, grown on demand; the
+  // parity tables [max_bodies][orb_cap] (keypoints and descriptors, apart from the feature slot, which later uploads
+  // replace) and the kept counts [max_bodies]; per body, the n_features_max of its last detection (-1: none since the
+  // tables were made or its texture modality was set)
+  DeviceBuffer<uint8_t> d_orb_scratch;
+  DeviceBuffer<float2> d_orb_xy;
+  DeviceBuffer<float> d_orb_angle, d_orb_response;
+  DeviceBuffer<int> d_orb_octave, d_orb_found;
+  DeviceBuffer<uint32_t> d_orb_desc;
+  int orb_cap = 0;
+  std::vector<int> orb_nmax;
 
   // pose refinement (m3tb_refine_poses): the lists of RefineSelection, grown on demand; `refine` is set while it runs
   DeviceBuffer<int> d_refine;
@@ -2318,6 +2329,7 @@ int m3tb_create(int device, int max_bodies, int max_cameras, int max_models, m3t
   ctx->attach_uploaded.assign(max_bodies, std::array<char, RS_COUNT>{});
   ctx->tex_feat_gen.assign(max_bodies, -1);
   ctx->tex_crop.assign(max_bodies, m3tb_ctx::TexCrop{});
+  ctx->orb_nmax.assign(max_bodies, -1);
   if (const char* e = std::getenv("M3TB_NO_TILES")) ctx->use_tiles = !(e[0] == '1');
   if (const char* e = std::getenv("M3TB_NO_ROI_INGEST")) ctx->roi_ingest = !(e[0] == '1');
   if (const char* e = std::getenv("M3TB_CLUSTER")) ctx->use_clusters = e[0] == '1';
@@ -4502,6 +4514,45 @@ int CheckTextureBody(m3tb_ctx* ctx, int body) {
   return M3TB_OK;
 }
 
+// The focused crop of texture body b at `pose`, as m3tb_texture_crop and m3tb_texture_detect_orb both make it: roi and
+// scale always (zero without a focus), and when the body has a focus with a non-empty output, the output size and the
+// source frame (returns true). The destination is the caller's.
+bool FocusCropJob(const m3tb_ctx* ctx, int b, const float* pose, TexCropJob* j) {
+  std::memset(j, 0, sizeof(*j));
+  int32_t r[4];
+  float s;
+  bool ok = TextureFocus(ctx, b, pose, r, &s);
+  // cv::resize's dsize for Size(): saturate_cast<int>(roi.w * double(scale)), rounded half to even
+  const int w = ok ? int(std::nearbyint(double(r[2]) * double(s))) : 0;
+  const int h = ok ? int(std::nearbyint(double(r[3]) * double(s))) : 0;
+  ok = ok && w >= 1 && h >= 1;  // cv::resize refuses an empty output
+  j->roi_x = r[0]; j->roi_y = r[1]; j->roi_w = r[2]; j->roi_h = r[3];
+  j->scale = s;
+  if (!ok) return false;
+  const CameraDev& c = ctx->h_ccams[ctx->h_bodies[b].texture_camera];
+  j->src = c.host_src ? c.host_src : c.image;  // a pinned frame is read in place: its device copy holds only ROIs
+  j->src_pitch = c.host_src ? c.host_pitch : c.pitch;
+  j->out_w = w;
+  j->out_h = h;
+  return true;
+}
+
+// Body b has no device detection any more (its texture modality was set or removed): no read-back, a count of 0
+int ForgetDetection(m3tb_ctx* ctx, int b) {
+  ctx->orb_nmax[b] = -1;
+  if (ctx->d_orb_found) CU(cudaMemsetAsync(ctx->d_orb_found + b, 0, sizeof(int), ctx->stream));
+  return M3TB_OK;
+}
+
+// Records body b's crop (of its camera's current frame) for m3tb_upload_texture_features_device; none without a focus
+void RecordCrop(m3tb_ctx* ctx, int b, const TexCropJob& j) {
+  m3tb_ctx::TexCrop& t = ctx->tex_crop[b];
+  t.roi_x = j.roi_x;
+  t.roi_y = j.roi_y;
+  t.scale = j.scale;
+  t.gen = j.out_w > 0 ? ctx->h_ccams[ctx->h_bodies[b].texture_camera].generation : -1;
+}
+
 }  // namespace
 
 extern "C" {
@@ -4521,6 +4572,8 @@ int m3tb_set_texture_modality(m3tb_ctx* ctx, int body, const m3tb_texture_params
         ctx->render_dirty = true;
       }
     if (ctx->d_tex_nonfinite) CU(cudaMemsetAsync(ctx->d_tex_nonfinite + body, 0, sizeof(int), ctx->stream));
+    int rc = ForgetDetection(ctx, body);
+    if (rc) return rc;
     ctx->tex_crop[body].gen = -1;
     B.has_texture = 0;
     ctx->n_texture--;
@@ -4587,7 +4640,7 @@ int m3tb_set_texture_modality(m3tb_ctx* ctx, int body, const m3tb_texture_params
   ctx->tex_feat_gen[body] = -1;
   ctx->tex_crop[body].gen = -1;
   ctx->bodies_dirty = true;
-  return M3TB_OK;
+  return ForgetDetection(ctx, body);
 }
 
 int m3tb_get_texture_focus(m3tb_ctx* ctx, int first, int count, int32_t* roi, float* scale, int32_t* valid) {
@@ -4699,39 +4752,21 @@ int m3tb_texture_crop(m3tb_ctx* ctx, const int* bodies, int count, uint8_t* out,
   bool too_large = false;
   for (int k = 0; k < count; ++k) {
     const int b = bodies[k];
-    int32_t r[4];
-    float s;
-    bool ok = TextureFocus(ctx, b, poses.data() + 12 * b, r, &s);
-    // cv::resize's dsize for Size(): saturate_cast<int>(roi.w * double(scale)), rounded half to even
-    const int w = ok ? int(std::nearbyint(double(r[2]) * double(s))) : 0;
-    const int h = ok ? int(std::nearbyint(double(r[3]) * double(s))) : 0;
-    ok = ok && w >= 1 && h >= 1;  // cv::resize refuses an empty output
-    too_large = too_large || (ok && (w > capacity_width || h > capacity_height));
-    if (roi) std::memcpy(roi + 4 * k, r, sizeof(r));
-    if (scale) scale[k] = s;
-    if (size) { size[2 * k] = ok ? w : 0; size[2 * k + 1] = ok ? h : 0; }
+    TexCropJob j;
+    const bool ok = FocusCropJob(ctx, b, poses.data() + 12 * b, &j);
+    too_large = too_large || (ok && (j.out_w > capacity_width || j.out_h > capacity_height));
+    if (roi) { roi[4 * k] = j.roi_x; roi[4 * k + 1] = j.roi_y; roi[4 * k + 2] = j.roi_w; roi[4 * k + 3] = j.roi_h; }
+    if (scale) scale[k] = j.scale;
+    if (size) { size[2 * k] = j.out_w; size[2 * k + 1] = j.out_h; }
     if (valid) valid[k] = ok ? 1 : 0;
     if (!ok) continue;
-    const CameraDev& c = ctx->h_ccams[ctx->h_bodies[b].texture_camera];
-    TexCropJob j;
-    j.src = c.host_src ? c.host_src : c.image;  // a pinned frame is read in place: its device copy holds only ROIs
-    j.src_pitch = c.host_src ? c.host_pitch : c.pitch;
     j.dst = out + body_stride * size_t(k);
-    j.roi_x = r[0]; j.roi_y = r[1]; j.roi_w = r[2]; j.roi_h = r[3];
-    j.out_w = w; j.out_h = h;
-    j.scale = s;
     jobs.push_back(j);
     job_body.push_back(b);
   }
   if (too_large) return Fail(ctx, M3TB_ERR_INVALID, "a crop is larger than the capacity (see size)");
   for (int k = 0; k < count; ++k) ctx->tex_crop[bodies[k]].gen = -1;
-  for (size_t k = 0; k < jobs.size(); ++k) {
-    m3tb_ctx::TexCrop& t = ctx->tex_crop[job_body[k]];
-    t.roi_x = jobs[k].roi_x;
-    t.roi_y = jobs[k].roi_y;
-    t.scale = jobs[k].scale;
-    t.gen = ctx->h_ccams[ctx->h_bodies[job_body[k]].texture_camera].generation;
-  }
+  for (size_t k = 0; k < jobs.size(); ++k) RecordCrop(ctx, job_body[k], jobs[k]);
   for (size_t first = 0; first < jobs.size(); first += kTexJobs) {
     TexCropArgs a;
     a.n_jobs = int(std::min<size_t>(kTexJobs, jobs.size() - first));
@@ -4844,6 +4879,211 @@ int m3tb_get_texture_feature_flags(m3tb_ctx* ctx, int first, int count, int32_t*
   CU(cudaMemcpyAsync(nonfinite, ctx->d_tex_nonfinite + first, sizeof(int32_t) * size_t(count), cudaMemcpyDeviceToHost,
                      ctx->stream));
   CU(cudaStreamSynchronize(ctx->stream));
+  return M3TB_OK;
+}
+
+void m3tb_orb_params_default(m3tb_orb_params* p) {
+  if (!p) return;
+  p->n_features = 300;  // texture_modality.h:410-412
+  p->scale_factor = 1.2f;
+  p->n_levels = 3;
+}
+
+}  // extern "C"
+
+namespace {
+
+// One body's ORB job from its crop size and settings (orb.cpp: getScale, the level sizes and nfeaturesPerLevel),
+// in the float arithmetic of cv::ORB
+TexOrbJob OrbJob(int body, int w, int h, const m3tb_orb_params& p) {
+  TexOrbJob j;
+  std::memset(&j, 0, sizeof(j));
+  j.body = body;
+  j.n_levels = p.n_levels;
+  const double sf = double(p.scale_factor);
+  for (int l = 0; l < p.n_levels; ++l) {
+    const float s = float(std::pow(sf, double(l)));
+    const float inv = 1.0f / s;
+    j.layer_scale[l] = s;
+    j.w[l] = w > 0 ? int(std::nearbyint(float(w) * inv)) : 0;
+    j.h[l] = h > 0 ? int(std::nearbyint(float(h) * inv)) : 0;
+  }
+  const float factor = float(1.0 / sf);
+  float desired = float(p.n_features) * (1.0f - factor) / (1.0f - float(std::pow(double(factor), double(p.n_levels))));
+  int sum = 0;
+  for (int l = 0; l < p.n_levels - 1; ++l) {
+    j.per_level[l] = int(std::nearbyint(desired));
+    sum += j.per_level[l];
+    desired *= factor;
+  }
+  j.per_level[p.n_levels - 1] = std::max(p.n_features - sum, 0);
+  return j;
+}
+
+}  // namespace
+
+extern "C" {
+
+int m3tb_texture_detect_orb(m3tb_ctx* ctx, const int* bodies, int count, const m3tb_orb_params* params) {
+  CHECK_CTX();
+  if (count < 0 || (count > 0 && !bodies)) return Fail(ctx, M3TB_ERR_INVALID, "bad detection arguments");
+  m3tb_orb_params defaults;
+  m3tb_orb_params_default(&defaults);
+  std::vector<char> listed(ctx->n_bodies, 0);
+  for (int k = 0; k < count; ++k) {  // every refusal before anything is allocated or launched
+    const int b = bodies[k];
+    int rc = CheckTextureBody(ctx, b);
+    if (rc) return rc;
+    if (listed[b]++) return Fail(ctx, M3TB_ERR_INVALID, "body listed twice");
+    if (ctx->h_bodies[b].tp.descriptor_type != M3TB_DESCRIPTOR_ORB)
+      return Fail(ctx, M3TB_ERR_INVALID, "device detection is cv::ORB: the body's descriptor type is not ORB");
+    const m3tb_orb_params& p = params ? params[k] : defaults;
+    if (p.n_features < 1 || !std::isfinite(p.scale_factor) || !(p.scale_factor > 1.0f) || p.n_levels < 1)
+      return Fail(ctx, M3TB_ERR_INVALID, "ORB settings: n_features >= 1, finite scale_factor > 1, n_levels >= 1");
+    if (p.n_levels > kOrbMaxLevels) return Fail(ctx, M3TB_ERR_UNSUPPORTED, "ORB n_levels above 8");
+    if (p.n_features > kOrbFeatureLimit) return Fail(ctx, M3TB_ERR_UNSUPPORTED, "ORB n_features above 2^24");
+    if (!ctx->h_ccams[ctx->h_bodies[b].texture_camera].image)
+      return Fail(ctx, M3TB_ERR_NOT_SET_UP, "texture detection: no colour frame uploaded");
+  }
+  if (count == 0) return M3TB_OK;
+  std::vector<float> poses(size_t(12) * ctx->n_bodies);
+  CU(cudaMemcpyAsync(poses.data(), ctx->d_poses, poses.size() * sizeof(float), cudaMemcpyDeviceToHost, ctx->stream));
+  CU(cudaStreamSynchronize(ctx->stream));
+  // the focus and crop of every body, as m3tb_texture_crop makes them
+  std::vector<TexCropJob> crops(count);
+  std::vector<TexOrbJob> jobs(count);
+  int width = 1, height = 1;
+  for (int k = 0; k < count; ++k) {
+    const int b = bodies[k];
+    const bool ok = FocusCropJob(ctx, b, poses.data() + 12 * b, &crops[k]);
+    width = std::max(width, crops[k].out_w);
+    height = std::max(height, crops[k].out_h);
+    jobs[k] = OrbJob(b, crops[k].out_w, crops[k].out_h, params ? params[k] : defaults);
+    jobs[k].n_features_max = ctx->h_bodies[b].tp.n_features_max;
+    jobs[k].roi_x = crops[k].roi_x;
+    jobs[k].roi_y = crops[k].roi_y;
+    jobs[k].scale = ok ? crops[k].scale : 1.0f;
+  }
+  const int pitch = (width + 15) / 16 * 16;
+  const size_t job_bytes = (size_t(pitch) * size_t(height) * kOrbScratchBytesPerPixel + 255) / 256 * 256;
+  const size_t scratch_bytes = job_bytes * size_t(std::min(count, kTexJobs));
+  // scratch and parity tables, each grown all or nothing before anything is committed
+  DeviceBuffer<uint8_t> scratch;
+  if (ctx->d_orb_scratch.size() < scratch_bytes) CU(scratch.create(scratch_bytes));
+  const bool tables = ctx->orb_cap != ctx->tex_cap || !ctx->d_orb_found;
+  DeviceBuffer<float2> t_xy;
+  DeviceBuffer<float> t_angle, t_response;
+  DeviceBuffer<int> t_octave, t_found;
+  DeviceBuffer<uint32_t> t_desc;
+  if (tables) {
+    const size_t slots = size_t(ctx->max_bodies) * size_t(ctx->tex_cap);
+    CU(t_xy.create(slots));
+    CU(t_angle.create(slots));
+    CU(t_response.create(slots));
+    CU(t_octave.create(slots));
+    CU(t_desc.create(slots * kTexDescWords));
+    if (!ctx->d_orb_found) CU(t_found.create(size_t(ctx->max_bodies)));
+  }
+  if (scratch) ctx->d_orb_scratch = std::move(scratch);
+  if (tables) {
+    // new tables at the current feature capacity: every other body's last detection is forgotten
+    ctx->d_orb_xy = std::move(t_xy);
+    ctx->d_orb_angle = std::move(t_angle);
+    ctx->d_orb_response = std::move(t_response);
+    ctx->d_orb_octave = std::move(t_octave);
+    ctx->d_orb_desc = std::move(t_desc);
+    if (t_found) ctx->d_orb_found = std::move(t_found);
+    ctx->orb_cap = ctx->tex_cap;
+    std::fill(ctx->orb_nmax.begin(), ctx->orb_nmax.end(), -1);
+    CU(cudaMemsetAsync(ctx->d_orb_found, 0, sizeof(int) * size_t(ctx->max_bodies), ctx->stream));
+  }
+  for (int k = 0; k < count; ++k) {
+    const int b = bodies[k];
+    RecordCrop(ctx, b, crops[k]);
+    ctx->tex_feat_gen[b] = ctx->h_ccams[ctx->h_bodies[b].texture_camera].generation;  // none without a focus
+    ctx->orb_nmax[b] = jobs[k].n_features_max;
+  }
+  for (int first = 0; first < count; first += kTexJobs) {
+    const int n = std::min(kTexJobs, count - first);
+    TexCropArgs ca;
+    ca.n_jobs = 0;
+    ca.dst_pitch = size_t(pitch);
+    size_t threads = 0;
+    for (int k = 0; k < n; ++k) {
+      if (crops[first + k].out_w == 0) continue;
+      TexCropJob cj = crops[first + k];
+      cj.dst = ctx->d_orb_scratch + job_bytes * size_t(k);
+      ca.jobs[ca.n_jobs++] = cj;
+      threads = std::max(threads, size_t((cj.out_w + kTexCropPixels - 1) / kTexCropPixels) * cj.out_h);
+    }
+    if (ca.n_jobs > 0) {
+      const unsigned blocks = unsigned((threads + kTexCropThreads - 1) / kTexCropThreads);
+      k_texture_crop<<<dim3(blocks, unsigned(ca.n_jobs)), kTexCropThreads, 0, ctx->stream>>>(ca);
+      CU(cudaGetLastError());
+      ctx->launches++;
+    }
+    TexOrbArgs oa;
+    for (int k = 0; k < n; ++k) oa.jobs[k] = jobs[first + k];
+    oa.scratch = ctx->d_orb_scratch;
+    oa.job_bytes = job_bytes;
+    oa.pitch = pitch;
+    oa.height = height;
+    oa.feat_xy = ctx->d_tex_xy;
+    oa.feat_desc = ctx->d_tex_desc;
+    oa.feat_n = ctx->d_tex_nfeat;
+    oa.orb_xy = ctx->d_orb_xy;
+    oa.orb_angle = ctx->d_orb_angle;
+    oa.orb_response = ctx->d_orb_response;
+    oa.orb_octave = ctx->d_orb_octave;
+    oa.orb_desc = ctx->d_orb_desc;
+    oa.found = ctx->d_orb_found;
+    oa.cap = ctx->tex_cap;
+    oa.orb_cap = ctx->orb_cap;
+    k_texture_orb<<<n, kOrbThreads, 0, ctx->stream>>>(oa);
+    CU(cudaGetLastError());
+    ctx->launches++;
+  }
+  return M3TB_OK;
+}
+
+int m3tb_get_texture_detections(m3tb_ctx* ctx, int first, int count, int32_t* n_found) {
+  CHECK_CTX();
+  if (first < 0 || count < 0 || first + count > ctx->n_bodies || (count > 0 && !n_found))
+    return Fail(ctx, M3TB_ERR_INVALID, "bad body range / null output");
+  if (count == 0) return M3TB_OK;
+  if (!ctx->d_orb_found) {
+    std::memset(n_found, 0, sizeof(int32_t) * size_t(count));
+    return M3TB_OK;
+  }
+  CU(cudaMemcpyAsync(n_found, ctx->d_orb_found + first, sizeof(int32_t) * size_t(count), cudaMemcpyDeviceToHost,
+                     ctx->stream));
+  CU(cudaStreamSynchronize(ctx->stream));
+  return M3TB_OK;
+}
+
+int m3tb_get_texture_orb_keypoints(m3tb_ctx* ctx, int body, float* xy, float* angle, float* response, int32_t* octave,
+                                   uint8_t* descriptors, int capacity, int* n_out) {
+  CHECK_CTX();
+  if (body < 0 || body >= ctx->n_bodies || capacity < 0 || !n_out) return Fail(ctx, M3TB_ERR_INVALID, "bad read-back arguments");
+  *n_out = 0;
+  if (!ctx->d_orb_found || ctx->orb_nmax[body] < 0) return M3TB_OK;
+  int found = 0;
+  CU(cudaMemcpyAsync(&found, ctx->d_orb_found + body, sizeof(int), cudaMemcpyDeviceToHost, ctx->stream));
+  CU(cudaStreamSynchronize(ctx->stream));
+  const int n = std::min(found <= ctx->orb_nmax[body] ? found : 0, capacity);
+  const size_t at = size_t(body) * size_t(ctx->orb_cap);
+  if (n > 0) {
+    if (xy) CU(cudaMemcpyAsync(xy, ctx->d_orb_xy + at, sizeof(float2) * n, cudaMemcpyDeviceToHost, ctx->stream));
+    if (angle) CU(cudaMemcpyAsync(angle, ctx->d_orb_angle + at, sizeof(float) * n, cudaMemcpyDeviceToHost, ctx->stream));
+    if (response)
+      CU(cudaMemcpyAsync(response, ctx->d_orb_response + at, sizeof(float) * n, cudaMemcpyDeviceToHost, ctx->stream));
+    if (octave) CU(cudaMemcpyAsync(octave, ctx->d_orb_octave + at, sizeof(int) * n, cudaMemcpyDeviceToHost, ctx->stream));
+    if (descriptors)
+      CU(cudaMemcpyAsync(descriptors, ctx->d_orb_desc + at * kTexDescWords, size_t(32) * n, cudaMemcpyDeviceToHost,
+                         ctx->stream));
+    CU(cudaStreamSynchronize(ctx->stream));
+  }
+  *n_out = n;
   return M3TB_OK;
 }
 

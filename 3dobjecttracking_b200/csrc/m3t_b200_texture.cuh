@@ -1,8 +1,8 @@
 // m3t_b200_texture.cuh — TextureModality on the device (texture_modality.cpp): keyframe reconstruction from the device
 // silhouette renderer, brute-force kNN matching (Hamming for ORB's 32-byte descriptors, L2 for SIFT / DAISY float
 // descriptors), and the Tukey-weighted reprojection gradient / Hessian that k_track adds to a body's link. Feature
-// detection stays with the caller; what it hands over (keypoints in image coordinates and descriptors) is all these
-// kernels read of the colour frame.
+// detection stays with the caller, or for ORB bodies runs in k_texture_orb (m3t_b200_orb.cu); the keypoints in image
+// coordinates and the descriptors are all the matching kernels read of the colour frame.
 #pragma once
 
 #include "m3t_b200_device.cuh"
@@ -130,6 +130,45 @@ struct TexFeatArgs {
 
 // one CTA of kTexThreads per job
 __global__ void k_texture_features(const __grid_constant__ TexFeatArgs a);
+
+// k_texture_orb: cv::ORB detect + compute on the crops k_texture_crop wrote into the scratch, one CTA per job.
+constexpr int kOrbThreads = 512;
+constexpr int kOrbMaxLevels = 8;
+constexpr int kOrbFeatureLimit = 1 << 24;  // n_features: the per-level counts stay exact in float and 2 n in int
+// scratch bytes per job: two ping-pong levels, the blurred level and the FAST scores (1 byte per pixel each), and the
+// candidate positions, keys and Harris responses (4 bytes per pixel each)
+constexpr int kOrbScratchBytesPerPixel = 4 + 3 * 4;
+
+struct TexOrbJob {
+  int body;
+  int n_levels;
+  int n_features_max;            // the body's capacity: more keypoints than this and it gets none
+  int roi_x, roi_y;
+  float scale;                   // crop scale: image keypoint = roi + pt / scale
+  int w[kOrbMaxLevels], h[kOrbMaxLevels];  // level sizes (w[0] = 0: no focus, no features)
+  int per_level[kOrbMaxLevels];  // nfeaturesPerLevel
+  float layer_scale[kOrbMaxLevels];
+};
+
+struct TexOrbArgs {
+  TexOrbJob jobs[kTexJobs];
+  uint8_t* scratch;              // job k at scratch + k * job_bytes; its level-0 crop there with rows `pitch` apart
+  size_t job_bytes;
+  int pitch, height;             // the largest crop of the launch
+  float2* feat_xy;               // TextureArgs' frame-feature tables, `cap` features per body
+  uint32_t* feat_desc;
+  int* feat_n;
+  float2* orb_xy;                // parity tables [n_bodies][orb_cap]: crop (level-0) keypoint, angle, response, octave
+  float* orb_angle;
+  float* orb_response;
+  int* orb_octave;
+  uint32_t* orb_desc;            // [n_bodies][orb_cap][8]
+  int* found;                    // [n_bodies] keypoints cv::ORB keeps, before the n_features_max check
+  int cap;                       // of the frame-feature tables
+  int orb_cap;                   // of the parity tables (the same; kept apart as the tables are made apart)
+};
+
+__global__ void k_texture_orb(const __grid_constant__ TexOrbArgs a);
 
 // TextureModality::TukeyNorm (texture_modality.cpp:1231-1237)
 __host__ __device__ __forceinline__ float TexTukeyNorm(float error, float c) {

@@ -1427,10 +1427,10 @@ class DepthModality : public Modality {
 };
 
 // ---- texture_modality.h ------------------------------------------------------------------------------------------------
-// Feature detection stays with the caller (no OpenCV here): instead of DetectAndComputeCorrKeypoints the caller asks for
-// the body's focus region with CalculateFocus, detects features in the cropped and scaled grey image and hands them
-// over with SetFeatures, once per frame. DescriptorType ORB (32-byte descriptors), SIFT and DAISY (float descriptors)
-// are implemented.
+// No OpenCV here. For ORB bodies DetectFeatures runs DetectAndComputeCorrKeypoints on the device (cv::ORB at the
+// orb_* settings, m3tb_texture_detect_orb). Otherwise the caller asks for the body's focus region with CalculateFocus,
+// detects features in the cropped and scaled grey image and hands them over with SetFeatures, once per frame.
+// DescriptorType ORB (32-byte descriptors), SIFT and DAISY (float descriptors) are implemented.
 class TextureModality : public Modality {
  public:
   enum class DescriptorType { BRISK = 0, DAISY = 1, FREAK = 2, SIFT = 3, ORB = 4, ORB_CUDA = 5 };  // texture_modality.h
@@ -1441,6 +1441,7 @@ class TextureModality : public Modality {
       : Modality(name, batch, body_ptr), color_camera_ptr_(color_camera_ptr) {
     silhouette_renderer_ptr_ = silhouette_renderer_ptr;
     m3tb_texture_params_default(&params_);
+    m3tb_orb_params_default(&orb_params_);
   }
   // setters of the reference (texture_modality.h:186-194, 218-226), same names
   void set_descriptor_type(DescriptorType v) { descriptor_type_ = v; set_up_ = false; }
@@ -1467,6 +1468,14 @@ class TextureModality : public Modality {
   void set_measured_occlusion_threshold(float v) { params_.measured_occlusion_threshold = v; set_up_ = false; }
   void set_modeled_occlusion_radius(float v) { params_.modeled_occlusion_radius = v; set_up_ = false; }
   void set_modeled_occlusion_threshold(float v) { params_.modeled_occlusion_threshold = v; set_up_ = false; }
+  // the detector settings of the reference (texture_modality.h:410-412: 300, 1.2, 3), used by DetectFeatures
+  void set_orb_n_features(int v) { orb_params_.n_features = v; set_up_ = false; }
+  void set_orb_scale_factor(float v) { orb_params_.scale_factor = v; set_up_ = false; }
+  void set_orb_n_levels(int v) { orb_params_.n_levels = v; set_up_ = false; }
+  int orb_n_features() const { return orb_params_.n_features; }
+  float orb_scale_factor() const { return orb_params_.scale_factor; }
+  int orb_n_levels() const { return orb_params_.n_levels; }
+  const m3tb_orb_params& orb_params() const { return orb_params_; }
   // A device capacity the reference does not have: the most features SetFeatures may hand over per frame, 512 (the
   // default) .. 4096. It sizes the context's texture tables (m3tb_texture_params::n_features_max).
   void set_n_features_max(int v) { params_.n_features_max = v; set_up_ = false; }
@@ -1617,6 +1626,49 @@ class TextureModality : public Modality {
     if (features.length != 0) batch_->NoteDeviceFeatures(body);
     return true;
   }
+  // DetectAndComputeCorrKeypoints for several ORB modalities of one Batch in ONE m3tb_texture_detect_orb call (one pose
+  // download, one stream synchronisation, two launches per 128 bodies): each body's focused crop of its camera's current
+  // frame and cv::ORB detect + compute on it at the modality's orb_* settings, the features stored for the next
+  // StartModality / CalculateCorrespondences / CalculateResults. A body without a focus gets no features, as the
+  // reference returns early. cv::ORB keeps every tie at its cuts, so it can keep more than orb_n_features; a body that
+  // keeps more than n_features_max gets none that frame (detections() reports the count). False, with nothing
+  // launched, for a modality that is not set up or not ORB, modalities of different batches or bad orb_* settings.
+  static bool DetectFeatures(const std::vector<std::shared_ptr<TextureModality>>& modalities) {
+    if (modalities.empty()) return true;
+    m3tb_ctx* ctx = modalities[0]->batch_->ctx();
+    std::vector<int> bodies;
+    std::vector<m3tb_orb_params> params;
+    for (auto& m : modalities) {
+      if (!m->IsSetup()) return false;
+      if (m->descriptor_type_ != DescriptorType::ORB) {
+        std::cerr << "Modality " << m->name_ << ": DetectFeatures runs cv::ORB; its descriptor type is not ORB"
+                  << std::endl;
+        return false;
+      }
+      if (m->batch_->ctx() != ctx) {
+        std::cerr << "TextureModality::DetectFeatures: the modalities belong to different batches" << std::endl;
+        return false;
+      }
+      bodies.push_back(m->body_ptr_->index());
+      params.push_back(m->orb_params_);
+    }
+    return Check(ctx, m3tb_texture_detect_orb(ctx, bodies.data(), int(bodies.size()), params.data()),
+                 "TextureModality::DetectFeatures");
+  }
+  // One modality's detection; each call synchronises the stream, so several bodies go through DetectFeatures(modalities)
+  bool DetectFeatures() {
+    std::vector<std::shared_ptr<TextureModality>> self{std::shared_ptr<TextureModality>(this, [](TextureModality*) {})};
+    return DetectFeatures(self);
+  }
+  // The keypoints cv::ORB kept at the body's last DetectFeatures (may exceed orb_n_features and n_features_max);
+  // -1 on an error. Synchronises the stream.
+  int detections() const {
+    int32_t n = -1;
+    if (!Check(batch_->ctx(), m3tb_get_texture_detections(batch_->ctx(), body_ptr_->index(), 1, &n),
+               "TextureModality::detections"))
+      return -1;
+    return n;
+  }
 
   bool StartModality(int iteration, int corr_iteration) override {
     if (!IsSetup()) return false;
@@ -1652,6 +1704,7 @@ class TextureModality : public Modality {
 
  private:
   m3tb_texture_params params_;
+  m3tb_orb_params orb_params_;  // DetectFeatures
   DescriptorType descriptor_type_ = DescriptorType::ORB;
   std::shared_ptr<ColorCamera> color_camera_ptr_;
   std::shared_ptr<DepthCamera> depth_camera_ptr_;  // MeasureOcclusions

@@ -479,7 +479,8 @@ int m3tb_get_histograms(m3tb_ctx* ctx, int body, float* histogram_f, float* hist
 int m3tb_share_color_histograms(m3tb_ctx* ctx, int body, int owner_body);
 
 /* ---- texture modality (TextureModality, texture_modality.cpp; k_texture_keyframe / k_texture_match, DESIGN.md §3) -----
- * Feature detection stays with the caller, as the renderers once did: per frame it asks for each body's focus region,
+ * Feature detection stays with the caller, as the renderers once did (for ORB bodies m3tb_texture_detect_orb below runs
+ * cv::ORB on the device instead): per frame it asks for each body's focus region,
  * crops and scales the grey image as DetectAndComputeCorrKeypoints does (texture_modality.cpp:866-868: cvtColor
  * BGR2GRAY, image(roi), resize by `scale` in both directions), runs cv::ORB, cv::SIFT or cv::xfeatures2d::DAISY on the
  * crop and hands the keypoints and descriptors over. Everything after detection runs on the device: keyframe
@@ -566,6 +567,46 @@ int m3tb_upload_texture_features_device(m3tb_ctx* ctx, const int* bodies, const 
 /* nonfinite[k] = 1 when body first + k's last m3tb_upload_texture_features_device held a non-finite descriptor
  * value (its features were dropped). Synchronises the stream. */
 int m3tb_get_texture_feature_flags(m3tb_ctx* ctx, int first, int count, int32_t* nonfinite);
+/* cv::ORB on the device (k_texture_orb, DESIGN.md §3 "k_texture_orb"). The detector settings M3T exposes
+ * (texture_modality.h:410-412); everything else is cv::ORB's default, which M3T never changes: edgeThreshold 31,
+ * firstLevel 0, WTA_K 2, HARRIS_SCORE, patchSize 31, fastThreshold 20. */
+typedef struct m3tb_orb_params {
+  int32_t n_features;   /* 300 (>= 1) */
+  float scale_factor;   /* 1.2 (finite, > 1) */
+  int32_t n_levels;     /* 3 (1 .. 8) */
+} m3tb_orb_params;
+void m3tb_orb_params_default(m3tb_orb_params* p);
+/* DetectAndComputeCorrKeypoints (texture_modality.cpp:858-888) for the ORB bodies bodies[0 .. count), from the current
+ * device poses and each body's camera's current frame: the focused crop (k_texture_crop, into context-owned scratch),
+ * then cv::ORB detect and compute on it (k_texture_orb), the keypoints and descriptors stored in the body's feature
+ * slot exactly as m3tb_upload_texture_features_device stores the same features in the same order (float(roi_x) +
+ * x / scale). params [count] (NULL: m3tb_orb_params_default for every body). The result is bit-equal to OpenCV 4's
+ * cv::ORB as a multiset of keypoints and descriptors. The order is canonical, not cv2's: level ascending, then
+ * row-major by the keypoint's pixel in its level (cv2's order within a level comes from nth_element / partition).
+ * cv::ORB can keep more than n_features keypoints, because its cuts keep every tie: a body that keeps more than its
+ * n_features_max gets no features this frame (m3tb_get_texture_detections reports the count). A body without a focus
+ * gets none either, as the reference returns early. Synchronises once (the poses); the counts stay on the device; two
+ * launches per 128 bodies (one when none of them has a focus). Records the crop as m3tb_texture_crop does.
+ * Refusals launch nothing and leave the context unchanged: M3TB_ERR_INVALID for a body without a texture modality, a
+ * body whose descriptor type is not ORB, a body listed twice, n_features < 1, a scale_factor that is not finite or
+ * not above 1 and n_levels < 1; M3TB_ERR_UNSUPPORTED for n_levels above 8 and n_features above 2^24;
+ * M3TB_ERR_NOT_SET_UP without a colour frame.
+ * Device memory: scratch of 16 bytes per pixel of the largest crop for up to 128 bodies (0.64 MB per body at
+ * 200 x 200), grown on demand, and parity tables of 52 bytes per feature slot, made again when the feature capacity of
+ * the context has grown (which forgets the other bodies' last detections); each growth is all or nothing. */
+int m3tb_texture_detect_orb(m3tb_ctx* ctx, const int* bodies, int count, const m3tb_orb_params* params);
+/* n_found[k]: the keypoints cv::ORB kept for body first + k at its last m3tb_texture_detect_orb (0 before one, and
+ * after m3tb_set_texture_modality sets or removes the body's modality), which may exceed n_features (ties) and
+ * n_features_max (the body then has no features). Synchronises the stream. */
+int m3tb_get_texture_detections(m3tb_ctx* ctx, int first, int count, int32_t* n_found);
+/* Parity read-back of body's last m3tb_texture_detect_orb, in the canonical order: xy [n][2] KeyPoint::pt in crop
+ * (level-0) coordinates, angle [n] (degrees), response [n] (Harris), octave [n], descriptors [n][32]. The detection's
+ * own copy: later feature uploads for the body do not change it. At most `capacity` keypoints; *n_out the number
+ * stored (0 when the body kept more than its n_features_max, and when it has no detection: none yet, its texture
+ * modality set or removed since, or the tables made again by a later detection of other bodies). Any output pointer
+ * but n_out may be NULL. Synchronises the stream. */
+int m3tb_get_texture_orb_keypoints(m3tb_ctx* ctx, int body, float* xy, float* angle, float* response, int32_t* octave,
+                                   uint8_t* descriptors, int capacity, int* n_out);
 /* TextureModality::CalculateCorrespondences (texture_modality.cpp:322-386) for every body with a texture modality:
  * matching at corr_iteration 0, the data points' projection (center) at every iteration. */
 int m3tb_texture_correspondences(m3tb_ctx* ctx, int iteration, int corr_iteration);
