@@ -4901,13 +4901,18 @@ TexOrbJob OrbJob(int body, int w, int h, const m3tb_orb_params& p) {
   j.body = body;
   j.n_levels = p.n_levels;
   const double sf = double(p.scale_factor);
+  bool empty_level = false;
   for (int l = 0; l < p.n_levels; ++l) {
     const float s = float(std::pow(sf, double(l)));
     const float inv = 1.0f / s;
     j.layer_scale[l] = s;
     j.w[l] = w > 0 ? int(std::nearbyint(float(w) * inv)) : 0;
     j.h[l] = h > 0 ? int(std::nearbyint(float(h) * inv)) : 0;
+    empty_level = empty_level || j.w[l] < 1 || j.h[l] < 1;
   }
+  // cv::ORB builds the whole pyramid before it detects, and cv::resize throws on a level of size 0: detect returns
+  // nothing for such a crop, keypoints of the earlier levels included. w[0] = 0 gives the body no keypoints.
+  if (empty_level) j.w[0] = 0;
   const float factor = float(1.0 / sf);
   float desired = float(p.n_features) * (1.0f - factor) / (1.0f - float(std::pow(double(factor), double(p.n_levels))));
   int sum = 0;

@@ -254,9 +254,10 @@ __global__ void __launch_bounds__(kOrbThreads) k_texture_orb(const __grid_consta
   uint32_t* orb_desc = a.orb_desc + size_t(b) * orb_cap * kTexDescWords;
 
   int total = 0;
+  // w[0] = 0: no focus, or a pyramid with a level of size 0 (cv::ORB detects nothing then); otherwise every level
+  // has at least one pixel
   for (int level = 0; level < j.n_levels && j.w[0] > 0; ++level) {
     const int w = j.w[level], h = j.h[level];
-    if (w < 1 || h < 1) break;  // cv::resize refuses an empty level; no level after it has keypoints either
     uint8_t* im = base + (level & 1) * area;
     if (level > 0) ResizeExact(base + ((level - 1) & 1) * area, j.w[level - 1], j.h[level - 1], im, w, h, pitch);
     __syncthreads();

@@ -145,7 +145,7 @@ struct TexOrbJob {
   int n_features_max;            // the body's capacity: more keypoints than this and it gets none
   int roi_x, roi_y;
   float scale;                   // crop scale: image keypoint = roi + pt / scale
-  int w[kOrbMaxLevels], h[kOrbMaxLevels];  // level sizes (w[0] = 0: no focus, no features)
+  int w[kOrbMaxLevels], h[kOrbMaxLevels];  // level sizes (w[0] = 0: no focus or an empty level, no features)
   int per_level[kOrbMaxLevels];  // nfeaturesPerLevel
   float layer_scale[kOrbMaxLevels];
 };

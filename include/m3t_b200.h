@@ -585,7 +585,10 @@ void m3tb_orb_params_default(m3tb_orb_params* p);
  * row-major by the keypoint's pixel in its level (cv2's order within a level comes from nth_element / partition).
  * cv::ORB can keep more than n_features keypoints, because its cuts keep every tie: a body that keeps more than its
  * n_features_max gets no features this frame (m3tb_get_texture_detections reports the count). A body without a focus
- * gets none either, as the reference returns early. Synchronises once (the poses); the counts stay on the device; two
+ * gets none either, as the reference returns early. Nor does a body whose pyramid has a level with a side of 0 pixels
+ * (a small crop at a large scale_factor and many levels): cv::ORB builds every level before it detects and
+ * cv::resize throws on the empty one, so cv::ORB returns no keypoints at all, the earlier levels' included; the
+ * body's count is 0, with no read-back and no features, and the other bodies of the call are unaffected. Synchronises once (the poses); the counts stay on the device; two
  * launches per 128 bodies (one when none of them has a focus). Records the crop as m3tb_texture_crop does.
  * Refusals launch nothing and leave the context unchanged: M3TB_ERR_INVALID for a body without a texture modality, a
  * body whose descriptor type is not ORB, a body listed twice, n_features < 1, a scale_factor that is not finite or

@@ -117,14 +117,20 @@ def resize_linear_exact(src, width, height):
     return np.clip(out, 0, 255).astype(np.uint8)
 
 
+def empty_pyramid(width, height, scale_factor, n_levels):
+    """Whether a level of the pyramid has a side of 0 pixels. cv::ORB builds every level before it detects, and
+    cv::resize refuses an empty size, so cv2 raises and detects nothing at all, on the earlier levels neither."""
+    return any(lw < 1 or lh < 1 for lw, lh in level_sizes(width, height, scale_factor, n_levels))
+
+
 def pyramid(image, scale_factor, n_levels):
-    """imagePyramid's levels: level 0 the image, level l resize(level l - 1, INTER_LINEAR_EXACT)."""
+    """imagePyramid's levels: level 0 the image, level l resize(level l - 1, INTER_LINEAR_EXACT). Every level has at
+    least one pixel (see empty_pyramid)."""
     h, w = image.shape
+    assert not empty_pyramid(w, h, scale_factor, n_levels)
     levels = [np.ascontiguousarray(image, dtype=np.uint8)]
     for (lw, lh) in level_sizes(w, h, scale_factor, n_levels)[1:]:
-        # cv::resize refuses an empty size (cv2 raises); such a level, and every one after it, has no keypoints
-        empty = lw < 1 or lh < 1 or levels[-1].size == 0
-        levels.append(np.zeros((max(lh, 0), max(lw, 0)), np.uint8) if empty else resize_linear_exact(levels[-1], lw, lh))
+        levels.append(resize_linear_exact(levels[-1], lw, lh))
     return levels
 
 
@@ -315,23 +321,33 @@ def orb(image, n_features=300, scale_factor=1.2, n_levels=3, pattern=None, stage
     """cv::ORB::create(n_features, scale_factor, n_levels): detect, then compute, in canonical order.
 
     Returns a dict of arrays: xy [n][2] float32 (level-0 coordinates, KeyPoint::pt), angle, response (float32),
-    octave (int32), descriptors [n][32] uint8, and lxy [n][2] the pixel in its level. `stages`, when a dict, receives
-    the per-level pyramid, blurred levels, FAST corners and the counts after each cut."""
+    octave (int32), descriptors [n][32] uint8, and lxy [n][2] the pixel in its level; nothing when a level of the
+    pyramid is empty (empty_pyramid). `stages`, when a dict, receives "empty_pyramid", the per-level counts
+    ("per_level") and, per level, the pyramid, blurred levels, the FAST corners found ("n_corners") and those inside
+    the border that the first cut ranks ("n_fast"), and the counts after each cut."""
     image = np.ascontiguousarray(image, dtype=np.uint8)
     if pattern is None:
         pattern = bit_pattern()
-    levels = pyramid(image, scale_factor, n_levels)
-    scales = level_scales(scale_factor, n_levels)
     per_level = features_per_level(n_features, scale_factor, n_levels)
-    out = {k: [] for k in ("xy", "lxy", "angle", "response", "octave", "descriptors")}
+    empty = empty_pyramid(image.shape[1], image.shape[0], scale_factor, n_levels)
+    if stages is not None:
+        stages["empty_pyramid"] = empty
+        stages["per_level"] = per_level
+    levels = [] if empty else pyramid(image, scale_factor, n_levels)
+    scales = level_scales(scale_factor, n_levels)
+    out = {k: [np.zeros((0,) + s, t)] for k, s, t in (("xy", (2,), np.float32), ("lxy", (2,), np.int32),
+                                                        ("angle", (), np.float32), ("response", (), np.float32),
+                                                        ("octave", (), np.int32), ("descriptors", (32,), np.uint8))}
     for level, img in enumerate(levels):
         h, w = img.shape
         xs, ys, sc = fast_corners(img)
+        n_corners = len(xs)
         if h <= 2 * EDGE_THRESHOLD or w <= 2 * EDGE_THRESHOLD:
             inside = np.zeros(len(xs), bool)
         else:
             inside = (xs >= EDGE_THRESHOLD) & (xs < w - EDGE_THRESHOLD) & (ys >= EDGE_THRESHOLD) & (ys < h - EDGE_THRESHOLD)
         xs, ys, sc = xs[inside], ys[inside], sc[inside]
+        n_fast = len(xs)
         keep = retain_best(sc.astype(np.float32), 2 * per_level[level])
         xs, ys = xs[keep], ys[keep]
         n_first = len(xs)
@@ -352,6 +368,8 @@ def orb(image, n_features=300, scale_factor=1.2, n_levels=3, pattern=None, stage
         if stages is not None:
             stages.setdefault("levels", []).append(img)
             stages.setdefault("blurred", []).append(blurred)
+            stages.setdefault("n_corners", []).append(n_corners)
+            stages.setdefault("n_fast", []).append(n_fast)
             stages.setdefault("n_first_cut", []).append(n_first)
             stages.setdefault("n_second_cut", []).append(len(xs))
     res = {k: np.concatenate(v) for k, v in out.items()}
@@ -388,14 +406,35 @@ def as_multiset(res):
 
 # ---- inputs shared by the CPU test and the golden generator ------------------------------------------------------
 
-def textured(h, w, seed):
-    """A random textured image: smoothed noise plus blobs and edges, so FAST finds corners at every level."""
+def textured(h, w, seed, block=4):
+    """A random textured image: random blocks of `block` pixels plus noise, so FAST finds corners at every level."""
     rng = np.random.default_rng(seed)
-    base = rng.integers(0, 256, size=(max(h // 4, 1) + 2, max(w // 4, 1) + 2)).astype(np.float64)
-    up = np.kron(base, np.ones((4, 4)))[:h, :w]
+    base = rng.integers(0, 256, size=(max(h // block, 1) + 2, max(w // block, 1) + 2)).astype(np.float64)
+    up = np.kron(base, np.ones((block, block)))[:h, :w]
     noise = rng.integers(-40, 41, size=(h, w))
     img = np.clip(up + noise, 0, 255).astype(np.uint8)
     return img
+
+
+def noise(h, w, seed):
+    """Uniform noise: FAST corners on most pixels, long candidate lists and many equal FAST scores."""
+    return np.random.default_rng(seed).integers(0, 256, size=(h, w)).astype(np.uint8)
+
+
+def binary_noise(h, w, seed):
+    """0 / 255 noise: FAST scores saturate, so the first cut ties on nearly every candidate."""
+    return (np.random.default_rng(seed).integers(0, 2, size=(h, w)) * 255).astype(np.uint8)
+
+
+def ramp(h, w):
+    """A smooth diagonal ramp: no FAST corner anywhere."""
+    yy, xx = np.mgrid[0:h, 0:w]
+    return ((xx + 2 * yy) * 255 // max(w + 2 * h - 3, 1)).astype(np.uint8)
+
+
+def as_frame(grey):
+    """A BGR frame whose grey image (BGR2GRAY) is `grey` itself."""
+    return np.ascontiguousarray(np.repeat(grey[:, :, None], 3, axis=2))
 
 
 def dot_grid(h=300, w=300, spacing=12):
@@ -429,3 +468,15 @@ def checkerboard(h=200, w=200, cell=5):
 
 SETTINGS = [(300, 1.2, 3), (20, 1.2, 3), (500, 1.2, 8), (300, 2.0, 3), (300, 1.2, 1), (4096, 1.2, 3)]
 RANDOM_SIZES = [1, 7, 62, 63, 64, 65, 70, 100, 200, 369]
+
+# The float just above 1, the smallest scale_factor cv::ORB accepts: every level has the size of level 0.
+NEXT_ABOVE_1 = float(np.nextafter(np.float32(1.0), np.float32(2.0)))
+# (n_features, scale_factor, n_levels) beyond SETTINGS: every n_features of {1, 2, 5, 20, 300, 1000, 4096, 2^24}, every
+# scale_factor of {NEXT_ABOVE_1, 1.05, 1.2, 1.3, 1.5, 2.0, 2.5, 3.0} and n_levels 1 .. 8. It has per-level counts of 0
+# (n_features up to 5, and 300 at 8 levels of 2.5 or 3.0), pyramids with an empty level (3.0 at 8 levels below 1094 px,
+# 2.5 at 8 levels below 305 px and at 5 levels below 20 px) and n_features 2^24, where the cuts keep everything and
+# keypoints with a Harris response <= 0 survive.
+SWEEP = [(1, 1.2, 3), (1, 3.0, 1), (2, NEXT_ABOVE_1, 8), (2, 2.5, 2), (5, 1.05, 4), (5, 1.5, 6), (20, 1.3, 7),
+         (20, 2.0, 5), (300, 1.2, 3), (300, 2.5, 8), (300, 3.0, 8), (300, NEXT_ABOVE_1, 2), (1000, 1.3, 4),
+         (1000, 1.5, 8), (1000, 2.0, 6), (4096, 1.2, 8), (4096, 1.05, 8), (4096, 3.0, 3), (1 << 24, 1.2, 3),
+         (1 << 24, 1.5, 1), (1 << 24, 2.5, 5), (1 << 24, NEXT_ABOVE_1, 4)]
