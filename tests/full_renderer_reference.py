@@ -17,11 +17,11 @@ f32 = np.float32
 GOLDEN = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden")
 
 
-def render_full(intr, world2camera, poses, geometry, bodies, z_min=0.02, z_max=10.0, id_type="body"):
+def render_full(intr, world2camera, poses, geometry, bodies, z_min=0.02, z_max=10.0, id_type="body", stats=None):
     """FullRenderer::StartRendering + Fetch{Depth,Silhouette,Normal}Image: dict(depth [H,W] u16 (65535 = nothing drawn),
     silhouette [H,W] u8 (0 = background), normal [H,W,4] u8, projection_term_a / b). poses / geometry: {body: [3,4]
-    body2world / rr.Geometry}; bodies: render_data_bodies order."""
-    normal, zbuf = vr.render_normal(intr, world2camera, poses, geometry, bodies, z_min, z_max)
+    body2world / rr.Geometry}; bodies: render_data_bodies order; stats: see rr.raster_keyed."""
+    normal, zbuf = vr.render_normal(intr, world2camera, poses, geometry, bodies, z_min, z_max, stats)
     depth = (zbuf >> np.uint64(48)).astype(np.uint16)  # the cleared key reads 65535
     ids = np.array([geometry[b].region_id if id_type == "region" else geometry[b].body_id for b in bodies] + [0],
                    np.uint8)

@@ -1,6 +1,6 @@
 """CPU restatement of depth-model generation (DESIGN.md §3 "k_model_raster / k_model_points"), operation for
 operation in float32 like the kernels built with -fmad=false, so that views, points, surface areas and the debug images
-are compared bit for bit. Rasterisation goes through render_reference.raster_triangle; the sampler replays
+are compared bit for bit. Rasterisation goes through render_reference.raster_keyed; the sampler replays
 std::mt19937{7} with numpy's RandomState(7), as tests/golden/reference_rig.py does. Test infrastructure only."""
 import ctypes
 import ctypes.util
@@ -151,62 +151,26 @@ def HALF_D(g):
     return f32(0.5) * f32(g.maximum_body_diameter)
 
 
-class _Sink:
-    """Stands in for rr.raster_triangle's u32 z-buffer: reads as cleared, records every fragment's depth16."""
-
-    def __getitem__(self, idx):
-        return np.full(len(idx[0]), 0xFFFFFFFF, np.uint32)
-
-    def __setitem__(self, idx, packed):
-        self.j, self.i, self.d16 = idx[0], idx[1], (np.asarray(packed) >> np.uint32(16)).astype(np.uint64)
-
-
-def raster(M, triangles, culling, S, draw, zbuf):
-    """Every triangle of one body through M into zbuf [S,S] uint64 (depth16 << 48 | draw << 32 | triangle)."""
-    tv = np.asarray(triangles, f32).reshape(-1, 3, 3)
-    vx, vy, vz = tv[..., 0], tv[..., 1], tv[..., 2]
-    clip = [M[4 * r] * vx + M[4 * r + 1] * vy + M[4 * r + 2] * vz + M[4 * r + 3] for r in range(4)]
-    dist = clip[2] + clip[3]
-    half = rr.HALF * f32(S)
-    for t in range(tv.shape[0]):
-        c = [tuple(clip[r][t, k] for r in range(4)) for k in range(3)]
-        d = [dist[t, k] for k in range(3)]
-        poly = []
-        for e in range(3):
-            e1 = 0 if e == 2 else e + 1
-            in0, in1 = d[e] >= 0, d[e1] >= 0
-            if in0:
-                poly.append(c[e])
-            if in0 != in1:
-                poly.append(rr._intersect(c[e], d[e], c[e1], d[e1]) if in0 else rr._intersect(c[e1], d[e1], c[e], d[e]))
-        if len(poly) < 3:
-            continue
-        win = [((p[0] / p[3] + f32(1)) * half, (p[1] / p[3] + f32(1)) * half, (p[2] / p[3] + f32(1)) * rr.HALF)
-               for p in poly]
-        fans = [(win[0], win[1], win[2])] + ([(win[0], win[2], win[3])] if len(win) == 4 else [])
-        tag = (np.uint64(draw) << np.uint64(32)) | np.uint64(t)
-        for v0, v1, v2 in fans:
-            sink = _Sink()
-            rr.raster_triangle(v0, v1, v2, culling, S, 0, sink)
-            if hasattr(sink, "d16"):
-                key = (sink.d16 << np.uint64(48)) | tag
-                np.minimum.at(zbuf, (sink.j, sink.i), key)
+def raster(M, triangles, culling, S, draw, zbuf, stats=None):
+    """Every triangle of one body through M into zbuf [S,S] uint64 (depth16 << 48 | draw << 32 | triangle):
+    rr.raster_keyed, whose `stats` count what it reaches."""
+    rr.raster_keyed(M, triangles, culling, S, S, draw, zbuf, stats)
 
 
 def _unorm8(c):
     return np.rint(np.fmin(np.fmax(c, f32(0)), f32(1)) * f32(255)).astype(np.uint8)
 
 
-def render_view(st: Setup, camera2body):
-    """The two z-buffers of one view and its normal (BGRA), depth and silhouette images."""
+def render_view(st: Setup, camera2body, stats=None):
+    """The two z-buffers of one view and its normal (BGRA), depth and silhouette images (stats: see rr.raster_keyed)."""
     S = st.S
     Ms, rot = st.matrices(camera2body)
     z0 = np.full((S, S), CLEAR, np.uint64)
-    raster(Ms[0][0], st.body.triangles, st.body.enable_culling, S, 0, z0)
+    raster(Ms[0][0], st.body.triangles, st.body.enable_culling, S, 0, z0, stats)
     if st.occlusion:
         zs = np.full((S, S), CLEAR, np.uint64)
         for g, G in enumerate([st.body] + st.occlusion):
-            raster(Ms[1][g], G.triangles, G.enable_culling, S, g, zs)
+            raster(Ms[1][g], G.triangles, G.enable_culling, S, g, zs, stats)
         sil = (zs != CLEAR) & (((zs >> np.uint64(32)) & np.uint64(0xFFFF)) == 0)
     else:
         sil = z0 != CLEAR

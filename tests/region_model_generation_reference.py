@@ -120,8 +120,9 @@ class Setup:
         self.projection_term_a = hi * lo * f32(65535) / (hi - lo)
         self.projection_term_b = hi * f32(65535) / (hi - lo)
 
-    def render(self, camera2body):
-        """dict(name -> silhouette [S,S] u8) and the main renderer's depth image [S,S] u16."""
+    def render(self, camera2body, stats=None):
+        """dict(name -> silhouette [S,S] u8) and the main renderer's depth image [S,S] u16 (stats: see
+        rr.raster_keyed)."""
         S = self.S
         fS = f32(S)
         P00 = f32(2) * self.fu / fS
@@ -142,7 +143,7 @@ class Setup:
                     M[8 + c] = P22 * T[8 + c]
                     M[12 + c] = T[8 + c]
                 M[11] = M[11] + P23
-                mg.raster(M, g.triangles, g.enable_culling, S, d, z)
+                mg.raster(M, g.triangles, g.enable_culling, S, d, z, stats)
             ids = np.array([i for _, i in draws] + [0], np.uint8)
             draw = np.where(z == mg.CLEAR, len(draws), (z >> np.uint64(32)) & np.uint64(0xFFFF)).astype(np.int64)
             sils[name] = ids[draw]
@@ -171,11 +172,15 @@ def view_points(st: Setup, camera2body, sils, depth, n_points, stride_depth_offs
     px = st.r / st.fu
     max_dd = px * MAX_SURFACE_GRADIENT
     same, occ = sils.get("same_region"), sils.get("occlusion")
+
+    def at(img, u, v):  # neighbours outside the image read as background
+        return img[v, u] if 0 <= u < S and 0 <= v < S else BACKGROUND_ID
+
     valid = []
     for c in contours:  # IsContourPointValid
         for x, y in c:
             nb = ((x, y + 1), (x, y - 1), (x + 1, y), (x - 1, y))
-            if same is not None and any(same[v, u] != BACKGROUND_ID for u, v in nb):
+            if same is not None and any(at(same, u, v) != BACKGROUND_ID for u, v in nb):
                 stats["same_region"] = stats.get("same_region", 0) + 1
                 continue
             if occ is not None and occ[y, x] != BACKGROUND_ID:
@@ -183,7 +188,7 @@ def view_points(st: Setup, camera2body, sils, depth, n_points, stride_depth_offs
                 continue
             s, n = f32(0), 0
             for u, v in nb:
-                if main[v, u] == DIFFERENT_BODY_ID:
+                if at(main, u, v) == DIFFERENT_BODY_ID:
                     s = s + dep(u, v)
                     n += 1
             if n > 0 and s / f32(n) < dep(x, y) - max_dd:

@@ -37,65 +37,10 @@ def clip_matrix(P, T):
     return M
 
 
-def raster_triangle(v0, v1, v2, culling, W, H, tag, zbuf):
-    """One window-space triangle into zbuf [H,W] uint64 (rr.raster_triangle with separate x and y limits)."""
-    A = (v1[0] - v0[0]) * (v2[1] - v0[1]) - (v2[0] - v0[0]) * (v1[1] - v0[1])
-    if not (A != 0):
-        return
-    if culling and A > 0:
-        return
-    if A < 0:
-        v1, v2 = v2, v1
-        A = -A
-    fW, fH = f32(W), f32(H)
-    lo_x = np.fmin(np.fmax(np.ceil(np.fmin(np.fmin(v0[0], v1[0]), v2[0]) - HALF), f32(0)), fW)
-    hi_x = np.fmin(np.fmax(np.floor(np.fmax(np.fmax(v0[0], v1[0]), v2[0]) - HALF), f32(-1)), fW - f32(1))
-    lo_y = np.fmin(np.fmax(np.ceil(np.fmin(np.fmin(v0[1], v1[1]), v2[1]) - HALF), f32(0)), fH)
-    hi_y = np.fmin(np.fmax(np.floor(np.fmax(np.fmax(v0[1], v1[1]), v2[1]) - HALF), f32(-1)), fH - f32(1))
-    i0, j0 = int(lo_x), int(lo_y)
-    nx, ny = int(hi_x) - i0 + 1, int(hi_y) - j0 + 1
-    if nx <= 0 or ny <= 0:
-        return
-    jj, ii = np.mgrid[j0:j0 + ny, i0:i0 + nx]
-    px = ii.astype(f32) + HALF
-    py = jj.astype(f32) + HALF
-    e0, e1, e2 = rr._edge(v1, v2, px, py), rr._edge(v2, v0, px, py), rr._edge(v0, v1, px, py)
-    inside = rr._covers(e0, v1, v2) & rr._covers(e1, v2, v0) & rr._covers(e2, v0, v1)
-    with np.errstate(invalid="ignore", over="ignore"):
-        z = (e0 * v0[2] + e1 * v1[2] + e2 * v2[2]) / A
-        q = np.rint(z * f32(65535))
-        keep = inside & (q < f32(65535))
-    d16 = np.fmax(q[keep], f32(0)).astype(np.uint64)
-    np.minimum.at(zbuf, (jj[keep], ii[keep]), (d16 << np.uint64(48)) | np.uint64(tag))
-
-
-def raster(M, triangles, culling, W, H, draw, zbuf):
-    """Every triangle of one body through M: near-plane clipping, window mapping onto W x H, fans."""
-    tv = np.asarray(triangles, f32).reshape(-1, 3, 3)
-    vx, vy, vz = tv[..., 0], tv[..., 1], tv[..., 2]
-    clip = [M[4 * r] * vx + M[4 * r + 1] * vy + M[4 * r + 2] * vz + M[4 * r + 3] for r in range(4)]
-    dist = clip[2] + clip[3]
-    half_x, half_y = HALF * f32(W), HALF * f32(H)
-    for t in range(tv.shape[0]):
-        c = [tuple(clip[r][t, k] for r in range(4)) for k in range(3)]
-        d = [dist[t, k] for k in range(3)]
-        poly = []
-        for e in range(3):
-            e1 = 0 if e == 2 else e + 1
-            in0, in1 = d[e] >= 0, d[e1] >= 0
-            if in0:
-                poly.append(c[e])
-            if in0 != in1:
-                poly.append(rr._intersect(c[e], d[e], c[e1], d[e1]) if in0 else rr._intersect(c[e1], d[e1], c[e], d[e]))
-        if len(poly) < 3:
-            continue
-        with np.errstate(divide="ignore", invalid="ignore", over="ignore"):
-            win = [((p[0] / p[3] + f32(1)) * half_x, (p[1] / p[3] + f32(1)) * half_y, (p[2] / p[3] + f32(1)) * HALF)
-                   for p in poly]
-        tag = (draw << 32) | t
-        raster_triangle(win[0], win[1], win[2], culling, W, H, tag, zbuf)
-        if len(win) == 4:
-            raster_triangle(win[0], win[2], win[3], culling, W, H, tag, zbuf)
+def raster(M, triangles, culling, W, H, draw, zbuf, stats=None):
+    """Every triangle of one body through M: near-plane clipping, window mapping onto W x H, fans, the z-buffer key
+    (rr.raster_keyed; `stats` counts what it reaches)."""
+    rr.raster_keyed(M, triangles, culling, W, H, draw, zbuf, stats)
 
 
 def encode_normals(zbuf, rots, normals):
@@ -118,7 +63,7 @@ def encode_normals(zbuf, rots, normals):
     return out
 
 
-def render_normal(intr, world2camera, poses, geometry, bodies, z_min=Z_MIN, z_max=Z_MAX):
+def render_normal(intr, world2camera, poses, geometry, bodies, z_min=Z_MIN, z_max=Z_MAX, stats=None):
     """FullNormalRenderer::StartRendering + FetchNormalImage: (normal [H,W,4] u8, zbuf [H,W] u64). poses /
     geometry: {body: [3,4] body2world / rr.Geometry}; bodies: render_data_bodies order."""
     W, H = int(intr.width), int(intr.height)
@@ -129,7 +74,7 @@ def render_normal(intr, world2camera, poses, geometry, bodies, z_min=Z_MIN, z_ma
     for g, b in enumerate(bodies):
         G = geometry[b]
         T = rr.pose_mul(w2c, rr.pose_mul(poses[b], G.geometry2body))
-        raster(clip_matrix(P, T), G.triangles, G.enable_culling, W, H, g, zbuf)
+        raster(clip_matrix(P, T), G.triangles, G.enable_culling, W, H, g, zbuf, stats)
         rots.append(T.reshape(3, 4)[:, :3].copy())
         normals.append(mg.face_normals(G.triangles))
     return encode_normals(zbuf, rots, normals), zbuf
