@@ -153,7 +153,7 @@ SYMBOLS = [
     "m3tb_texture_correspondences", "m3tb_texture_gradient_hessian", "m3tb_get_texture_points",
     "m3tb_get_texture_keyframes", "m3tb_texture_crop", "m3tb_upload_texture_features_device",
     "m3tb_get_texture_feature_flags", "m3tb_orb_params_default", "m3tb_texture_detect_orb",
-    "m3tb_get_texture_detections", "m3tb_get_texture_orb_keypoints",
+    "m3tb_get_texture_detections", "m3tb_get_texture_orb_keypoints", "m3tb_refine_poses_orb",
 ]
 
 KERNEL_NAMES = {0: None, 1: "k_track", 2: "k_track2", 3: "k_track_cluster"}
@@ -241,6 +241,7 @@ def lib():
     L.m3tb_n_structures.argtypes = [vp]
     L.m3tb_calculate_consistent_poses.argtypes = [vp]
     L.m3tb_refine_poses.argtypes = [vp, C.POINTER(ci), ci, C.POINTER(ci), ci, ci, ci]
+    L.m3tb_refine_poses_orb.argtypes = [vp, C.POINTER(ci), ci, C.POINTER(ci), ci, ci, ci, C.POINTER(OrbParams)]
     L.m3tb_reset_joint_poses.argtypes = [vp]
     L.m3tb_prefetch_frames.argtypes = [vp]
     L.m3tb_detach_frames.argtypes = [vp]
@@ -859,6 +860,29 @@ class Context:
         ip = C.POINTER(C.c_int)
         self._ck(self.L.m3tb_refine_poses(self.h, b.ctypes.data_as(ip), len(b), s.ctypes.data_as(ip), len(s),
                                           n_corr_iterations, n_update_iterations))
+
+    def refine_poses_orb(self, bodies=(), structures=(), n_corr_iterations=7, n_update_iterations=2, orb_params=None):
+        """refine_poses with refined ORB texture bodies taking part (m3tb_refine_poses_orb): their features are
+        detected on the device before every correspondence iteration. orb_params: None (defaults), one
+        (n_features, scale_factor, n_levels) tuple / OrbParams for every body, or a dict body -> tuple / OrbParams
+        (the other bodies take the defaults)."""
+        b = np.ascontiguousarray(list(bodies), dtype=np.int32)
+        s = np.ascontiguousarray(list(structures), dtype=np.int32)
+        ip = C.POINTER(C.c_int)
+        arr = None
+        if orb_params is not None:
+            as_params = lambda p: p if isinstance(p, OrbParams) else OrbParams(int(p[0]), float(p[1]), int(p[2]))
+            arr = (OrbParams * max(self.n_bodies, 1))()
+            for k in range(len(arr)):
+                self.L.m3tb_orb_params_default(C.byref(arr[k]))
+            if isinstance(orb_params, dict):
+                for body, p in orb_params.items():
+                    arr[int(body)] = as_params(p)
+            else:
+                for k in range(len(arr)):
+                    arr[k] = as_params(orb_params)
+        self._ck(self.L.m3tb_refine_poses_orb(self.h, b.ctypes.data_as(ip), len(b), s.ctypes.data_as(ip), len(s),
+                                              n_corr_iterations, n_update_iterations, arr))
 
     def get_link_poses(self, structure, n_links):
         """(body2joint, joint2parent, link2world), each [n_links, 3, 4]."""

@@ -113,6 +113,9 @@ struct RefineSelection {
   int n_hist_groups = 0;                //   owner[n] | first[n + 1] | summed[n] | members (refined ones first)
   bool ingested = false;                // k_ingest ran for the refined bodies
   std::vector<std::pair<int, int>> runs;  // k_track: (first body, count) of each run of consecutive refined bodies
+  const int* texture = nullptr;         // k_texture_keyframe / _match / _knn_*: the refined texture bodies
+  int n_texture = 0;                    //   (m3tb_refine_poses_orb only)
+  std::vector<int> texture_ids;         // host copy
 };
 
 }  // namespace
@@ -569,6 +572,9 @@ int SyncStructures(m3tb_ctx* ctx);
 int LaunchRender(m3tb_ctx* ctx, int which);
 int LaunchTexture(m3tb_ctx* ctx, bool keyframe, int mode);
 int ValidateTexture(m3tb_ctx* ctx);
+int ValidateTextureBody(m3tb_ctx* ctx, int b);
+int CheckOrbDetection(m3tb_ctx* ctx, int b, const m3tb_orb_params& p);
+int DetectOrb(m3tb_ctx* ctx, const int* bodies, int count, const m3tb_orb_params* params);
 
 // cuTensorMapEncodeTiled through the runtime (libcuda is not linked: the library must load on machines without a driver)
 PFN_cuTensorMapEncodeTiled_v12000 TensorMapEncoder() {
@@ -2920,14 +2926,20 @@ int m3tb_calculate_consistent_poses(m3tb_ctx* ctx) {
   return LaunchStructure(ctx, 1, false);
 }
 
+}  // extern "C"
+
+namespace {
+
 // Refiner::RefinePoses (refiner.cpp:76-117) for the named optimisers: Refiner::CalculateConsistentPoses, then per
 // correspondence iteration StartModalities (render, ClearMemory, StartModality(0, corr), InitializeHistograms),
 // CalculateCorrespondences (render, CalculateCorrespondences(0, corr)) and n_update x (CalculateGradientAndHessian,
 // CalculateOptimization). The launches are the tracking step's, restricted to the refined bodies, structures and
-// renderers through RefineSelection; every other body keeps its state.
-int m3tb_refine_poses(m3tb_ctx* ctx, const int* bodies, int n_bodies, const int* structures, int n_structures,
-                      int n_corr_iterations, int n_update_iterations) {
-  CHECK_CTX();
+// renderers through RefineSelection; every other body keeps its state. With `texture` (m3tb_refine_poses_orb) refined
+// ORB texture bodies take part: TextureModality::StartModality is device detection (orb[body], or the defaults when
+// `orb` is null) and k_texture_keyframe, and the bodies match at correspondence iteration 0; without it a refined
+// texture body is refused.
+int RefinePoses(m3tb_ctx* ctx, const int* bodies, int n_bodies, const int* structures, int n_structures,
+                int n_corr_iterations, int n_update_iterations, bool texture, const m3tb_orb_params* orb) {
   if (n_bodies < 0 || n_structures < 0 || (n_bodies > 0 && !bodies) || (n_structures > 0 && !structures))
     return Fail(ctx, M3TB_ERR_INVALID, "bad body / structure list");
   if (n_corr_iterations < 0 || n_update_iterations < 0) return Fail(ctx, M3TB_ERR_INVALID, "negative iteration count");
@@ -2970,13 +2982,28 @@ int m3tb_refine_poses(m3tb_ctx* ctx, const int* bodies, int n_bodies, const int*
       }
     }
   // TextureModality::StartModality detects features in a pose-dependent focus region before every correspondence
-  // iteration; with detection left to the caller one call cannot serve it
-  for (int b : track)
-    if (ctx->h_bodies[b].has_texture)
+  // iteration; with detection left to the caller one call cannot serve it, so only device detection (cv::ORB) can
+  RefineSelection sel;
+  std::vector<m3tb_orb_params> orb_settings;  // of sel.texture_ids
+  m3tb_orb_params defaults;
+  m3tb_orb_params_default(&defaults);
+  for (int b : track) {
+    const BodyDev& B = ctx->h_bodies[b];
+    if (!B.has_texture) continue;
+    if (!texture)
       return Fail(ctx, M3TB_ERR_UNSUPPORTED, "body " + std::to_string(b) + " has a texture modality: it cannot be refined");
+    if (B.tp.descriptor_type != M3TB_DESCRIPTOR_ORB)
+      return Fail(ctx, M3TB_ERR_UNSUPPORTED, "body " + std::to_string(b) +
+                                                 ": SIFT / DAISY features have no device detector: it cannot be refined");
+    const m3tb_orb_params& p = orb ? orb[b] : defaults;
+    int rc = CheckOrbDetection(ctx, b, p);
+    if (!rc) rc = ValidateTextureBody(ctx, b);
+    if (rc) return rc;
+    sel.texture_ids.push_back(b);
+    orb_settings.push_back(p);
+  }
   if (track.empty()) return M3TB_OK;  // if (!optimizer_found) return true
 
-  RefineSelection sel;
   std::vector<int> struct_list;
   if (HasStructures(ctx)) {
     int rc = SyncStructures(ctx);
@@ -2993,9 +3020,12 @@ int m3tb_refine_poses(m3tb_ctx* ctx, const int* bodies, int n_bodies, const int*
     for (int which : {int(kRenderAttached), int(kRenderRegion)}) {
       std::vector<char> use(ctx->renderers.size(), 0);
       for (int b : track)
-        for (int slot = 0; slot < RS_TEXTURE_SILHOUETTE; ++slot) {
+        for (int slot = 0; slot < RS_COUNT; ++slot) {  // the lists of SyncRenderTables
           const int r = ctx->attached[b][slot];
-          if (r >= 0 && (which == kRenderAttached || slot == RS_REGION_DEPTH || slot == RS_REGION_SILHOUETTE)) use[r] = 1;
+          if (r >= 0 && (which == kRenderAttached ? slot < RS_TEXTURE_SILHOUETTE
+                                                  : slot == RS_REGION_DEPTH || slot == RS_REGION_SILHOUETTE ||
+                                                        slot >= RS_TEXTURE_SILHOUETTE))
+            use[r] = 1;
         }
       for (int r = 0; r < int(use.size()); ++r) {
         if (!use[r]) continue;
@@ -3023,7 +3053,8 @@ int m3tb_refine_poses(m3tb_ctx* ctx, const int* bodies, int n_bodies, const int*
   }
   g_first.push_back(int(g_members.size()));
 
-  // one device table: bodies | structures | renderers (attached) | renderers (region) | shared-object groups
+  // one device table: bodies | structures | renderers (attached) | renderers (region) | texture bodies | shared-object
+  // groups
   std::vector<int> h(track);
   const size_t o_struct = h.size();
   h.insert(h.end(), struct_list.begin(), struct_list.end());
@@ -3032,6 +3063,8 @@ int m3tb_refine_poses(m3tb_ctx* ctx, const int* bodies, int n_bodies, const int*
     o_render[which] = h.size();
     h.insert(h.end(), sel.renderer_ids[which].begin(), sel.renderer_ids[which].end());
   }
+  const size_t o_texture = h.size();
+  h.insert(h.end(), sel.texture_ids.begin(), sel.texture_ids.end());
   const size_t o_groups = h.size();
   if (!g_owner.empty()) {
     h.insert(h.end(), g_owner.begin(), g_owner.end());
@@ -3063,6 +3096,8 @@ int m3tb_refine_poses(m3tb_ctx* ctx, const int* bodies, int n_bodies, const int*
     sel.renderers[which] = d + o_render[which];
     sel.n_renderers[which] = int(sel.renderer_ids[which].size());
   }
+  sel.texture = d + o_texture;
+  sel.n_texture = int(sel.texture_ids.size());
   sel.hist_groups = d + o_groups;
   sel.n_hist_groups = int(g_owner.size());
 
@@ -3079,14 +3114,22 @@ int m3tb_refine_poses(m3tb_ctx* ctx, const int* bodies, int n_bodies, const int*
   for (int b : track) ctx->h_bodies[b].first_iteration = 0;  // StartModality(0, corr)
   ctx->bodies_dirty = true;
   const unsigned corr_phases = PH_REGION_CORR | PH_DEPTH_CORR | PH_STORE_REGION | PH_STORE_DEPTH;
+  const bool textured = sel.n_texture > 0;
+  const unsigned tex = textured ? unsigned(PH_TEXTURE_GH) : 0u;
   for (int corr = 0; corr < n_corr_iterations; ++corr) {
-    if (ctx->n_attached > 0) rc = LaunchRender(ctx, kRenderRegion);  // start_modality_renderer_ptrs
+    // DetectAndComputeCorrKeypoints at the pose this iteration starts from. It goes before the start renders (it reads
+    // only the pose and the colour frame): a detection that fails to grow its scratch then leaves the refined bodies as
+    // the completed iterations left them.
+    if (textured) rc = DetectOrb(ctx, sel.texture_ids.data(), sel.n_texture, orb_settings.data());
+    if (!rc && ctx->n_attached > 0) rc = LaunchRender(ctx, kRenderRegion);  // start_modality_renderer_ptrs
     if (!rc) rc = LaunchHistogram(ctx, 0, 0);
+    if (!rc && textured) rc = LaunchTexture(ctx, true, 0);  // ComputeKeyframeData
     if (!rc && ctx->n_attached > 0) rc = LaunchRender(ctx, kRenderAttached);  // correspondence_renderer_ptrs
+    if (!rc && textured && corr == 0) rc = LaunchTexture(ctx, false, 1);  // the texture matches (corr 0 only)
     if (rc) return rc;
     if (!structured) {
       rc = LaunchTrack(ctx, 0, corr, corr + 1, n_update_iterations, 0,
-                       corr_phases | PH_REGION_GH | PH_DEPTH_GH | PH_SOLVE);
+                       corr_phases | PH_REGION_GH | PH_DEPTH_GH | PH_SOLVE | tex);
       if (rc) return rc;
       continue;
     }
@@ -3098,12 +3141,30 @@ int m3tb_refine_poses(m3tb_ctx* ctx, const int* bodies, int n_bodies, const int*
     for (int upd = 0; upd < n_update_iterations; ++upd) {
       rc = LaunchTrack(ctx, 0, corr, corr + 1, 1, upd,
                        (upd == 0 ? corr_phases : unsigned(PH_LOAD_REGION | PH_LOAD_DEPTH)) | PH_REGION_GH | PH_DEPTH_GH |
-                           PH_STORE_LINK_GH);
+                           PH_STORE_LINK_GH | tex);
       if (!rc) rc = LaunchStructure(ctx, 0, false);
       if (rc) return rc;
     }
   }
   return M3TB_OK;
+}
+
+}  // namespace
+
+extern "C" {
+
+int m3tb_refine_poses(m3tb_ctx* ctx, const int* bodies, int n_bodies, const int* structures, int n_structures,
+                      int n_corr_iterations, int n_update_iterations) {
+  CHECK_CTX();
+  return RefinePoses(ctx, bodies, n_bodies, structures, n_structures, n_corr_iterations, n_update_iterations, false,
+                     nullptr);
+}
+
+int m3tb_refine_poses_orb(m3tb_ctx* ctx, const int* bodies, int n_bodies, const int* structures, int n_structures,
+                          int n_corr_iterations, int n_update_iterations, const m3tb_orb_params* orb_params) {
+  CHECK_CTX();
+  return RefinePoses(ctx, bodies, n_bodies, structures, n_structures, n_corr_iterations, n_update_iterations, true,
+                     orb_params);
 }
 
 int m3tb_get_link_poses(m3tb_ctx* ctx, int structure, float* body2joint, float* joint2parent, float* link2world) {
@@ -4386,28 +4447,47 @@ int EnsureTextureTables(m3tb_ctx* ctx, bool l2, bool knn, int cap) {
 // m3tb_set_body assigned the body a depth camera (its depth modality's, or its region modality's for measured occlusions)
 bool HasDepthCamera(const BodyDev& B) { return B.has_depth || (B.has_region && B.rp.measure_occlusions); }
 
-// TextureModality::SetUp's conditions, checked before every texture launch ("Set up ... first")
+// TextureModality::SetUp's conditions for body b (a set body with a texture modality)
+int ValidateTextureBody(m3tb_ctx* ctx, int b) {
+  const BodyDev& B = ctx->h_bodies[b];
+  if (ctx->attached[b][RS_TEXTURE_SILHOUETTE] < 0)
+    return Fail(ctx, M3TB_ERR_NOT_SET_UP, "texture modality of body " + std::to_string(b) + ": no silhouette renderer attached");
+  if (B.tp.model_occlusions && ctx->attached[b][RS_TEXTURE_DEPTH] < 0)
+    return Fail(ctx, M3TB_ERR_NOT_SET_UP, "texture modality: model_occlusions needs a depth renderer attached");
+  if (B.tp.measure_occlusions) {
+    if (!HasDepthCamera(B)) return Fail(ctx, M3TB_ERR_NOT_SET_UP, "texture measure_occlusions: the body has no depth camera");
+    const CameraDev& d = ctx->h_dcams[B.depth_camera];
+    if (!d.set || !d.image) return Fail(ctx, M3TB_ERR_NOT_SET_UP, "texture measure_occlusions: depth camera not set / no image uploaded");
+  }
+  return M3TB_OK;
+}
+
+// TextureModality::SetUp's conditions, checked before every texture launch ("Set up ... first"): of every texture body,
+// or of the refined ones while a refinement runs
 int ValidateTexture(m3tb_ctx* ctx) {
+  if (const RefineSelection* sel = ctx->refine) {
+    for (int b : sel->texture_ids) {
+      int rc = ValidateTextureBody(ctx, b);
+      if (rc) return rc;
+    }
+    return M3TB_OK;
+  }
   for (int b = 0; b < ctx->n_bodies; ++b) {
     const BodyDev& B = ctx->h_bodies[b];
     if (!B.set || !B.has_texture) continue;
-    if (ctx->attached[b][RS_TEXTURE_SILHOUETTE] < 0)
-      return Fail(ctx, M3TB_ERR_NOT_SET_UP, "texture modality of body " + std::to_string(b) + ": no silhouette renderer attached");
-    if (B.tp.model_occlusions && ctx->attached[b][RS_TEXTURE_DEPTH] < 0)
-      return Fail(ctx, M3TB_ERR_NOT_SET_UP, "texture modality: model_occlusions needs a depth renderer attached");
-    if (B.tp.measure_occlusions) {
-      if (!HasDepthCamera(B)) return Fail(ctx, M3TB_ERR_NOT_SET_UP, "texture measure_occlusions: the body has no depth camera");
-      const CameraDev& d = ctx->h_dcams[B.depth_camera];
-      if (!d.set || !d.image) return Fail(ctx, M3TB_ERR_NOT_SET_UP, "texture measure_occlusions: depth camera not set / no image uploaded");
-    }
+    int rc = ValidateTextureBody(ctx, b);
+    if (rc) return rc;
   }
   return M3TB_OK;
 }
 
 // Features belong to the colour frame they were uploaded for: a body whose camera has received a newer frame since
-// has none (the reference's detection on that frame found nothing to work with).
+// has none (the reference's detection on that frame found nothing to work with). A refinement touches only its bodies.
 int SyncTextureFeatures(m3tb_ctx* ctx) {
-  for (int b = 0; b < ctx->n_bodies; ++b) {
+  const RefineSelection* sel = ctx->refine;
+  const int n = sel ? sel->n_texture : ctx->n_bodies;
+  for (int k = 0; k < n; ++k) {
+    const int b = sel ? sel->texture_ids[k] : k;
     const BodyDev& B = ctx->h_bodies[b];
     if (!B.has_texture) continue;
     const int gen = ctx->h_ccams[B.texture_camera].generation;
@@ -4419,10 +4499,12 @@ int SyncTextureFeatures(m3tb_ctx* ctx) {
   return M3TB_OK;
 }
 
-// k_texture_keyframe (keyframe = true) or k_texture_match over every body; mode as TextureArgs::mode. Matching
-// (mode 1) first runs k_texture_knn_l2 when an L2 body has keyframe descriptors to match.
+// k_texture_keyframe (keyframe = true) or k_texture_match over every body, or over the refined texture bodies while a
+// refinement runs; mode as TextureArgs::mode. Matching (mode 1) first runs k_texture_knn_l2 when an L2 body has keyframe
+// descriptors to match.
 int LaunchTexture(m3tb_ctx* ctx, bool keyframe, int mode) {
-  if (ctx->n_texture == 0) return M3TB_OK;
+  const RefineSelection* sel = ctx->refine;
+  if (ctx->n_texture == 0 || (sel && sel->n_texture == 0)) return M3TB_OK;
   int rc = ValidateTexture(ctx);
   if (!rc) rc = SyncTables(ctx);
   if (!rc) rc = SyncTextureFeatures(ctx);
@@ -4447,10 +4529,12 @@ int LaunchTexture(m3tb_ctx* ctx, bool keyframe, int mode) {
   a.counts = ctx->d_tex_counts;
   a.mode = mode;
   a.cap = ctx->tex_cap;
+  a.list = sel ? sel->texture : nullptr;
+  const int n_launch = sel ? sel->n_texture : ctx->n_bodies;
   // the longest descriptor, deque and n_features_max of the L2 bodies and of the ORB bodies matched by kNN
   int l2_length = 0, l2_keyframes = 0, l2_features = 0, ham_keyframes = 0, ham_features = 0;
-  for (int b = 0; b < ctx->n_bodies; ++b) {
-    const BodyDev& B = ctx->h_bodies[b];
+  for (int k = 0; k < n_launch; ++k) {
+    const BodyDev& B = ctx->h_bodies[sel ? sel->texture_ids[k] : k];
     if (!B.set || !B.has_texture) continue;
     if (B.tp.l2) {
       l2_length = std::max(l2_length, B.tp.descriptor_length);
@@ -4463,19 +4547,19 @@ int LaunchTexture(m3tb_ctx* ctx, bool keyframe, int mode) {
   }
   if (!keyframe && mode == 1 && l2_length > 0) {  // a body without a length has no features, hence no keyframe points
     CU(cudaFuncSetAttribute(k_texture_knn_l2, cudaFuncAttributeMaxDynamicSharedMemorySize, KnnSharedBytes(l2_length)));
-    const dim3 grid(kKnnSplits * l2_keyframes * KnnTilesPerKeyframe(l2_features), ctx->n_bodies);
+    const dim3 grid(kKnnSplits * l2_keyframes * KnnTilesPerKeyframe(l2_features), n_launch);
     k_texture_knn_l2<<<grid, kKnnThreads, KnnSharedBytes(l2_length), ctx->stream>>>(a);
     CU(cudaGetLastError());
     ctx->launches++;
   }
   if (!keyframe && mode == 1 && ham_features > 0) {
-    const dim3 grid(kKnnSplits * ham_keyframes * KnnTilesPerKeyframe(ham_features), ctx->n_bodies);
+    const dim3 grid(kKnnSplits * ham_keyframes * KnnTilesPerKeyframe(ham_features), n_launch);
     k_texture_knn_hamming<<<grid, kKnnThreads, KnnSharedBytes(kTexDescWords), ctx->stream>>>(a);
     CU(cudaGetLastError());
     ctx->launches++;
   }
-  if (keyframe) k_texture_keyframe<<<ctx->n_bodies, kTexThreads, 0, ctx->stream>>>(a);
-  else k_texture_match<<<ctx->n_bodies, kTexThreads, 0, ctx->stream>>>(a);
+  if (keyframe) k_texture_keyframe<<<n_launch, kTexThreads, 0, ctx->stream>>>(a);
+  else k_texture_match<<<n_launch, kTexThreads, 0, ctx->stream>>>(a);
   CU(cudaGetLastError());
   ctx->launches++;
   return M3TB_OK;
@@ -4936,31 +5020,22 @@ TexOrbJob OrbJob(int body, int w, int h, const m3tb_orb_params& p) {
   return j;
 }
 
-}  // namespace
+// The refusals of device detection for ORB texture body b with settings p, apart from the body checks
+int CheckOrbDetection(m3tb_ctx* ctx, int b, const m3tb_orb_params& p) {
+  if (p.n_features < 1 || !std::isfinite(p.scale_factor) || !(p.scale_factor > 1.0f) || p.n_levels < 1)
+    return Fail(ctx, M3TB_ERR_INVALID, "ORB settings: n_features >= 1, finite scale_factor > 1, n_levels >= 1");
+  if (p.n_levels > kOrbMaxLevels) return Fail(ctx, M3TB_ERR_UNSUPPORTED, "ORB n_levels above 8");
+  if (p.n_features > kOrbFeatureLimit) return Fail(ctx, M3TB_ERR_UNSUPPORTED, "ORB n_features above 2^24");
+  if (!ctx->h_ccams[ctx->h_bodies[b].texture_camera].image)
+    return Fail(ctx, M3TB_ERR_NOT_SET_UP, "texture detection: no colour frame uploaded");
+  return M3TB_OK;
+}
 
-extern "C" {
-
-int m3tb_texture_detect_orb(m3tb_ctx* ctx, const int* bodies, int count, const m3tb_orb_params* params) {
-  CHECK_CTX();
-  if (count < 0 || (count > 0 && !bodies)) return Fail(ctx, M3TB_ERR_INVALID, "bad detection arguments");
-  m3tb_orb_params defaults;
-  m3tb_orb_params_default(&defaults);
-  std::vector<char> listed(ctx->n_bodies, 0);
-  for (int k = 0; k < count; ++k) {  // every refusal before anything is allocated or launched
-    const int b = bodies[k];
-    int rc = CheckTextureBody(ctx, b);
-    if (rc) return rc;
-    if (listed[b]++) return Fail(ctx, M3TB_ERR_INVALID, "body listed twice");
-    if (ctx->h_bodies[b].tp.descriptor_type != M3TB_DESCRIPTOR_ORB)
-      return Fail(ctx, M3TB_ERR_INVALID, "device detection is cv::ORB: the body's descriptor type is not ORB");
-    const m3tb_orb_params& p = params ? params[k] : defaults;
-    if (p.n_features < 1 || !std::isfinite(p.scale_factor) || !(p.scale_factor > 1.0f) || p.n_levels < 1)
-      return Fail(ctx, M3TB_ERR_INVALID, "ORB settings: n_features >= 1, finite scale_factor > 1, n_levels >= 1");
-    if (p.n_levels > kOrbMaxLevels) return Fail(ctx, M3TB_ERR_UNSUPPORTED, "ORB n_levels above 8");
-    if (p.n_features > kOrbFeatureLimit) return Fail(ctx, M3TB_ERR_UNSUPPORTED, "ORB n_features above 2^24");
-    if (!ctx->h_ccams[ctx->h_bodies[b].texture_camera].image)
-      return Fail(ctx, M3TB_ERR_NOT_SET_UP, "texture detection: no colour frame uploaded");
-  }
+// cv::ORB on the focused crops of `count` checked ORB texture bodies at their current poses, with settings params[k]
+// for bodies[k] (m3tb_texture_detect_orb, and m3tb_refine_poses_orb before every correspondence iteration). Reads the
+// poses back (one host synchronisation) to size the crops; the scratch and parity tables grow all or nothing before
+// anything is committed, so a failed allocation returns M3TB_ERR_CUDA with every body as it was.
+int DetectOrb(m3tb_ctx* ctx, const int* bodies, int count, const m3tb_orb_params* params) {
   if (count == 0) return M3TB_OK;
   std::vector<float> poses(size_t(12) * ctx->n_bodies);
   CU(cudaMemcpyAsync(poses.data(), ctx->d_poses, poses.size() * sizeof(float), cudaMemcpyDeviceToHost, ctx->stream));
@@ -4974,7 +5049,7 @@ int m3tb_texture_detect_orb(m3tb_ctx* ctx, const int* bodies, int count, const m
     const bool ok = FocusCropJob(ctx, b, poses.data() + 12 * b, &crops[k]);
     width = std::max(width, crops[k].out_w);
     height = std::max(height, crops[k].out_h);
-    jobs[k] = OrbJob(b, crops[k].out_w, crops[k].out_h, params ? params[k] : defaults);
+    jobs[k] = OrbJob(b, crops[k].out_w, crops[k].out_h, params[k]);
     jobs[k].n_features_max = ctx->h_bodies[b].tp.n_features_max;
     jobs[k].roi_x = crops[k].roi_x;
     jobs[k].roi_y = crops[k].roi_y;
@@ -5060,6 +5135,31 @@ int m3tb_texture_detect_orb(m3tb_ctx* ctx, const int* bodies, int count, const m
     ctx->launches++;
   }
   return M3TB_OK;
+}
+
+}  // namespace
+
+extern "C" {
+
+int m3tb_texture_detect_orb(m3tb_ctx* ctx, const int* bodies, int count, const m3tb_orb_params* params) {
+  CHECK_CTX();
+  if (count < 0 || (count > 0 && !bodies)) return Fail(ctx, M3TB_ERR_INVALID, "bad detection arguments");
+  m3tb_orb_params defaults;
+  m3tb_orb_params_default(&defaults);
+  std::vector<char> listed(ctx->n_bodies, 0);
+  std::vector<m3tb_orb_params> settings(count);
+  for (int k = 0; k < count; ++k) {  // every refusal before anything is allocated or launched
+    const int b = bodies[k];
+    int rc = CheckTextureBody(ctx, b);
+    if (rc) return rc;
+    if (listed[b]++) return Fail(ctx, M3TB_ERR_INVALID, "body listed twice");
+    if (ctx->h_bodies[b].tp.descriptor_type != M3TB_DESCRIPTOR_ORB)
+      return Fail(ctx, M3TB_ERR_INVALID, "device detection is cv::ORB: the body's descriptor type is not ORB");
+    settings[k] = params ? params[k] : defaults;
+    rc = CheckOrbDetection(ctx, b, settings[k]);
+    if (rc) return rc;
+  }
+  return DetectOrb(ctx, bodies, count, settings.data());
 }
 
 int m3tb_get_texture_detections(m3tb_ctx* ctx, int first, int count, int32_t* n_found) {

@@ -113,7 +113,7 @@ __device__ void Orientation(const float* b2c, float* o) {
 // StartModality (mode 0: PrecalculatePoseVariables from the current pose, then ComputeKeyframeData) and CalculateResults
 // (mode 1: the rotation / age rule with the pose of the last gradient pass, texture_modality.cpp:456-472).
 __global__ void __launch_bounds__(kTexThreads) k_texture_keyframe(const __grid_constant__ TextureArgs a) {
-  const int b = blockIdx.x, tid = threadIdx.x;
+  const int b = a.list ? a.list[blockIdx.x] : int(blockIdx.x), tid = threadIdx.x;
   const BodyDev& body = a.bodies[b];
   if (!body.set || !body.has_texture) return;
   __shared__ float b2c[12], c2b[12], b2d[12];
@@ -289,7 +289,7 @@ __device__ __forceinline__ void KnnAccumulate(const uint4& q, const uint4& t, fl
 template <bool kHamming>
 __device__ __forceinline__ void KnnTile(const TextureArgs& a) {
   namespace cg = cooperative_groups;
-  const int b = blockIdx.y, tid = threadIdx.x;
+  const int b = a.list ? a.list[blockIdx.y] : int(blockIdx.y), tid = threadIdx.x;
   const BodyDev& body = a.bodies[b];
   // every return before the first cluster barrier depends on (body, tile) alone: a cluster leaves or stays whole
   if (!body.set || !body.has_texture || (kHamming ? !TexHammingKnn(body.tp) : !body.tp.l2)) return;
@@ -397,7 +397,7 @@ __global__ void __cluster_dims__(kKnnSplits, 1, 1) __launch_bounds__(kKnnThreads
 // matched here (Hamming, the train set in shared memory); k_texture_knn_l2 / _hamming have matched the others just
 // before. Every call then projects the data points with the current pose (data_point.center) and records that pose.
 __global__ void __launch_bounds__(kTexThreads) k_texture_match(const __grid_constant__ TextureArgs a) {
-  const int b = blockIdx.x, tid = threadIdx.x;
+  const int b = a.list ? a.list[blockIdx.x] : int(blockIdx.x), tid = threadIdx.x;
   const BodyDev& body = a.bodies[b];
   if (!body.set || !body.has_texture) return;
   __shared__ uint4 s_train[kTexMaxFeatures * 2];

@@ -52,6 +52,7 @@ struct TextureArgs {
   int* counts;                  // [n_bodies]
   int mode;                     // k_texture_keyframe: 0 StartModality, 1 CalculateResults; k_texture_match: 1 = match
   int cap;                      // features per body of every table above (kTexMaxFeatures .. kTexFeatureLimit)
+  const int* list = nullptr;    // the bodies of the launch, one per CTA (grid y for the kNN kernels); null: every body
 };
 
 // k_texture_match reads an ORB body's matches from knn (k_texture_knn_hamming) instead of scanning its train set
@@ -66,7 +67,8 @@ __global__ void k_texture_match(const __grid_constant__ TextureArgs a);
 // kKnnSplits CTAs per tile of kKnnQueries queries of one keyframe. The train set is walked in chunks of kKnnChunk rows;
 // CTA r of the cluster scans rows [c * kKnnChunk + r * kKnnTrain, ... + kKnnTrain) of every chunk c and rank 0 merges
 // the partial top-2 lists. Grid: (kKnnSplits * keyframes * KnnTilesPerKeyframe(features), n_bodies), with the longest
-// deque and the largest n_features_max of the bodies the kernel matches; dynamic shared memory KnnSharedBytes(row
+// deque and the largest n_features_max of the bodies the kernel matches (n_bodies: the length of TextureArgs::list when
+// it has one); dynamic shared memory KnnSharedBytes(row
 // length in 32-bit words: the longest descriptor of the context's L2 bodies, kTexDescWords for Hamming).
 constexpr int kKnnQueries = 64, kKnnTrain = 64, kKnnThreads = 256;
 constexpr int kKnnSplits = 8;                       // the portable cluster size

@@ -2222,7 +2222,9 @@ class Tracker {
 // ---- refiner.h ------------------------------------------------------------------------------------------------------
 // Refiner (refiner.h): refines the poses of the named optimizers, e.g. after a detector, while every other body keeps
 // tracking undisturbed. RefinePoses is one m3tb_refine_poses call: a rigid optimizer is refined through its body, a
-// kinematic structure as a whole.
+// kinematic structure as a whole. When a named optimizer's links carry a TextureModality it is one
+// m3tb_refine_poses_orb call instead, which detects the ORB features before every correspondence iteration at each
+// modality's orb_* settings; SIFT / DAISY modalities have no device detector and cannot be refined.
 class Refiner {
  public:
   Refiner(const std::string& name, int n_corr_iterations = 7, int n_update_iterations = 2)
@@ -2260,17 +2262,37 @@ class Refiner {
       return false;
     }
     std::vector<int> bodies, structures;
+    std::vector<std::pair<int, m3tb_orb_params>> texture;  // (body, orb_* settings) of the named texture modalities
     for (auto& o : optimizer_ptrs_) {
       if (names.find(o->name()) == names.end()) continue;
       if (o->structure_index() >= 0) structures.push_back(o->structure_index());
       else bodies.push_back(o->root_link_ptr()->body_ptr()->index());
+      for (auto& l : o->ReferencedLinks())
+        for (auto& m : l->modality_ptrs())
+          if (auto t = std::dynamic_pointer_cast<TextureModality>(m)) {
+            if (t->descriptor_type() != TextureModality::DescriptorType::ORB) {
+              std::cerr << "Modality " << t->name() << ": only ORB features are detected on the device between the "
+                        << "correspondence iterations; optimizer " << o->name() << " cannot be refined" << std::endl;
+              return false;
+            }
+            texture.emplace_back(t->body_ptr()->index(), t->orb_params());
+          }
     }
     if (bodies.empty() && structures.empty()) return true;
     const auto& batch = optimizer_ptrs_.front()->batch();
-    const bool ok = Check(batch->ctx(),
-                          m3tb_refine_poses(batch->ctx(), bodies.data(), int(bodies.size()), structures.data(),
-                                            int(structures.size()), n_corr_iterations_, n_update_iterations_),
-                          "Refiner::RefinePoses");
+    m3tb_ctx* ctx = batch->ctx();
+    int rc;
+    if (texture.empty()) {
+      rc = m3tb_refine_poses(ctx, bodies.data(), int(bodies.size()), structures.data(), int(structures.size()),
+                             n_corr_iterations_, n_update_iterations_);
+    } else {
+      std::vector<m3tb_orb_params> orb(std::max(m3tb_n_bodies(ctx), 1));
+      for (auto& p : orb) m3tb_orb_params_default(&p);
+      for (auto& t : texture) orb[t.first] = t.second;
+      rc = m3tb_refine_poses_orb(ctx, bodies.data(), int(bodies.size()), structures.data(), int(structures.size()),
+                                 n_corr_iterations_, n_update_iterations_, orb.data());
+    }
+    const bool ok = Check(ctx, rc, "Refiner::RefinePoses");
     batch->PosesChanged();
     return ok;
   }

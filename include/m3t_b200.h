@@ -706,9 +706,32 @@ int m3tb_calculate_consistent_poses(m3tb_ctx* ctx);
  * Both lists empty: M3TB_OK, nothing is launched. M3TB_ERR_INVALID: an id that is out of range or not set, an id listed
  * twice, a negative iteration count, or a body that is a link or an extra body of a structure (name the structure).
  * M3TB_ERR_UNSUPPORTED: a refined body, or a body of a refined structure, has a texture modality
- * (TextureModality::StartModality detects features before every correspondence iteration, which the caller does). */
+ * (TextureModality::StartModality detects features before every correspondence iteration, which the caller does; for
+ * ORB texture bodies m3tb_refine_poses_orb detects them on the device). */
 int m3tb_refine_poses(m3tb_ctx* ctx, const int* bodies, int n_bodies, const int* structures, int n_structures,
                       int n_corr_iterations, int n_update_iterations);
+/* m3tb_refine_poses with refined ORB texture bodies taking part, as Refiner::RefinePoses runs them: per correspondence
+ * iteration, TextureModality::StartModality is DetectAndComputeCorrKeypoints on the device at the pose the iteration
+ * starts from (m3tb_texture_detect_orb with orb_params[body]: one crop + ORB launch pair per 128 refined texture bodies)
+ * and ComputeKeyframeData (k_texture_keyframe over the refined texture bodies: one new keyframe per iteration, at most
+ * n_keyframes kept, age 0); their silhouette and depth renderers render with the start renderers. The bodies match
+ * at correspondence iteration 0 only (texture_modality.cpp:332; kNN first where a body needs it), and every update adds
+ * their texture term (k_track, or k_track + k_structure for structures). So a refined texture body ends with the
+ * corr-0 data points and the features of the last iteration's detection. orb_params: NULL (m3tb_orb_params_default for
+ * every body) or [m3tb_n_bodies(ctx)] entries by body id, of which only the refined texture bodies' are read.
+ * A selection without texture bodies launches exactly what m3tb_refine_poses launches, with the same results.
+ * Synchronises the host once per correspondence iteration with a texture body: detection reads the poses back to size
+ * the focus crops. The detection scratch grows on demand, all or nothing; as the crop size follows the pose, it may
+ * have to grow at a later iteration, and if that allocation fails the call returns M3TB_ERR_CUDA with the refined
+ * bodies as the completed iterations left them (as the reference's loop returns false mid-way) and every other body
+ * untouched; the context stays usable.
+ * Refusals launch nothing and change nothing: every refusal of m3tb_refine_poses but the texture one;
+ * M3TB_ERR_UNSUPPORTED for a refined texture body whose descriptor type is SIFT or DAISY (no device detector, and a
+ * detection by the caller cannot run between the iterations of one call); the ORB-setting refusals of
+ * m3tb_texture_detect_orb; M3TB_ERR_NOT_SET_UP when a refined texture body's camera has no colour frame, or the body
+ * misses a renderer its texture modality needs. */
+int m3tb_refine_poses_orb(m3tb_ctx* ctx, const int* bodies, int n_bodies, const int* structures, int n_structures,
+                          int n_corr_iterations, int n_update_iterations, const m3tb_orb_params* orb_params);
 /* Link::body2joint_pose / joint2parent_pose / link2world_pose of every link of one structure after the last update,
  * each [n_links][12]; any pointer may be NULL. */
 int m3tb_get_link_poses(m3tb_ctx* ctx, int structure, float* body2joint, float* joint2parent, float* link2world);
