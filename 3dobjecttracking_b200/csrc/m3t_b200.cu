@@ -487,6 +487,11 @@ int SyncTables(m3tb_ctx* ctx) {
 // a stride of 0 (a scan that never ends, in the reference too) or a negative offset index
 bool RadiusValid(float r) { return r >= 0.0f && std::isfinite(r); }
 
+// The region modality's depth-offset id (region_modality.cpp:975-976, 985-986) as the kernels compute it. The reference
+// checks only radius <= max_radius; when max_radius / stride lies in [29.5, 30) a radius near the maximum rounds to
+// id 30, one past the table, so ValidateBodies refuses any id of 30 or more.
+int RegionOffsetId(float radius, const ModelDev& m) { return int(radius / m.stride_depth_offset + 0.5f); }
+
 // Checks that every set body references set-up objects ("Set up ... first").
 int ValidateBodies(m3tb_ctx* ctx) {
   if (ctx->n_bodies == 0) return Fail(ctx, M3TB_ERR_NOT_SET_UP, "no body set");
@@ -497,15 +502,21 @@ int ValidateBodies(m3tb_ctx* ctx) {
       if (!ctx->h_rmodels[B.region_model].set) return Fail(ctx, M3TB_ERR_NOT_SET_UP, "region model not set");
       const CameraDev& c = ctx->h_ccams[B.color_camera];
       if (!c.set || !c.image) return Fail(ctx, M3TB_ERR_NOT_SET_UP, "color camera not set / no image uploaded");
+      const ModelDev& m = ctx->h_rmodels[B.region_model];
       if (B.rp.measure_occlusions) {  // RegionModality::SetUp / PrecalculateModelVariables (region_modality.cpp:965-977)
         const CameraDev& d = ctx->h_dcams[B.depth_camera];
         if (!d.set || !d.image) return Fail(ctx, M3TB_ERR_NOT_SET_UP, "measure_occlusions: depth camera not set / no image uploaded");
-        if (B.rp.measured_depth_offset_radius > ctx->h_rmodels[B.region_model].max_radius_depth_offset)
+        if (B.rp.measured_depth_offset_radius > m.max_radius_depth_offset)
           return Fail(ctx, M3TB_ERR_INVALID, "Measured depth offset radius too large");
+        if (RegionOffsetId(B.rp.measured_depth_offset_radius, m) >= kDepthOffsets)
+          return Fail(ctx, M3TB_ERR_INVALID, "Measured depth offset radius rounds past the model's 30 depth offsets");
       }
-      if (B.rp.model_occlusions &&  // region_modality.cpp:979-991
-          B.rp.modeled_depth_offset_radius > ctx->h_rmodels[B.region_model].max_radius_depth_offset)
-        return Fail(ctx, M3TB_ERR_INVALID, "Modeled depth offset radius too large");
+      if (B.rp.model_occlusions) {  // region_modality.cpp:979-991
+        if (B.rp.modeled_depth_offset_radius > m.max_radius_depth_offset)
+          return Fail(ctx, M3TB_ERR_INVALID, "Modeled depth offset radius too large");
+        if (RegionOffsetId(B.rp.modeled_depth_offset_radius, m) >= kDepthOffsets)
+          return Fail(ctx, M3TB_ERR_INVALID, "Modeled depth offset radius rounds past the model's 30 depth offsets");
+      }
     }
     if (B.has_depth) {
       if (!ctx->h_dmodels[B.depth_model].set) return Fail(ctx, M3TB_ERR_NOT_SET_UP, "depth model not set");
@@ -1402,6 +1413,11 @@ int SetModel(m3tb_ctx* ctx, bool region, int model_id, int n_views, int n_points
              const float* scalars, const void* points, float stride_depth_offset, float max_radius_depth_offset) {
   if (model_id < 0 || model_id >= ctx->max_models || n_views <= 0 || n_points <= 0 || !orientations || !points)
     return Fail(ctx, M3TB_ERR_INVALID, "bad model arguments");
+  // what model generation refuses (CheckModelParams), and an infinite stride besides: a stride of 0, a negative or
+  // non-finite one, or more than 30 depth offsets would give depth-offset ids outside the table
+  if (!(stride_depth_offset > 0.0f) || !std::isfinite(stride_depth_offset) || !(max_radius_depth_offset >= 0.0f) ||
+      !std::isfinite(max_radius_depth_offset) || int(max_radius_depth_offset / stride_depth_offset + 1.0f) > kDepthOffsets)
+    return Fail(ctx, M3TB_ERR_INVALID, "bad model depth-offset parameters");
   // Repack the .bin AoS DataPoints (152 B / 144 B) into the 32 B records the kernels read:
   // region (cx,cy,cz,nx)(ny,nz,fg,bg), depth (cx,cy,cz,nx)(ny,nz,0,0). One-time setup, not on the hot path.
   const int fl = region ? M3TB_REGION_POINT_BYTES / 4 : M3TB_DEPTH_POINT_BYTES / 4;

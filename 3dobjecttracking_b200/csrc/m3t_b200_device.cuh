@@ -157,6 +157,12 @@ constexpr float kRegionOffset = 2.0f;  // region_modality.h:147
 constexpr int kDepthOffsets = 30;        // DataPoint::depth_offsets (region_model.h:97, depth_model.h:74)
 constexpr int kMaxNOcclusionStrides = 5; // region_modality.h:145, depth_modality.h:113
 
+// Whether an occlusion window of this diameter [px] is scanned. A NaN diameter or one in (-5, 0) gives a stride of 0
+// (float-to-int conversion maps NaN to 0), so the reference's scan would never end; a non-finite or negative diameter
+// comes from an item behind or level with the camera or from a non-finite pose. Such a window scans nothing and counts
+// as unoccluded (DESIGN.md §3).
+__device__ __forceinline__ bool ScanDiameterValid(float diameter) { return diameter >= 0.0f && diameter <= 3.40282347e38f; }
+
 // Parameters of m3t::TextureModality (texture_modality.h:400-436)
 struct TextureParamsDev {
   int focused_image_size;

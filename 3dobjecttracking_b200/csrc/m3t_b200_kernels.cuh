@@ -258,6 +258,7 @@ struct LineState {  // RegionModality::DataLine (region_modality.h:150-165), the
 // truncation to int and reduction modulo 2^16 (identical to the oracle).
 static __device__ __noinline__ bool WindowUnoccluded(const Tile& t, const uint16_t* tile, const FrameView& f, int w_m1, int h_m1,
                                               float center_u, float center_v, float diameter, float min_depth_value) {
+  if (!ScanDiameterValid(diameter)) return true;
   const int stride = int(diameter / float(kMaxNOcclusionStrides) + 1.0f);
   const int n_strides = int(diameter / float(stride) + 0.5f);
   const int rounded_diameter = n_strides * stride;
@@ -310,6 +311,7 @@ __device__ __forceinline__ bool LineUnoccludedMeasured(const RegionOcclusion& o,
 // DepthModality::IsPointUnoccludedModeled (depth_modality.cpp:778-824) in the focused depth rendering.
 static __device__ __noinline__ bool ModeledWindowUnoccluded(const RenderingDev& r, float center_u, float center_v, float diameter,
                                                             float min_allowed_depth) {
+  if (!ScanDiameterValid(diameter)) return true;
   const int stride = int(diameter / float(kMaxNOcclusionStrides) + 1.0f);
   const int n_strides = int(diameter / float(stride) + 0.5f);
   const int rounded_diameter = n_strides * stride;
@@ -521,7 +523,7 @@ __device__ __forceinline__ void RegionLine(const RegionIter& it, const RegionPar
   float continuous_distance = fminf(p1.w, p1.z) * it.fu / (z * it.fscale);
   // IsLineValid (:1252-1291)
   if (continuous_distance < rp.min_continuous_distance) return;
-  if (z <= 0.0f) return;
+  if (!(z > 0.0f)) return;
   int icu = int(center_u + 0.5f), icv = int(center_v + 0.5f);
   if (icu < 0 || icu > it.w_m1 || icv < 0 || icv > it.h_m1) return;
   if (OCC) {  // region checking (:1269-1274), measured occlusions (:1274-1281), modeled occlusions (:1283-1289)
@@ -746,7 +748,7 @@ __device__ __forceinline__ void DepthPoint(const DepthIter& it, const DepthParam
   float center_u = x * it.fu / z + it.ppu;
   float center_v = y * it.fv / z + it.ppv;
   // IsPointValid (:697-726)
-  if (z <= 0.0f) return;
+  if (!(z > 0.0f)) return;
   int icu = int(center_u + 0.5f), icv = int(center_v + 0.5f);
   if (icu < 0 || icu > it.w_m1 || icv < 0 || icv > it.h_m1) return;
   if (OCC) {  // IsPointOnValidSilhouette (:728-734) via FocusedSilhouetteRenderer::SilhouetteValue
@@ -2045,7 +2047,7 @@ __global__ void __launch_bounds__(kBlockThreads) k_histogram(HistArgs args) {
     float4 p0 = __ldg(pts + 2 * i), p1 = __ldg(pts + 2 * i + 1);
     float x, y, z;
     PoseApply(it.b2c, p0.x, p0.y, p0.z, x, y, z);
-    if (z <= 0.0f) continue;
+    if (!(z > 0.0f)) continue;
     float center_u = x * it.fu / z + it.ppu;
     float center_v = y * it.fv / z + it.ppv;
     int icu = int(center_u + 0.5f), icv = int(center_v + 0.5f);

@@ -41,6 +41,7 @@ __device__ bool UnoccludedMeasured(const CameraDev& d, const float* b2d, const T
   const float center_u = x * d.fu / z + d.ppu, center_v = y * d.fv / z + d.ppv;
   const float meter_to_pixel = d.fu / z;
   const float diameter = 2.0f * tp.measured_occlusion_radius * meter_to_pixel;
+  if (!ScanDiameterValid(diameter)) return true;
   const int stride = int(diameter / float(kMaxNOcclusionStrides) + 1.0f);
   const int n_strides = int(diameter / float(stride) + 0.5f);
   const int rounded_diameter = n_strides * stride;
@@ -75,6 +76,7 @@ __device__ bool UnoccludedModeled(const CameraDev& c, const RenderingDev& r, con
   const float z = b2c[8] * bx + b2c[9] * by + b2c[10] * bz + b2c[11];
   const float meter_to_pixel = (c.fu / z) * r.scale;
   const float diameter = 2.0f * tp.modeled_occlusion_radius * meter_to_pixel;
+  if (!ScanDiameterValid(diameter)) return true;
   const int stride = int(diameter / float(kMaxNOcclusionStrides) + 1.0f);
   const int n_strides = int(diameter / float(stride) + 0.5f);
   const int rounded_diameter = n_strides * stride;

@@ -85,15 +85,19 @@ typedef struct m3tb_region_params {
   float learning_rate_b;           /* 0.2 */
   float unconsidered_line_length;  /* 0.5 */
   float max_considered_line_length; /* 20 */
+  /* Occlusion windows: an item whose window diameter is not finite or is negative (behind or level with the camera
+   * that is scanned, or a non-finite pose) scans nothing and counts as unoccluded; items whose depth in the tracking
+   * camera is not above 0 (NaN included) are dropped before any check. The reference's scans would not end there. */
   int32_t measure_occlusions;      /* 0 */
-  float measured_depth_offset_radius; /* 0.01 */
+  float measured_depth_offset_radius; /* 0.01; must not exceed the model's max_radius_depth_offset nor round to a
+                                         depth-offset id of 30 or more (M3TB_ERR_INVALID at the next launch) */
   float measured_occlusion_radius;    /* 0.01 */
   float measured_occlusion_threshold; /* 0.03 */
   int32_t n_unoccluded_iterations; /* 10 */
   int32_t min_n_unoccluded_lines;  /* 0 */
   /* checks that read renderer images (handed over with m3tb_upload_*_rendering), region_modality.h:424-431 */
   int32_t model_occlusions;        /* 0  RegionModality::ModelOcclusions (focused depth rendering) */
-  float modeled_depth_offset_radius;  /* 0.01 */
+  float modeled_depth_offset_radius;  /* 0.01; the same limits as measured_depth_offset_radius */
   float modeled_occlusion_radius;     /* 0.01 */
   float modeled_occlusion_threshold;  /* 0.03 */
   int32_t use_region_checking;     /* 0  RegionModality::UseRegionChecking (focused silhouette rendering) */
@@ -249,6 +253,10 @@ int m3tb_set_region_model(m3tb_ctx* ctx, int model_id, int n_views, int n_points
                           const float* orientations, const float* contour_lengths,
                           const void* points, float stride_depth_offset,
                           float max_radius_depth_offset);
+/* Both model setters refuse (M3TB_ERR_INVALID, the context unchanged) a stride_depth_offset that is not finite and
+ * above 0, a max_radius_depth_offset that is not finite and >= 0, and int(max_radius_depth_offset /
+ * stride_depth_offset + 1) above 30: what model generation refuses, and an infinite stride besides (every radius
+ * would select depth offset 0 of a table the model cannot have been generated with). */
 /* Replaces DepthModel::views_ (depth_model.h:73-86); `points` are 144-B DepthModel::DataPoint. */
 int m3tb_set_depth_model(m3tb_ctx* ctx, int model_id, int n_views, int n_points,
                          const float* orientations, const float* surface_areas,

@@ -757,12 +757,18 @@ int orc_closest_view(const orc_model* model, const float body2camera[12], int ro
 namespace {
 constexpr int kMaxNOcclusionStrides = 5;  // region_modality.h:145, depth_modality.h:113
 
+// A NaN diameter or one in (-5, 0) gives the reference's scans a stride of 0 and a loop that never ends. A window whose
+// diameter is not finite or is negative (an item behind or level with the camera, a non-finite pose) scans nothing and
+// counts as unoccluded, as in the library.
+bool ScanDiameterValid(float diameter) { return diameter >= 0.0f && diameter <= 3.40282347e38f; }
+
 // The strided window scan shared by RegionModality::IsLineUnoccludedMeasured (region_modality.cpp:1355-1388) and
 // DepthModality::IsPointUnoccludedMeasured (depth_modality.cpp:739-775): false if any valid depth sample inside the
 // window lies in front of min_depth. The reference converts the float threshold with ushort(x); that is restated as
 // truncation to int followed by reduction modulo 2^16 (what x86 does), so that a negative threshold behaves the same
 // on both sides of the parity tests.
 bool WindowUnoccluded(const orc_depth_frame* f, float center_u, float center_v, float diameter, float min_depth_value) {
+  if (!ScanDiameterValid(diameter)) return true;
   int stride = int(diameter / kMaxNOcclusionStrides + 1.0f);
   int n_strides = int(diameter / stride + 0.5f);
   int rounded_diameter = n_strides * stride;
@@ -799,15 +805,20 @@ bool LineUnoccludedMeasured(const orc_region_params* p, const orc_depth_frame* f
                           (cd[2] - depth_offset - p->measured_occlusion_threshold) / f->depth_scale);
 }
 
-// measured_depth_offset_id_ (region_modality.cpp:965-977); -1 if the radius exceeds the model's table
+// measured_depth_offset_id_ (region_modality.cpp:965-977); -1 if the radius exceeds the model's table or rounds to an
+// id past its 30 entries (max_radius / stride in [29.5, 30) passes the reference's radius test), which the library
+// refuses
+int RegionOffsetIdOf(float radius, const orc_model* model) {
+  if (radius > model->max_radius_depth_offset) return -1;
+  const int id = int(radius / model->stride_depth_offset + 0.5f);
+  return id < ORC_N_DEPTH_OFFSETS ? id : -1;
+}
 int RegionOffsetId(const orc_region_params* p, const orc_model* model) {
-  if (p->measured_depth_offset_radius > model->max_radius_depth_offset) return -1;
-  return int(p->measured_depth_offset_radius / model->stride_depth_offset + 0.5f);
+  return RegionOffsetIdOf(p->measured_depth_offset_radius, model);
 }
 // modeled_depth_offset_id_ (region_modality.cpp:979-991)
 int RegionModeledOffsetId(const orc_region_params* p, const orc_model* model) {
-  if (p->modeled_depth_offset_radius > model->max_radius_depth_offset) return -1;
-  return int(p->modeled_depth_offset_radius / model->stride_depth_offset + 0.5f);
+  return RegionOffsetIdOf(p->modeled_depth_offset_radius, model);
 }
 
 constexpr int kNRegionStride = 5;      // region_modality.h:146
@@ -820,6 +831,7 @@ inline uint8_t SilhouetteAt(const orc_rendering* r, int v, int u) {
 // The strided minimum scan shared by RegionModality::IsLineUnoccludedModeled (region_modality.cpp:1391-1431) and
 // DepthModality::IsPointUnoccludedModeled (depth_modality.cpp:778-824), in the focused depth rendering.
 bool ModeledWindowUnoccluded(const orc_rendering* r, float center_u, float center_v, float diameter, float min_allowed_depth) {
+  if (!ScanDiameterValid(diameter)) return true;
   int stride = int(diameter / kMaxNOcclusionStrides + 1.0f);
   int n_strides = int(diameter / stride + 0.5f);
   int rounded_diameter = n_strides * stride;
@@ -975,7 +987,7 @@ void orc_region_add_line_pixels_occ(const orc_region_params* p, const orc_model*
     float foreground_distance = dp[6], background_distance = dp[7];
     float cc[3];
     PoseApply(v.body2camera, center_f_body, cc);
-    if (cc[2] <= 0.0f) continue;
+    if (!(cc[2] > 0.0f)) continue;
     float center_u = cc[0] * v.fu / cc[2] + v.ppu;
     float center_v = cc[1] * v.fv / cc[2] + v.ppv;
     int i_center_u = int(center_u + 0.5f);
@@ -1089,7 +1101,7 @@ int orc_region_correspondences(const orc_region_params* p, const orc_model* mode
       float continuous_distance = std::min(dp[7], dp[6]) * v.fu / (cc[2] * v.fscale);
       // IsLineValid (:1252-1291)
       if (continuous_distance < p->min_continuous_distance) continue;
-      if (cc[2] <= 0.0f) continue;
+      if (!(cc[2] > 0.0f)) continue;
       int i_center_u = int(L.center_u + 0.5f);
       int i_center_v = int(L.center_v + 0.5f);
       if (i_center_u < 0 || i_center_u > v.w_m1 || i_center_v < 0 || i_center_v > v.h_m1) continue;
@@ -1195,7 +1207,7 @@ int orc_depth_correspondences(const orc_depth_params* p, const orc_model* model,
       float center_v = cc[1] * v.fv / cc[2] + v.ppv;
       float depth = cc[2];
       // IsPointValid (:697-726)
-      if (depth <= 0.0f) continue;
+      if (!(depth > 0.0f)) continue;
       int i_center_u = int(center_u + 0.5f);
       int i_center_v = int(center_v + 0.5f);
       if (i_center_u < 0 || i_center_u > v.w_m1 || i_center_v < 0 || i_center_v > v.h_m1) continue;

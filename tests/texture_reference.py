@@ -106,6 +106,12 @@ def keyframe_fires(b2c_stale, last_orientation, age, max_rotation, max_age):
     return bool(diff > f32(max_rotation) or age > max_age), age
 
 
+def _scanned(diameter):
+    """A window whose diameter is not finite or is negative scans nothing and counts as unoccluded (its stride would be
+    0 or negative)."""
+    return bool(diameter >= f32(0)) and not np.isinf(diameter)
+
+
 def _window(center_u, center_v, diameter, w_m1, h_m1):
     stride = int(diameter / f32(5) + f32(1))  # kMaxNOcclusionStrides
     n_strides = int(diameter / f32(stride) + f32(0.5))
@@ -124,6 +130,8 @@ def unoccluded_measured(X, m):
     x, y, z = apply(m["b2d"], X)
     cu, cv = x * fu / z + ppu, y * fv / z + ppv
     diameter = f32(2) * f32(m["radius"]) * (fu / z)
+    if not _scanned(diameter):
+        return True
     u0, v0, u1, v1, stride = _window(cu, cv, diameter, int(intr["width"]) - 1, int(intr["height"]) - 1)
     min_depth = int((z - f32(m["threshold"])) / f32(m["depth_scale"])) & 0xFFFF
     img = m["image"]
@@ -143,6 +151,8 @@ def unoccluded_modeled(X, m):
     x, y, z = apply(m["b2c"], X)
     sc = f32(r["scale"])
     diameter = f32(2) * f32(m["radius"]) * ((fu / z) * sc)
+    if not _scanned(diameter):
+        return True
     cu, cv = x * fu / z + ppu, y * fv / z + ppv
     fcu, fcv = (cu - f32(r["corner_u"])) * sc, (cv - f32(r["corner_v"])) * sc
     S = r["depth"].shape[0]
