@@ -2469,6 +2469,22 @@ int m3tb_set_body(m3tb_ctx* ctx, int body, const m3tb_region_params* region, con
       (depth && !(RadiusValid(depth->measured_depth_offset_radius) && RadiusValid(depth->measured_occlusion_radius) &&
                   RadiusValid(depth->modeled_depth_offset_radius) && RadiusValid(depth->modeled_occlusion_radius))))
     return Fail(ctx, M3TB_ERR_INVALID, "occlusion and depth-offset radii must be finite and >= 0");
+  if (depth) {  // checked before anything is written, so that a refused call leaves the context as it was
+    if (depth->n_considered_distances < 1 || depth->n_considered_distances > M3TB_MAX_SCHEDULE ||
+        depth->n_standard_deviations < 1 || depth->n_standard_deviations > M3TB_MAX_SCHEDULE ||
+        depth->n_points_max < 1 || !(depth->stride_length > 0.0f))
+      return Fail(ctx, M3TB_ERR_INVALID, "bad depth schedule / n_points_max / stride_length");
+    // FindCorrespondence divides the window diameter by max_n_strides_ = int(d / stride_length + 0.5f)
+    // (depth_modality.cpp:651, :835): a distance below half the stride length, or NaN, gives 0 and an infinite stride,
+    // and 2^31 strides or more overflow the int (the device saturates, x86 gives INT_MIN and a stride of 0)
+    for (int i = 0; i < depth->n_considered_distances; ++i) {
+      const float d = depth->considered_distances[i];
+      const float strides = d / depth->stride_length + 0.5f;
+      if (!(d > 0.0f) || !std::isfinite(d) || !(strides >= 1.0f) || !(strides < 2147483648.0f))
+        return Fail(ctx, M3TB_ERR_INVALID,
+                    "considered distances must be finite, at least half the stride length and under 2^31 strides");
+    }
+  }
   BodyDev B;
   std::memset(&B, 0, sizeof(B));
   B.first_iteration = ctx->h_bodies[body].first_iteration;
@@ -2559,10 +2575,6 @@ int m3tb_set_body(m3tb_ctx* ctx, int body, const m3tb_region_params* region, con
   if (depth) {
     if (depth_model < 0 || depth_model >= ctx->max_models || depth_camera < 0 || depth_camera >= ctx->max_cameras)
       return Fail(ctx, M3TB_ERR_INVALID, "depth model / depth camera id out of range");
-    if (depth->n_considered_distances < 1 || depth->n_considered_distances > M3TB_MAX_SCHEDULE ||
-        depth->n_standard_deviations < 1 || depth->n_standard_deviations > M3TB_MAX_SCHEDULE ||
-        depth->n_points_max < 1 || !(depth->stride_length > 0.0f))
-      return Fail(ctx, M3TB_ERR_INVALID, "bad depth schedule / n_points_max / stride_length");
     DepthParamsDev& d = B.dp;
     d.measure_occlusions = depth->measure_occlusions ? 1 : 0;
     d.n_unoccluded_iterations = depth->n_unoccluded_iterations;

@@ -632,7 +632,7 @@ __device__ __forceinline__ void RegionLine(const RegionIter& it, const RegionPar
     var += (dd * dd) * L.dist[d];
   }
   L.mean = mean_from_begin - (float(kDistributionLength) - 1.0f) / 2.0f;
-  L.var = fmaxf(var, rp.min_expected_variance);
+  L.var = var < rp.min_expected_variance ? rp.min_expected_variance : var;  // std::max: a NaN variance stays NaN
   L.valid = true;
 }
 
@@ -820,13 +820,17 @@ __device__ __forceinline__ void DepthPoint(const DepthIter& it, const DepthParam
     // The reference's tests, restated so that most samples cost a handful of instructions (results unchanged):
     //  * depth > min && depth < max on the raw integer sample (a u16 is exact in float: raw > m <=> raw >= floor(m) + 1);
     //  * dz * dz >= best: the exact early-out (d2 >= dz * dz under round-to-nearest);
-    //  * a SCREEN with reciprocal multiplies instead of the two divisions: its squared distance differs from the exact
-    //    one by < 1e-7 m^2 (|tx|, |ty| < 1 m, relative error of x * (1 / f) against x / f < 2e-7), so a sample whose
-    //    screened value exceeds best by more than 1e-6 m^2 cannot pass the strict test d2 < best; everything else is
-    //    evaluated with the reference's expression, and only those values are ever stored.
+    //  * a SCREEN with reciprocal multiplies instead of the two divisions: whenever d2 < best, its squared distance s
+    //    satisfies s <= best * (1 + 2^-9) + 2^-34 * (|x| + |y|)^2 (DESIGN.md section 3), so a sample with
+    //    s > best * (1 + 2^-8) + 2^-33 * (|x| + |y|)^2 + 2^-126 cannot pass the strict test d2 < best, at any depth,
+    //    depth scale or considered distance. Everything else is evaluated with the reference's expression, and only
+    //    those values are ever stored.
     const int raw_lo = int(floorf(fmaxf(min_depth_value, -2.0f))) + 1;
     const int raw_hi = int(ceilf(fminf(max_depth_value, 70000.0f))) - 1;
     const float rfu = 1.0f / it.fu, rfv = 1.0f / it.fv;
+    const float q = fabsf(x) + fabsf(y);
+    const float k = 0x1p-33f * (q * q) + 0x1p-126f;  // 2^-126: the roundings of k where q * q is subnormal
+    float screen = best * (1.0f + 0x1p-8f) + k;
     for (int v = v_min; v <= v_max; v += stride, trow += row_step) {
       const float vy = float(v) - it.ppv;
 #pragma unroll 4
@@ -839,12 +843,12 @@ __device__ __forceinline__ void DepthPoint(const DepthIter& it, const DepthParam
           if (dz2 >= best) continue;
           const float ux = float(u) - it.ppu;
           const float ax = ux * depth * rfu - x, ay = vy * depth * rfv - y;
-          if (ax * ax + ay * ay + dz2 > best + 1.0e-6f) continue;
+          if (ax * ax + ay * ay + dz2 > screen) continue;
           float tx = ux * depth / it.fu;
           float ty = vy * depth / it.fv;
           float dx = tx - x, dy = ty - y, dz = depth - z;
           float d2 = dx * dx + dy * dy + dz * dz;
-          if (d2 < best) { bx = tx; by = ty; bz = depth; best = d2; }
+          if (d2 < best) { bx = tx; by = ty; bz = depth; best = d2; screen = best * (1.0f + 0x1p-8f) + k; }
         }
       }
     }

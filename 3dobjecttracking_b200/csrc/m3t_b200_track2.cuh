@@ -299,7 +299,7 @@ __device__ __forceinline__ void RegionLine2(const RegionIter& it, const RegionPa
   float continuous_distance = fminf(p1.w, p1.z) * it.fu / (z * it.fscale);
   // IsLineValid (:1252-1291)
   if (continuous_distance < rp.min_continuous_distance) return;
-  if (z <= 0.0f) return;
+  if (!(z > 0.0f)) return;
   int icu = int(center_u + 0.5f), icv = int(center_v + 0.5f);
   if (icu < 0 || icu > it.w_m1 || icv < 0 || icv > it.h_m1) return;
   // CalculateSegmentProbabilities (:1433-1573); horizontal / vertical cases folded into major / minor axes
@@ -370,7 +370,7 @@ __device__ __forceinline__ void RegionLine2(const RegionIter& it, const RegionPa
     var += (dd * dd) * dist[d];
   }
   L.mean = mean_from_begin - (float(kDistributionLength) - 1.0f) / 2.0f;
-  L.var = fmaxf(var, rp.min_expected_variance);
+  L.var = var < rp.min_expected_variance ? rp.min_expected_variance : var;  // std::max: a NaN variance stays NaN
   L.valid = true;
 }
 

@@ -20,6 +20,7 @@
 
 #include <algorithm>
 #include <array>
+#include <cmath>
 #include <cstdint>
 #include <cstdio>
 #include <cstring>
@@ -1367,11 +1368,19 @@ class DepthModality : public Modality {
     m3tb_depth_params_default(&params_);
   }
   void set_n_points_max(int v) { params_.n_points_max = v; set_up_ = false; }
-  void set_stride_length(float v) { params_.stride_length = v; set_up_ = false; }
-  void set_considered_distances(const std::vector<float>& v) {
+  // Each value must be finite and positive (refused here, whatever the order of the calls); SetUp refuses a schedule
+  // whose considered distances are not at least half the stride length, as m3tb_set_body does.
+  bool set_stride_length(float v) {
+    if (!(v > 0.0f) || !std::isfinite(v)) return Refuse("stride_length must be finite and positive");
+    params_.stride_length = v; set_up_ = false; return true;
+  }
+  bool set_considered_distances(const std::vector<float>& v) {
+    for (float d : v)
+      if (!(d > 0.0f) || !std::isfinite(d)) return Refuse("considered distances must be finite and positive");
     params_.n_considered_distances = int(v.size());
     for (size_t i = 0; i < v.size() && i < M3TB_MAX_SCHEDULE; ++i) params_.considered_distances[i] = v[i];
     set_up_ = false;
+    return true;
   }
   void set_standard_deviations(const std::vector<float>& v) {
     params_.n_standard_deviations = int(v.size());
@@ -1393,6 +1402,12 @@ class DepthModality : public Modality {
   const std::shared_ptr<DepthModel>& depth_model_ptr() const { return depth_model_ptr_; }
 
   bool SetUp() override {
+    const int n = std::min(params_.n_considered_distances, int(M3TB_MAX_SCHEDULE));
+    for (int k = 0; k < n; ++k) {  // max_n_strides_ = int(d / stride_length + 0.5f) must lie in [1, 2^31)
+      const float strides = params_.considered_distances[k] / params_.stride_length + 0.5f;
+      if (!(strides >= 1.0f) || !(strides < 2147483648.0f))
+        return Refuse("considered distances must be at least half the stride length and under 2^31 strides");
+    }
     if (!CheckRenderers(IDType::BODY)) return false;
     set_up_ = true;
     return true;
@@ -1421,6 +1436,10 @@ class DepthModality : public Modality {
   bool CalculateResults(int) override { return IsSetup(); }  // depth_modality.cpp:393
 
  private:
+  bool Refuse(const char* what) const {
+    std::cerr << "Modality " << name_ << ": " << what << std::endl;
+    return false;
+  }
   m3tb_depth_params params_;
   std::shared_ptr<DepthCamera> depth_camera_ptr_;
   std::shared_ptr<DepthModel> depth_model_ptr_;

@@ -4,6 +4,7 @@
 // objects that are not set up refuse to run, structural setters clear set_up. Runs on a machine without GPU: the Batch
 // then has no context (there is no CPU fallback) and everything that would need it must fail cleanly.
 #include <iostream>
+#include <limits>
 #include <memory>
 
 #include "m3t_b200/m3t_b200.hpp"
@@ -46,6 +47,21 @@ int main() {
   EXPECT(!optimizer->set_up());
   EXPECT(!optimizer->CalculateOptimization(0, 0, 0)); // "Set up optimizer ... first"
   EXPECT(!optimizer->CalculateConsistentPoses());
+
+  // Depth modality schedule: a malformed value is refused by its setter whatever the order of the calls; a considered
+  // distance below half the stride length, or 2^31 strides or more, is refused by SetUp (as by m3tb_set_body)
+  auto depth = std::make_shared<DepthModality>("depth", batch, body, nullptr, nullptr);
+  EXPECT(!depth->set_considered_distances({0.05f, 0.0f}) && !depth->set_considered_distances({-0.01f}));
+  EXPECT(!depth->set_considered_distances({std::numeric_limits<float>::quiet_NaN()}));
+  EXPECT(!depth->set_considered_distances({std::numeric_limits<float>::infinity()}));
+  EXPECT(!depth->set_stride_length(0.0f) && !depth->set_stride_length(std::numeric_limits<float>::infinity()));
+  EXPECT(depth->params().n_considered_distances == 3 && depth->params().stride_length == 0.005f);
+  EXPECT(depth->set_stride_length(0.1f));              // 0.01 / 0.1 + 0.5 < 1 until the schedule follows
+  EXPECT(!depth->SetUp() && !depth->set_up());
+  EXPECT(depth->set_stride_length(1e-12f));            // 0.05 / 1e-12 strides overflow an int
+  EXPECT(!depth->SetUp());
+  EXPECT(depth->set_considered_distances({0.2f, 0.1f}) && depth->set_stride_length(0.1f));
+  EXPECT(depth->params().n_considered_distances == 2 && depth->params().stride_length == 0.1f);
 
   // Constraints
   auto constraint = std::make_shared<Constraint>("constraint", root, child);

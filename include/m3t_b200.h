@@ -111,7 +111,7 @@ typedef struct m3tb_depth_params {
   float reference_surface_area;    /* 0 */
   float stride_length;             /* 0.005 */
   int32_t n_considered_distances;  /* 3 */
-  float considered_distances[M3TB_MAX_SCHEDULE]; /* {0.05,0.02,0.01} */
+  float considered_distances[M3TB_MAX_SCHEDULE]; /* {0.05,0.02,0.01}; finite, >= stride_length / 2, < 2^31 strides */
   int32_t n_standard_deviations;   /* 3 */
   float standard_deviations[M3TB_MAX_SCHEDULE];  /* {0.05,0.03,0.02} */
   int32_t measure_occlusions;      /* 0 */

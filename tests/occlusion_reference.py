@@ -18,9 +18,9 @@ The rule the reference leaves undefined: a window whose diameter is not finite o
 earlier guards instead (z <= 0 as the only projection test, no diameter test, region depth-offset ids not limited to
 the table): a scan that would not end is then reported in stats["stride0_scans"] rather than looped.
 
-What is not restated: the closest view, the line's segment probabilities and the depth point's correspondence search.
-`geometric_valid` (an item's validity with every check off, from a run without them) and `view` come from the caller;
-the predicted valid flag is geometric_valid and the checks.
+What is not restated here: the closest view; the line's segment probabilities and the depth point's correspondence
+search are restated in tests/correspondence_reference.py. `geometric_valid` (an item's validity with every check off,
+from a run without them) and `view` come from the caller; the predicted valid flag is geometric_valid and the checks.
 """
 from __future__ import annotations
 
