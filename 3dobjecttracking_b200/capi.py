@@ -80,7 +80,8 @@ class Constraint(C.Structure):
                 ("standard_deviation_rotation", C.c_float), ("standard_deviation_translation", C.c_float)]
 
 
-DESCRIPTOR_DAISY, DESCRIPTOR_SIFT, DESCRIPTOR_ORB = 1, 3, 4  # M3TB_DESCRIPTOR_*
+DESCRIPTOR_BRISK, DESCRIPTOR_DAISY, DESCRIPTOR_FREAK, DESCRIPTOR_SIFT, DESCRIPTOR_ORB = 0, 1, 2, 3, 4  # M3TB_DESCRIPTOR_*
+BINARY_BYTES = {DESCRIPTOR_ORB: 32, DESCRIPTOR_BRISK: 64, DESCRIPTOR_FREAK: 64}  # NORM_HAMMING descriptor widths
 
 
 def texture_params_default():
@@ -107,8 +108,8 @@ TEXTURE_POINT_LIMIT = 8 * 4096  # a full deque of 8 keyframes at n_features_max 
 
 class DeviceFeatures(C.Structure):
     """m3tb_device_features: one body's keypoints (x[i * xy_stride], y[i * xy_stride], crop coordinates) and descriptor
-    rows (descriptor_pitch bytes apart; 32-byte ORB rows with length 0, `length` floats for SIFT / DAISY) in device
-    memory."""
+    rows (descriptor_pitch bytes apart; with length 0 binary rows, 32 bytes for ORB and 64 for BRISK / FREAK; `length`
+    floats for SIFT / DAISY) in device memory."""
     _fields_ = [("n", C.c_int), ("length", C.c_int), ("x", C.c_void_p), ("y", C.c_void_p), ("xy_stride", C.c_int),
                 ("descriptors", C.c_void_p), ("descriptor_pitch", C.c_size_t)]
 
@@ -424,6 +425,7 @@ class Context:
         self.h = h
         self.n_bodies = 0
         self._texture_length = {}  # SIFT / DAISY bodies: descriptor length of their uploads (0 before the first)
+        self._texture_bytes = {}   # ORB / BRISK / FREAK bodies: bytes per binary descriptor
         if stream is not None:
             self.set_stream(stream)
 
@@ -908,8 +910,11 @@ class Context:
         self._ck(self.L.m3tb_set_texture_modality(self.h, body, C.byref(params) if params is not None else None,
                                                   color_camera))
         self._texture_length.pop(body, None)
+        self._texture_bytes.pop(body, None)
         if params is not None and params.descriptor_type in (DESCRIPTOR_DAISY, DESCRIPTOR_SIFT):
             self._texture_length[body] = 0
+        elif params is not None:
+            self._texture_bytes[body] = BINARY_BYTES[params.descriptor_type]
 
     def get_texture_focus(self, first=0, count=None):
         """(roi [count, 4] int32 x, y, width, height; scale [count] float32; valid [count] bool)."""
@@ -923,8 +928,8 @@ class Context:
         return roi[:count], scale[:count], valid[:count].astype(bool)
 
     def upload_texture_features(self, body, keypoints_xy, descriptors, roi_x, roi_y, scale):
-        """keypoints_xy [n, 2] float32 in crop coordinates; descriptors [n, 32] uint8 (ORB) or [n, length] float32
-        (SIFT / DAISY, m3tb_upload_texture_float_features)."""
+        """keypoints_xy [n, 2] float32 in crop coordinates; descriptors [n, 32] uint8 (ORB), [n, 64] uint8 (BRISK /
+        FREAK) or [n, length] float32 (SIFT / DAISY, m3tb_upload_texture_float_features)."""
         xy = np.ascontiguousarray(np.asarray(keypoints_xy, np.float32).reshape(-1, 2))
         if isinstance(descriptors, np.ndarray) and descriptors.dtype == np.float32:
             d = np.ascontiguousarray(descriptors)
@@ -934,7 +939,14 @@ class Context:
             if self._texture_length.get(body) == 0:
                 self._texture_length[body] = d.shape[1]
             return
-        d = np.ascontiguousarray(np.asarray(descriptors, np.uint8).reshape(-1, 32))
+        width = self._texture_bytes.get(body, 32)
+        if width == 32:
+            d = np.ascontiguousarray(np.asarray(descriptors, np.uint8).reshape(-1, 32))
+        else:
+            d = np.ascontiguousarray(descriptors)
+            if d.dtype != np.uint8 or d.shape != (xy.shape[0], width):
+                raise ValueError("descriptors of a BRISK / FREAK body are (n, %d) uint8, got %s %s"
+                                 % (width, d.shape, d.dtype))
         self._ck(self.L.m3tb_upload_texture_features(self.h, body, _p(xy), d.ctypes.data_as(C.c_void_p), xy.shape[0],
                                                      int(roi_x), int(roi_y), float(scale)))
 
@@ -955,7 +967,8 @@ class Context:
         return roi[:n], scale[:n], size[:n], valid[:n].astype(bool)
 
     def upload_texture_features_device(self, bodies, features):
-        """features: one DeviceFeatures per body (m3tb_upload_texture_features_device); does not synchronise."""
+        """features: one DeviceFeatures per body (m3tb_upload_texture_features_device); does not synchronise. A BRISK /
+        FREAK body's rows are 64 bytes: length 0 and descriptor_pitch >= 64, which the library checks."""
         ids = np.ascontiguousarray(bodies, np.int32).reshape(-1)
         arr = (DeviceFeatures * max(len(ids), 1))(*features)
         self._ck(self.L.m3tb_upload_texture_features_device(self.h, ids.ctypes.data_as(C.POINTER(C.c_int)), arr,
@@ -1024,12 +1037,14 @@ class Context:
 
     def get_texture_keyframes(self, body, capacity=TEXTURE_POINT_LIMIT):
         """dict(sizes [n_keyframes], points [total, 3] float32, descriptors, age, orientation [3]). descriptors:
-        [total, 32] uint8 for ORB; [total, length] float32 for a SIFT / DAISY body, length that of its uploads."""
+        [total, 32] uint8 for ORB, [total, 64] uint8 for BRISK / FREAK; [total, length] float32 for a SIFT / DAISY
+        body, length that of its uploads."""
         length = self._texture_length.get(body)
         nk, age = C.c_int(0), C.c_int(0)
         sizes = np.zeros(8, np.int32)
         pts = np.zeros((capacity, 3), np.float32)
-        desc = np.zeros((capacity, 32), np.uint8) if length is None else np.zeros((capacity, length), np.float32)
+        desc = (np.zeros((capacity, self._texture_bytes.get(body, 32)), np.uint8) if length is None
+                else np.zeros((capacity, length), np.float32))
         o = np.zeros(3, np.float32)
         self._ck(self.L.m3tb_get_texture_keyframes(self.h, body, C.byref(nk), sizes.ctypes.data_as(C.POINTER(C.c_int)),
                                                    _p(pts), desc.ctypes.data_as(C.c_void_p), capacity, C.byref(age),

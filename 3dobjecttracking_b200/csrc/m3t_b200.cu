@@ -291,9 +291,9 @@ struct m3tb_ctx {
   DeviceBuffer<int> d_tex_nfeat, d_tex_kf_n, d_tex_counts;
   DeviceBuffer<float> d_tex_kf_points, d_tex_points, d_tex_pose, d_gh_texture;
   DeviceBuffer<TexKeyframeState> d_tex_kf_state;
-  // float descriptors (SIFT / DAISY): made by the first m3tb_set_texture_modality with an L2 descriptor type; the
-  // matches of k_texture_knn_l2 / _hamming: made with them or by the first ORB body above kTexMaxFeatures. Contexts
-  // whose ORB bodies keep the default n_features_max have neither.
+  // the wide descriptor tables (TexWideRows: SIFT / DAISY floats, BRISK / FREAK 64-byte rows): made by the first
+  // m3tb_set_texture_modality with such a type; the matches of k_texture_knn_l2 / _hamming: made with them or by the
+  // first ORB body above kTexMaxFeatures. Contexts whose ORB bodies keep the default n_features_max have neither.
   DeviceBuffer<float> d_tex_fdesc, d_tex_kf_fdesc;
   DeviceBuffer<int> d_tex_knn;
   // device front end (m3tb_texture_crop / m3tb_upload_texture_features_device): per body, the focus of its last crop
@@ -327,6 +327,12 @@ namespace {
 int Fail(m3tb_ctx* ctx, int code, const std::string& msg) {
   if (ctx) ctx->err = msg;
   return code;
+}
+
+// TextureModality::DescriptorType's names, for refusals
+const char* DescriptorName(int type) {
+  static const char* const names[] = {"BRISK", "DAISY", "FREAK", "SIFT", "ORB", "ORB_CUDA"};
+  return type >= 0 && type < 6 ? names[type] : "unknown";
 }
 
 #define CU(call)                                                                                       \
@@ -3021,8 +3027,8 @@ int RefinePoses(m3tb_ctx* ctx, const int* bodies, int n_bodies, const int* struc
     if (!texture)
       return Fail(ctx, M3TB_ERR_UNSUPPORTED, "body " + std::to_string(b) + " has a texture modality: it cannot be refined");
     if (B.tp.descriptor_type != M3TB_DESCRIPTOR_ORB)
-      return Fail(ctx, M3TB_ERR_UNSUPPORTED, "body " + std::to_string(b) +
-                                                 ": SIFT / DAISY features have no device detector: it cannot be refined");
+      return Fail(ctx, M3TB_ERR_UNSUPPORTED, "body " + std::to_string(b) + ": " + DescriptorName(B.tp.descriptor_type) +
+                                                 " features have no device detector: it cannot be refined");
     const m3tb_orb_params& p = orb ? orb[b] : defaults;
     int rc = CheckOrbDetection(ctx, b, p);
     if (!rc) rc = ValidateTextureBody(ctx, b);
@@ -4395,17 +4401,17 @@ struct TexTable {
 };
 
 // The texture tables for max_bodies at `cap` features per body (m3tb_set_texture_modality): the base tables, with knn
-// the kNN match table, with l2 also the float descriptor tables. Whatever is missing is made, and when `cap` exceeds
-// the capacity of the existing tables every capacity-sized table is remade at `cap` with its contents kept; all of it
-// in one all-or-nothing step. A context whose bodies keep kTexMaxFeatures never grows.
-int EnsureTextureTables(m3tb_ctx* ctx, bool l2, bool knn, int cap) {
+// the kNN match table, with wide also the wide descriptor tables (and the match table). Whatever is missing is made,
+// and when `cap` exceeds the capacity of the existing tables every capacity-sized table is remade at `cap` with its
+// contents kept; all of it in one all-or-nothing step. A context whose bodies keep kTexMaxFeatures never grows.
+int EnsureTextureTables(m3tb_ctx* ctx, bool wide, bool knn, int cap) {
   const size_t nb = size_t(ctx->max_bodies), K = kTexMaxKeyframes;
   const bool base = !ctx->d_tex_xy;
   cap = std::max(cap, base ? kTexMaxFeatures : ctx->tex_cap);
   const bool grow = !base && cap > ctx->tex_cap;
-  l2 = l2 || ctx->d_tex_fdesc;
-  knn = knn || l2 || ctx->d_tex_knn;
-  if (!base && !grow && (!l2 || ctx->d_tex_fdesc) && (!knn || ctx->d_tex_knn)) return M3TB_OK;
+  wide = wide || ctx->d_tex_fdesc;
+  knn = knn || wide || ctx->d_tex_knn;
+  if (!base && !grow && (!wide || ctx->d_tex_fdesc) && (!knn || ctx->d_tex_knn)) return M3TB_OK;
   TexTable<float> fdesc{ctx->d_tex_fdesc, nb, kTexMaxFloatDesc};
   TexTable<float> kf_fdesc{ctx->d_tex_kf_fdesc, nb * K, kTexMaxFloatDesc};
   TexTable<int> knn_t{ctx->d_tex_knn, nb * K, 1};
@@ -4414,8 +4420,8 @@ int EnsureTextureTables(m3tb_ctx* ctx, bool l2, bool knn, int cap) {
   TexTable<uint32_t> kf_desc{ctx->d_tex_kf_desc, nb * K, kTexDescWords};
   TexTable<float> kf_points{ctx->d_tex_kf_points, nb * K * 3, 1};
   TexTable<float> points{ctx->d_tex_points, nb * TF_COUNT, K};
-  CU(fdesc.make(l2, grow, cap));
-  CU(kf_fdesc.make(l2, grow, cap));
+  CU(fdesc.make(wide, grow, cap));
+  CU(kf_fdesc.make(wide, grow, cap));
   CU(knn_t.make(knn, grow, cap));
   CU(xy.make(true, grow, cap));
   CU(desc.make(true, grow, cap));
@@ -4529,7 +4535,7 @@ int SyncTextureFeatures(m3tb_ctx* ctx) {
 
 // k_texture_keyframe (keyframe = true) or k_texture_match over every body, or over the refined texture bodies while a
 // refinement runs; mode as TextureArgs::mode. Matching (mode 1) first runs k_texture_knn_l2 when an L2 body has keyframe
-// descriptors to match.
+// descriptors to match, and k_texture_knn_hamming once for every TexHammingKnn body.
 int LaunchTexture(m3tb_ctx* ctx, bool keyframe, int mode) {
   const RefineSelection* sel = ctx->refine;
   if (ctx->n_texture == 0 || (sel && sel->n_texture == 0)) return M3TB_OK;
@@ -4559,16 +4565,17 @@ int LaunchTexture(m3tb_ctx* ctx, bool keyframe, int mode) {
   a.cap = ctx->tex_cap;
   a.list = sel ? sel->texture : nullptr;
   const int n_launch = sel ? sel->n_texture : ctx->n_bodies;
-  // the longest descriptor, deque and n_features_max of the L2 bodies and of the ORB bodies matched by kNN
-  int l2_length = 0, l2_keyframes = 0, l2_features = 0, ham_keyframes = 0, ham_features = 0;
+  // the widest row, longest deque and largest n_features_max of the L2 bodies and of the Hamming bodies matched by kNN
+  int l2_length = 0, l2_keyframes = 0, l2_features = 0, ham_words = 0, ham_keyframes = 0, ham_features = 0;
   for (int k = 0; k < n_launch; ++k) {
     const BodyDev& B = ctx->h_bodies[sel ? sel->texture_ids[k] : k];
     if (!B.set || !B.has_texture) continue;
-    if (B.tp.l2) {
-      l2_length = std::max(l2_length, B.tp.descriptor_length);
+    if (!TexHamming(B.tp.descriptor_type)) {
+      l2_length = std::max(l2_length, TexRowWords(B.tp));
       l2_keyframes = std::max(l2_keyframes, B.tp.n_keyframes);
       l2_features = std::max(l2_features, B.tp.n_features_max);
     } else if (TexHammingKnn(B.tp)) {
+      ham_words = std::max(ham_words, TexRowWords(B.tp));
       ham_keyframes = std::max(ham_keyframes, B.tp.n_keyframes);
       ham_features = std::max(ham_features, B.tp.n_features_max);
     }
@@ -4582,7 +4589,7 @@ int LaunchTexture(m3tb_ctx* ctx, bool keyframe, int mode) {
   }
   if (!keyframe && mode == 1 && ham_features > 0) {
     const dim3 grid(kKnnSplits * ham_keyframes * KnnTilesPerKeyframe(ham_features), n_launch);
-    k_texture_knn_hamming<<<grid, kKnnThreads, KnnSharedBytes(kTexDescWords), ctx->stream>>>(a);
+    k_texture_knn_hamming<<<grid, kKnnThreads, KnnSharedBytes(ham_words), ctx->stream>>>(a);
     CU(cudaGetLastError());
     ctx->launches++;
   }
@@ -4702,9 +4709,19 @@ int m3tb_set_texture_modality(m3tb_ctx* ctx, int body, const m3tb_texture_params
     return M3TB_OK;
   }
   const m3tb_texture_params& p = *params;
-  const bool l2 = p.descriptor_type == M3TB_DESCRIPTOR_SIFT || p.descriptor_type == M3TB_DESCRIPTOR_DAISY;
-  if (p.descriptor_type != M3TB_DESCRIPTOR_ORB && !l2)
-    return Fail(ctx, M3TB_ERR_UNSUPPORTED, "only DescriptorType::ORB (NORM_HAMMING), SIFT and DAISY (NORM_L2) are implemented");
+  if (p.descriptor_type != M3TB_DESCRIPTOR_ORB && p.descriptor_type != M3TB_DESCRIPTOR_BRISK &&
+      p.descriptor_type != M3TB_DESCRIPTOR_FREAK && p.descriptor_type != M3TB_DESCRIPTOR_SIFT &&
+      p.descriptor_type != M3TB_DESCRIPTOR_DAISY)
+    return Fail(ctx, M3TB_ERR_UNSUPPORTED,
+                "only DescriptorType::ORB, BRISK, FREAK (NORM_HAMMING), SIFT and DAISY (NORM_L2) are implemented");
+  // m3tb_upload_texture_features and m3tb_get_texture_keyframes take no row width: the body's type sets it. A body's
+  // modality therefore moves between the 64-byte types and the others only through its removal (NULL params), so that
+  // the same calls on the same body never read or write the caller's buffers at a width they were not sized for.
+  const auto binary64 = [](int type) { return TexHamming(type) && TexWideRows(type); };
+  if (B.has_texture && binary64(B.tp.descriptor_type) != binary64(p.descriptor_type))
+    return Fail(ctx, M3TB_ERR_UNSUPPORTED, std::string("the body's texture modality is ") +
+                                               DescriptorName(B.tp.descriptor_type) + ": remove it before setting " +
+                                               DescriptorName(p.descriptor_type));
   if (p.n_keyframes > kTexMaxKeyframes) return Fail(ctx, M3TB_ERR_UNSUPPORTED, "n_keyframes above 8");
   if (p.n_features_max > kTexFeatureLimit) return Fail(ctx, M3TB_ERR_UNSUPPORTED, "n_features_max above 4096");
   if (p.n_features_max < kTexMaxFeatures) return Fail(ctx, M3TB_ERR_INVALID, "n_features_max below 512");
@@ -4723,7 +4740,7 @@ int m3tb_set_texture_modality(m3tb_ctx* ctx, int body, const m3tb_texture_params
     return Fail(ctx, M3TB_ERR_INVALID, "measure_occlusions needs the body's depth camera");
   if (!ctx->h_geometry[body].set)
     return Fail(ctx, M3TB_ERR_INVALID, "the texture modality needs the body's geometry (m3tb_set_body_geometry)");
-  int rc = EnsureTextureTables(ctx, l2, !l2 && p.n_features_max > kTexMaxFeatures, p.n_features_max);
+  int rc = EnsureTextureTables(ctx, TexWideRows(p.descriptor_type), p.n_features_max > kTexMaxFeatures, p.n_features_max);
   if (rc) return rc;
   CU(cudaStreamSynchronize(ctx->stream));  // a launch in flight may still read this body's keyframes
   CU(cudaMemsetAsync(ctx->d_tex_kf_state + body, 0, sizeof(TexKeyframeState), ctx->stream));
@@ -4745,9 +4762,8 @@ int m3tb_set_texture_modality(m3tb_ctx* ctx, int body, const m3tb_texture_params
   t.model_occlusions = p.model_occlusions ? 1 : 0;
   t.modeled_occlusion_radius = p.modeled_occlusion_radius;
   t.modeled_occlusion_threshold = p.modeled_occlusion_threshold;
-  t.l2 = l2 ? 1 : 0;
   t.descriptor_type = p.descriptor_type;
-  t.descriptor_length = 0;  // the next upload fixes it
+  t.descriptor_length = 0;  // SIFT / DAISY: the next upload fixes it
   t.n_features_max = p.n_features_max;
   if (B.has_texture && B.texture_camera != color_camera)  // renderers of the old camera no longer fit
     for (int slot = RS_TEXTURE_SILHOUETTE; slot < RS_COUNT; ++slot)
@@ -4785,8 +4801,8 @@ int m3tb_get_texture_focus(m3tb_ctx* ctx, int first, int count, int32_t* roi, fl
 
 namespace {
 
-// m3tb_upload_texture_features (l2 false: 32-byte rows) and m3tb_upload_texture_float_features (l2 true: rows of
-// `length` floats)
+// m3tb_upload_texture_features (l2 false: binary rows of the body's width) and m3tb_upload_texture_float_features
+// (l2 true: rows of `length` floats)
 int UploadTextureFeatures(m3tb_ctx* ctx, int body, const float* keypoints_xy, const void* descriptors, bool l2, int n,
                           int length, int roi_x, int roi_y, float scale) {
   int rc = CheckTextureBody(ctx, body);
@@ -4797,9 +4813,9 @@ int UploadTextureFeatures(m3tb_ctx* ctx, int body, const float* keypoints_xy, co
     return Fail(ctx, M3TB_ERR_INVALID, "bad feature arguments");
   TextureParamsDev& tp = ctx->h_bodies[body].tp;
   const float* float_descriptors = static_cast<const float*>(descriptors);
-  if (l2 != (tp.l2 != 0))
-    return Fail(ctx, M3TB_ERR_INVALID, tp.l2 ? "SIFT / DAISY descriptors are uploaded as floats"
-                                             : "ORB descriptors are uploaded as 32-byte rows");
+  if (l2 == TexHamming(tp.descriptor_type))
+    return Fail(ctx, M3TB_ERR_INVALID, l2 ? "ORB, BRISK and FREAK descriptors are uploaded as binary rows"
+                                          : "SIFT / DAISY descriptors are uploaded as floats");
   if (l2) {
     if (tp.descriptor_type == M3TB_DESCRIPTOR_SIFT ? length != 128 : (length < 1 || length > kTexMaxFloatDesc))
       return Fail(ctx, M3TB_ERR_INVALID, "descriptor length: 128 for SIFT, 1 .. 256 for DAISY");
@@ -4818,10 +4834,11 @@ int UploadTextureFeatures(m3tb_ctx* ctx, int body, const float* keypoints_xy, co
     const size_t cap = size_t(ctx->tex_cap);
     CU(cudaMemcpyAsync(ctx->d_tex_xy + size_t(body) * cap, xy.data(), sizeof(float2) * n, cudaMemcpyHostToDevice,
                        ctx->stream));
-    if (l2)
-      CU(cudaMemcpy2DAsync(ctx->d_tex_fdesc + size_t(body) * cap * kTexMaxFloatDesc,
-                           sizeof(float) * kTexMaxFloatDesc, float_descriptors, sizeof(float) * length,
-                           sizeof(float) * length, n, cudaMemcpyHostToDevice, ctx->stream));
+    // a row is `length` floats or the binary width of the body's type, copied bit for bit
+    const size_t row = l2 ? sizeof(float) * length : sizeof(uint32_t) * TexRowWords(tp);
+    if (TexWideRows(tp.descriptor_type))
+      CU(cudaMemcpy2DAsync(ctx->d_tex_fdesc + size_t(body) * cap * kTexMaxFloatDesc, sizeof(float) * kTexMaxFloatDesc,
+                           descriptors, row, row, n, cudaMemcpyHostToDevice, ctx->stream));
     else
       CU(cudaMemcpyAsync(ctx->d_tex_desc + size_t(body) * cap * kTexDescWords, descriptors, size_t(32) * n,
                          cudaMemcpyHostToDevice, ctx->stream));
@@ -4924,16 +4941,16 @@ int m3tb_upload_texture_features_device(m3tb_ctx* ctx, const int* bodies, const 
       return Fail(ctx, M3TB_ERR_INVALID, "bad feature arguments");
     const TextureParamsDev& tp = ctx->h_bodies[b].tp;
     const bool l2 = f.length != 0;
-    if (l2 != (tp.l2 != 0))
-      return Fail(ctx, M3TB_ERR_INVALID, tp.l2 ? "SIFT / DAISY descriptors are uploaded as floats"
-                                               : "ORB descriptors are uploaded as 32-byte rows");
+    if (l2 == TexHamming(tp.descriptor_type))
+      return Fail(ctx, M3TB_ERR_INVALID, l2 ? "ORB, BRISK and FREAK descriptors are binary rows (length 0)"
+                                            : "SIFT / DAISY descriptors are uploaded as floats");
     if (l2) {
       if (tp.descriptor_type == M3TB_DESCRIPTOR_SIFT ? f.length != 128 : (f.length < 1 || f.length > kTexMaxFloatDesc))
         return Fail(ctx, M3TB_ERR_INVALID, "descriptor length: 128 for SIFT, 1 .. 256 for DAISY");
       if (tp.descriptor_length != 0 && f.length != tp.descriptor_length)
         return Fail(ctx, M3TB_ERR_INVALID, "descriptor length differs from the first upload's");
     }
-    const size_t row = l2 ? sizeof(float) * size_t(f.length) : 32;
+    const size_t row = l2 ? sizeof(float) * size_t(f.length) : sizeof(uint32_t) * TexRowWords(tp);
     if (f.n > 1 && f.descriptor_pitch < row) return Fail(ctx, M3TB_ERR_INVALID, "descriptor pitch smaller than a row");
     if (l2 && ((reinterpret_cast<uintptr_t>(f.descriptors) | f.descriptor_pitch) & 3))
       return Fail(ctx, M3TB_ERR_INVALID, "float descriptors not aligned to 4 bytes");
@@ -4972,7 +4989,10 @@ int m3tb_upload_texture_features_device(m3tb_ctx* ctx, const int* bodies, const 
       j.roi_x = c.roi_x;
       j.roi_y = c.roi_y;
       j.scale = c.scale;
-      j.pad = 0;
+      const TextureParamsDev& tp = ctx->h_bodies[j.body].tp;
+      j.words = TexRowWords(tp);
+      j.wide = TexWideRows(tp.descriptor_type) ? 1 : 0;
+      j.pad[0] = j.pad[1] = j.pad[2] = 0;
     }
     k_texture_features<<<a.n_jobs, kTexThreads, 0, ctx->stream>>>(a);
     CU(cudaGetLastError());
@@ -5287,12 +5307,12 @@ int m3tb_get_texture_keyframes(m3tb_ctx* ctx, int body, int* n_keyframes, int* s
   if (capacity < 0) return Fail(ctx, M3TB_ERR_INVALID, "bad capacity");
   TexKeyframeState st;
   const TextureParamsDev& tp = ctx->h_bodies[body].tp;
-  // a descriptor is `width` bytes in rows of `stride` words: 32 of 8 for ORB, 4 * length of kTexMaxFloatDesc for L2
-  const int stride = tp.l2 ? kTexMaxFloatDesc : kTexDescWords;
-  const size_t width = tp.l2 ? sizeof(float) * tp.descriptor_length : 32;
+  // a descriptor is `width` bytes in rows of `stride` words (m3t_b200_texture.cuh)
+  const size_t stride = TexRowStride(tp), width = sizeof(uint32_t) * TexRowWords(tp);
   const size_t cap = size_t(ctx->tex_cap);
   std::vector<int> kn(kTexMaxKeyframes);
-  const uint32_t* kd_src = tp.l2 ? reinterpret_cast<const uint32_t*>(ctx->d_tex_kf_fdesc.get()) : ctx->d_tex_kf_desc.get();
+  const uint32_t* kd_src = TexWideRows(tp.descriptor_type) ? reinterpret_cast<const uint32_t*>(ctx->d_tex_kf_fdesc.get())
+                                                           : ctx->d_tex_kf_desc.get();
   CU(cudaMemcpyAsync(&st, ctx->d_tex_kf_state + body, sizeof(st), cudaMemcpyDeviceToHost, ctx->stream));
   CU(cudaMemcpyAsync(kn.data(), ctx->d_tex_kf_n + body * kTexMaxKeyframes, sizeof(int) * kn.size(), cudaMemcpyDeviceToHost,
                      ctx->stream));

@@ -175,13 +175,14 @@ struct TextureParamsDev {
   float measured_occlusion_radius, measured_occlusion_threshold;
   int model_occlusions;
   float modeled_occlusion_radius, modeled_occlusion_threshold;
-  // l2 0: 32-byte binary descriptors (ORB, NORM_HAMMING); 1: float descriptors (SIFT / DAISY, NORM_L2) of
-  // descriptor_length floats, fixed by the first upload after m3tb_set_texture_modality (0 before it)
-  int descriptor_type, l2, descriptor_length;
+  // descriptor_type: M3TB_DESCRIPTOR_*, whose table, row width and distance m3t_b200_texture.cuh states (TexWideRows,
+  // TexRowWords, TexHamming); descriptor_length: the floats of a SIFT / DAISY descriptor, fixed by the first upload
+  // after m3tb_set_texture_modality (0 before it, and for binary types)
+  int descriptor_type, descriptor_length;
   // m3tb_texture_params::n_features_max: a body above kTexMaxFeatures matches ORB descriptors with
   // k_texture_knn_hamming instead of k_texture_match's in-CTA scan
   int n_features_max;
-  int pad[3];  // keeps BodyDev::rend 16-byte aligned
+  int pad[4];  // keeps BodyDev::rend 16-byte aligned
 };
 
 struct BodyDev {

@@ -1,6 +1,6 @@
-// m3t_b200_texture.cu — k_texture_keyframe, k_texture_knn_l2 and k_texture_match (TextureModality,
+// m3t_b200_texture.cu — k_texture_keyframe, k_texture_knn_l2 / _hamming and k_texture_match (TextureModality,
 // texture_modality.cpp). k_texture_keyframe / k_texture_match: one CTA of kTexThreads threads per body;
-// k_texture_knn_l2: clusters over a body's queries (m3t_b200_texture.cuh). Bodies without a texture modality return
+// the kNN kernels: clusters over a body's queries (m3t_b200_texture.cuh). Bodies without a texture modality return
 // at once.
 #include <cfloat>
 #include <climits>
@@ -162,15 +162,14 @@ __global__ void __launch_bounds__(kTexThreads) k_texture_keyframe(const __grid_c
   const int n = a.feat_n[b];
   const size_t cap = size_t(a.cap);
   const float2* xy = a.feat_xy + size_t(b) * cap;
-  // a descriptor is `words` 32-bit words in rows of `stride`: 8 of 8 for ORB, descriptor_length floats of
-  // kTexMaxFloatDesc for SIFT / DAISY
-  const bool l2 = tp.l2 != 0;
-  const int words = l2 ? tp.descriptor_length : kTexDescWords, stride = l2 ? kTexMaxFloatDesc : kTexDescWords;
-  const uint32_t* desc = l2 ? reinterpret_cast<const uint32_t*>(a.feat_fdesc) : a.feat_desc;
+  // a descriptor is TexRowWords 32-bit words, copied as words (binary or float alike) in rows of TexRowStride
+  const bool wide = TexWideRows(tp.descriptor_type);
+  const int words = TexRowWords(tp), stride = int(TexRowStride(tp));
+  const uint32_t* desc = wide ? reinterpret_cast<const uint32_t*>(a.feat_fdesc) : a.feat_desc;
   desc += size_t(b) * cap * stride;
   const int slot = s_slot;
   float* kp = a.kf_points + (size_t(b) * kTexMaxKeyframes + slot) * 3 * cap;
-  uint32_t* kd = l2 ? reinterpret_cast<uint32_t*>(a.kf_fdesc) : a.kf_desc;
+  uint32_t* kd = wide ? reinterpret_cast<uint32_t*>(a.kf_fdesc) : a.kf_desc;
   kd += (size_t(b) * kTexMaxKeyframes + slot) * cap * stride;
   int written = 0;
   for (int i0 = 0; i0 < n; i0 += kTexThreads) {
@@ -266,7 +265,7 @@ __device__ __forceinline__ void StageRows(const uint32_t* src, size_t src_stride
 }
 
 // The distance sums of one (query, train) pair over four 32-bit words: L2, float descriptors: squared differences
-// in descriptor order; Hamming, 32-byte binary descriptors: bits that differ
+// in descriptor order; Hamming, binary descriptors: bits that differ
 template <bool kHamming>
 __device__ __forceinline__ void KnnAccumulate(const uint4& q, const uint4& t, float& acc) {
   if constexpr (kHamming) {
@@ -287,14 +286,16 @@ __device__ __forceinline__ void KnnAccumulate(const uint4& q, const uint4& t, fl
 // frame's train set. Each thread holds a 4 x 4 block of (query, train) sums, queries ty + 16 i and train rows tx + 16 j
 // of the CTA's slice of a chunk, and a running top-2 list per query over its train rows in increasing index: the
 // insertion of cv::batchDistance. The lists of the 16 lanes sharing a query and then of the cluster's CTAs are merged
-// under (distance, train index) order, which is what that insertion gives over the union.
-template <bool kHamming>
-__device__ __forceinline__ void KnnTile(const TextureArgs& a) {
+// under (distance, train index) order, which is what that insertion gives over the union. kWords: the body's
+// TexRowWords as a constant of the inner loop (the caller has checked it), 0 for a width known at run time only.
+template <bool kHamming, int kWords>
+__device__ __forceinline__ void KnnTile(const TextureArgs& a, int b) {
   namespace cg = cooperative_groups;
-  const int b = a.list ? a.list[blockIdx.y] : int(blockIdx.y), tid = threadIdx.x;
+  const int tid = threadIdx.x;
   const BodyDev& body = a.bodies[b];
   // every return before the first cluster barrier depends on (body, tile) alone: a cluster leaves or stays whole
-  if (!body.set || !body.has_texture || (kHamming ? !TexHammingKnn(body.tp) : !body.tp.l2)) return;
+  if (!body.set || !body.has_texture || (kHamming ? !TexHammingKnn(body.tp) : TexHamming(body.tp.descriptor_type)))
+    return;
   const int rank = blockIdx.x % kKnnSplits, tile = blockIdx.x / kKnnSplits;
   const int tiles = KnnTilesPerKeyframe(body.tp.n_features_max);
   const int k = tile / tiles, q0 = tile % tiles * kKnnQueries;
@@ -304,10 +305,11 @@ __device__ __forceinline__ void KnnTile(const TextureArgs& a) {
   const int nq = min(kKnnQueries, a.kf_n[b * kTexMaxKeyframes + slot] - q0);
   if (nq <= 0) return;
   // rows of `length` words, `src_stride` words apart in the tables
-  const int length = kHamming ? kTexDescWords : body.tp.descriptor_length, stride = KnnStride(length);
-  const size_t src_stride = kHamming ? kTexDescWords : kTexMaxFloatDesc, cap = size_t(a.cap);
-  const uint32_t* kf_rows = kHamming ? a.kf_desc : reinterpret_cast<const uint32_t*>(a.kf_fdesc);
-  const uint32_t* feat_rows = kHamming ? a.feat_desc : reinterpret_cast<const uint32_t*>(a.feat_fdesc);
+  const int length = kWords ? kWords : TexRowWords(body.tp), stride = KnnStride(length);
+  const size_t src_stride = TexRowStride(body.tp), cap = size_t(a.cap);
+  const bool wide = TexWideRows(body.tp.descriptor_type);
+  const uint32_t* kf_rows = wide ? reinterpret_cast<const uint32_t*>(a.kf_fdesc) : a.kf_desc;
+  const uint32_t* feat_rows = wide ? reinterpret_cast<const uint32_t*>(a.feat_fdesc) : a.feat_desc;
   const int n_train = a.feat_n[b];
   extern __shared__ uint4 s_dyn[];
   uint32_t* s_q = reinterpret_cast<uint32_t*>(s_dyn);
@@ -383,21 +385,26 @@ __device__ __forceinline__ void KnnTile(const TextureArgs& a) {
 // integer below 2^24, so any order gives OpenCV's distance bit for bit (DESIGN.md section 3).
 __global__ void __cluster_dims__(kKnnSplits, 1, 1) __launch_bounds__(kKnnThreads)
     k_texture_knn_l2(const __grid_constant__ TextureArgs a) {
-  KnnTile<false>(a);
+  KnnTile<false, 0>(a, a.list ? a.list[blockIdx.y] : int(blockIdx.y));
 }
 
-// cv::BFMatcher(NORM_HAMMING).knnMatch(k = 2) and the ratio test for every ORB body whose n_features_max is above
-// kTexMaxFeatures, at correspondence iteration 0. Distances are bit counts, exact as floats.
-__global__ void __cluster_dims__(kKnnSplits, 1, 1) __launch_bounds__(kKnnThreads)
+// cv::BFMatcher(NORM_HAMMING).knnMatch(k = 2) and the ratio test for every TexHammingKnn body (ORB above
+// kTexMaxFeatures, BRISK, FREAK), at correspondence iteration 0. Distances are bit counts, exact as floats. The row
+// width is the CTA's body's, the same for the whole cluster (grid y), and a constant of each inner loop. Three CTAs
+// per SM, as before 16-word rows: unbounded, their unrolled loop takes 127 registers, and every body of the launch,
+// ORB's included, would run at two.
+__global__ void __cluster_dims__(kKnnSplits, 1, 1) __launch_bounds__(kKnnThreads, 3)
     k_texture_knn_hamming(const __grid_constant__ TextureArgs a) {
-  KnnTile<true>(a);
+  const int b = a.list ? a.list[blockIdx.y] : int(blockIdx.y);
+  if (TexRowWords(a.bodies[b].tp) == kTexBinary64Words) KnnTile<true, kTexBinary64Words>(a, b);
+  else KnnTile<true, kTexDescWords>(a, b);
 }
 
 // CalculateCorrespondences (texture_modality.cpp:322-386): with mode 1 (correspondence iteration 0) every keyframe's
 // descriptors (queries) are matched against the frame's (train set) by brute-force kNN, k = 2, and the matches that pass
 // the ratio test become the data points, keyframe by keyframe in query order. ORB bodies up to kTexMaxFeatures are
-// matched here (Hamming, the train set in shared memory); k_texture_knn_l2 / _hamming have matched the others just
-// before. Every call then projects the data points with the current pose (data_point.center) and records that pose.
+// matched here (Hamming, the train set in shared memory); k_texture_knn_l2 / _hamming have matched the others, BRISK
+// and FREAK bodies always, just before. Every call then projects the data points with the current pose (data_point.center) and records that pose.
 __global__ void __launch_bounds__(kTexThreads) k_texture_match(const __grid_constant__ TextureArgs a) {
   const int b = a.list ? a.list[blockIdx.x] : int(blockIdx.x), tid = threadIdx.x;
   const BodyDev& body = a.bodies[b];
@@ -409,7 +416,7 @@ __global__ void __launch_bounds__(kTexThreads) k_texture_match(const __grid_cons
   const CameraDev& cam = a.color_cams[body.texture_camera];
   if (a.mode == 1) {
     const int n_train = a.feat_n[b];
-    const bool knn_matched = body.tp.l2 != 0 || TexHammingKnn(body.tp);
+    const bool knn_matched = !TexHamming(body.tp.descriptor_type) || TexHammingKnn(body.tp);
     const uint4* train = reinterpret_cast<const uint4*>(a.feat_desc + size_t(b) * cap * kTexDescWords);
     if (!knn_matched)
       for (int k = tid; k < 2 * n_train; k += kTexThreads) s_train[k] = train[k];
@@ -555,7 +562,8 @@ __global__ void __launch_bounds__(kTexCropThreads) k_texture_crop(const __grid_c
 }
 
 // The host upload's conversion (UploadTextureFeatures): keypoint roi + pt / scale, descriptors into the frame tables.
-// Float descriptors are checked here: a body with a non-finite value gets no features and its flag is raised.
+// Float descriptors are checked here: a body with a non-finite value gets no features and its flag is raised. Binary
+// rows are copied byte by byte, never read as floats.
 __global__ void __launch_bounds__(kTexThreads) k_texture_features(const __grid_constant__ TexFeatArgs a) {
   const TexFeatJob& j = a.jobs[blockIdx.x];
   const int tid = threadIdx.x, b = j.body;
@@ -567,10 +575,13 @@ __global__ void __launch_bounds__(kTexThreads) k_texture_features(const __grid_c
   }
   int bad = 0;
   if (j.length == 0) {
-    uint32_t* dst = a.feat_desc + size_t(b) * cap * kTexDescWords;
-    for (int e = tid; e < j.n * 32; e += kTexThreads) {  // byte by byte: the caller's rows need no alignment
-      const int i = e >> 5, c = e & 31;
-      reinterpret_cast<uint8_t*>(dst)[e] = j.desc[size_t(i) * j.desc_pitch + c];
+    const size_t stride = j.wide ? kTexMaxFloatDesc : kTexDescWords;
+    uint8_t* dst = reinterpret_cast<uint8_t*>((j.wide ? reinterpret_cast<uint32_t*>(a.feat_fdesc) : a.feat_desc) +
+                                              size_t(b) * cap * stride);
+    const int width = 4 * j.words;
+    for (int e = tid; e < j.n * width; e += kTexThreads) {  // byte by byte: the caller's rows need no alignment
+      const int i = e / width, c = e - i * width;
+      dst[size_t(i) * 4 * stride + c] = j.desc[size_t(i) * j.desc_pitch + c];
     }
   } else {
     float* dst = a.feat_fdesc + size_t(b) * cap * kTexMaxFloatDesc;

@@ -1,10 +1,11 @@
 // m3t_b200_texture.cuh — TextureModality on the device (texture_modality.cpp): keyframe reconstruction from the device
-// silhouette renderer, brute-force kNN matching (Hamming for ORB's 32-byte descriptors, L2 for SIFT / DAISY float
-// descriptors), and the Tukey-weighted reprojection gradient / Hessian that k_track adds to a body's link. Feature
-// detection stays with the caller, or for ORB bodies runs in k_texture_orb (m3t_b200_orb.cu); the keypoints in image
-// coordinates and the descriptors are all the matching kernels read of the colour frame.
+// silhouette renderer, brute-force kNN matching (Hamming for ORB's 32-byte and BRISK / FREAK's 64-byte descriptors,
+// L2 for SIFT / DAISY float descriptors), and the Tukey-weighted reprojection gradient / Hessian that k_track adds to a
+// body's link. Feature detection stays with the caller, or for ORB bodies runs in k_texture_orb (m3t_b200_orb.cu); the
+// keypoints in image coordinates and the descriptors are all the matching kernels read of the colour frame.
 #pragma once
 
+#include "m3t_b200.h"  // M3TB_DESCRIPTOR_*
 #include "m3t_b200_device.cuh"
 
 namespace m3tb {
@@ -12,12 +13,12 @@ namespace m3tb {
 // Frame features per body: n_features_max, kTexMaxFeatures (the default) .. kTexFeatureLimit. The tables of a context
 // hold TextureArgs::cap features per body, the largest n_features_max any of its texture bodies has asked for.
 // k_texture_match stages an ORB body's train set in shared memory up to kTexMaxFeatures; ORB bodies above it and every
-// L2 body are matched by the cluster kNN kernels below.
+// BRISK, FREAK and L2 body are matched by the cluster kNN kernels below.
 constexpr int kTexMaxFeatures = 512;
 constexpr int kTexFeatureLimit = 4096;
 constexpr int kTexMaxKeyframes = 8;    // n_keyframes
 constexpr int kTexDescWords = 8;       // 32-byte ORB descriptors
-constexpr int kTexMaxFloatDesc = 256;  // float descriptor cap and the stride of the float tables (SIFT 128, DAISY 104)
+constexpr int kTexMaxFloatDesc = 256;  // float descriptor cap and the stride of the wide tables (SIFT 128, DAISY 104)
 constexpr int kTexThreads = 256;
 constexpr int kTexRoiMargin = 10;      // kRegionOfInterestMargin, texture_modality.h:132
 
@@ -39,11 +40,11 @@ struct TextureArgs {
   const CameraDev* depth_cams;
   const float2* feat_xy;        // [n_bodies][cap] keypoints_ in image coordinates
   const uint32_t* feat_desc;    // [n_bodies][cap][8]
-  const float* feat_fdesc;      // [n_bodies][cap][kTexMaxFloatDesc] (L2 bodies; null without any)
+  const float* feat_fdesc;      // [n_bodies][cap][kTexMaxFloatDesc] the wide table (TexWideRows; null without any)
   const int* feat_n;            // [n_bodies]
   float* kf_points;             // [n_bodies][kTexMaxKeyframes][3][cap]
   uint32_t* kf_desc;            // [n_bodies][kTexMaxKeyframes][cap][8]
-  float* kf_fdesc;              // [n_bodies][kTexMaxKeyframes][cap][kTexMaxFloatDesc] (L2 bodies)
+  float* kf_fdesc;              // [n_bodies][kTexMaxKeyframes][cap][kTexMaxFloatDesc] (TexWideRows)
   int* knn;                     // [n_bodies][kTexMaxKeyframes][cap] k_texture_knn_l2 / _hamming: the train index of
                                 // a query's best match that passes the ratio test, -1 otherwise (by keyframe slot)
   int* kf_n;                    // [n_bodies][kTexMaxKeyframes]
@@ -55,21 +56,42 @@ struct TextureArgs {
   const int* list = nullptr;    // the bodies of the launch, one per CTA (grid y for the kNN kernels); null: every body
 };
 
-// k_texture_match reads an ORB body's matches from knn (k_texture_knn_hamming) instead of scanning its train set
+// Where a descriptor type's rows live, how wide they are and how they are matched. Every kernel and host path reads
+// these three facts from here:
+//   type          table                                   words per row                  distance
+//   ORB           feat_desc / kf_desc (kTexDescWords)     kTexDescWords (32 bytes)       Hamming
+//   BRISK, FREAK  feat_fdesc / kf_fdesc (kTexMaxFloatDesc) kTexBinary64Words (64 bytes)  Hamming
+//   SIFT, DAISY   feat_fdesc / kf_fdesc (kTexMaxFloatDesc) descriptor_length floats      L2
+// In parentheses: the words from one row to the next. Binary rows are copied bit for bit and never read as floats.
+constexpr int kTexBinary64Words = 16;
+__host__ __device__ __forceinline__ bool TexWideRows(int type) { return type != M3TB_DESCRIPTOR_ORB; }
+__host__ __device__ __forceinline__ bool TexHamming(int type) {
+  return type == M3TB_DESCRIPTOR_ORB || type == M3TB_DESCRIPTOR_BRISK || type == M3TB_DESCRIPTOR_FREAK;
+}
+__host__ __device__ __forceinline__ int TexRowWords(const TextureParamsDev& tp) {
+  if (!TexWideRows(tp.descriptor_type)) return kTexDescWords;
+  return TexHamming(tp.descriptor_type) ? kTexBinary64Words : tp.descriptor_length;
+}
+__host__ __device__ __forceinline__ size_t TexRowStride(const TextureParamsDev& tp) {
+  return TexWideRows(tp.descriptor_type) ? kTexMaxFloatDesc : kTexDescWords;
+}
+
+// k_texture_match reads a Hamming body's matches from knn (k_texture_knn_hamming) instead of scanning its train set:
+// ORB above kTexMaxFeatures, every BRISK / FREAK body. k_texture_match stages only 8-word rows.
 __host__ __device__ __forceinline__ bool TexHammingKnn(const TextureParamsDev& tp) {
-  return !tp.l2 && tp.n_features_max > kTexMaxFeatures;
+  return TexHamming(tp.descriptor_type) && (TexWideRows(tp.descriptor_type) || tp.n_features_max > kTexMaxFeatures);
 }
 
 __global__ void k_texture_keyframe(const __grid_constant__ TextureArgs a);
 __global__ void k_texture_match(const __grid_constant__ TextureArgs a);
 
-// k_texture_knn_l2 (SIFT / DAISY bodies) and k_texture_knn_hamming (ORB bodies above kTexMaxFeatures): a cluster of
+// k_texture_knn_l2 (SIFT / DAISY bodies) and k_texture_knn_hamming (TexHammingKnn bodies): a cluster of
 // kKnnSplits CTAs per tile of kKnnQueries queries of one keyframe. The train set is walked in chunks of kKnnChunk rows;
 // CTA r of the cluster scans rows [c * kKnnChunk + r * kKnnTrain, ... + kKnnTrain) of every chunk c and rank 0 merges
 // the partial top-2 lists. Grid: (kKnnSplits * keyframes * KnnTilesPerKeyframe(features), n_bodies), with the longest
 // deque and the largest n_features_max of the bodies the kernel matches (n_bodies: the length of TextureArgs::list when
-// it has one); dynamic shared memory KnnSharedBytes(row
-// length in 32-bit words: the longest descriptor of the context's L2 bodies, kTexDescWords for Hamming).
+// it has one); dynamic shared memory KnnSharedBytes(the widest TexRowWords of the bodies the kernel matches).
+// k_texture_knn_hamming matches 8-word and 16-word rows in one launch, each CTA at its body's width.
 constexpr int kKnnQueries = 64, kKnnTrain = 64, kKnnThreads = 256;
 constexpr int kKnnSplits = 8;                       // the portable cluster size
 constexpr int kKnnChunk = kKnnSplits * kKnnTrain;   // 512 train rows per chunk
@@ -111,12 +133,13 @@ __global__ void k_texture_crop(const __grid_constant__ TexCropArgs a);
 struct TexFeatJob {
   const float* x;        // keypoint i at x[i * xy_stride], y[i * xy_stride] (crop coordinates)
   const float* y;
-  const uint8_t* desc;   // descriptor row i at desc + i * desc_pitch: 32 bytes (ORB) or `length` floats
+  const uint8_t* desc;   // descriptor row i at desc + i * desc_pitch: 4 * words bytes (binary) or `length` floats
   size_t desc_pitch;
-  int body, n, xy_stride, length;  // length 0: ORB
+  int body, n, xy_stride, length;  // length 0: a binary type
   int roi_x, roi_y;
   float scale;
-  int pad;
+  int words;             // TexRowWords of the body; its rows are TexRowStride words apart in the table of TexWideRows
+  int wide, pad[3];
 };
 
 struct TexFeatArgs {

@@ -1449,7 +1449,8 @@ class DepthModality : public Modality {
 // No OpenCV here. For ORB bodies DetectFeatures runs DetectAndComputeCorrKeypoints on the device (cv::ORB at the
 // orb_* settings, m3tb_texture_detect_orb). Otherwise the caller asks for the body's focus region with CalculateFocus,
 // detects features in the cropped and scaled grey image and hands them over with SetFeatures, once per frame.
-// DescriptorType ORB (32-byte descriptors), SIFT and DAISY (float descriptors) are implemented.
+// DescriptorType ORB (32-byte descriptors), BRISK and FREAK (64-byte descriptors), SIFT and DAISY (float descriptors)
+// are implemented; ORB_CUDA is not.
 class TextureModality : public Modality {
  public:
   enum class DescriptorType { BRISK = 0, DAISY = 1, FREAK = 2, SIFT = 3, ORB = 4, ORB_CUDA = 5 };  // texture_modality.h
@@ -1500,6 +1501,10 @@ class TextureModality : public Modality {
   void set_n_features_max(int v) { params_.n_features_max = v; set_up_ = false; }
   int n_features_max() const { return params_.n_features_max; }
   DescriptorType descriptor_type() const { return descriptor_type_; }
+  static const char* DescriptorName(DescriptorType type) {
+    static const char* const names[] = {"BRISK", "DAISY", "FREAK", "SIFT", "ORB", "ORB_CUDA"};
+    return int(type) >= 0 && int(type) < 6 ? names[int(type)] : "unknown";
+  }
   const m3tb_texture_params& params() const { return params_; }
   const std::shared_ptr<ColorCamera>& color_camera_ptr() const { return color_camera_ptr_; }
   const std::shared_ptr<DepthCamera>& depth_camera_ptr() const { return depth_camera_ptr_; }
@@ -1509,9 +1514,8 @@ class TextureModality : public Modality {
   // TextureModality::SetUp (texture_modality.cpp:39-88); the body's device record is written by Optimizer::SetUp
   bool SetUp() override {
     set_up_ = false;
-    if (descriptor_type_ != DescriptorType::ORB && descriptor_type_ != DescriptorType::SIFT &&
-        descriptor_type_ != DescriptorType::DAISY) {
-      std::cerr << "Modality " << name_ << ": only DescriptorType::ORB, SIFT and DAISY are implemented" << std::endl;
+    if (descriptor_type_ == DescriptorType::ORB_CUDA) {
+      std::cerr << "Modality " << name_ << ": DescriptorType::ORB_CUDA is not implemented" << std::endl;
       return false;
     }
     if (!silhouette_renderer_ptr_) {
@@ -1556,13 +1560,15 @@ class TextureModality : public Modality {
       return false;
     return valid != 0;
   }
-  // SetFeatures: the keypoints (x, y in crop coordinates, keypoints_xy[2 n]) and 32-byte ORB descriptors
-  // (descriptors[32 n]) detected in the crop of CalculateFocus
+  // SetFeatures: the keypoints (x, y in crop coordinates, keypoints_xy[2 n]) and binary descriptors detected in the
+  // crop of CalculateFocus: 32 bytes each for ORB (descriptors[32 n]), 64 for BRISK and FREAK (descriptors[64 n])
   bool SetFeatures(const std::vector<float>& keypoints_xy, const std::vector<uint8_t>& descriptors,
                    const std::array<int32_t, 4>& roi, float scale) {
     const int n = int(keypoints_xy.size() / 2);
-    if (descriptors.size() != size_t(32) * n) {
-      std::cerr << "Modality " << name_ << ": one 32-byte descriptor per keypoint" << std::endl;
+    const size_t width = descriptor_type_ == DescriptorType::BRISK || descriptor_type_ == DescriptorType::FREAK ? 64 : 32;
+    if (descriptors.size() != width * n) {
+      std::cerr << "Modality " << name_ << ": one " << width << "-byte " << DescriptorName(descriptor_type_)
+                << " descriptor per keypoint" << std::endl;
       return false;
     }
     return Check(batch_->ctx(),
@@ -1660,7 +1666,8 @@ class TextureModality : public Modality {
     for (auto& m : modalities) {
       if (!m->IsSetup()) return false;
       if (m->descriptor_type_ != DescriptorType::ORB) {
-        std::cerr << "Modality " << m->name_ << ": DetectFeatures runs cv::ORB; its descriptor type is not ORB"
+        std::cerr << "Modality " << m->name_ << ": DetectFeatures runs cv::ORB; its descriptor type is "
+                  << DescriptorName(m->descriptor_type_)
                   << std::endl;
         return false;
       }
@@ -2291,7 +2298,9 @@ class Refiner {
           if (auto t = std::dynamic_pointer_cast<TextureModality>(m)) {
             if (t->descriptor_type() != TextureModality::DescriptorType::ORB) {
               std::cerr << "Modality " << t->name() << ": only ORB features are detected on the device between the "
-                        << "correspondence iterations; optimizer " << o->name() << " cannot be refined" << std::endl;
+                        << "correspondence iterations, its descriptor type is "
+                        << TextureModality::DescriptorName(t->descriptor_type()) << "; optimizer " << o->name()
+                        << " cannot be refined" << std::endl;
               return false;
             }
             texture.emplace_back(t->body_ptr()->index(), t->orb_params());

@@ -1,14 +1,15 @@
 // texture_mirror_tracker.cpp — drives the C++ mirror's TextureModality on a seeded synthetic scene: one rigid body and
 // one 3-link chain (root with 6 DoF, revolute-x children at Tx(0.01)), every body with region, depth and texture
 // modalities on its own RGB-D pair and its own focused silhouette renderer. The features a detector would find are
-// generated here from a seed: points on the prism's mid-plane with random 32-byte descriptors (orb) or 128
-// whole-number floats in 0 .. 255, as cv::SIFT writes them (sift), seen at the start pose for StartModality and at the
+// generated here from a seed: points on the prism's mid-plane with random 32-byte descriptors (orb), 64-byte
+// descriptors (brisk, matched through k_texture_knn_hamming at every n_features_max) or 128 whole-number floats in
+// 0 .. 255, as cv::SIFT writes them (sift), seen at the start pose for StartModality and at the
 // ground-truth pose for the tracked frame. The scene is tracked once through Tracker::ExecuteTrackingStep and once
 // through ExecuteTrackingStepObjectWise; both pose sets are printed as JSON for tests/test_gpu_texture_mirror.py and
 // tests/test_gpu_texture_l2.py. Above 512 features per body (up to 4096) every texture modality raises its
 // n_features_max to n_features, so the frame's features are matched in full (k_texture_knn_hamming for orb).
 //
-//   usage: texture_mirror_tracker [seed=1] [n_features=300] [orb|sift]
+//   usage: texture_mirror_tracker [seed=1] [n_features=300] [orb|sift|brisk]
 #include <algorithm>
 #include <array>
 #include <cmath>
@@ -81,10 +82,10 @@ constexpr int kSiftLength = 128;
 // a body's texture: n points on the prism's triangular mid-plane (body frame) and their descriptors
 struct Texture {
   std::vector<float> points;  // [n][3]
-  std::vector<uint8_t> descriptors;  // [n][32] (orb)
+  std::vector<uint8_t> descriptors;  // [n][32] (orb) or [n][64] (brisk)
   std::vector<float> float_descriptors;  // [n][kSiftLength] (sift)
 };
-Texture MakeTexture(uint64_t seed, int body, int n, bool sift) {
+Texture MakeTexture(uint64_t seed, int body, int n, bool sift, int binary_bytes) {
   std::mt19937 rng(uint32_t(seed * 7919u + uint64_t(body)));
   std::uniform_real_distribution<float> u(0.0f, 1.0f);
   std::uniform_int_distribution<int> byte(0, 255);
@@ -98,7 +99,7 @@ Texture MakeTexture(uint64_t seed, int body, int n, bool sift) {
     if (sift)
       for (int k = 0; k < kSiftLength; ++k) t.float_descriptors.push_back(float(byte(rng)));
     else
-      for (int k = 0; k < 32; ++k) t.descriptors.push_back(uint8_t(byte(rng)));
+      for (int k = 0; k < binary_bytes; ++k) t.descriptors.push_back(uint8_t(byte(rng)));
   }
   return t;
 }
@@ -151,6 +152,7 @@ int main(int argc, char** argv) {
   const uint64_t seed = argc > 1 ? std::strtoull(argv[1], nullptr, 10) : 1;
   const int n_features = argc > 2 ? std::atoi(argv[2]) : 300;
   const bool sift = argc > 3 && std::string(argv[3]) == "sift";
+  const bool brisk = argc > 3 && std::string(argv[3]) == "brisk";
   const int n_lines = 200, n_points = 200, n_divides = 2;
   float prism_diameter = 0.0f;
   const std::vector<float> prism = PrismTriangles(&prism_diameter);
@@ -191,7 +193,7 @@ int main(int argc, char** argv) {
     }
     m3ts_render_color(&sci, Mul(color_w2c, gt[b]).data(), seed * 1000003 + b, fg, bg, 10.0f, color[b].data(), cpitch);
     m3ts_render_depth(&sdi, Mul(depth_w2c, gt[b]).data(), seed * 1000003 + b, 1.0f, 0.001f, 0.01f, 0.001f, depth[b].data(), dpitch);
-    textures.push_back(MakeTexture(seed, b, n_features, sift));
+    textures.push_back(MakeTexture(seed, b, n_features, sift, brisk ? 64 : 32));
   }
 
   std::vector<Transform3fA> start;
@@ -225,6 +227,7 @@ int main(int argc, char** argv) {
       dm->set_n_points_max(n_points);
       auto tm = std::make_shared<TextureModality>("texture_modality_" + std::to_string(b), s.batch, body, cc, silhouette);
       if (sift) tm->set_descriptor_type(TextureModality::DescriptorType::SIFT);
+      if (brisk) tm->set_descriptor_type(TextureModality::DescriptorType::BRISK);
       tm->set_n_features_max(std::max(n_features, tm->n_features_max()));
       auto link = std::make_shared<Link>("link_" + std::to_string(b), body);
       link->AddModality(rm);
@@ -268,7 +271,7 @@ int main(int argc, char** argv) {
   if (!fused.tracker->ExecuteTrackingStep(0)) return 3;
   if (!object_wise.tracker->ExecuteTrackingStepObjectWise(0)) return 4;
   std::printf("{\"descriptor\": \"%s\", \"n_bodies\": %d, \"n_features_max\": %d, \"texture_points\": [",
-              sift ? "sift" : "orb", kBodies, fused.textures[0]->n_features_max());
+              sift ? "sift" : brisk ? "brisk" : "orb", kBodies, fused.textures[0]->n_features_max());
   for (int b = 0; b < kBodies; ++b) {
     std::vector<m3tb_texture_point> pts(512);
     int n = 0;

@@ -192,14 +192,16 @@ typedef struct m3tb_depth_point {
 } m3tb_depth_point;
 
 /* Parameters of m3t::TextureModality, defaults texture_modality.h:400-436. DescriptorType::ORB (32-byte binary
- * descriptors, NORM_HAMMING), SIFT (128 floats) and DAISY (1 .. 256 floats, 104 at M3T's defaults), both NORM_L2, are
- * implemented; the detector's own settings stay with the caller, who detects. */
-#define M3TB_DESCRIPTOR_DAISY 1   /* TextureModality::DescriptorType::DAISY, texture_modality.h:153-162 */
+ * descriptors), BRISK and FREAK (64-byte binary descriptors), all NORM_HAMMING, and SIFT (128 floats) and DAISY
+ * (1 .. 256 floats, 104 at M3T's defaults), both NORM_L2, are implemented; the detector's own settings stay with the
+ * caller, who detects. */
+#define M3TB_DESCRIPTOR_BRISK 0   /* TextureModality::DescriptorType::BRISK, texture_modality.h:153-162 */
+#define M3TB_DESCRIPTOR_DAISY 1   /* TextureModality::DescriptorType::DAISY */
+#define M3TB_DESCRIPTOR_FREAK 2   /* TextureModality::DescriptorType::FREAK */
 #define M3TB_DESCRIPTOR_SIFT 3    /* TextureModality::DescriptorType::SIFT */
 #define M3TB_DESCRIPTOR_ORB 4     /* TextureModality::DescriptorType::ORB */
 typedef struct m3tb_texture_params {
-  int32_t descriptor_type;                 /* M3TB_DESCRIPTOR_ORB, _SIFT or _DAISY (BRISK 0, FREAK 2, ORB_CUDA 5:
-                                              M3TB_ERR_UNSUPPORTED) */
+  int32_t descriptor_type;                 /* M3TB_DESCRIPTOR_* (ORB_CUDA 5: M3TB_ERR_UNSUPPORTED) */
   int32_t focused_image_size;              /* 200 */
   float descriptor_distance_threshold;     /* 0.7 */
   float tukey_norm_constant;               /* 20 */
@@ -496,8 +498,9 @@ int m3tb_share_color_histograms(m3tb_ctx* ctx, int body, int owner_body);
  * BGR2GRAY, image(roi), resize by `scale` in both directions), runs cv::ORB, cv::SIFT or cv::xfeatures2d::DAISY on the
  * crop and hands the keypoints and descriptors over. Everything after detection runs on the device: keyframe
  * reconstruction from the device silhouette renderer with the occlusion checks, kNN matching with the ratio test
- * (Hamming for ORB, with k_texture_knn_hamming at correspondence iteration 0 for bodies above 512 features; L2 for SIFT
- * and DAISY, k_texture_knn_l2 at correspondence iteration 0), the Tukey-weighted
+ * (Hamming for ORB, BRISK and FREAK, with k_texture_knn_hamming at correspondence iteration 0 for ORB bodies above 512
+ * features and every BRISK / FREAK body; L2 for SIFT and DAISY, k_texture_knn_l2 at correspondence iteration 0), the
+ * Tukey-weighted
  * reprojection gradient / Hessian in every update (inside k_track, added to the link after region and depth) and the
  * keyframe refresh. Bodies with a texture modality are tracked by k_track; contexts without one launch what they
  * launched before. A texture body may be the body of a link of a kinematic structure, or one of its extra bodies with
@@ -505,16 +508,19 @@ int m3tb_share_color_histograms(m3tb_ctx* ctx, int body, int owner_body);
 /* TextureModality + SetUp for body `body` (set with m3tb_set_body and m3tb_set_body_geometry, whose
  * maximum_body_diameter the focus region uses) on colour camera `color_camera`; NULL params remove the modality and
  * detach its renderers. Setting it again starts with an empty keyframe deque and, for SIFT / DAISY, clears the
- * descriptor length. M3TB_ERR_UNSUPPORTED for BRISK, FREAK and ORB_CUDA and for n_keyframes above 8;
+ * descriptor length. M3TB_ERR_UNSUPPORTED for ORB_CUDA and for n_keyframes above 8, and for a change in place between
+ * BRISK / FREAK and the other types: the binary upload and the keyframe read-back take no width, so a body that has a
+ * texture modality of ORB, SIFT or DAISY gets BRISK or FREAK (or back) only after its removal (NULL params);
  * M3TB_ERR_INVALID for bad ids, an unset camera, a body without geometry, non-positive standard deviations or Tukey
  * constant, a negative or non-finite measured / modeled occlusion radius (a window stride of 0, a scan that never
  * ends), and measure_occlusions without the body's depth camera; a refused call changes nothing in the context.
  * M3TB_ERR_UNSUPPORTED for n_features_max above 4096 and M3TB_ERR_INVALID below 512.
  * Device memory: the tables hold C features per body slot for max_bodies, C the largest n_features_max any texture
  * body of the context has asked for (512 while every body keeps the default). The first call allocates the base
- * tables, 616 C bytes per slot (0.32 MB at 512, 2.5 MB at 4096); the first call with SIFT or DAISY adds the float
- * descriptor tables and the match table, 9248 C bytes per slot (C frame and 8 x C keyframe rows of 256 floats, and
- * 8 x C match results: 4.7 MB at 512, 37.9 MB at 4096); the first ORB body above 512 adds the match table alone
+ * tables, 616 C bytes per slot (0.32 MB at 512, 2.5 MB at 4096); the first call with SIFT, DAISY, BRISK or FREAK adds
+ * the wide descriptor tables and the match table, 9248 C bytes per slot (C frame and 8 x C keyframe rows of 256 words,
+ * and 8 x C match results: 4.7 MB at 512, 37.9 MB at 4096; a BRISK / FREAK row uses 16 of its 256 words, so the
+ * tables stay shared by every wide type); the first ORB body above 512 adds the match table alone
  * (32 C bytes per slot). A call that raises C remakes every table at the new C and keeps what the other bodies hold.
  * Each of these steps is all or nothing: on failure the context is as it was. */
 int m3tb_set_texture_modality(m3tb_ctx* ctx, int body, const m3tb_texture_params* params, int color_camera);
@@ -524,17 +530,18 @@ int m3tb_set_texture_modality(m3tb_ctx* ctx, int body, const m3tb_texture_params
  * modality (roi and scale are then 0). Synchronises the stream. */
 int m3tb_get_texture_focus(m3tb_ctx* ctx, int first, int count, int32_t* roi, float* scale, int32_t* valid);
 /* The keypoints_ / descriptors_ of the current colour frame of one body: `n` (0 .. n_features_max) keypoints as (x, y) in crop
- * coordinates, which become roi + pt / scale in the image (texture_modality.cpp:884-887), and n 32-byte ORB
- * descriptors. One upload per frame serves m3tb_start_modalities, correspondence iteration 0 (both detect on the same
+ * coordinates, which become roi + pt / scale in the image (texture_modality.cpp:884-887), and n binary descriptors of
+ * the body's width: 32 bytes for ORB, 64 bytes for BRISK and FREAK, copied bit for bit. One upload per frame serves m3tb_start_modalities, correspondence iteration 0 (both detect on the same
  * frame at the same pose) and m3tb_calculate_results. A body whose camera received a newer frame since its last upload
  * has no features, as when the reference's detection returns early. M3TB_ERR_UNSUPPORTED above the body's
  * n_features_max features;
- * M3TB_ERR_INVALID for a SIFT / DAISY body (m3tb_upload_texture_float_features). */
+ * M3TB_ERR_INVALID for a SIFT / DAISY body (m3tb_upload_texture_float_features). The signature is ORB's; a BRISK or
+ * FREAK body reads 64 n bytes from `descriptors`. */
 int m3tb_upload_texture_features(m3tb_ctx* ctx, int body, const float* keypoints_xy, const uint8_t* descriptors, int n,
                                  int roi_x, int roi_y, float scale);
 /* As m3tb_upload_texture_features for a SIFT or DAISY body: descriptors [n][length] floats, length 128 for SIFT and
  * 1 .. 256 for DAISY. The first upload after m3tb_set_texture_modality fixes the length; M3TB_ERR_INVALID for another
- * length later, for a non-finite descriptor value and for an ORB body. */
+ * length later, for a non-finite descriptor value and for an ORB, BRISK or FREAK body. */
 int m3tb_upload_texture_float_features(m3tb_ctx* ctx, int body, const float* keypoints_xy, const float* descriptors,
                                        int n, int length, int roi_x, int roi_y, float scale);
 /* The focused grey images of bodies[0 .. count) on the device (k_texture_crop, one launch per 128 bodies): what
@@ -555,7 +562,9 @@ int m3tb_texture_crop(m3tb_ctx* ctx, const int* bodies, int count, uint8_t* out,
 /* One body's features in device memory (cv::cuda::ORB's GpuMat keypoints and descriptors, a torch detector's
  * tensors): keypoint i at x[i * xy_stride], y[i * xy_stride] in crop coordinates (GpuMat rows: x and y rows of the
  * keypoint matrix, stride 1; interleaved xy: y = x + 1, stride 2); descriptor row i at descriptors + i *
- * descriptor_pitch bytes, 32 bytes for ORB (length 0) or `length` floats for SIFT / DAISY (4-byte aligned). */
+ * descriptor_pitch bytes: with length 0 the binary width of the body's type (32 bytes for ORB, 64 for BRISK / FREAK;
+ * descriptor_pitch at least that, no alignment needed, copied bit for bit and never checked as floats), or `length`
+ * floats for SIFT / DAISY (4-byte aligned). */
 typedef struct m3tb_device_features {
   int n;
   int length;
@@ -569,8 +578,9 @@ typedef struct m3tb_device_features {
  * launch per 128 bodies and without synchronising: keypoints become float(roi_x) + x / scale with the roi and scale of
  * the body's last m3tb_texture_crop. Replaces, per body and frame, the host copy of the detector's output
  * (DetectAndComputeCorrKeypoints, texture_modality.cpp:870-887). Refusals as the host upload (M3TB_ERR_UNSUPPORTED
- * above the body's n_features_max features; M3TB_ERR_INVALID for the other descriptor kind, a bad length and a length other than the first
- * upload's), and M3TB_ERR_INVALID for a body whose last crop is not of its camera's current frame; nothing is launched
+ * above the body's n_features_max features; M3TB_ERR_INVALID for the other descriptor kind, i.e. a nonzero length for a
+ * binary body or 0 for a SIFT / DAISY body, a bad length and a length other than the first upload's), and
+ * M3TB_ERR_INVALID for a body whose last crop is not of its camera's current frame; nothing is launched
  * when any body is refused. Float descriptors are checked on the device: a body with a non-finite value gets no
  * features this frame and its flag (m3tb_get_texture_feature_flags) is raised. The caller keeps the buffers unchanged
  * until the stream has passed the upload (any synchronising call). */
@@ -636,7 +646,8 @@ int m3tb_get_texture_points(m3tb_ctx* ctx, int body, m3tb_texture_point* points,
 /* Parity read-back of the keyframe deque, front to back: *n_keyframes deques entries, sizes[k] points each (sizes holds
  * 8 entries), their center_f_body [total][3] and descriptors (at most `capacity` points in all), the keyframe_age_ and
  * orientation_last_keyframe_[3]. Each descriptor is written at the body's width: [total][32] bytes for ORB,
- * [total][length] floats (4 * length bytes) for SIFT and DAISY. Any output pointer may be NULL. */
+ * [total][64] bytes for BRISK and FREAK, [total][length] floats (4 * length bytes) for SIFT and DAISY. Any output
+ * pointer may be NULL. */
 int m3tb_get_texture_keyframes(m3tb_ctx* ctx, int body, int* n_keyframes, int* sizes, float* points, uint8_t* descriptors,
                                int capacity, int* age, float* orientation);
 
@@ -734,7 +745,7 @@ int m3tb_refine_poses(m3tb_ctx* ctx, const int* bodies, int n_bodies, const int*
  * bodies as the completed iterations left them (as the reference's loop returns false mid-way) and every other body
  * untouched; the context stays usable.
  * Refusals launch nothing and change nothing: every refusal of m3tb_refine_poses but the texture one;
- * M3TB_ERR_UNSUPPORTED for a refined texture body whose descriptor type is SIFT or DAISY (no device detector, and a
+ * M3TB_ERR_UNSUPPORTED for a refined texture body whose descriptor type is SIFT, DAISY, BRISK or FREAK (no device detector, and a
  * detection by the caller cannot run between the iterations of one call); the ORB-setting refusals of
  * m3tb_texture_detect_orb; M3TB_ERR_NOT_SET_UP when a refined texture body's camera has no colour frame, or the body
  * misses a renderer its texture modality needs. */

@@ -24,7 +24,13 @@ feature near the body's centre, so all become keyframe points), for ORB and SIFT
     k_texture_knn_l2 for SIFT;
   - one tracking step (n_corr x n_update of the workload).
 
-    python scripts/texture_timing.py [K] [--descriptor sift|daisy] [--features N]"""
+With --descriptor brisk it measures the 64-byte Hamming matcher (random 64-byte descriptors, every feature near the
+body's centre) at n_features_max 512, 2048 and 4096 for 1, 8 and 128 bodies: k_texture_knn_hamming per launch, and
+one tracking step. In the same run it times k_texture_knn_hamming for ORB at 4096 features (8 and 128 bodies) on this
+build and on the build given by --parent-lib PATH (another libm3t_b200.so, e.g. of the parent commit), alternating
+between the two in fresh processes, three rounds each, so that a change of the 8-word path shows beside its spread.
+
+    python scripts/texture_timing.py [K] [--descriptor sift|daisy|brisk] [--features N] [--parent-lib PATH]"""
 import importlib
 import json
 import os
@@ -43,16 +49,21 @@ synth = pkg.synth
 ARGS = [a for a in sys.argv[1:] if not a.startswith("--")]
 DESCRIPTOR = sys.argv[sys.argv.index("--descriptor") + 1] if "--descriptor" in sys.argv else None
 FEATURES = int(sys.argv[sys.argv.index("--features") + 1]) if "--features" in sys.argv else None
-ARGS = [a for a in ARGS if a not in (DESCRIPTOR, str(FEATURES))]
+PARENT_LIB = sys.argv[sys.argv.index("--parent-lib") + 1] if "--parent-lib" in sys.argv else None
+ORB_KNN = "--orb-knn-4096" in sys.argv  # one round of the ORB comparison, run by brisk_main in a fresh process
+ARGS = [a for a in ARGS if a not in (DESCRIPTOR, str(FEATURES), PARENT_LIB)]
 K = int(ARGS[0]) if ARGS else 100
 N_FEAT = 300
 L2_LENGTH = {"sift": 128, "daisy": 104}
 L2_TYPE = {"sift": capi.DESCRIPTOR_SIFT, "daisy": capi.DESCRIPTOR_DAISY}
+TYPE = dict(L2_TYPE, brisk=capi.DESCRIPTOR_BRISK)
 
 
 def descriptors(rng, kind, n):
     if kind is None:
         return rng.integers(0, 256, (n, 32), dtype=np.uint8)
+    if kind == "brisk":
+        return rng.integers(0, 256, (n, 64), dtype=np.uint8)
     if kind == "sift":
         return rng.integers(0, 256, (n, 128)).astype(np.float32)
     v = rng.random((n, L2_LENGTH[kind])).astype(np.float32)
@@ -60,7 +71,7 @@ def descriptors(rng, kind, n):
 
 
 def perturbed(rng, kind, desc):
-    if kind is None:
+    if kind is None or kind == "brisk":
         desc = desc.copy()
         desc[:, ::4] ^= 1
         return desc
@@ -71,7 +82,7 @@ def perturbed(rng, kind, desc):
 def make(wl, texture, kind=None, n_feat=N_FEAT, n_keyframes=1, central=False):
     """A context of the workload; with texture, every body gets a texture modality on its own camera, a keyframe from
     the first frame's features and the next frame's features (the same ones, a few descriptor bits flipped).
-    kind: None (ORB) or an L2 descriptor; n_keyframes > 1 refreshes the keyframe every frame until the deque is full;
+    kind: None (ORB), "brisk" or an L2 descriptor; n_keyframes > 1 refreshes the keyframe every frame until the deque is full;
     central puts every feature near the body's centre, so that all become keyframe points."""
     ctx = capi.context_from_workload(wl)
     tri, diam = synth.prism_triangles()
@@ -81,7 +92,7 @@ def make(wl, texture, kind=None, n_feat=N_FEAT, n_keyframes=1, central=False):
         rng = np.random.default_rng(0)
         params = capi.texture_params_default()
         if kind is not None:
-            params.descriptor_type = L2_TYPE[kind]
+            params.descriptor_type = TYPE[kind]
         params.n_keyframes = n_keyframes
         params.n_features_max = max(params.n_features_max, n_feat)
         params.max_keyframe_age = 0 if n_keyframes > 1 else params.max_keyframe_age
@@ -143,8 +154,9 @@ def knn_kernel_ms(ctx, kernel="k_texture_knn_l2"):
         ctx.synchronize()
         torch.cuda.synchronize()
     rows = [e for e in prof.key_averages() if kernel in e.key]
-    assert len(rows) == 1 and rows[0].count == K, [(e.key, e.count) for e in rows]
-    return max(rows[0].self_device_time_total, rows[0].device_time_total) / K / 1e3
+    assert len(rows) == 1 and 0 < rows[0].count <= K, [(e.key, e.count) for e in rows]
+    # the profiler may drop a few events of a long run: the mean over the launches it recorded
+    return max(rows[0].self_device_time_total, rows[0].device_time_total) / rows[0].count / 1e3
 
 
 def l2_main(kind):
@@ -195,6 +207,56 @@ def features_main(n_feat):
     print(json.dumps(dict(features=n_feat, K=K, shapes=shapes, gpu=gpu_name())))
 
 
+def orb_knn_round():
+    """k_texture_knn_hamming for ORB at 4096 features per body, 8 and 128 bodies: {bodies: ms per launch}."""
+    import torch
+    torch.cuda.init()
+    out = {}
+    for n_bodies in (8, 128):
+        wl = synth.make_workload("c4", n_bodies=n_bodies, n_divides=2, seed=0)
+        wl, ctx = make(wl, True, None, n_feat=4096, central=True)
+        out[n_bodies] = knn_kernel_ms(ctx, "k_texture_knn_hamming")
+        ctx.close()
+    return out
+
+
+def brisk_main():
+    import torch
+    torch.cuda.init()
+    shapes = []
+    for n_feat in (512, 2048, 4096):
+        for n_bodies in (1, 8, 128):
+            wl = synth.make_workload("c4", n_bodies=n_bodies, n_divides=2, seed=0)
+            wl, ctx = make(wl, True, "brisk", n_feat=n_feat, central=True)
+            queries = sum(int(ctx.get_texture_keyframes(b)["sizes"].sum()) for b in range(n_bodies))
+            ms = knn_kernel_ms(ctx, "k_texture_knn_hamming")
+            ms_step = time_calls(ctx, step(ctx, wl.n_corr_iterations, wl.n_update_iterations))
+            points = int(np.mean([len(ctx.get_texture_points(b)) for b in range(n_bodies)]))
+            shapes.append(dict(descriptor="brisk", bodies=n_bodies, queries=queries, train_per_body=n_feat,
+                               ms_knn_hamming=ms, ms_step=ms_step, mean_data_points_per_body=points,
+                               n_corr=wl.n_corr_iterations, n_update=wl.n_update_iterations))
+            ctx.close()
+    orb = {"this": [], "parent": []}
+    if PARENT_LIB:
+        script = os.path.abspath(__file__)
+        for _ in range(3):
+            for name, lib_path in (("this", None), ("parent", PARENT_LIB)):
+                env = dict(os.environ)
+                env.pop("M3TB_LIB", None)
+                if lib_path:
+                    env["M3TB_LIB"] = os.path.abspath(lib_path)
+                r = subprocess.run([sys.executable, script, str(K), "--orb-knn-4096"], env=env, capture_output=True,
+                                   text=True, check=True)
+                orb[name].append(json.loads(r.stdout.strip().split("\n")[-1]))
+    print(json.dumps(dict(descriptor="brisk", K=K, shapes=shapes, orb_knn_hamming_4096_ms=orb, gpu=gpu_name())))
+
+
+if ORB_KNN:
+    print(json.dumps(orb_knn_round()))
+    sys.exit(0)
+if DESCRIPTOR == "brisk":
+    brisk_main()
+    sys.exit(0)
 if FEATURES is not None:
     assert 512 <= FEATURES <= 4096, FEATURES
     features_main(FEATURES)
