@@ -157,7 +157,7 @@ SYMBOLS = [
     "m3tb_get_texture_detections", "m3tb_get_texture_orb_keypoints", "m3tb_refine_poses_orb",
 ]
 
-KERNEL_NAMES = {0: None, 1: "k_track", 2: "k_track2", 3: "k_track_cluster"}
+KERNEL_NAMES = {0: None, 1: "k_track", 2: "k_track2"}
 
 
 class LaunchInfo(C.Structure):
@@ -1072,8 +1072,8 @@ class Context:
         return out
 
     def last_launch(self):
-        """The tracking-kernel variant of the last tracking launch as a dict (kernel: "k_track2" | "k_track" |
-        "k_track_cluster" | None before the first launch)."""
+        """The tracking-kernel variant of the last tracking launch as a dict (kernel: "k_track2" | "k_track" | None
+        before the first launch)."""
         info = LaunchInfo()
         self._ck(self.L.m3tb_debug_last_launch(self.h, C.byref(info)))
         d = {k: int(getattr(info, k)) for k, _ in LaunchInfo._fields_}

@@ -36,7 +36,7 @@ extern template __global__ void k_track2<512, false>(const __grid_constant__ Tra
 extern template __global__ void k_track2<1024, true>(const __grid_constant__ TrackArgs);
 extern template __global__ void k_track2<1024, false>(const __grid_constant__ TrackArgs);
 // the fused kernel's variants are compiled in m3t_b200_track_<g>.cu
-#define M3TB_DECLARE(T_, K_, L_, O_, C_) extern template __global__ void k_track<T_, K_, L_, O_, C_>(const __grid_constant__ TrackArgs);
+#define M3TB_DECLARE(T_, K_, L_, O_) extern template __global__ void k_track<T_, K_, L_, O_>(const __grid_constant__ TrackArgs);
 M3TB_TRACK_ALL(M3TB_DECLARE)
 #undef M3TB_DECLARE
 }  // namespace m3tb
@@ -191,7 +191,6 @@ struct m3tb_ctx {
   bool structures_dirty = false;
   int n_struct_launch = 0;                 // user structures + one implicit structure per unreferenced body
   std::vector<int> h_link_bodies;          // body index of every launched link
-  bool use_clusters = false;               // M3TB_CLUSTER=1: cluster-fused structure path (see DESIGN.md: measured slower)
   std::vector<StructureDev> h_structures;
   DeviceBuffer<StructureDev> d_structures;
   DeviceBuffer<LinkDev> d_links;
@@ -747,9 +746,8 @@ TrackArgs RunArgs(const TrackArgs& a, int first) {
   return r;
 }
 
-// cluster > 0: one thread-block cluster of `cluster` CTAs per kinematic structure (PH_CLUSTER_SOLVE)
 int LaunchTrack(m3tb_ctx* ctx, int iteration, int corr_begin, int corr_end, int n_update, int opt_base,
-                unsigned phases, int cluster = 0) {
+                unsigned phases) {
   int rc = ValidateBodies(ctx);
   if (!rc && (phases & PH_TEXTURE_GH)) rc = ValidateTexture(ctx);
   if (rc) return rc;
@@ -801,12 +799,6 @@ int LaunchTrack(m3tb_ctx* ctx, int iteration, int corr_begin, int corr_end, int 
   a.phases = phases;
   a.phase_clock = ctx->d_phase_clock;
   a.roi = ctx->d_roi;
-  a.structures = ctx->d_structures;
-  a.links = ctx->d_links;
-  a.constraints = ctx->d_constraints;
-  a.theta_out = ctx->d_theta;
-  a.struct_status = ctx->d_struct_status;
-  a.struct_offset = 0u;
   // thread <-> line mapping: T threads per body, K lines and K points per thread (state in registers)
   const int items = std::max(ctx->line_cap, ctx->point_cap);
   bool lut_smem = true;  // normalised LUT staged in shared memory when every region body has <= 16 bins (32 KB)
@@ -814,15 +806,12 @@ int LaunchTrack(m3tb_ctx* ctx, int iteration, int corr_begin, int corr_end, int 
     if (ctx->h_bodies[b].has_region && ctx->h_bodies[b].rp.n_bins > 16) lut_smem = false;
   // dynamic shared memory: [normalised LUT 32 KB (16 bins)] [colour bin-index tile] [depth tile]
   const size_t lut_bytes = lut_smem ? size_t(16 * 16 * 16) * sizeof(float2) : 0;
-  // with cluster-fused structures the solver workspace sits at the end of the dynamic shared memory
-  const size_t struct_bytes = cluster > 0 ? Align(ctx->struct_smem, 128) : 0;
   bool bins_fit_u16 = true;  // the colour tile holds 16-bit bin indices: 64 bins (18 bits) go without tiles
   for (int b = 0; b < ctx->n_bodies; ++b)
     if (ctx->h_bodies[b].has_region && ctx->h_bodies[b].rp.n_bins > 32) bins_fit_u16 = false;
-  const bool tiles = ctx->use_tiles && cluster == 0 && bins_fit_u16;
-  const size_t dyn = tiles ? size_t(kDynSmemBytes) : lut_bytes + struct_bytes;
-  a.tile_bytes = tiles ? int(dyn - lut_bytes - struct_bytes) : 0;
-  a.struct_offset = unsigned(dyn - struct_bytes);
+  const bool tiles = ctx->use_tiles && bins_fit_u16;
+  const size_t dyn = tiles ? size_t(kDynSmemBytes) : lut_bytes;
+  a.tile_bytes = tiles ? int(dyn - lut_bytes) : 0;
   bool occ = false;  // measured occlusion handling anywhere: the kernel variant that carries the depth-window scans
   for (int b = 0; b < ctx->n_bodies; ++b) {
     const BodyDev& B = ctx->h_bodies[b];
@@ -837,7 +826,7 @@ int LaunchTrack(m3tb_ctx* ctx, int iteration, int corr_begin, int corr_end, int 
   {
     const unsigned k2_phases = PH_REGION_CORR | PH_DEPTH_CORR | PH_REGION_GH | PH_DEPTH_GH | PH_SOLVE | PH_STORE_REGION |
                                PH_STORE_DEPTH;
-    bool ok = ctx->use_track2 && !ctx->refine && bins_fit_u16 && cluster == 0 && !occ && items <= kGroup && (phases & ~k2_phases) == 0 &&
+    bool ok = ctx->use_track2 && !ctx->refine && bins_fit_u16 && !occ && items <= kGroup && (phases & ~k2_phases) == 0 &&
               (n_update == 0 || (phases & PH_SOLVE));
     bool both = false, have_lookup = false;
     for (int b = 0; b < ctx->n_bodies && ok; ++b) {
@@ -878,35 +867,11 @@ int LaunchTrack(m3tb_ctx* ctx, int iteration, int corr_begin, int corr_end, int 
   }
 #define M3TB_LAUNCH1(T_, K_, L_, O_)                                                                                   \
   do {                                                                                                                 \
-    CU(cudaFuncSetAttribute(k_track<T_, K_, L_, O_, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, int(dyn)));   \
+    CU(cudaFuncSetAttribute(k_track<T_, K_, L_, O_>, cudaFuncAttributeMaxDynamicSharedMemorySize, int(dyn)));           \
     for (size_t r_ = 0; r_ < n_runs; ++r_)                                                                             \
-      k_track<T_, K_, L_, O_, false><<<runs_begin[r_].second, T_, dyn, ctx->stream>>>(RunArgs(a, runs_begin[r_].first)); \
+      k_track<T_, K_, L_, O_><<<runs_begin[r_].second, T_, dyn, ctx->stream>>>(RunArgs(a, runs_begin[r_].first));       \
     n_launches = int(n_runs);                                                                                          \
     info = {M3TB_KERNEL_TRACK, T_, K_, L_ ? 1 : 0, O_ ? 1 : 0, tiles ? 1 : 0, -1};                                     \
-  } while (0)
-#define M3TB_LAUNCH_CLUSTER(T_, K_, L_)                                                                                \
-  do {                                                                                                                 \
-    CU(cudaFuncSetAttribute(k_track<T_, K_, L_, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, int(dyn))); \
-    cudaLaunchConfig_t cfg = {};                                                                                       \
-    cfg.gridDim = dim3(unsigned(ctx->n_bodies));                                                                       \
-    cfg.blockDim = dim3(T_);                                                                                           \
-    cfg.dynamicSmemBytes = dyn;                                                                                        \
-    cfg.stream = ctx->stream;                                                                                          \
-    cudaLaunchAttribute attr;                                                                                          \
-    attr.id = cudaLaunchAttributeClusterDimension;                                                                     \
-    attr.val.clusterDim.x = unsigned(cluster);                                                                         \
-    attr.val.clusterDim.y = 1;                                                                                         \
-    attr.val.clusterDim.z = 1;                                                                                         \
-    cfg.attrs = &attr;                                                                                                 \
-    cfg.numAttrs = 1;                                                                                                  \
-    if (ctx->d_phase_clock) {                                                                                          \
-      int n_clusters = -1;                                                                                             \
-      cudaOccupancyMaxActiveClusters(&n_clusters, k_track<T_, K_, L_, false, true>, &cfg);                             \
-      std::fprintf(stderr, "m3tb: cluster launch %d x %d CTAs, dyn smem %zu, max active clusters %d\n",                \
-                   ctx->n_bodies / cluster, cluster, size_t(dyn), n_clusters);                                         \
-    }                                                                                                                  \
-    CU(cudaLaunchKernelEx(&cfg, k_track<T_, K_, L_, false, true>, a));                                                 \
-    info = {M3TB_KERNEL_TRACK_CLUSTER, T_, K_, L_ ? 1 : 0, 0, 0, -1};                                                  \
   } while (0)
 #define M3TB_LAUNCH(T_, K_)                                       \
   do {                                                            \
@@ -921,20 +886,13 @@ int LaunchTrack(m3tb_ctx* ctx, int iteration, int corr_begin, int corr_end, int 
   const std::pair<int, int> all_bodies(0, ctx->n_bodies);
   const std::pair<int, int>* runs_begin = ctx->refine ? ctx->refine->runs.data() : &all_bodies;
   const size_t n_runs = ctx->refine ? ctx->refine->runs.size() : 1;
-  if (cluster > 0) {
-    // cluster-fused structures: 256-thread CTAs without ROI tiles, so that two CTAs share an SM and every cluster of
-    // a 32-chain shard is resident at once (with 220 KB tiles at most 16 clusters of 8 fit on the 132 SMs)
-    if (items <= 256) { if (lut_smem) M3TB_LAUNCH_CLUSTER(256, 1, true); else M3TB_LAUNCH_CLUSTER(256, 1, false); }
-    else if (items <= 512) { if (lut_smem) M3TB_LAUNCH_CLUSTER(256, 2, true); else M3TB_LAUNCH_CLUSTER(256, 2, false); }
-    else return Fail(ctx, M3TB_ERR_UNSUPPORTED, "cluster-fused structures: n_lines_max / n_points_max above 512");
-  } else if (items <= 256) M3TB_LAUNCH(256, 1);
+  if (items <= 256) M3TB_LAUNCH(256, 1);
   else if (items <= 512) M3TB_LAUNCH(512, 1);
   else if (items <= 1024) M3TB_LAUNCH(512, 2);
   else if (items <= 2048) M3TB_LAUNCH(512, 4);
   else return Fail(ctx, M3TB_ERR_UNSUPPORTED, "n_lines_max / n_points_max above 2048");
 #undef M3TB_LAUNCH
 #undef M3TB_LAUNCH1
-#undef M3TB_LAUNCH_CLUSTER
   CU(cudaGetLastError());
   ctx->launches += n_launches;
   ctx->last_launch = info;
@@ -1112,30 +1070,6 @@ int LaunchStructure(m3tb_ctx* ctx, int mode, bool from_modalities) {
   return M3TB_OK;
 }
 
-// Can every structure run as one thread-block cluster inside k_track? All structures have the same number of links
-// (2..8, the portable cluster size), every link carries a body, and structure s, link l is body s * n_links + l, so
-// that CTA rank = link index. Anything else takes the general multi-launch path below.
-int ClusterLinks(m3tb_ctx* ctx) {
-  if (!ctx->use_clusters || ctx->n_struct_launch == 0) return 0;
-  const int nl = ctx->h_structures[0].n_links;
-  if (nl < 2 || nl > 8 || ctx->n_struct_launch * nl != ctx->n_bodies) return 0;
-  for (int si = 0; si < ctx->n_struct_launch; ++si) {
-    const StructureDev& d = ctx->h_structures[si];
-    if (d.n_links != nl) return 0;
-    for (int l = 0; l < nl; ++l)
-      if (ctx->h_link_bodies[d.first_link + l] != si * nl + l) return 0;
-    if (si < int(ctx->structures.size()))
-      for (const auto& lk : ctx->structures[si].links)
-        if (lk.n_extra > 0) return 0;
-  }
-  for (int b = 0; b < ctx->n_bodies; ++b) {
-    const BodyDev& B = ctx->h_bodies[b];
-    if ((B.has_region && B.rp.measure_occlusions) || (B.has_depth && B.dp.measure_occlusions)) return 0;
-    if ((B.has_region && B.rp.n_lines_max > 512) || (B.has_depth && B.dp.n_points_max > 512)) return 0;
-  }
-  return nl;
-}
-
 // Tracker::ExecuteTrackingStep's loop nest (tracker.cpp:344-361) when the optimisers are kinematic structures: the
 // per-body work stays in k_track (correspondences, gradient / Hessian of region, depth and texture -> gh_link), every
 // Optimizer::CalculateOptimization is one k_structure launch over all structures. Texture matching runs once per frame,
@@ -1143,21 +1077,12 @@ int ClusterLinks(m3tb_ctx* ctx) {
 int StructureStep(m3tb_ctx* ctx, int iteration, int corr_begin, int corr_end, int n_update) {
   int rc0 = SyncStructures(ctx);
   // TextureModality::SetUp's conditions first: a texture modality then has its silhouette renderer attached, so a
-  // textured context renders (below) and never takes the cluster-fused path, which has no texture term
+  // textured context renders (below)
   if (!rc0 && ctx->n_texture > 0) rc0 = ValidateTexture(ctx);
   if (rc0) return rc0;
   // device renderers refresh their images before every correspondence iteration
   const bool render = ctx->n_attached > 0;
   const unsigned tex = ctx->n_texture > 0 ? unsigned(PH_TEXTURE_GH) : 0u;
-  if (const int nl = render ? 0 : ClusterLinks(ctx)) {
-    // fused: the whole corr x update loop nest in ONE launch, one cluster per structure, CalculateOptimization over
-    // distributed shared memory
-    if (n_update > 0)
-      return LaunchTrack(ctx, iteration, corr_begin, corr_end, n_update, 0,
-                         PH_REGION_CORR | PH_DEPTH_CORR | PH_REGION_GH | PH_DEPTH_GH | PH_CLUSTER_SOLVE | PH_STORE_REGION |
-                             PH_STORE_DEPTH,
-                         nl);
-  }
   for (int corr = corr_begin; corr < corr_end; ++corr) {
     if (render) {
       int rc = LaunchRender(ctx, kRenderAttached);
@@ -2364,7 +2289,6 @@ int m3tb_create(int device, int max_bodies, int max_cameras, int max_models, m3t
   ctx->orb_nmax.assign(max_bodies, -1);
   if (const char* e = std::getenv("M3TB_NO_TILES")) ctx->use_tiles = !(e[0] == '1');
   if (const char* e = std::getenv("M3TB_NO_ROI_INGEST")) ctx->roi_ingest = !(e[0] == '1');
-  if (const char* e = std::getenv("M3TB_CLUSTER")) ctx->use_clusters = e[0] == '1';
   if (const char* e = std::getenv("M3TB_KERNEL")) ctx->use_track2 = !(e[0] == '1');
   if (const char* e = std::getenv("M3TB_TMA")) ctx->tma_mode = (e[0] >= '0' && e[0] <= '2') ? e[0] - '0' : 1;
   const char* timing_env = std::getenv("M3TB_TIMING");

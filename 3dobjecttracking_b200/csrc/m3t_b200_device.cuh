@@ -48,8 +48,6 @@ enum Phase : unsigned {
   PH_LOAD_REGION = 32u, PH_LOAD_DEPTH = 64u, PH_STORE_REGION = 128u, PH_STORE_DEPTH = 256u,
   PH_STORE_GH = 512u, PH_LOAD_GH = 1024u,
   PH_STORE_LINK_GH = 2048u,  // sum over the body's modalities -> gh_link (input of k_structure)
-  PH_CLUSTER_SOLVE = 4096u,  // one thread-block cluster per kinematic structure: Optimizer::CalculateOptimization
-                             // over distributed shared memory inside k_track (CLUSTER variants only)
   PH_TEXTURE_GH = 8192u      // TextureModality::CalculateGradientAndHessian of the bodies with a texture modality
 };
 
@@ -219,13 +217,6 @@ struct TrackArgs {
   int tile_bytes;               // dynamic shared memory available for the colour / depth ROI tiles (0: no tiling)
   RoiRecord* roi;               // [n_bodies][2]: colour, depth
   long long* phase_clock;       // optional [n_bodies][kPhaseSlots] clock64() stamps of thread 0 (profiling aid), or null
-  // cluster-fused kinematic structures (PH_CLUSTER_SOLVE): CTA rank r of cluster c handles link r of structure c
-  const struct StructureDev* structures;
-  struct LinkDev* links;
-  const struct ConstraintDev* constraints;
-  float* theta_out;             // [n_structures][kMaxSystem]
-  int* struct_status;           // [n_structures]
-  unsigned struct_offset;       // byte offset of the solver workspace in dynamic shared memory
   // k_track2: TMA tensor maps over the image pools ([camera][row][column] u16), one per tile width; the box is
   // kTileBoxRows rows high. tma_ok = 0: the pools cannot be described (private images): k_track2 is not launched.
   CUtensorMap bin_maps[kTileWidths];

@@ -16,8 +16,6 @@
 //   k_lut        per-bin normalisation of (hist_f, hist_b) -> float2 LUT.
 #pragma once
 
-#include <cooperative_groups.h>
-
 #include "m3t_b200_device.cuh"
 #include "m3t_b200_structures.cuh"
 #include "m3t_b200_texture.cuh"
@@ -50,7 +48,6 @@ struct Shared {
   float a[36];                   // normal matrix, full symmetric
   float b[6];
   float x[6];
-  float link_gh[32];             // this link's g[6] + H lower[21], read by the cluster leader over DSMEM
   unsigned best_key[2][2][kMaxWarps];  // [call parity][model][warp]
   int best_idx[2][2][kMaxWarps];
   unsigned long long lut_bar;    // mbarrier of the LUT bulk copy
@@ -1108,7 +1105,7 @@ __device__ __forceinline__ void FitTile(Tile& t, int budget, int align_x) {
 // The fused kernel
 // ---------------------------------------------------------------------------------------------
 
-template <int T, int K, bool LUT_SMEM, bool OCC, bool CLUSTER>
+template <int T, int K, bool LUT_SMEM, bool OCC>
 __global__ void __launch_bounds__(T, 512 / T) k_track(const __grid_constant__ TrackArgs args) {
   extern __shared__ __align__(128) unsigned char dyn[];
   __shared__ Shared sh;
@@ -1495,7 +1492,6 @@ __global__ void __launch_bounds__(T, 512 / T) k_track(const __grid_constant__ Tr
           if (args.phases & PH_TEXTURE_GH) args.gh_texture[27 * body_id + l] = v;
         }
         if (args.phases & PH_STORE_LINK_GH) args.gh_link[27 * body_id + l] = v;
-        if (CLUSTER && (args.phases & PH_CLUSTER_SOLVE)) sh.link_gh[l] = v;
         if (args.phases & PH_LOAD_GH) {  // Link::CalculateGradientAndHessian (link.cpp:184-193): region, depth, texture
           v = 0.0f + args.gh_region[27 * body_id + l] + args.gh_depth[27 * body_id + l];
           if (body.has_texture) v = v + args.gh_texture[27 * body_id + l];
@@ -1519,59 +1515,12 @@ __global__ void __launch_bounds__(T, 512 / T) k_track(const __grid_constant__ Tr
       }
       if (args.phases & PH_SOLVE) M3TB_STAMP();  // solve + pose products (warp 0)
       __syncthreads();
-      if (CLUSTER && (args.phases & PH_CLUSTER_SOLVE)) {
-        // One cluster = one kinematic structure, CTA rank = link index. The leader CTA gathers every link's pose and
-        // gradient / Hessian sums over distributed shared memory, runs Optimizer::CalculateOptimization for the whole
-        // structure (all T threads), and writes the new link poses back into every CTA's shared memory.
-        namespace cg = cooperative_groups;
-        cg::cluster_group cluster = cg::this_cluster();
-        cluster.sync();
-        const int nl = int(cluster.num_blocks());
-        constexpr int kSolveThreads = T < kStructThreads ? T : kStructThreads;  // the first four warps solve
-        if (cluster.block_rank() == 0 && tid < kSolveThreads) {
-          const int sidx = body_id / nl;
-          const StructureDev st = args.structures[sidx];
-          LinkDev* links = args.links + st.first_link;
-          const ConstraintDev* cons = args.constraints + st.first_constraint;
-          StructSmem s = CarveStructSmem(reinterpret_cast<float*>(dyn + args.struct_offset), nl, st.dof, st.dof + st.n_rows,
-                                         st.n_constraints);
-          for (int e = tid; e < nl * 12; e += kSolveThreads) {
-            const int l = e / 12, k = e - 12 * l;
-            s.l2w[e] = cluster.map_shared_rank(sh.pose, l)[k];
-          }
-          for (int e = tid; e < nl * 42; e += kSolveThreads) {
-            const int l = e / 42, k = e - 42 * l;
-            int src = k;
-            if (k >= 6) {
-              const int i = (k - 6) / 6, j = (k - 6) - 6 * i;
-              src = 6 + (i >= j ? Tri(i, j) : Tri(j, i));
-            }
-            const float val = cluster.map_shared_rank(sh.link_gh, l)[src];
-            if (k < 6) s.g[6 * l + k] = val; else s.H[36 * l + k - 6] = val;
-          }
-          const bool updated = StructureSolveBlock(st, links, cons, s, args.theta_out + size_t(sidx) * kMaxSystem, tid, kSolveThreads);
-          if (tid == 0) args.struct_status[sidx] = updated ? 1 : 0;
-          if (updated)
-            for (int e = tid; e < nl * 12; e += kSolveThreads) {
-              const int l = e / 12, k = e - 12 * l;
-              cluster.map_shared_rank(sh.pose, l)[k] = s.l2w[e];
-            }
-        }
-        cluster.sync();
-        if (warp == 0) {
-          float pose[12];
-#pragma unroll
-          for (int i = 0; i < 12; ++i) pose[i] = sh.pose[i];
-          PublishPoseProducts(pose, ccam != nullptr, dcam != nullptr, /*store_pose=*/false, sh);
-        }
-        __syncthreads();
-      }
       M3TB_STAMP();  // solve + pose update
     }
   }
 
   // ---------------- epilogue ----------------------------------------------------------------------
-  if (args.phases & (PH_SOLVE | PH_CLUSTER_SOLVE))
+  if (args.phases & PH_SOLVE)
     if (tid < 12) args.poses[12 * body_id + tid] = sh.pose[tid];
   if (args.phases & PH_STORE_REGION) {
 #pragma unroll

@@ -278,8 +278,8 @@ __device__ inline StructSmem CarveStructSmem(float* base, int nl, int dof, int n
   return s;
 }
 
-// The solver runs on the first T threads of a CTA (T a multiple of 32): the whole CTA in k_structure, the first four
-// warps of the leader CTA in the cluster-fused k_track. Named barrier 1 keeps it independent of the other warps.
+// The solver's barriers over the first T threads of a CTA (T a multiple of 32; k_structure passes its whole CTA).
+// Named barrier 1 keeps them independent of any other warps of the CTA.
 __device__ __forceinline__ void StructSync(int T) { asm volatile("bar.sync 1, %0;" ::"r"(T) : "memory"); }
 __device__ __forceinline__ int StructSyncOr(int T, int pred) {
   int out;
@@ -348,8 +348,7 @@ __device__ inline void UpdatePosesBlock(const StructSmem& s, LinkDev* links, int
 // Optimizer::CalculateOptimization for one structure, executed by the first T threads of one CTA (tid < T). In: s.l2w (link poses),
 // s.g / s.H (the links' summed modality gradients / Hessians), the links' joint poses in global memory. Out: s.l2w,
 // joint poses, theta_out[n] (optional). Returns false when the NaN guard (optimizer.cpp:165) skipped the update.
-// Not inlined: it is shared by k_structure and by the cluster-fused variant of k_track, whose register allocation
-// must not be disturbed by this (rarely executed, latency-bound) code.
+// Not inlined: this rarely executed, latency-bound code is kept out of its caller's register allocation.
 static __device__ __noinline__ bool StructureSolveBlock(const StructureDev& st, LinkDev* links, const ConstraintDev* cons,
                                                  const StructSmem& s, float* theta_out, int tid, int T) {
   const int nl = st.n_links, dof = st.dof, nc = st.n_constraints, n = st.dof + st.n_rows;

@@ -4,7 +4,7 @@
 #include "m3t_b200_track_variants.h"
 
 namespace m3tb {
-#define M3TB_INSTANTIATE(T_, K_, L_, O_, C_) template __global__ void k_track<T_, K_, L_, O_, C_>(const __grid_constant__ TrackArgs);
+#define M3TB_INSTANTIATE(T_, K_, L_, O_) template __global__ void k_track<T_, K_, L_, O_>(const __grid_constant__ TrackArgs);
 M3TB_TRACK_GROUP_3(M3TB_INSTANTIATE)
 #undef M3TB_INSTANTIATE
 }  // namespace m3tb

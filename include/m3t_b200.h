@@ -800,8 +800,7 @@ int m3tb_debug_phase_clocks(m3tb_ctx* ctx, int body, long long* out, int capacit
 typedef enum {
   M3TB_KERNEL_NONE = 0,
   M3TB_KERNEL_TRACK = 1,         /* k_track, the general kernel */
-  M3TB_KERNEL_TRACK2 = 2,        /* k_track2, the fused rigid-body kernel */
-  M3TB_KERNEL_TRACK_CLUSTER = 3  /* k_track with thread-block clusters (M3TB_CLUSTER=1, kinematic structures) */
+  M3TB_KERNEL_TRACK2 = 2         /* k_track2, the fused rigid-body kernel */
 } m3tb_kernel;
 typedef struct m3tb_launch_info {
   int32_t kernel;            /* m3tb_kernel */

@@ -25,7 +25,7 @@ from helpers import pose_error
 pytestmark = pytest.mark.gpu
 
 f32 = np.float32
-_ENV = ("M3TB_TMA", "M3TB_TMA_MAXW", "M3TB_NO_TILES", "M3TB_NO_ROI_INGEST", "M3TB_KERNEL", "M3TB_CLUSTER")
+_ENV = ("M3TB_TMA", "M3TB_TMA_MAXW", "M3TB_NO_TILES", "M3TB_NO_ROI_INGEST", "M3TB_KERNEL")
 LINE_FIELDS = ("center_f_body", "center_u", "center_v", "normal_u", "normal_v")
 LINE_FIELDS_VALID = ("delta_r", "normal_component_to_scale", "distribution", "mean", "measured_variance")
 

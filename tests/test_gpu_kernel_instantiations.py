@@ -1,21 +1,19 @@
-"""GPU parity along the instantiation axis: every compiled k_track2<T, LUT_SMEM> and k_track<T, K, LUT_SMEM, OCC, CLUSTER>
-runs in at least one case here, and every case asserts the exact variant it runs (m3tb_debug_last_launch: kernel,
+"""GPU parity along the instantiation axis: every compiled k_track2<T, LUT_SMEM> and k_track<T, K, LUT_SMEM, OCC> runs
+in at least one case here, and every case asserts the exact variant it runs (m3tb_debug_last_launch: kernel,
 threads, items per thread, LUT in shared memory, occlusion variant), so that a routing change cannot make a case
 vacuous. COVERAGE maps each variant to its cases; test_kernel_instantiation_inventory.py holds it equal to what the
 sources instantiate, so an instantiation without a case (or a row for one that does not exist) fails on any machine.
 
 LaunchTrack picks the variant from max(n_lines_max, n_points_max) (<= 256: 256 threads x 1 item, <= 512: 512 x 1,
 <= 1024: 512 x 2, <= 2048: 512 x 4; k_track2 takes <= 512 items), whether every region body has <= 16 histogram bins
-(LUT in shared memory), whether any body measures occlusions or reads renderer images (OCC), whether a body carries
-both modalities (k_track2 at 1024 threads) and M3TB_CLUSTER (cluster-fused kinematic structures, 256 threads).
+(LUT in shared memory), whether any body measures occlusions or reads renderer images (OCC) and whether a body
+carries both modalities (k_track2 at 1024 threads).
 
 Bars as in test_gpu_edges / test_gpu_parameter_space (helpers.per_iteration_parity): closest views and per-line /
 per-point records bit-exact against the mirror oracle, g within 1e-4 and H within 1e-5 of max|H|, poses within 1e-5 of
 the mirror oracle (5e-5 at 4 items per thread: 4096 summands, as in test_gpu_bench_shape.test_many_items_per_thread)
 and within 1e-4 of the reference-faithful oracle after every correspondence iteration; StartModalities /
-CalculateResults histograms bit-exact wherever a region modality exists. Cluster-fused chains are held to the
-reference-faithful oracle per correspondence iteration with body and joint poses re-synchronised (1e-4 m / 1e-4 rad,
-joint poses within 1e-4), as in test_gpu_structures.
+CalculateResults histograms bit-exact wherever a region modality exists.
 """
 import dataclasses
 
@@ -27,7 +25,7 @@ from helpers import (TOL, assert_lines_bit_equal, assert_points_bit_equal, per_i
 
 pytestmark = pytest.mark.gpu
 
-_ENV = ("M3TB_TMA", "M3TB_TMA_MAXW", "M3TB_NO_TILES", "M3TB_NO_ROI_INGEST", "M3TB_KERNEL", "M3TB_CLUSTER")
+_ENV = ("M3TB_TMA", "M3TB_TMA_MAXW", "M3TB_NO_TILES", "M3TB_NO_ROI_INGEST", "M3TB_KERNEL")
 
 # ---- the cases ----------------------------------------------------------------------------------------------------------
 # A. k_track2 with two-modality bodies: bins -> (bins, upload, environment)
@@ -41,18 +39,14 @@ K_TRACK = {"200_16_kernel1": (200, 16, True, 4), "300_16_kernel1": (300, 16, Tru
            "300_32_kernel1": (300, 32, True, 4), "600_32": (600, 32, False, 3), "1500_32": (1500, 32, False, 3)}
 # D. k_track with measured occlusions: n_lines = n_points, bins
 OCCLUSION = [(n, bins) for n in (200, 300, 600, 1500) for bins in (16, 32)]
-# E. cluster-fused chains: (variant, items, bins)
-CLUSTER = [(v, n, bins) for v in ("projected", "constrained") for n in (200, 300) for bins in (16, 32)]
 
 CASES = ([f"test_track2_two_modalities[{k}]" for k in TWO_MODALITIES] + ["test_track2_two_modalities_border_32_bins"] +
          [f"test_track2_one_modality_per_body[{b}]" for b in ONE_MODALITY_BINS] +
          [f"test_k_track[{k}]" for k in K_TRACK] +
          [f"test_k_track_measured_occlusion[{n}_{b}]" for n, b in OCCLUSION] +
-         ["test_k_track_occlusion_fallback_600", "test_k_track_renderer_checks_600"] +
-         [f"test_cluster_chain[{v}_{n}_{b}]" for v, n, b in CLUSTER])
+         ["test_k_track_occlusion_fallback_600", "test_k_track_renderer_checks_600"])
 
 # (kernel, threads, items_per_thread, lut_smem, occ) as m3tb_debug_last_launch reports it -> the cases that launch it.
-# The cluster launch reports occ = 0: k_track is only instantiated with OCC = false under CLUSTER.
 COVERAGE = {
     ("k_track2", 1024, 1, 1, 0): ["test_track2_two_modalities[16_full]"],
     ("k_track2", 1024, 1, 0, 0): ["test_track2_two_modalities[32_full]", "test_track2_two_modalities[32_tma0]",
@@ -75,10 +69,6 @@ COVERAGE = {
     ("k_track", 512, 1, 0, 1): ["test_k_track_measured_occlusion[300_32]"],
     ("k_track", 512, 2, 0, 1): ["test_k_track_measured_occlusion[600_32]", "test_k_track_occlusion_fallback_600"],
     ("k_track", 512, 4, 0, 1): ["test_k_track_measured_occlusion[1500_32]"],
-    ("k_track_cluster", 256, 1, 1, 0): ["test_cluster_chain[projected_200_16]", "test_cluster_chain[constrained_200_16]"],
-    ("k_track_cluster", 256, 1, 0, 0): ["test_cluster_chain[projected_200_32]", "test_cluster_chain[constrained_200_32]"],
-    ("k_track_cluster", 256, 2, 1, 0): ["test_cluster_chain[projected_300_16]", "test_cluster_chain[constrained_300_16]"],
-    ("k_track_cluster", 256, 2, 0, 0): ["test_cluster_chain[projected_300_32]", "test_cluster_chain[constrained_300_32]"],
 }
 _FIELDS = ("kernel", "threads", "items_per_thread", "lut_smem", "occ")
 
@@ -423,96 +413,3 @@ def test_k_track_renderer_checks_600(capi, oracle, synth, case):
     assert dl > 0 and dp > 0, (dl, dp)
     # region checking against start-pose renderings keeps few lines: 2081 of 16800 line slots (12 %) on an H100
     _parity(capi, oracle, wl, case, min_valid_lines=0.1, min_valid_points=0.3)
-
-
-# ---- E. cluster-fused kinematic structures --------------------------------------------------------------------------
-def _sync_joint_poses(dst, src):
-    """The joint poses of oracle `src`'s structures into oracle `dst`'s (same workload)."""
-    for d, so in zip(dst.structure_objs, src.structure_objs):
-        b2j, j2p = so.joint_poses()
-        for k in range(len(so.spec.links)):
-            d.links[k].body2joint[:] = b2j[k].reshape(12).tolist()
-            d.links[k].joint2parent[:] = j2p[k].reshape(12).tolist()
-
-
-@pytest.mark.parametrize("variant,n,bins", CLUSTER, ids=[f"{v}_{n}_{b}" for v, n, b in CLUSTER])
-def test_cluster_chain(capi, oracle, synth, monkeypatch, case, variant, n, bins):
-    """M3TB_CLUSTER=1: two 2-link chains, each one thread-block cluster running the whole corr x update loop nest in
-    one k_track launch (1 item per thread at 200 lines / points, 2 at 300; the LUT in shared memory at 16 bins and in
-    global memory at 32), Optimizer::CalculateOptimization by the cluster leader.
-
-    Every correspondence iteration starts all three sides (device, mirror oracle, reference-faithful oracle) from the
-    faithful oracle's body and joint poses (test_gpu_structures._resync). Per-line / per-point records are bit-exact
-    against the mirror oracle; body and joint poses within 1e-4 of the faithful oracle (test_gpu_structures' bars)
-    except where the two oracle modes themselves end the iteration further apart than that, and within 1e-5 of the
-    mirror oracle everywhere. Such a split moves every link of the chain at once (one optimisation), so it is counted
-    per structure: measured on an H100, the constrained chains at 32 bins split once (2.6e-3 rad at 200 items,
-    1.2e-4 rad at 300), identically on the cluster-fused and on the multi-launch path."""
-    from test_gpu_structures import TOL_POSE_M, TOL_POSE_RAD, _resync
-    wl = synth.make_chain_workload(n_chains=2, n_links=2, n_lines=n, n_points=n, n_divides=2, variant=variant, seed=4)
-    wl.region = dataclasses.replace(wl.region, n_histogram_bins=bins)
-    monkeypatch.setenv("M3TB_CLUSTER", "1")   # read at context creation
-    ctx = capi.context_from_workload(wl)
-    monkeypatch.delenv("M3TB_CLUSTER")
-    assert ctx.n_structures() == 2
-    faithful = oracle.OracleTracker(wl, rotation_mode=oracle.ROTATION_POLAR, exp_mode=oracle.EXP_PADE)
-    mirror = oracle.OracleTracker(wl, rotation_mode=oracle.ROTATION_LINEAR, exp_mode=oracle.EXP_RODRIGUES)
-    for o in (faithful, mirror):
-        o.start_modalities(0)
-    ctx.start_modalities(0)
-    worst = dict(mirror_m=0.0, mirror_rad=0.0, mirror_joint=0.0, faithful_m=0.0, faithful_rad=0.0, faithful_joint=0.0)
-    launch = None
-    n_links = wl.notes["n_links"]
-    structure_of = np.array([i for i, sp in enumerate(wl.structures) for _ in sp.links])
-    mode_splits = valid_lines = valid_points = 0
-    for corr in range(wl.n_corr_iterations):
-        _resync(ctx, faithful, wl)
-        mirror.set_poses(faithful.get_poses())
-        _sync_joint_poses(mirror, faithful)
-        before = ctx.launch_count
-        ctx.corr_iteration(0, corr, wl.n_update_iterations)
-        assert ctx.launch_count - before == 1, (case, corr)   # the fused path, not k_track + k_structure
-        launch = launch or ctx.last_launch()
-        for b in range(wl.n_bodies):
-            nl_, view = mirror.region_correspondences(b, 0, corr)
-            assert ctx.get_closest_views(b)[0] == view, (case, corr, b)
-            lines = ctx.get_region_lines(b, wl.lines_per_body)
-            assert_lines_bit_equal(lines, mirror.lines[b][:nl_])
-            valid_lines += int((lines["valid"] != 0).sum())
-            np_, view = mirror.depth_correspondences(b, 0, corr)
-            assert ctx.get_closest_views(b)[1] == view, (case, corr, b)
-            pts = ctx.get_depth_points(b, wl.points_per_body)
-            assert_points_bit_equal(pts, mirror.points[b][:np_])
-            valid_points += int((pts["valid"] != 0).sum())
-        for o in (faithful, mirror):
-            o.tracking_step(0, n_corr=corr + 1, corr_begin=corr)
-        gpu = ctx.get_poses()
-        st, sr = pose_error(mirror.get_poses(), faithful.get_poses())
-        split = np.zeros(len(wl.structures), bool)
-        np.logical_or.at(split, structure_of, (st >= TOL_POSE_M) | (sr >= TOL_POSE_RAD))
-        mode_splits += int(split.sum())
-        comparable = ~split[structure_of]
-        for side, o in (("mirror", mirror), ("faithful", faithful)):
-            dt, dr = pose_error(gpu, o.get_poses())
-            keep = np.ones(wl.n_bodies, bool) if side == "mirror" else comparable
-            if keep.any():
-                worst[f"{side}_m"] = max(worst[f"{side}_m"], dt[keep].max())
-                worst[f"{side}_rad"] = max(worst[f"{side}_rad"], dr[keep].max())
-            for i, so in enumerate(o.structure_objs):
-                if side == "faithful" and split[i]:
-                    continue
-                b2j, j2p, _ = ctx.get_link_poses(i, n_links)
-                ob2j, oj2p = so.joint_poses()
-                worst[f"{side}_joint"] = max(worst[f"{side}_joint"], np.abs(j2p - oj2p).max(), np.abs(b2j - ob2j).max())
-    ctx.close()
-    record(case, bodies=wl.n_bodies, valid_lines=valid_lines, valid_points=valid_points, oracle_mode_splits=mode_splits,
-           launch=launch, **{k: float(f"{v:.3e}") for k, v in worst.items()})
-    _check_launch(case, launch)
-    n_slots = wl.n_bodies * wl.n_corr_iterations
-    assert valid_lines > 0.3 * wl.lines_per_body * n_slots and valid_points > 0.3 * wl.points_per_body * n_slots, \
-        (valid_lines, valid_points)
-    assert mode_splits <= max(1, 0.05 * len(wl.structures) * wl.n_corr_iterations), mode_splits
-    assert worst["mirror_m"] < 1e-5 and worst["mirror_rad"] < 1e-5 and worst["mirror_joint"] < 1e-5, worst
-    assert worst["faithful_m"] < TOL_POSE_M and worst["faithful_rad"] < TOL_POSE_RAD, worst
-    assert worst["faithful_joint"] < 1e-4, worst
-    _histograms_exact(capi, oracle, wl, case)

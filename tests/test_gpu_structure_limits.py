@@ -1,4 +1,4 @@
-"""The device's kinematic-structure solve (k_structure; the cluster-fused k_track) against the float64 restatement of
+"""The device's kinematic-structure solve (k_structure) against the float64 restatement of
 Optimizer::CalculateOptimization (tests/structure_reference.py) at the limits m3tb_set_structure accepts and in its
 degenerate cases.
 
@@ -16,7 +16,7 @@ import numpy as np
 import pytest
 
 import structure_reference as sr
-from helpers import pose_error, record
+from helpers import record
 
 pytestmark = pytest.mark.gpu
 
@@ -259,52 +259,3 @@ def test_singular_system_pseudo_inverse(capi, oracle, synth, wl64):
         assert np.all(np.delete(theta_g, leaf_t) != 0.0)
     run.report("structure_pseudo_inverse", zero_pivots=3, zeroed_unknowns=leaf_t)
     run.close()
-
-
-def _cluster_limit_structure(synth, wl, chain):
-    """The chain's constrained shape (8 six-DoF links, 7 constraints of 5 rows) with 9 of its constraints repeated:
-    48 DoF + 80 hard rows = 128 unknowns, the largest system a cluster of 8 CTAs can be handed. The repeated rows are
-    bit-identical copies, so the multipliers' split between copies is decided by rounding - but the same rounding on
-    both paths, whose per-body sums agree bit for bit with at most 256 lines / points per body."""
-    import copy
-    spec = copy.deepcopy(wl.structures[chain])
-    base = [c for c in spec.constraints if not c.soft]
-    spec.constraints = base + [copy.deepcopy(base[k % len(base)]) for k in range(9)]
-    return spec
-
-
-def test_cluster_fused_solve_at_128_unknowns(capi, synth, monkeypatch):
-    wl = synth.make_chain_workload(n_chains=2, n_links=8, n_lines=200, n_points=200, n_divides=2, variant="constrained",
-                                   seed=8)
-    wl.structures = [_cluster_limit_structure(synth, wl, c) for c in range(2)]
-    spec = wl.structures[0]
-    assert (sr.dof_of(spec), sr.n_unknowns(spec), len(spec.constraints)) == (48, 128, 16)
-    smem = sr.spec_smem_bytes(spec)
-    assert smem > SMEM_48K
-    monkeypatch.setenv("M3TB_CLUSTER", "1")   # read at context creation
-    ctx_a = capi.context_from_workload(wl)
-    monkeypatch.delenv("M3TB_CLUSTER")
-    ctx_b = capi.context_from_workload(wl)
-    for c in (ctx_a, ctx_b):
-        c.start_modalities(0)
-    la, lb = ctx_a.launch_count, ctx_b.launch_count
-    ctx_a.corr_iteration(0, 0, wl.n_update_iterations)
-    ctx_b.corr_iteration(0, 0, wl.n_update_iterations)
-    launch = ctx_a.last_launch()
-    assert launch["kernel"] == "k_track_cluster" and ctx_a.launch_count - la == 1, launch
-    assert ctx_b.launch_count - lb == 2 * wl.n_update_iterations
-    dt, dr = pose_error(ctx_a.get_poses(), ctx_b.get_poses())
-    assert dt.max() < 1e-5 and dr.max() < 1e-4, (dt.max(), dr.max())
-    worst = 0.0
-    for i in range(2):
-        ta, ua = ctx_a.get_structure_theta(i)
-        tb, ub = ctx_b.get_structure_theta(i)
-        assert len(ta) == 128 and ua and ub
-        dev = np.abs(ta - tb).max()
-        assert dev <= 1e-3 * np.abs(tb).max(), (i, dev, np.abs(tb).max())
-        worst = max(worst, dev / np.abs(tb).max())
-    record("structure_cluster_128", kernel=launch["kernel"], struct_smem_bytes=smem,
-           dyn_smem_bytes=32768 + (smem + 127) // 128 * 128, theta_rel_dev=float(f"{worst:.3e}"),
-           pose_m=float(f"{dt.max():.3e}"), pose_rad=float(f"{dr.max():.3e}"))
-    ctx_a.close()
-    ctx_b.close()

@@ -242,42 +242,6 @@ def test_rigid_bodies_through_structure_path(capi, synth):
     ctx_b.close()
 
 
-@pytest.mark.parametrize("variant", ["projected", "constrained"])
-def test_cluster_fused_path_matches_multi_launch_path(capi, synth, variant, monkeypatch):
-    """Opt-in variant (M3TB_CLUSTER=1): chains whose links map 1:1 onto the CTAs of a thread-block cluster run the
-    whole corr x update loop nest in ONE k_track launch, Optimizer::CalculateOptimization being executed by the
-    cluster leader over distributed shared memory. Same per-line arithmetic and the same solver code as the general
-    path (k_track + k_structure per update iteration); the per-body sums are taken over 256 instead of 512 threads, so
-    the two agree to rounding: tightly after one correspondence iteration, within the chain's error growth after a
-    whole step."""
-    wl = synth.make_chain_workload(n_chains=5, n_links=8, n_lines=300, n_points=300, n_divides=4, variant=variant, seed=8)
-    monkeypatch.setenv("M3TB_CLUSTER", "1")   # read at context creation
-    ctx_a = capi.context_from_workload(wl)
-    monkeypatch.delenv("M3TB_CLUSTER")
-    ctx_b = capi.context_from_workload(wl)
-    for c in (ctx_a, ctx_b):
-        c.start_modalities(0)
-    la, lb = ctx_a.launch_count, ctx_b.launch_count
-    ctx_a.corr_iteration(0, 0, wl.n_update_iterations)
-    ctx_b.corr_iteration(0, 0, wl.n_update_iterations)
-    assert ctx_a.launch_count - la == 1
-    assert ctx_b.launch_count - lb == 2 * wl.n_update_iterations
-    dt, dr = pose_error(ctx_a.get_poses(), ctx_b.get_poses())
-    assert dt.max() < 1e-5 and dr.max() < 1e-4, (dt.max(), dr.max())
-    for i in range(5):
-        ta, ua = ctx_a.get_structure_theta(i)
-        tb, ub = ctx_b.get_structure_theta(i)
-        assert ua and ub and np.abs(ta - tb).max() <= 1e-3 * np.abs(tb).max()
-    ctx_a.set_poses(wl.start_body2world); ctx_a.reset_joint_poses()
-    ctx_b.set_poses(wl.start_body2world); ctx_b.reset_joint_poses()
-    ctx_a.tracking_step(0, wl.n_corr_iterations, wl.n_update_iterations)
-    ctx_b.tracking_step(0, wl.n_corr_iterations, wl.n_update_iterations)
-    dt, dr = pose_error(ctx_a.get_poses(), ctx_b.get_poses())
-    assert np.median(dt) < 5e-4 and np.median(dr) < 1e-2, (dt, dr)
-    ctx_a.close()
-    ctx_b.close()
-
-
 def test_reset_joint_poses_keeps_other_structures_defaults(capi, synth):
     """Link::ResetJointPoses restores each link's OWN defaults (link.cpp:243-246): re-declaring structure 1 after
     tracking must not turn structure 0's tracked joint poses into its defaults (ADVICE r01)."""

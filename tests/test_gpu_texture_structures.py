@@ -395,8 +395,7 @@ def test_removed_link_texture_leaves_no_stale_term(capi, synth):
 
 def test_textured_structure_without_silhouette_renderer_is_refused(capi, synth):
     """TextureModality::SetUp's conditions hold in the structure step too: a texture modality whose silhouette renderer
-    was detached refuses the step (M3TB_ERR_NOT_SET_UP) instead of tracking without its texture term, also where the
-    cluster-fused chain path would otherwise take the step."""
+    was detached refuses the step (M3TB_ERR_NOT_SET_UP) instead of tracking without its texture term."""
     ctx, _ = _context(capi, synth, CHAIN_POSES, texture=(0, 1, 2))
     ctx.set_structure(0, _chain(synth))
     _start(ctx, (0, 1, 2))

@@ -1,6 +1,6 @@
 """Every tracking kernel the library compiles has a GPU case that runs it, and every such case names a kernel that
 exists (no GPU needed). The instantiations are read from the sources: the M3TB_TRACK_GROUP_* lists of
-m3t_b200_track_variants.h (k_track<T, K, LUT_SMEM, OCC, CLUSTER>) and the explicit k_track2<T, LUT_SMEM> instantiations
+m3t_b200_track_variants.h (k_track<T, K, LUT_SMEM, OCC>) and the explicit k_track2<T, LUT_SMEM> instantiations
 of m3t_b200_track2_*.cu. Each becomes the tuple m3tb_debug_last_launch reports for it, (kernel, threads,
 items_per_thread, lut_smem, occ), and the set must equal the keys of test_gpu_kernel_instantiations.COVERAGE, whose
 cases assert exactly that launch."""
@@ -14,7 +14,7 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 CSRC = os.path.join(ROOT, "3dobjecttracking_b200", "csrc")
 
 _B = r"\s*(true|false)\s*"
-_X = re.compile(r"X\(\s*(\d+)\s*,\s*(\d+)\s*," + _B + "," + _B + "," + _B + r"\)")
+_X = re.compile(r"X\(\s*(\d+)\s*,\s*(\d+)\s*," + _B + "," + _B + r"\)")
 _K2 = re.compile(r"template\s+__global__\s+void\s+k_track2<\s*(\d+)\s*," + _B + ">")
 
 
@@ -24,15 +24,14 @@ def _read(path):
 
 
 def _k_track_groups():
-    """{group number: [(T, K, LUT_SMEM, OCC, CLUSTER)]} of m3t_b200_track_variants.h."""
+    """{group number: [(T, K, LUT_SMEM, OCC)]} of m3t_b200_track_variants.h."""
     text = _read(os.path.join(CSRC, "m3t_b200_track_variants.h"))
     joined = text.replace("\\\n", " ")
     groups = {}
     for line in joined.splitlines():
         m = re.match(r"\s*#define\s+M3TB_TRACK_GROUP_(\d+)\(X\)(.*)", line)
         if m:
-            groups[int(m.group(1))] = [(int(t), int(k), l == "true", o == "true", c == "true")
-                                       for t, k, l, o, c in _X.findall(m.group(2))]
+            groups[int(m.group(1))] = [(int(t), int(k), l == "true", o == "true") for t, k, l, o in _X.findall(m.group(2))]
     # an X(...) outside the group lists would not be compiled where this test looks for it
     assert len(_X.findall(text)) == sum(len(v) for v in groups.values()), "X(...) entry outside M3TB_TRACK_GROUP_*"
     return groups, joined
@@ -52,8 +51,8 @@ def compiled_instantiations():
     assert {g: len(u) for g, u in units.items()} == {g: 1 for g in groups}, units
     out = []
     for entries in groups.values():
-        for t, k, lut, occ, cluster in entries:
-            out.append(("k_track_cluster" if cluster else "k_track", t, k, int(lut), int(occ)))
+        for t, k, lut, occ in entries:
+            out.append(("k_track", t, k, int(lut), int(occ)))
     k2 = []
     for path in sorted(glob.glob(os.path.join(CSRC, "m3t_b200_track2_*.cu"))):
         k2 += [("k_track2", int(t), 1, int(lut == "true"), 0) for t, lut in _K2.findall(_read(path))]
@@ -68,7 +67,7 @@ def test_every_instantiation_has_a_case_and_every_case_an_instantiation():
     covered = set(COVERAGE)
     assert not compiled - covered, f"instantiations without a GPU case: {sorted(compiled - covered)}"
     assert not covered - compiled, f"COVERAGE rows without an instantiation: {sorted(covered - compiled)}"
-    assert len(compiled) == 24, len(compiled)   # 4 x k_track2, 16 x k_track, 4 x cluster-fused k_track
+    assert len(compiled) == 20, len(compiled)   # 4 x k_track2, 16 x k_track
 
 
 def test_coverage_names_each_case_once():
