@@ -154,7 +154,7 @@ SYMBOLS = [
     "m3tb_texture_correspondences", "m3tb_texture_gradient_hessian", "m3tb_get_texture_points",
     "m3tb_get_texture_keyframes", "m3tb_texture_crop", "m3tb_upload_texture_features_device",
     "m3tb_get_texture_feature_flags", "m3tb_orb_params_default", "m3tb_texture_detect_orb",
-    "m3tb_get_texture_detections", "m3tb_get_texture_orb_keypoints", "m3tb_refine_poses_orb",
+    "m3tb_get_texture_detections", "m3tb_get_texture_orb_keypoints", "m3tb_refine_poses_orb", "m3tb_debug_bin_image",
 ]
 
 KERNEL_NAMES = {0: None, 1: "k_track", 2: "k_track2"}
@@ -164,6 +164,22 @@ class LaunchInfo(C.Structure):
     """m3tb_launch_info: the tracking-kernel variant of the last tracking launch."""
     _fields_ = [("kernel", C.c_int32), ("threads", C.c_int32), ("items_per_thread", C.c_int32), ("lut_smem", C.c_int32),
                 ("occ", C.c_int32), ("tiles", C.c_int32), ("tma_mode", C.c_int32)]
+
+
+class RoiRecord(C.Structure):
+    """m3tb_roi_record: the colour rectangle [x0, x1) x [y0, y1) k_ingest fetched for `body`, and from which generation."""
+    _fields_ = [("body", C.c_int32), ("x0", C.c_int32), ("y0", C.c_int32), ("x1", C.c_int32), ("y1", C.c_int32),
+                ("generation", C.c_int32)]
+
+
+class BinImageInfo(C.Structure):
+    """m3tb_bin_image_info."""
+    _fields_ = [("state", C.c_int32), ("pinned", C.c_int32), ("has_image", C.c_int32), ("width", C.c_int32),
+                ("height", C.c_int32), ("generation", C.c_int32), ("n_rois", C.c_int32), ("roi_capacity", C.c_int32),
+                ("rois", C.POINTER(RoiRecord))]
+
+
+BINS_NONE, BINS_AT_INGEST = -1, -2  # m3tb_bin_image_info::state besides a bit shift
 
 
 class ModelParams(C.Structure):
@@ -255,6 +271,7 @@ def lib():
     L.m3tb_set_gradient_hessian.argtypes = [vp, ci, fp, fp]
     L.m3tb_debug_rigid_solve.argtypes = [vp, ci, ci, fp, fp, fp, fp, C.POINTER(ci)]
     L.m3tb_debug_last_launch.argtypes = [vp, C.POINTER(LaunchInfo)]
+    L.m3tb_debug_bin_image.argtypes = [vp, ci, vp, C.c_size_t, C.POINTER(BinImageInfo)]
     L.m3tb_set_body_geometry.argtypes = [vp, ci, fp, ci, fp, C.c_float, ci, ci, ci]
     L.m3tb_set_focused_renderer.argtypes = [vp, ci, ci, ci, ci, C.c_float, C.c_float, ci, ip, ci, ip, ci]
     L.m3tb_attach_renderer.argtypes = [vp, ci, ci, ci, ci]
@@ -1079,6 +1096,21 @@ class Context:
         d = {k: int(getattr(info, k)) for k, _ in LaunchInfo._fields_}
         d["kernel"] = KERNEL_NAMES.get(d["kernel"], d["kernel"])
         return d
+
+    def debug_bin_image(self, cam):
+        """(image, info) of m3tb_debug_bin_image: colour camera `cam`'s bin-index image ([H, W] u16 lookup-table slots,
+        None when the camera has none) and its state as a dict (state, pinned, generation, rois: one dict per region
+        body on the camera)."""
+        rois = (RoiRecord * max(self.n_bodies, 1))()
+        info = BinImageInfo(roi_capacity=max(self.n_bodies, 1), rois=rois)
+        self._ck(self.L.m3tb_debug_bin_image(self.h, cam, None, 0, C.byref(info)))
+        img = None
+        if info.has_image:
+            img = np.zeros((info.height, info.width), np.uint16)
+            self._ck(self.L.m3tb_debug_bin_image(self.h, cam, img.ctypes.data, img.strides[0], C.byref(info)))
+        d = {k: int(getattr(info, k)) for k in ("state", "pinned", "has_image", "width", "height", "generation")}
+        d["rois"] = [{k: int(getattr(rois[i], k)) for k, _ in RoiRecord._fields_} for i in range(info.n_rois)]
+        return img, d
 
     def get_closest_views(self, body):
         a, b = C.c_int(0), C.c_int(0)

@@ -3656,6 +3656,36 @@ int m3tb_debug_last_launch(m3tb_ctx* ctx, m3tb_launch_info* out) {
   return M3TB_OK;
 }
 
+int m3tb_debug_bin_image(m3tb_ctx* ctx, int cam, uint16_t* out, size_t out_pitch, m3tb_bin_image_info* info) {
+  CHECK_CTX();
+  if (cam < 0 || cam >= ctx->max_cameras || !info) return Fail(ctx, M3TB_ERR_INVALID, "bad bin-image arguments");
+  const CameraDev& c = ctx->h_ccams[cam];
+  if (out && c.bins && out_pitch < size_t(c.width) * 2) return Fail(ctx, M3TB_ERR_INVALID, "pitch smaller than a row");
+  if (ctx->pf.ingest_stream) CU(cudaStreamSynchronize(ctx->pf.ingest_stream));  // a prefetched ingest writes the image
+  CU(cudaStreamSynchronize(ctx->stream));
+  info->state = ctx->bin_shift[cam];
+  info->pinned = c.host_src ? 1 : 0;
+  info->has_image = c.bins ? 1 : 0;
+  info->width = c.width;
+  info->height = c.height;
+  info->generation = c.generation;
+  info->n_rois = 0;
+  std::vector<RoiRecord> roi(2 * size_t(ctx->max_bodies));
+  CU(cudaMemcpy(roi.data(), ctx->d_roi, sizeof(RoiRecord) * roi.size(), cudaMemcpyDeviceToHost));
+  for (int b = 0; b < ctx->n_bodies; ++b) {
+    const BodyDev& B = ctx->h_bodies[b];
+    if (!B.set || !B.has_region || B.color_camera != cam) continue;
+    if (info->rois && info->n_rois < info->roi_capacity) {
+      const RoiRecord& r = roi[2 * size_t(b)];
+      info->rois[info->n_rois] = m3tb_roi_record{b, r.x0, r.y0, r.x1, r.y1, r.generation};
+    }
+    info->n_rois++;
+  }
+  if (out && c.bins)
+    CU(cudaMemcpy2D(out, out_pitch, c.bins, c.bin_pitch, size_t(c.width) * 2, c.height, cudaMemcpyDeviceToHost));
+  return M3TB_OK;
+}
+
 int m3tb_debug_closest_view(const float* orientations, int n_views, const float* queries, int n_queries,
                             const int* prev, int* out_scan, int* out_pruned, int* out_evaluated) {
   if (!orientations || n_views <= 0 || !queries || n_queries < 0 || !out_scan || !out_pruned) return M3TB_ERR_INVALID;

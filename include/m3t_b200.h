@@ -813,6 +813,30 @@ typedef struct m3tb_launch_info {
 } m3tb_launch_info;
 int m3tb_debug_last_launch(m3tb_ctx* ctx, m3tb_launch_info* out);
 
+/* Test aid: the histogram bin-index image of colour camera `cam` (one u16 lookup-table slot per pixel, the source of
+ * k_track2's colour tiles) and the state that says which of its pixels are meant to be valid. Waits for the context's
+ * stream and any prefetched ingest first. `out` (rows `out_pitch` bytes apart, width x height u16) may be null; nothing
+ * is copied when the camera has no bin-index image (its frame is not in the shared pool, or the pool's width is not a
+ * multiple of 4). info->rois (capacity info->roi_capacity, set by the caller) receives the colour ROI record of every
+ * region body on the camera, in body order; info->n_rois is their number even when it exceeds the capacity. */
+typedef struct m3tb_roi_record {
+  int32_t body;
+  int32_t x0, y0, x1, y1;    /* the rectangle k_ingest fetched: [x0, x1) x [y0, y1) */
+  int32_t generation;        /* the camera generation it was fetched from, -1: never */
+} m3tb_roi_record;
+typedef struct m3tb_bin_image_info {
+  int32_t state;             /* bit shift the image was written with; -1 none that matches the frame; -2 a pinned frame
+                                whose bin indices the next ingest writes */
+  int32_t pinned;            /* 1: the camera holds a pinned frame (device copy valid inside the ROIs only) */
+  int32_t has_image;         /* 1: the camera has a bin-index image (and `out` received it) */
+  int32_t width, height;
+  int32_t generation;        /* the camera's frame generation */
+  int32_t n_rois;
+  int32_t roi_capacity;      /* in: capacity of rois */
+  m3tb_roi_record* rois;     /* in: caller memory, may be null */
+} m3tb_bin_image_info;
+int m3tb_debug_bin_image(m3tb_ctx* ctx, int cam, uint16_t* out, size_t out_pitch, m3tb_bin_image_info* info);
+
 /* Host only, meant for tests. *live (if not null) receives the number of CUDA resources the library holds across all
  * contexts: device allocations, pinned host allocations, streams and events. fail_after > 0 makes the fail_after-th
  * resource creation from now on fail as an allocation failure (cudaErrorMemoryAllocation) without calling CUDA;
