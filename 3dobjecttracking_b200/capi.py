@@ -155,6 +155,8 @@ SYMBOLS = [
     "m3tb_get_texture_keyframes", "m3tb_texture_crop", "m3tb_upload_texture_features_device",
     "m3tb_get_texture_feature_flags", "m3tb_orb_params_default", "m3tb_texture_detect_orb",
     "m3tb_get_texture_detections", "m3tb_get_texture_orb_keypoints", "m3tb_refine_poses_orb", "m3tb_debug_bin_image",
+    "m3tb_set_focused_normal_renderer", "m3tb_render_focused_normals", "m3tb_get_focused_normal_rendering",
+    "m3tb_get_normalized_depth_image",
 ]
 
 KERNEL_NAMES = {0: None, 1: "k_track", 2: "k_track2"}
@@ -313,6 +315,10 @@ def lib():
     L.m3tb_undistortion_map.argtypes = [C.POINTER(Intrinsics), fp, C.POINTER(Intrinsics), vp, C.c_size_t]
     L.m3tb_set_camera_undistortion.argtypes = [vp, ci, ci, vp, C.c_size_t, ci, C.c_int32]
     L.m3tb_get_camera_image.argtypes = [vp, ci, ci, vp, C.c_size_t]
+    L.m3tb_set_focused_normal_renderer.argtypes = [vp, ci, ci, ci, ci, C.c_float, C.c_float, ip, ci, ip, ci]
+    L.m3tb_render_focused_normals.argtypes = [vp]
+    L.m3tb_get_focused_normal_rendering.argtypes = [vp, ci, vp, vp, fp, fp, fp, fp, fp, ip]
+    L.m3tb_get_normalized_depth_image.argtypes = [vp, ci, ci, C.c_float, C.c_float, vp, C.c_size_t]
     _lib = L
     return L
 
@@ -656,6 +662,61 @@ class Context:
         self._ck(self.L.m3tb_get_full_rendering(self.h, renderer, depth_ptr, depth_pitch, silhouette_ptr,
                                                 silhouette_pitch, normal_ptr, normal_pitch, C.byref(a), C.byref(b)))
         return dict(projection_term_a=np.float32(a.value), projection_term_b=np.float32(b.value))
+
+    def set_focused_normal_renderer(self, renderer, camera_kind, camera, geometry_bodies, referenced_bodies,
+                                    image_size=200, z_min=0.02, z_max=10.0):
+        """FocusedNormalRenderer of camera `camera` (camera_kind "color" | "depth", or 0 | 1) drawing `geometry_bodies`
+        in that order and focusing on `referenced_bodies`."""
+        kind = {"color": 0, "depth": 1}.get(camera_kind, camera_kind)
+        g = np.ascontiguousarray(geometry_bodies, np.int32)
+        r = np.ascontiguousarray(referenced_bodies, np.int32)
+        ip = C.POINTER(C.c_int)
+        self._ck(self.L.m3tb_set_focused_normal_renderer(self.h, renderer, int(kind), camera, image_size, z_min, z_max,
+                                                         g.ctypes.data_as(ip), g.size, r.ctypes.data_as(ip), r.size))
+        self._focused_normal_refs = getattr(self, "_focused_normal_refs", {})
+        self._focused_normal_refs[renderer] = (image_size, r.size)
+
+    def render_focused_normals(self):
+        """FocusedNormalRenderer::StartRendering of every focused normal renderer from the current poses."""
+        self._ck(self.L.m3tb_render_focused_normals(self.h))
+
+    def get_focused_normal_rendering(self, renderer):
+        """dict(depth [S,S] u16, normal [S,S,4] u8 in GL_BGRA order, corner_u, corner_v, scale, projection_term_a / b
+        (float32), visible [n_referenced] int32) of the renderer's last render."""
+        S, _ = self._focused_normal_refs[renderer]
+        depth = np.zeros((S, S), np.uint16)
+        normal = np.zeros((S, S, 4), np.uint8)
+        out = self.get_focused_normal_rendering_to(renderer, depth.ctypes.data, normal.ctypes.data)
+        out.update(depth=depth, normal=normal)
+        return out
+
+    def get_focused_normal_rendering_to(self, renderer, depth_ptr=None, normal_ptr=None):
+        """The images into caller memory, host or device (e.g. torch tensors' data_ptr()), rows packed; a None pointer
+        skips that image. Returns dict(corner_u, corner_v, scale, projection_term_a / b, visible)."""
+        _, n_ref = self._focused_normal_refs[renderer]
+        f = [C.c_float(0.0) for _ in range(5)]
+        vis = np.zeros(n_ref, np.int32)
+        self._ck(self.L.m3tb_get_focused_normal_rendering(self.h, renderer, depth_ptr, normal_ptr,
+                                                          *[C.byref(x) for x in f],
+                                                          vis.ctypes.data_as(C.POINTER(C.c_int))))
+        out = dict(zip(("corner_u", "corner_v", "scale", "projection_term_a", "projection_term_b"),
+                       (np.float32(x.value) for x in f)))
+        out.update(visible=vis)
+        return out
+
+    def get_normalized_depth_image(self, source, id, min_depth, max_depth, width, height):
+        """NormalizedDepthImage(min_depth, max_depth) [H,W] u8 of depth camera `id` (source "camera" / 0) or full
+        renderer `id` (source "full_renderer" / 1)."""
+        out = np.zeros((height, width), np.uint8)
+        self.get_normalized_depth_image_to(source, id, min_depth, max_depth, out.ctypes.data, out.strides[0])
+        return out
+
+    def get_normalized_depth_image_to(self, source, id, min_depth, max_depth, ptr, pitch):
+        """The same into caller memory, host or device (e.g. a torch uint8 tensor's data_ptr()), rows `pitch` bytes
+        apart."""
+        src = {"camera": 0, "full_renderer": 1}.get(source, source)
+        self._ck(self.L.m3tb_get_normalized_depth_image(self.h, int(src), id, min_depth, max_depth, C.c_void_p(ptr),
+                                                        pitch))
 
     def generate_depth_model(self, model_id, body, occlusion_bodies=(), params=None):
         """DepthModel::GenerateModel on the device from the geometry of m3tb_set_body_geometry (params: ModelParams,

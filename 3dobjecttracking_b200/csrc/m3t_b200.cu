@@ -245,7 +245,7 @@ struct m3tb_ctx {
     DeviceBuffer<uint64_t> zbuf;          // cleared; k_view_resolve clears it again after each draw
     DeviceBuffer<uint8_t> normal;
     DeviceBuffer<uint8_t> image;          // viewers: the frame blended with the normal image
-    DeviceBuffer<uint16_t> depth;         // VK_FULL
+    DeviceBuffer<uint16_t> depth;         // VK_FULL, VK_FOCUSED
     DeviceBuffer<uint8_t> silhouette;     // VK_FULL
   };
   struct ViewSlotHost {
@@ -254,12 +254,26 @@ struct m3tb_ctx {
     std::vector<int> geometry;
     float opacity = 0.0f, min_depth = 0.0f, max_depth = 0.0f;  // viewers
     int id_type = 0;                                           // VK_FULL
-    float z_min = 0.0f, z_max = 0.0f;                          // VK_FULL
-    int width = 0, height = 0;            // of the images (the camera's size when they were made)
+    float z_min = 0.0f, z_max = 0.0f;                          // VK_FULL, VK_FOCUSED
+    int image_size = 0;                                        // VK_FOCUSED
+    std::vector<int> referenced;                               // VK_FOCUSED
+    int first_referenced = 0;             // VK_FOCUSED: where its visible flags are in d_focus_visible after a render
+    int width = 0, height = 0;            // of the images (the camera's size when they were made; VK_FOCUSED: S x S)
     ViewImages images;
     bool drawn = false;                   // the images hold a result (m3tb_get_viewer_image / m3tb_get_full_rendering)
   };
   std::vector<ViewSlotHost> viewers, full_renderers;
+  // focused normal renderers (m3tb_set_focused_normal_renderer / m3tb_render_focused_normals, VK_FOCUSED), dense ids of
+  // their own, and the k_view_focus tables of their last render, grown lazily, each set all or nothing
+  std::vector<ViewSlotHost> focused_normal_renderers;
+  std::vector<FocusDev> h_focus;
+  std::vector<int> h_focus_referenced;
+  std::vector<float> h_focus_radius;
+  DeviceBuffer<FocusDev> d_focus;
+  DeviceBuffer<int> d_focus_referenced, d_focus_visible;
+  DeviceBuffer<float> d_focus_radius;
+  DeviceBuffer<RenderOutDev> d_focus_out;
+  DeviceBuffer<uint8_t> d_normalized_depth;  // m3tb_get_normalized_depth_image into host memory, grown lazily
   // tables of one update (or one full render), grown lazily, each set all or nothing
   std::vector<ViewerDev> h_view_viewers;
   std::vector<ViewDrawDev> h_view_draws;
@@ -3943,9 +3957,9 @@ using ViewSlotHost = m3tb_ctx::ViewSlotHost;
 static int MakeViewImages(m3tb_ctx* ctx, int kind, int width, int height, m3tb_ctx::ViewImages& im) {
   const size_t n = size_t(width) * height;
   CU(im.zbuf.create(n));
-  if (kind == VK_FULL) {
+  if (kind == VK_FULL || kind == VK_FOCUSED) {
     CU(im.depth.create(n));
-    CU(im.silhouette.create(n));
+    if (kind == VK_FULL) CU(im.silhouette.create(n));
     CU(im.normal.create(4 * n));
   } else {
     CU(im.normal.create(4 * n));
@@ -3955,7 +3969,14 @@ static int MakeViewImages(m3tb_ctx* ctx, int kind, int width, int height, m3tb_c
   return M3TB_OK;
 }
 
-static int LaunchView(m3tb_ctx* ctx, size_t n_triangles, int max_triangles, int max_pixels);
+static int LaunchView(m3tb_ctx* ctx, size_t n_triangles, int max_triangles, int max_pixels, const FocusArgs* focus);
+
+// The image size of a slot: its camera's, or image_size x image_size for a focused normal renderer
+static void SlotSize(m3tb_ctx* ctx, const ViewSlotHost& s, int& width, int& height) {
+  const CameraDev& c = CameraOf(ctx, s.camera_kind == 0, s.camera);
+  width = s.kind == VK_FOCUSED ? s.image_size : c.width;
+  height = s.kind == VK_FOCUSED ? s.image_size : c.height;
+}
 
 // FullRenderer::CalculateProjectionMatrix (renderer.cpp:257-264) from the camera's intrinsics, and its world2camera
 static void FullProjection(const CameraDev& c, float z_min, float z_max, ViewerDev& d) {
@@ -3974,25 +3995,26 @@ static void FullProjection(const CameraDev& c, float z_min, float z_max, ViewerD
 // of the table or the next free one. The images of the slot it replaces are kept while the camera has their size;
 // otherwise new ones are made before anything changes.
 static int InstallViewSlot(m3tb_ctx* ctx, std::vector<ViewSlotHost>& table, int id, ViewSlotHost& slot) {
-  const CameraDev& c = CameraOf(ctx, slot.camera_kind == 0, slot.camera);
+  int W, H;
+  SlotSize(ctx, slot, W, H);
   ViewSlotHost* old = id < int(table.size()) ? &table[id] : nullptr;
-  if (!old || old->width != c.width || old->height != c.height) {
-    int rc = MakeViewImages(ctx, slot.kind, c.width, c.height, slot.images);
+  if (!old || old->width != W || old->height != H) {
+    int rc = MakeViewImages(ctx, slot.kind, W, H, slot.images);
     if (rc) return rc;
     if (old) CU(cudaStreamSynchronize(ctx->stream));  // a draw in flight may still use the old images
   } else {
     slot.images = std::move(old->images);
   }
-  slot.width = c.width;
-  slot.height = c.height;
+  slot.width = W;
+  slot.height = H;
   if (old) *old = std::move(slot);
   else table.push_back(std::move(slot));
   return M3TB_OK;
 }
 
-// One draw of every slot of `table` (ctx->viewers or ctx->full_renderers) from the current poses: the three k_view_*
-// launches over tables filled here
-static int DrawViewSlots(m3tb_ctx* ctx, std::vector<ViewSlotHost>& table) {
+// One draw of every slot of `table` (ctx->viewers, ctx->full_renderers or ctx->focused_normal_renderers) from the
+// current poses: the three k_view_* launches over tables filled here, after k_view_focus when `focus` is given
+static int DrawViewSlots(m3tb_ctx* ctx, std::vector<ViewSlotHost>& table, const FocusArgs* focus = nullptr) {
   const int ns = int(table.size());
   if (ns == 0) return M3TB_OK;
   // images of slots whose camera changed size since they were made (m3tb_set_*_camera), all or nothing
@@ -4000,9 +4022,10 @@ static int DrawViewSlots(m3tb_ctx* ctx, std::vector<ViewSlotHost>& table) {
   bool any_remade = false;
   for (int v = 0; v < ns; ++v) {
     const auto& h = table[v];
-    const CameraDev& c = CameraOf(ctx, h.camera_kind == 0, h.camera);
-    if (h.width == c.width && h.height == c.height) continue;
-    int rc = MakeViewImages(ctx, h.kind, c.width, c.height, remade[v]);
+    int W, H;
+    SlotSize(ctx, h, W, H);
+    if (h.width == W && h.height == H) continue;
+    int rc = MakeViewImages(ctx, h.kind, W, H, remade[v]);
     if (rc) return rc;
     any_remade = true;
   }
@@ -4011,9 +4034,7 @@ static int DrawViewSlots(m3tb_ctx* ctx, std::vector<ViewSlotHost>& table) {
     for (int v = 0; v < ns; ++v) {
       if (!remade[v].zbuf) continue;
       auto& h = table[v];
-      const CameraDev& c = CameraOf(ctx, h.camera_kind == 0, h.camera);
-      h.width = c.width;
-      h.height = c.height;
+      SlotSize(ctx, h, h.width, h.height);
       h.images = std::move(remade[v]);
       h.drawn = false;
     }
@@ -4030,7 +4051,11 @@ static int DrawViewSlots(m3tb_ctx* ctx, std::vector<ViewSlotHost>& table) {
     const CameraDev& c = CameraOf(ctx, h.camera_kind == 0, h.camera);
     ViewerDev& d = V[v];
     d.kind = h.kind;
-    if (h.kind == VK_FULL) {
+    if (h.kind == VK_FOCUSED) {  // the projection is k_view_focus's
+      d.width = d.height = h.image_size;
+      std::memcpy(d.w2c, c.w2c, sizeof(d.w2c));
+      d.depth = h.images.depth;
+    } else if (h.kind == VK_FULL) {
       FullProjection(c, h.z_min, h.z_max, d);
       d.depth = h.images.depth;
       d.silhouette = h.images.silhouette;
@@ -4065,9 +4090,9 @@ static int DrawViewSlots(m3tb_ctx* ctx, std::vector<ViewSlotHost>& table) {
       n_triangles += size_t(G.n_triangles);
       max_triangles = std::max(max_triangles, G.n_triangles);
     }
-    max_pixels = std::max(max_pixels, c.width * c.height);
+    max_pixels = std::max(max_pixels, d.width * d.height);
   }
-  int rc = LaunchView(ctx, n_triangles, max_triangles, max_pixels);
+  int rc = LaunchView(ctx, n_triangles, max_triangles, max_pixels, focus);
   if (rc) return rc;
   for (auto& h : table) h.drawn = true;
   return M3TB_OK;
@@ -4105,8 +4130,9 @@ int m3tb_update_viewers(m3tb_ctx* ctx) {
   return DrawViewSlots(ctx, ctx->viewers);
 }
 
-// The three k_view_* launches over the tables in ctx->h_view_viewers / h_view_draws (viewers or full renderers)
-static int LaunchView(m3tb_ctx* ctx, size_t n_triangles, int max_triangles, int max_pixels) {
+// The three k_view_* launches over the tables in ctx->h_view_viewers / h_view_draws (viewers, full renderers or focused
+// normal renderers), after k_view_focus when `focus` is given
+static int LaunchView(m3tb_ctx* ctx, size_t n_triangles, int max_triangles, int max_pixels, const FocusArgs* focus) {
   const std::vector<ViewerDev>& V = ctx->h_view_viewers;
   const std::vector<ViewDrawDev>& D = ctx->h_view_draws;
   const int nv = int(V.size());
@@ -4153,6 +4179,14 @@ static int LaunchView(m3tb_ctx* ctx, size_t n_triangles, int max_triangles, int 
   a.fan_tile = ctx->d_view_fan_tile;
   a.fan_cap = int(fan_cap);
   a.counter = ctx->d_view_counter;
+  if (focus) {
+    FocusArgs f = *focus;
+    f.viewers = ctx->d_view_viewers;
+    f.draws = ctx->d_view_draws;
+    k_view_focus<<<unsigned((f.n_focus + kViewThreads - 1) / kViewThreads), kViewThreads, 0, ctx->stream>>>(f);
+    CU(cudaGetLastError());
+    ctx->launches++;
+  }
   // the three launches always run (a grid dimension of 0 is not launchable, so empty ones get one idle block)
   const dim3 setup_grid(unsigned(std::max(1, (max_triangles + kViewThreads - 1) / kViewThreads)),
                         unsigned(std::max(1, n_draws)));
@@ -4258,6 +4292,209 @@ int m3tb_get_full_rendering(m3tb_ctx* ctx, int renderer, void* depth_u16, size_t
   if (projection_term_a) *projection_term_a = h.z_max * h.z_min * float(USHRT_MAX) / (h.z_max - h.z_min);
   if (projection_term_b) *projection_term_b = h.z_max * float(USHRT_MAX) / (h.z_max - h.z_min);
   if (to_host) CU(cudaStreamSynchronize(ctx->stream));
+  return M3TB_OK;
+}
+
+// ---- focused normal renderers (FocusedNormalRenderer, normal_renderer.cpp:295-423) ---------------------------------
+
+int m3tb_set_focused_normal_renderer(m3tb_ctx* ctx, int renderer, int camera_kind, int camera, int image_size,
+                                     float z_min, float z_max, const int* geometry_bodies, int n_geometry,
+                                     const int* referenced_bodies, int n_referenced) {
+  CHECK_CTX();
+  if (renderer < 0 || renderer > int(ctx->focused_normal_renderers.size()))
+    return Fail(ctx, M3TB_ERR_INVALID, "focused normal renderer ids must be dense (0..n)");
+  if (camera_kind != 0 && camera_kind != 1) return Fail(ctx, M3TB_ERR_INVALID, "camera_kind must be 0 (colour) or 1 (depth)");
+  int rc = CheckCameraSet(ctx, camera_kind, camera);
+  if (rc) return rc;
+  if (image_size > kFocusedNormalMaxImageSize)
+    return Fail(ctx, M3TB_ERR_UNSUPPORTED, "image_size above " + std::to_string(kFocusedNormalMaxImageSize));
+  if (image_size < 1 || !(z_min > 0.0f) || !(z_max > z_min) || !std::isfinite(z_max))
+    return Fail(ctx, M3TB_ERR_INVALID, "bad image_size / z_min / z_max");
+  if (!geometry_bodies || n_geometry < 1 || n_geometry > 65535 || !referenced_bodies || n_referenced < 1)
+    return Fail(ctx, M3TB_ERR_INVALID, "a renderer needs geometry bodies and referenced bodies");
+  rc = CheckBodyList(ctx, geometry_bodies, n_geometry);
+  if (!rc) rc = CheckBodyList(ctx, referenced_bodies, n_referenced);
+  if (rc) return rc;
+  ViewSlotHost nr;
+  nr.kind = VK_FOCUSED;
+  nr.camera_kind = camera_kind;
+  nr.camera = camera;
+  nr.image_size = image_size;
+  nr.z_min = z_min;
+  nr.z_max = z_max;
+  nr.geometry.assign(geometry_bodies, geometry_bodies + n_geometry);
+  nr.referenced.assign(referenced_bodies, referenced_bodies + n_referenced);
+  return InstallViewSlot(ctx, ctx->focused_normal_renderers, renderer, nr);
+}
+
+int m3tb_render_focused_normals(m3tb_ctx* ctx) {
+  CHECK_CTX();
+  auto& table = ctx->focused_normal_renderers;
+  const int n = int(table.size());
+  if (n == 0) return M3TB_OK;
+  // k_view_focus's tables: one FocusDev per renderer, the referenced bodies and their radii
+  std::vector<FocusDev>& F = ctx->h_focus;
+  std::vector<int>& ref = ctx->h_focus_referenced;
+  std::vector<float>& radius = ctx->h_focus_radius;
+  F.assign(n, FocusDev{});
+  ref.clear();
+  radius.clear();
+  for (int v = 0; v < n; ++v) {
+    const auto& h = table[v];
+    FocusDev& f = F[v];
+    f.cam = CameraOf(ctx, h.camera_kind == 0, h.camera);
+    f.image_size = h.image_size;
+    f.z_min = h.z_min;
+    f.z_max = h.z_max;
+    f.viewer = v;
+    f.first_referenced = int(ref.size());
+    f.n_referenced = int(h.referenced.size());
+    for (int b : h.referenced) {
+      ref.push_back(b);
+      radius.push_back(ctx->h_geometry[b].radius);
+    }
+  }
+  // grown tables stay local until the render has been launched, so that a failure leaves the context as it was
+  DeviceBuffer<FocusDev> focus;
+  DeviceBuffer<int> referenced, visible;
+  DeviceBuffer<float> radii;
+  DeviceBuffer<RenderOutDev> out;
+  int rc = GrowTable(ctx, ctx->d_focus, focus, size_t(n));
+  if (!rc) rc = GrowTable(ctx, ctx->d_focus_referenced, referenced, ref.size());
+  if (!rc) rc = GrowTable(ctx, ctx->d_focus_radius, radii, ref.size());
+  if (!rc) rc = GrowTable(ctx, ctx->d_focus_visible, visible, ref.size());
+  if (!rc) rc = GrowTable(ctx, ctx->d_focus_out, out, size_t(n));
+  if (rc) return rc;
+  FocusDev* d_focus = focus ? focus.get() : ctx->d_focus.get();
+  int* d_referenced = referenced ? referenced.get() : ctx->d_focus_referenced.get();
+  float* d_radius = radii ? radii.get() : ctx->d_focus_radius.get();
+  CU(cudaMemcpyAsync(d_focus, F.data(), sizeof(FocusDev) * n, cudaMemcpyHostToDevice, ctx->stream));
+  CU(cudaMemcpyAsync(d_referenced, ref.data(), sizeof(int) * ref.size(), cudaMemcpyHostToDevice, ctx->stream));
+  CU(cudaMemcpyAsync(d_radius, radius.data(), sizeof(float) * radius.size(), cudaMemcpyHostToDevice, ctx->stream));
+  FocusArgs fa = {};
+  fa.focus = d_focus;
+  fa.n_focus = n;
+  fa.referenced = d_referenced;
+  fa.radius = d_radius;
+  fa.poses = ctx->d_poses;
+  fa.visible = visible ? visible.get() : ctx->d_focus_visible.get();
+  fa.out = out ? out.get() : ctx->d_focus_out.get();
+  const int64_t launches = ctx->launches;
+  rc = DrawViewSlots(ctx, table, &fa);
+  if (rc) {
+    // k_view_focus ran but a later launch failed: the flags and focus in the tables no longer match the images
+    if (ctx->launches != launches)
+      for (auto& h : table) h.drawn = false;
+    return rc;
+  }
+  // the replaced tables are released after the device-wide synchronisation of cudaFree (a render in flight may still
+  // use them)
+  if (focus) ctx->d_focus = std::move(focus);
+  if (referenced) ctx->d_focus_referenced = std::move(referenced);
+  if (radii) ctx->d_focus_radius = std::move(radii);
+  if (visible) ctx->d_focus_visible = std::move(visible);
+  if (out) ctx->d_focus_out = std::move(out);
+  for (int v = 0; v < n; ++v) table[v].first_referenced = F[v].first_referenced;
+  return M3TB_OK;
+}
+
+int m3tb_get_focused_normal_rendering(m3tb_ctx* ctx, int renderer, void* depth_u16, void* normal_bgra, float* corner_u,
+                                      float* corner_v, float* scale, float* projection_term_a,
+                                      float* projection_term_b, int* visible_flags) {
+  CHECK_CTX();
+  if (renderer < 0 || renderer >= int(ctx->focused_normal_renderers.size()))
+    return Fail(ctx, M3TB_ERR_INVALID, "focused normal renderer not set");
+  const auto& h = ctx->focused_normal_renderers[renderer];
+  if (!h.drawn) return Fail(ctx, M3TB_ERR_NOT_SET_UP, "focused normal renderer has not rendered since it was set");
+  const size_t S = size_t(h.image_size);
+  bool to_host = false;
+  if (depth_u16) {
+    CU(cudaMemcpyAsync(depth_u16, h.images.depth, 2 * S * S, cudaMemcpyDefault, ctx->stream));
+    to_host = to_host || !IsDevicePointer(depth_u16);
+  }
+  if (normal_bgra) {
+    CU(cudaMemcpyAsync(normal_bgra, h.images.normal, 4 * S * S, cudaMemcpyDefault, ctx->stream));
+    to_host = to_host || !IsDevicePointer(normal_bgra);
+  }
+  RenderOutDev o;
+  const bool want_focus = corner_u || corner_v || scale || projection_term_a || projection_term_b;
+  if (want_focus)
+    CU(cudaMemcpyAsync(&o, ctx->d_focus_out + renderer, sizeof(o), cudaMemcpyDeviceToHost, ctx->stream));
+  if (visible_flags)
+    CU(cudaMemcpyAsync(visible_flags, ctx->d_focus_visible + h.first_referenced, sizeof(int) * h.referenced.size(),
+                       cudaMemcpyDeviceToHost, ctx->stream));
+  if (to_host || want_focus || visible_flags) CU(cudaStreamSynchronize(ctx->stream));
+  if (corner_u) *corner_u = o.corner_u;
+  if (corner_v) *corner_v = o.corner_v;
+  if (scale) *scale = o.scale;
+  if (projection_term_a) *projection_term_a = o.projection_term_a;
+  if (projection_term_b) *projection_term_b = o.projection_term_b;
+  return M3TB_OK;
+}
+
+// ---- NormalizedDepthImage (DepthCamera, camera.cpp:108-115; FullDepthRenderer, renderer.cpp:407-427) ---------------
+
+int m3tb_get_normalized_depth_image(m3tb_ctx* ctx, int source, int id, float min_depth, float max_depth, void* dst,
+                                    size_t pitch) {
+  CHECK_CTX();
+  if ((source != M3TB_NORMALIZED_DEPTH_CAMERA && source != M3TB_NORMALIZED_DEPTH_FULL_RENDERER) || !dst)
+    return Fail(ctx, M3TB_ERR_INVALID, "bad normalized depth image arguments");
+  if (!(max_depth > min_depth)) return Fail(ctx, M3TB_ERR_INVALID, "max_depth must exceed min_depth");
+  NormalizedDepthArgs a = {};
+  if (source == M3TB_NORMALIZED_DEPTH_CAMERA) {
+    if (id < 0 || id >= ctx->max_cameras || !ctx->h_dcams[id].set)
+      return Fail(ctx, M3TB_ERR_INVALID, "depth camera not set");
+    const CameraDev& c = ctx->h_dcams[id];
+    if (!c.image) return Fail(ctx, M3TB_ERR_NOT_SET_UP, "depth camera has no image");
+    if (ctx->prefetched) CU(cudaStreamWaitEvent(ctx->stream, ctx->pf.ev_ingest_done, 0));
+    // Camera::image(): a pinned frame's device copy is valid only inside the ROIs, the frame itself is read in place
+    a.src = c.host_src ? c.host_src : c.image;
+    a.src_pitch = c.host_src ? c.host_pitch : c.pitch;
+    a.width = c.width;
+    a.height = c.height;
+    a.alpha = 255.0f / ((max_depth - min_depth) / c.depth_scale);
+    a.beta = -(min_depth / c.depth_scale) * a.alpha;
+  } else {
+    if (id < 0 || id >= int(ctx->full_renderers.size())) return Fail(ctx, M3TB_ERR_INVALID, "full renderer not set");
+    const auto& h = ctx->full_renderers[id];
+    const CameraDev& c = CameraOf(ctx, h.camera_kind == 0, h.camera);
+    if (!h.drawn || h.width != c.width || h.height != c.height)
+      return Fail(ctx, M3TB_ERR_NOT_SET_UP, "full renderer has not rendered since it was set or its camera changed size");
+    a.src = reinterpret_cast<const uint8_t*>(static_cast<const uint16_t*>(h.images.depth));
+    a.src_pitch = unsigned(2 * h.width);
+    a.width = h.width;
+    a.height = h.height;
+    a.renderer = 1;
+    a.a = h.z_max * h.z_min * float(USHRT_MAX) / (h.z_max - h.z_min);  // renderer.cpp:476-477
+    a.b = h.z_max * float(USHRT_MAX) / (h.z_max - h.z_min);
+    a.min_depth = min_depth;
+    a.delta = max_depth - min_depth;
+    a.scale = 255.0f / a.delta;
+  }
+  const size_t W = size_t(a.width), H = size_t(a.height);
+  if (pitch < W) return Fail(ctx, M3TB_ERR_INVALID, "pitch smaller than a row");
+  const bool to_host = !IsDevicePointer(dst);
+  if (to_host) {  // the kernel writes into device scratch, which is then copied
+    DeviceBuffer<uint8_t> grown;
+    int rc = GrowTable(ctx, ctx->d_normalized_depth, grown, W * H);
+    if (rc) return rc;
+    if (grown) {
+      CU(cudaStreamSynchronize(ctx->stream));  // a copy in flight may still read the scratch that is replaced
+      ctx->d_normalized_depth = std::move(grown);
+    }
+    a.dst = ctx->d_normalized_depth;
+    a.dst_pitch = W;
+  } else {
+    a.dst = static_cast<uint8_t*>(dst);
+    a.dst_pitch = pitch;
+  }
+  k_normalized_depth<<<unsigned((W * H + kViewThreads - 1) / kViewThreads), kViewThreads, 0, ctx->stream>>>(a);
+  CU(cudaGetLastError());
+  ctx->launches++;
+  if (to_host) {
+    CU(cudaMemcpy2DAsync(dst, pitch, a.dst, W, W, H, cudaMemcpyDeviceToHost, ctx->stream));
+    CU(cudaStreamSynchronize(ctx->stream));
+  }
   return M3TB_OK;
 }
 

@@ -3,8 +3,6 @@
 // depth / silhouette images and of the renderer-image records k_track / k_histogram read. Float32 throughout, one
 // rounding per operation in the order written (the library is built with -fmad=false); DESIGN.md §3 "k_render" states
 // the contract and tests/render_reference.py restates it.
-#include <cfloat>
-
 #include "m3t_b200_raster.cuh"
 #include "m3t_b200_render.cuh"
 
@@ -25,57 +23,14 @@ __global__ void __launch_bounds__(kRenderThreads) k_render(const __grid_constant
 
   // ---- focus: FocusedRenderer::CalculateProjectionMatrix (renderer.cpp:348-405) -------------------------------------
   if (tid == 0) {
-    const float* w = cam.w2c;
-    float u_min = FLT_MAX, u_max = FLT_MIN, v_min = FLT_MAX, v_max = FLT_MIN;  // numeric_limits<float>::min() as written
-    int any = 0;
-    for (int k = 0; k < R.n_referenced; ++k) {
+    auto body = [&](int k, float& rr, const float*& p) {
       const int b = a.referenced_bodies[R.first_referenced + k];
-      int vis = 0;
-      const float rr = a.geometry[b].radius;
-      const float* p = a.poses + 12 * b;
-      const float x = w[0] * p[3] + w[1] * p[7] + w[2] * p[11] + w[3];
-      const float y = w[4] * p[3] + w[5] * p[7] + w[6] * p[11] + w[7];
-      const float z = w[8] * p[3] + w[9] * p[7] + w[10] * p[11] + w[11];
-      if (!(z < rr * 1.5f || z - rr < R.z_min || z + rr > R.z_max)) {
-        const float abs_x = fabsf(x), abs_y = fabsf(y);
-        const float x2 = x * x, y2 = y * y, z2 = z * z, r2 = rr * rr, rz = rr * z;
-        const float z2_r2 = z2 - r2;
-        const float z3_zr2 = z2_r2 * z;
-        const float r_u = cam.fu * (abs_x * r2 + rz * sqrtf(z2_r2 + x2)) / z3_zr2;
-        const float r_v = cam.fv * (abs_y * r2 + rz * sqrtf(z2_r2 + y2)) / z3_zr2;
-        const float center_u = x * cam.fu / z + cam.ppu;
-        const float center_v = y * cam.fv / z + cam.ppv;
-        const float u_min_body = center_u - r_u, u_max_body = center_u + r_u;
-        const float v_min_body = center_v - r_v, v_max_body = center_v + r_v;
-        if (!(u_min_body > float(cam.width) || u_max_body < 0.0f || v_min_body > float(cam.height) || v_max_body < 0.0f)) {
-          u_min = u_min_body < u_min ? u_min_body : u_min;  // std::min(a, b) = b < a ? b : a
-          u_max = u_max < u_max_body ? u_max_body : u_max;  // std::max(a, b) = a < b ? b : a
-          v_min = v_min_body < v_min ? v_min_body : v_min;
-          v_max = v_max < v_max_body ? v_max_body : v_max;
-          vis = 1;
-          any = 1;
-        }
-      }
-      a.visible[R.first_referenced + k] = vis;
-    }
-    const float du = u_max - u_min, dv = v_max - v_min;
-    const float d = (du < dv ? dv : du) * 1.05f;  // kImageSizeSafetyMargin
+      rr = a.geometry[b].radius;
+      p = a.poses + 12 * b;
+    };
     RenderOutDev o;
-    o.corner_u = 0.5f * (u_min + u_max - d);
-    o.corner_v = 0.5f * (v_min + v_max - d);
-    o.scale = float(S) / d;
-    o.projection_term_a = R.z_max * R.z_min * 65535.0f / (R.z_max - R.z_min);  // renderer.cpp:567-570
-    o.projection_term_b = R.z_max * 65535.0f / (R.z_max - R.z_min);
+    s_any = FocusProjection(cam, S, R.z_min, R.z_max, R.n_referenced, body, a.visible + R.first_referenced, o, sP);
     a.out[r] = o;
-    const float ppu_scaled = (cam.ppu - o.corner_u) * o.scale;
-    const float ppv_scaled = (cam.ppv - o.corner_v) * o.scale;
-    sP[0] = 2.0f * cam.fu / d;
-    sP[1] = 2.0f * (ppu_scaled + 0.5f) / float(S) - 1.0f;
-    sP[2] = 2.0f * cam.fv / d;
-    sP[3] = 2.0f * (ppv_scaled + 0.5f) / float(S) - 1.0f;
-    sP[4] = (R.z_max + R.z_min) / (R.z_max - R.z_min);
-    sP[5] = -2.0f * R.z_max * R.z_min / (R.z_max - R.z_min);
-    s_any = any;  // no visible body: the matrix is not finite, nothing is drawn, the images stay cleared
   }
   __syncthreads();
 

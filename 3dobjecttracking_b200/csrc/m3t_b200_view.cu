@@ -3,7 +3,9 @@
 // (FullBasicDepthRenderer / FullSilhouetteRenderer / FullNormalRenderer, m3tb_render_full). Three launches for all
 // viewers (or all full renderers) of a context: k_view_setup clips and sets up every triangle, k_view_raster walks
 // (triangle, screen tile) pairs so that a large triangle is shared by many warps, k_view_resolve writes the normal and
-// viewer images (the depth, silhouette and normal images of a full renderer). Float32,
+// viewer images (the depth, silhouette and normal images of a full renderer). Focused normal renderers
+// (FocusedNormalRenderer, m3tb_render_focused_normals) take a fourth launch first, k_view_focus, which focuses each on
+// its referenced bodies from the current poses. k_normalized_depth writes NormalizedDepthImage. Float32,
 // one rounding per operation in the order written (-fmad=false); DESIGN.md §3 "k_view_setup / k_view_raster /
 // k_view_resolve" states the contract, tests/viewer_reference.py restates it.
 #include "m3t_b200_view.cuh"
@@ -70,6 +72,30 @@ __device__ __forceinline__ unsigned DepthGray(unsigned d, float alpha, float bet
 }
 
 }  // namespace
+
+__global__ void __launch_bounds__(kViewThreads) k_view_focus(const __grid_constant__ FocusArgs a) {
+  const int f = blockIdx.x * blockDim.x + threadIdx.x;
+  if (f >= a.n_focus) return;
+  const FocusDev& F = a.focus[f];
+  auto body = [&](int k, float& rr, const float*& p) {
+    rr = a.radius[F.first_referenced + k];
+    p = a.poses + 12 * a.referenced[F.first_referenced + k];
+  };
+  float P[6];
+  RenderOutDev o;
+  const bool any =
+      FocusProjection(F.cam, F.image_size, F.z_min, F.z_max, F.n_referenced, body, a.visible + F.first_referenced, o, P);
+  a.out[f] = o;
+  ViewerDev& V = a.viewers[F.viewer];
+  V.P00 = P[0];
+  V.P02 = P[1];
+  V.P11 = P[2];
+  V.P12 = P[3];
+  V.P22 = P[4];
+  V.P23 = P[5];
+  if (!any)  // as k_render: nothing is drawn, the images stay cleared
+    for (int g = 0; g < V.n_draws; ++g) a.draws[V.first_draw + g].n_triangles = 0;
+}
 
 __global__ void __launch_bounds__(kViewThreads) k_view_setup(const __grid_constant__ ViewArgs a) {
   const int d = blockIdx.y;
@@ -152,10 +178,10 @@ __global__ void __launch_bounds__(kViewThreads) k_view_resolve(const __grid_cons
   }
 #pragma unroll
   for (int k = 0; k < 4; ++k) V.normal[4 * size_t(p) + k] = uint8_t(nb[k]);
-  if (V.kind == VK_FULL) {
+  if (V.kind >= VK_FULL) {
     // glReadPixels of GL_DEPTH_COMPONENT16 (the cleared key reads 65535) and of the silhouette id attachment
     V.depth[p] = uint16_t(key >> 48);
-    V.silhouette[p] = key != kViewClear ? uint8_t(a.draws[d].silhouette_id) : uint8_t(0);
+    if (V.kind == VK_FULL) V.silhouette[p] = key != kViewClear ? uint8_t(a.draws[d].silhouette_id) : uint8_t(0);
     return;
   }
   unsigned cam[3];
@@ -174,6 +200,24 @@ __global__ void __launch_bounds__(kViewThreads) k_view_resolve(const __grid_cons
 #pragma unroll
   for (int k = 0; k < 3; ++k)
     V.image[3 * size_t(p) + k] = uint8_t(CharOf(float(cam[k]) * alpha_inv + float(nb[k]) * alpha));
+}
+
+__global__ void __launch_bounds__(kViewThreads) k_normalized_depth(const __grid_constant__ NormalizedDepthArgs a) {
+  const int p = blockIdx.x * blockDim.x + threadIdx.x;
+  if (p >= a.width * a.height) return;
+  const int i = p % a.width, j = p / a.width;
+  const unsigned v = reinterpret_cast<const uint16_t*>(a.src + size_t(j) * a.src_pitch)[i];
+  unsigned g;
+  if (!a.renderer) {
+    g = DepthGray(v, a.alpha, a.beta);  // DepthCamera::NormalizedDepthImage, as NormalDepthViewer reads its frame
+  } else {  // FullDepthRenderer::NormalizedDepthImage (renderer.cpp:407-427)
+    float depth = a.a / (a.b - float(v));
+    depth = depth - a.min_depth;
+    depth = depth < 0.0f ? 0.0f : depth;        // std::max(depth - min_depth, 0.0f)
+    depth = a.delta < depth ? a.delta : depth;  // std::min(..., delta_depth)
+    g = CharOf(depth * a.scale);                // uchar(depth * scale)
+  }
+  a.dst[size_t(j) * a.dst_pitch + i] = uint8_t(g);
 }
 
 }  // namespace m3tb

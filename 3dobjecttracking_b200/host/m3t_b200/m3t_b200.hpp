@@ -11,10 +11,11 @@
 //   m3t::Tracker::ExecuteTrackingStep                  -> m3tb_tracking_step + m3tb_calculate_results (fast path)
 //
 // Focused depth / silhouette renderers exist as device renderers (k_render), full depth / silhouette / normal
-// renderers and the normal viewers as k_view_*, model generation as DepthModel::GenerateModel (k_model_raster /
+// renderers, the focused normal renderer and the normal viewers as k_view_*, the image viewers on the camera frames and
+// NormalizedDepthImage (k_normalized_depth), model generation as DepthModel::GenerateModel (k_model_raster /
 // k_model_points) and RegionModel::GenerateModel (k_model_raster / k_region_contours / k_region_points), the texture
 // modality as TextureModality (ORB; the caller detects the features). Everything else the reference has outside this
-// path (focused normal renderer, detectors, feature detection, YAML metafiles) is out of scope here (DESIGN.md). Poses use a minimal Transform3fA (row-major 3x4).
+// path (detectors, feature detection, YAML metafiles) is out of scope here (DESIGN.md). Poses use a minimal Transform3fA (row-major 3x4).
 #ifndef M3T_B200_HPP_
 #define M3T_B200_HPP_
 
@@ -100,6 +101,7 @@ class Batch {
   int NextStructure() { return n_structures_++; }
   int NextViewer() { return n_viewers_++; }
   int NextFullRenderer() { return n_full_renderers_++; }
+  int NextFocusedNormalRenderer() { return n_focused_normal_renderers_++; }
   // every m3tb_update_viewers renders all viewers of the batch: read-backs older than the last update are stale
   void ViewersUpdated() { ++viewer_version_; }
   long viewer_version() const { return viewer_version_; }
@@ -135,7 +137,7 @@ class Batch {
  private:
   m3tb_ctx* ctx_ = nullptr;
   int max_bodies_ = 0, n_bodies_ = 0, n_renderers_ = 0, n_color_ = 0, n_depth_ = 0, n_rmodels_ = 0, n_dmodels_ = 0, n_structures_ = 0;
-  int n_viewers_ = 0, n_full_renderers_ = 0;
+  int n_viewers_ = 0, n_full_renderers_ = 0, n_focused_normal_renderers_ = 0;
   long viewer_version_ = 0;
   long pose_version_ = 0;
   Key done_[kNPhases];
@@ -221,6 +223,7 @@ class Camera {
   const Transform3fA& world2camera_pose() const { return world2camera_pose_; }
   int index() const { return index_; }
   bool set_up() const { return set_up_; }
+  const std::shared_ptr<Batch>& batch() const { return batch_; }
 
  protected:
   Camera(const std::string& name, const std::shared_ptr<Batch>& batch) : name_(name), batch_(batch) {}
@@ -278,6 +281,17 @@ class DepthCamera : public Camera {
       return false;
     }
     return Check(batch_->ctx(), m3tb_upload_depth(batch_->ctx(), index_, depth, pitch), "DepthCamera::UpdateImage");
+  }
+  // DepthCamera::NormalizedDepthImage (camera.cpp:108-115) of the frame the camera holds: width x height u8 (empty on
+  // failure)
+  std::vector<uint8_t> NormalizedDepthImage(float min_depth, float max_depth) const {
+    std::vector<uint8_t> image(size_t(intrinsics_.width) * size_t(intrinsics_.height));
+    if (!Check(batch_->ctx(),
+               m3tb_get_normalized_depth_image(batch_->ctx(), M3TB_NORMALIZED_DEPTH_CAMERA, index_, min_depth, max_depth,
+                                               image.data(), size_t(intrinsics_.width)),
+               "DepthCamera::NormalizedDepthImage"))
+      image.clear();
+    return image;
   }
 
  private:
@@ -925,6 +939,18 @@ class FullDepthRenderer {
   void set_z_max(float v) { z_max_ = v; set_up_ = false; }
   bool set_up() const { return set_up_; }
   int index() const { return index_; }
+  // FullDepthRenderer::NormalizedDepthImage (renderer.cpp:407-427) of the last render: height x width u8 (empty on
+  // failure or before the first render)
+  std::vector<uint8_t> NormalizedDepthImage(float min_depth, float max_depth) const {
+    std::vector<uint8_t> image(size_t(intrinsics_.width) * size_t(intrinsics_.height));
+    if (!set_up_ || !rendered_ ||
+        !Check(batch_->ctx(),
+               m3tb_get_normalized_depth_image(batch_->ctx(), M3TB_NORMALIZED_DEPTH_FULL_RENDERER, index_, min_depth,
+                                               max_depth, image.data(), size_t(intrinsics_.width)),
+               "FullDepthRenderer::NormalizedDepthImage"))
+      image.clear();
+    return image;
+  }
 
  protected:
   static constexpr float USHRT_MAX_F = 65535.0f;
@@ -1007,6 +1033,155 @@ class FullNormalRenderer : public FullDepthRenderer {
   const std::vector<uint8_t>& normal_image() const { return normal_image_; }
 };
 
+using Vec4b = std::array<uint8_t, 4>;  // cv::Vec4b
+
+// FocusedNormalRenderer (normal_renderer.h:135-176) on a focused-normal-renderer slot of its own
+// (m3tb_set_focused_normal_renderer), with FocusedDepthRenderer's getters. StartRendering renders every focused normal
+// renderer of the batch in one m3tb_render_focused_normals call; the images, focus and visible flags are those of the
+// last Fetch...Image.
+class FocusedNormalRenderer {
+ public:
+  FocusedNormalRenderer(const std::string& name, const std::shared_ptr<Batch>& batch,
+                        const std::shared_ptr<RendererGeometry>& renderer_geometry_ptr,
+                        const std::shared_ptr<Camera>& camera_ptr, int image_size = 200, float z_min = 0.02f,
+                        float z_max = 10.0f)
+      : name_(name), batch_(batch), renderer_geometry_ptr_(renderer_geometry_ptr), camera_ptr_(camera_ptr),
+        image_size_(image_size), z_min_(z_min), z_max_(z_max) {
+    index_ = batch->NextFocusedNormalRenderer();
+  }
+  bool AddReferencedBody(const std::shared_ptr<Body>& body_ptr) {
+    for (auto& b : referenced_body_ptrs_)
+      if (b->name() == body_ptr->name()) {
+        std::cerr << "Body " << body_ptr->name() << " already exists" << std::endl;
+        return false;
+      }
+    referenced_body_ptrs_.push_back(body_ptr);
+    set_up_ = false;
+    return true;
+  }
+  bool SetUp() {
+    set_up_ = false;
+    rendered_ = false;
+    if (!renderer_geometry_ptr_ || !renderer_geometry_ptr_->set_up()) {
+      std::cerr << "Set up renderer geometry of renderer " << name_ << " first" << std::endl;
+      return false;
+    }
+    if (!camera_ptr_ || !camera_ptr_->set_up()) {
+      std::cerr << "Set up camera of renderer " << name_ << " first" << std::endl;
+      return false;
+    }
+    if (referenced_body_ptrs_.empty()) {
+      std::cerr << "No referenced bodys were assigned to renderer " << name_ << std::endl;
+      return false;
+    }
+    std::vector<int> geo, ref;
+    for (auto& b : renderer_geometry_ptr_->body_ptrs()) geo.push_back(b->index());
+    for (auto& b : referenced_body_ptrs_) ref.push_back(b->index());
+    const int kind = std::dynamic_pointer_cast<ColorCamera>(camera_ptr_) ? 0 : 1;
+    if (!Check(batch_->ctx(),
+               m3tb_set_focused_normal_renderer(batch_->ctx(), index_, kind, camera_ptr_->index(), image_size_, z_min_,
+                                                z_max_, geo.data(), int(geo.size()), ref.data(), int(ref.size())),
+               "FocusedNormalRenderer::SetUp"))
+      return false;
+    // FocusedDepthRenderer::CalculateProjectionTerms (renderer.cpp:567-570)
+    projection_term_a_ = z_max_ * z_min_ * 65535.0f / (z_max_ - z_min_);
+    projection_term_b_ = z_max_ * 65535.0f / (z_max_ - z_min_);
+    set_up_ = true;
+    return true;
+  }
+  bool StartRendering() {
+    if (!set_up_) {
+      std::cerr << "Set up renderer " << name_ << " first" << std::endl;
+      return false;
+    }
+    if (!Check(batch_->ctx(), m3tb_render_focused_normals(batch_->ctx()), "FocusedNormalRenderer::StartRendering"))
+      return false;
+    rendered_ = true;
+    return true;
+  }
+  bool FetchNormalImage() { return Fetch("FocusedNormalRenderer::FetchNormalImage"); }
+  bool FetchDepthImage() { return Fetch("FocusedNormalRenderer::FetchDepthImage"); }
+  // BGRA8, image_size x image_size, GL_BGRA order (byte 0 encodes x)
+  const std::vector<uint8_t>& focused_normal_image() const { return normal_; }
+  const std::vector<uint16_t>& focused_depth_image() const { return depth_; }
+  // normal_renderer.cpp:393-415
+  std::array<float, 3> NormalVector(Vec4b normal_image_value) const {
+    return {1.0f - float(normal_image_value[0]) / 127.5f, 1.0f - float(normal_image_value[1]) / 127.5f,
+            1.0f - float(normal_image_value[2]) / 127.5f};
+  }
+  std::array<float, 3> NormalVector(const Point2i& image_coordinate) const {
+    return NormalVector(NormalImageValue(image_coordinate));
+  }
+  Vec4b NormalImageValue(const Point2i& image_coordinate) const {
+    const int u = int((image_coordinate.x - corner_u_) * scale_ + 0.5f);
+    const int v = int((image_coordinate.y - corner_v_) * scale_ + 0.5f);
+    const uint8_t* p = normal_.data() + 4 * (size_t(v) * size_t(image_size_) + size_t(u));
+    return {p[0], p[1], p[2], p[3]};
+  }
+  bool IsBodyVisible(const std::string& body_name) const {
+    for (size_t k = 0; k < referenced_body_ptrs_.size() && k < visible_.size(); ++k)
+      if (referenced_body_ptrs_[k]->name() == body_name) return visible_[k] != 0;
+    return false;
+  }
+  bool IsBodyReferenced(const std::string& body_name) const {
+    for (auto& b : referenced_body_ptrs_)
+      if (b->name() == body_name) return true;
+    return false;
+  }
+  float corner_u() const { return corner_u_; }
+  float corner_v() const { return corner_v_; }
+  float scale() const { return scale_; }
+  float projection_term_a() const { return projection_term_a_; }
+  float projection_term_b() const { return projection_term_b_; }
+  int image_size() const { return image_size_; }
+  float z_min() const { return z_min_; }
+  float z_max() const { return z_max_; }
+  void set_image_size(int v) { image_size_ = v; set_up_ = false; }
+  void set_z_min(float v) { z_min_ = v; set_up_ = false; }
+  void set_z_max(float v) { z_max_ = v; set_up_ = false; }
+  bool set_up() const { return set_up_; }
+  int index() const { return index_; }
+  const std::string& name() const { return name_; }
+  const std::shared_ptr<Camera>& camera_ptr() const { return camera_ptr_; }
+  const std::vector<std::shared_ptr<Body>>& referenced_body_ptrs() const { return referenced_body_ptrs_; }
+
+ private:
+  // one read-back of the last render: both images, the focus and the visible flags; fails before SetUp and before the
+  // first render
+  bool Fetch(const char* what) {
+    if (!set_up_) {
+      std::cerr << "Set up renderer " << name_ << " first" << std::endl;
+      return false;
+    }
+    if (!rendered_) {
+      std::cerr << "Renderer " << name_ << " has not rendered" << std::endl;
+      return false;
+    }
+    const size_t n = size_t(image_size_) * size_t(image_size_);
+    depth_.resize(n);
+    normal_.resize(4 * n);
+    visible_.assign(referenced_body_ptrs_.size(), 0);
+    return Check(batch_->ctx(),
+                 m3tb_get_focused_normal_rendering(batch_->ctx(), index_, depth_.data(), normal_.data(), &corner_u_,
+                                                   &corner_v_, &scale_, &projection_term_a_, &projection_term_b_,
+                                                   visible_.data()),
+                 what);
+  }
+  std::string name_;
+  std::shared_ptr<Batch> batch_;
+  std::shared_ptr<RendererGeometry> renderer_geometry_ptr_;
+  std::shared_ptr<Camera> camera_ptr_;
+  std::vector<std::shared_ptr<Body>> referenced_body_ptrs_;
+  int image_size_;
+  float z_min_, z_max_;
+  int index_ = 0;
+  bool set_up_ = false, rendered_ = false;
+  std::vector<uint16_t> depth_;
+  std::vector<uint8_t> normal_;
+  std::vector<int> visible_;
+  float corner_u_ = 0, corner_v_ = 0, scale_ = 0, projection_term_a_ = 0, projection_term_b_ = 0;
+};
+
 // ---- normal_viewer.h -----------------------------------------------------------------------------------------------
 // The FullNormalRenderer of a viewer (normal_viewer.h:59,104) over the whole image of its camera. On the device it is
 // the renderer of one viewer slot (m3tb_set_viewer); StartRendering renders every viewer of the batch in one
@@ -1082,14 +1257,31 @@ class ViewerNormalRenderer {
   std::vector<uint8_t> normal_, image_;
 };
 
-// Viewer (viewer.h): UpdateViewer renders and blends; the blended BGR8 image is read back by image() instead of being
+// Viewer (viewer.h): SetUp, UpdateViewer, and the image of the last update, read back by image() instead of being
 // displayed or saved
 class Viewer {
  public:
   virtual ~Viewer() = default;
   virtual bool SetUp() = 0;
-  // UpdateViewer(save_index): one m3tb_update_viewers for every viewer of the batch
-  bool UpdateViewer(int /*save_index*/) {
+  virtual bool UpdateViewer(int save_index) = 0;
+  virtual const std::vector<uint8_t>& image() = 0;
+  // true for the normal viewers, which m3tb_update_viewers draws all together (Tracker::UpdateViewers)
+  virtual bool drawn_by_update_viewers() const { return false; }
+  const std::string& name() const { return name_; }
+  bool set_up() const { return set_up_; }
+  bool dirty() const { return dirty_; }
+
+ protected:
+  explicit Viewer(const std::string& name) : name_(name) {}
+  std::string name_;
+  bool set_up_ = false, dirty_ = false;
+};
+
+// The normal viewers (normal_viewer.h): UpdateViewer renders and blends; image() is the blended BGR8 image
+class NormalViewer : public Viewer {
+ public:
+  // UpdateViewer(save_index): one m3tb_update_viewers for every normal viewer of the batch
+  bool UpdateViewer(int /*save_index*/) override {
     if (!set_up_) {
       std::cerr << "Set up viewer " << name_ << " first" << std::endl;
       return false;
@@ -1098,19 +1290,17 @@ class Viewer {
     return renderer_.StartRendering();
   }
   // the image CalculateAlphaBlend returned at the last update: width x height BGR8
-  const std::vector<uint8_t>& image() { return renderer_.blended_image(); }
+  const std::vector<uint8_t>& image() override { return renderer_.blended_image(); }
+  bool drawn_by_update_viewers() const override { return true; }
   ViewerNormalRenderer& renderer() { return renderer_; }
   void set_opacity(float opacity) { opacity_ = opacity; dirty_ = true; }
   float opacity() const { return opacity_; }
-  const std::string& name() const { return name_; }
-  bool set_up() const { return set_up_; }
-  bool dirty() const { return dirty_; }
 
  protected:
-  Viewer(const std::string& name, const std::shared_ptr<Batch>& batch,
-         const std::shared_ptr<RendererGeometry>& renderer_geometry_ptr, const std::shared_ptr<Camera>& camera_ptr,
-         float opacity)
-      : name_(name), renderer_("renderer", batch, renderer_geometry_ptr, camera_ptr), opacity_(opacity) {}
+  NormalViewer(const std::string& name, const std::shared_ptr<Batch>& batch,
+               const std::shared_ptr<RendererGeometry>& renderer_geometry_ptr, const std::shared_ptr<Camera>& camera_ptr,
+               float opacity)
+      : Viewer(name), renderer_("renderer", batch, renderer_geometry_ptr, camera_ptr), opacity_(opacity) {}
   bool SetUpWith(float min_depth, float max_depth) {
     set_up_ = false;
     if (!renderer_.camera_ptr()->set_up()) {
@@ -1122,28 +1312,26 @@ class Viewer {
     dirty_ = false;
     return true;
   }
-  std::string name_;
   ViewerNormalRenderer renderer_;
   float opacity_;
-  bool set_up_ = false, dirty_ = false;
 };
 
-class NormalColorViewer : public Viewer {
+class NormalColorViewer : public NormalViewer {
  public:
   NormalColorViewer(const std::string& name, const std::shared_ptr<Batch>& batch,
                     const std::shared_ptr<ColorCamera>& color_camera_ptr,
                     const std::shared_ptr<RendererGeometry>& renderer_geometry_ptr, float opacity = 0.5f)
-      : Viewer(name, batch, renderer_geometry_ptr, color_camera_ptr, opacity) {}
+      : NormalViewer(name, batch, renderer_geometry_ptr, color_camera_ptr, opacity) {}
   bool SetUp() override { return SetUpWith(0.0f, 1.0f); }
 };
 
-class NormalDepthViewer : public Viewer {
+class NormalDepthViewer : public NormalViewer {
  public:
   NormalDepthViewer(const std::string& name, const std::shared_ptr<Batch>& batch,
                     const std::shared_ptr<DepthCamera>& depth_camera_ptr,
                     const std::shared_ptr<RendererGeometry>& renderer_geometry_ptr, float min_depth = 0.0f,
                     float max_depth = 1.0f, float opacity = 0.5f)
-      : Viewer(name, batch, renderer_geometry_ptr, depth_camera_ptr, opacity), min_depth_(min_depth),
+      : NormalViewer(name, batch, renderer_geometry_ptr, depth_camera_ptr, opacity), min_depth_(min_depth),
         max_depth_(max_depth) {}
   bool SetUp() override { return SetUpWith(min_depth_, max_depth_); }
   void set_min_depth(float v) { min_depth_ = v; dirty_ = true; }
@@ -1151,6 +1339,76 @@ class NormalDepthViewer : public Viewer {
 
  private:
   float min_depth_, max_depth_;
+};
+
+// ImageColorViewer (image_viewer.cpp:9-35): image() is the frame the colour camera holds (Camera::image()), width x
+// height BGR8, read at each UpdateViewer
+class ImageColorViewer : public Viewer {
+ public:
+  ImageColorViewer(const std::string& name, const std::shared_ptr<ColorCamera>& color_camera_ptr)
+      : Viewer(name), color_camera_ptr_(color_camera_ptr) {}
+  bool SetUp() override {
+    set_up_ = false;
+    if (!color_camera_ptr_->set_up()) {
+      std::cerr << "Color camera " << color_camera_ptr_->name() << " was not set up" << std::endl;
+      return false;
+    }
+    set_up_ = true;
+    return true;
+  }
+  bool UpdateViewer(int /*save_index*/) override {
+    if (!set_up_) {
+      std::cerr << "Set up image color viewer " << name_ << " first" << std::endl;
+      return false;
+    }
+    const Intrinsics& in = color_camera_ptr_->intrinsics();
+    image_.resize(size_t(in.width) * size_t(in.height) * 3);
+    const auto& batch = color_camera_ptr_->batch();
+    return Check(batch->ctx(),
+                 m3tb_get_camera_image(batch->ctx(), 0, color_camera_ptr_->index(), image_.data(), size_t(in.width) * 3),
+                 "ImageColorViewer::UpdateViewer");
+  }
+  const std::vector<uint8_t>& image() override { return image_; }
+
+ private:
+  std::shared_ptr<ColorCamera> color_camera_ptr_;
+  std::vector<uint8_t> image_;
+};
+
+// ImageDepthViewer (image_viewer.cpp:50-78): image() is DepthCamera::NormalizedDepthImage(min_depth, max_depth) of the
+// frame the depth camera holds, width x height u8, computed at each UpdateViewer
+class ImageDepthViewer : public Viewer {
+ public:
+  ImageDepthViewer(const std::string& name, const std::shared_ptr<DepthCamera>& depth_camera_ptr, float min_depth = 0.0f,
+                   float max_depth = 1.0f)
+      : Viewer(name), depth_camera_ptr_(depth_camera_ptr), min_depth_(min_depth), max_depth_(max_depth) {}
+  bool SetUp() override {
+    set_up_ = false;
+    if (!depth_camera_ptr_->set_up()) {
+      std::cerr << "Depth camera " << depth_camera_ptr_->name() << " was not set up" << std::endl;
+      return false;
+    }
+    set_up_ = true;
+    return true;
+  }
+  bool UpdateViewer(int /*save_index*/) override {
+    if (!set_up_) {
+      std::cerr << "Set up image depth viewer " << name_ << " first" << std::endl;
+      return false;
+    }
+    image_ = depth_camera_ptr_->NormalizedDepthImage(min_depth_, max_depth_);
+    return !image_.empty();
+  }
+  const std::vector<uint8_t>& image() override { return image_; }
+  void set_min_depth(float v) { min_depth_ = v; }
+  void set_max_depth(float v) { max_depth_ = v; }
+  float min_depth() const { return min_depth_; }
+  float max_depth() const { return max_depth_; }
+
+ private:
+  std::shared_ptr<DepthCamera> depth_camera_ptr_;
+  float min_depth_, max_depth_;
+  std::vector<uint8_t> image_;
 };
 
 // ---- modality.h ----------------------------------------------------------------------------------------------------
@@ -2164,11 +2422,16 @@ class Tracker {
     viewer_ptrs_.push_back(v);
     return true;
   }
-  // Tracker::UpdateViewers (tracker.cpp:373): one m3tb_update_viewers for all viewers, from the current poses and frames
-  bool UpdateViewers(int /*iteration*/) {
-    if (viewer_ptrs_.empty()) return true;
-    for (auto& v : viewer_ptrs_)
+  // Tracker::UpdateViewers (tracker.cpp:373): one m3tb_update_viewers for all normal viewers, from the current poses and
+  // frames, and UpdateViewer of every image viewer
+  bool UpdateViewers(int iteration) {
+    bool any_normal = false;
+    for (auto& v : viewer_ptrs_) {
       if (v->dirty() && !v->SetUp()) return false;
+      if (v->drawn_by_update_viewers()) any_normal = true;
+      else if (!v->UpdateViewer(iteration)) return false;
+    }
+    if (!any_normal) return true;
     batch_->ViewersUpdated();
     return Check(batch_->ctx(), m3tb_update_viewers(batch_->ctx()), "Tracker::UpdateViewers");
   }

@@ -416,6 +416,55 @@ int m3tb_get_full_rendering(m3tb_ctx* ctx, int renderer, void* depth_u16, size_t
                             size_t silhouette_pitch, void* normal_bgra, size_t normal_pitch, float* projection_term_a,
                             float* projection_term_b);
 
+/* ---- focused normal renderers (FocusedNormalRenderer, normal_renderer.h:135-176, normal_renderer.cpp:295-423) -------
+ * A focused normal renderer focuses on its referenced bodies as a focused renderer does
+ * (FocusedRenderer::CalculateProjectionMatrix, renderer.cpp:348-405) and draws its geometry bodies into an
+ * image_size x image_size depth image and normal image with the full renderers' rasteriser (DESIGN.md §3 "Focused normal
+ * renderers"). Its depth image follows k_render's contract: up to the focused renderers' image_size limit of 240 it
+ * equals, bit for bit, the depth image of a device focused renderer (m3tb_set_focused_renderer) with the same camera,
+ * size, z range and bodies. */
+/* FocusedNormalRenderer(name, renderer_geometry, camera, image_size, z_min, z_max) + AddReferencedBody + SetUp of the
+ * colour (camera_kind 0) or depth (1) camera `camera`: `geometry_bodies` are drawn in that order
+ * (RendererGeometry::render_data_bodies), each with the geometry given by m3tb_set_body_geometry and its own culling
+ * flag; `referenced_bodies` are the bodies the image focuses on. Defaults (renderer.h:112-113,222): image_size 200, z_min
+ * 0.02, z_max 10. Ids are dense (0..n) and separate from the focused renderers', the full renderers' and the viewers';
+ * setting an existing id replaces it. M3TB_ERR_INVALID as for m3tb_set_focused_renderer; image_size above 4096 returns
+ * M3TB_ERR_UNSUPPORTED (the z-buffer takes 8 bytes per pixel of device memory). */
+int m3tb_set_focused_normal_renderer(m3tb_ctx* ctx, int renderer, int camera_kind, int camera, int image_size,
+                                     float z_min, float z_max, const int* geometry_bodies, int n_geometry,
+                                     const int* referenced_bodies, int n_referenced);
+/* FocusedNormalRenderer::StartRendering (normal_renderer.cpp:361-369) of every focused normal renderer from the current
+ * poses, in stream order after any tracking launch. Four kernel launches for all of them together. Never called by
+ * m3tb_tracking_step, m3tb_render, m3tb_render_full or m3tb_update_viewers; none set: nothing is launched. */
+int m3tb_render_focused_normals(m3tb_ctx* ctx);
+/* Read-back of focused normal renderer `renderer`'s last render, image_size x image_size, rows packed:
+ * FetchDepthImage (u16, GL_DEPTH_COMPONENT16, 65535 where nothing was drawn, row v = image row v), FetchNormalImage
+ * (focused_normal_image(): BGRA8 as m3tb_get_full_rendering), corner_u / corner_v / scale, FocusedDepthRenderer's
+ * projection terms (depth = a / (b - value)) and one FocusedRenderer::IsBodyVisible flag per referenced body. Any pointer
+ * may be NULL. The images may go to host or device memory; the scalars and flags go to host memory. The call waits
+ * unless every image goes to device memory and no scalar or flag is asked for. M3TB_ERR_NOT_SET_UP before the first
+ * render since the renderer was set. */
+int m3tb_get_focused_normal_rendering(m3tb_ctx* ctx, int renderer, void* depth_u16, void* normal_bgra, float* corner_u,
+                                      float* corner_v, float* scale, float* projection_term_a,
+                                      float* projection_term_b, int* visible_flags);
+
+/* ---- normalised depth images (DepthCamera::NormalizedDepthImage, camera.cpp:108-115;
+ * FullDepthRenderer::NormalizedDepthImage, renderer.cpp:407-427) ------------------------------------------------------ */
+#define M3TB_NORMALIZED_DEPTH_CAMERA 0        /* source: depth camera `id` */
+#define M3TB_NORMALIZED_DEPTH_FULL_RENDERER 1 /* source: full renderer `id` (m3tb_set_full_renderer) */
+/* NormalizedDepthImage(min_depth, max_depth) as a u8 image of the source's size, rows `pitch` bytes apart, in host or
+ * device memory (the call waits only for a host destination). One kernel launch.
+ * - Depth camera: convertTo(CV_8UC1, alpha, beta) with alpha = 255 / ((max - min) / depth_scale) and
+ *   beta = -(min / depth_scale) * alpha, as NormalDepthViewer computes it: one fused multiply-add, rounding half to even,
+ *   saturation. It reads the frame the camera holds (the rectified frame when an undistortion is set; a pinned frame is
+ *   read in place).
+ * - Full renderer: per pixel uchar(min(max(a / (b - value) - min, 0), max - min) * 255 / (max - min)) of its last render.
+ * M3TB_ERR_INVALID for a bad source, an unset camera or full renderer, max_depth <= min_depth (or NaN) and a pitch
+ * smaller than a row; M3TB_ERR_NOT_SET_UP for a camera without a frame and a full renderer that has not rendered since
+ * it was set or its camera changed size. */
+int m3tb_get_normalized_depth_image(m3tb_ctx* ctx, int source, int id, float min_depth, float max_depth, void* dst,
+                                    size_t pitch);
+
 /* Loader-style batch ingest: `count` frames for cameras [first_cam, first_cam+count), frame k at
  * base + k*frame_stride bytes. Cameras of equal size share one device pool, so this is a single
  * host->device copy when the host frames are contiguous (frame_stride == height*pitch). */
