@@ -79,6 +79,19 @@ def build_host_example(force=False):
     return out
 
 
+def build_pose_scoring_example(force=False):
+    """g++ build of examples/pose_scoring_selftest.cpp: the mirror's EvaluationModel and evaluators as plain C++17."""
+    src = os.path.join(_ROOT, "examples", "pose_scoring_selftest.cpp")
+    hdr = os.path.join(_HERE, "host", "m3t_b200", "m3t_b200.hpp")
+    out = os.path.join(_ROOT, "examples", "pose_scoring_selftest")
+    csrc = os.path.join(_HERE, "csrc")
+    if force or _stale(out, [src, hdr, os.path.join(csrc, "libm3t_b200.so")]):
+        subprocess.run(["g++", "-std=c++17", "-O2", "-Wall", "-I", os.path.join(_ROOT, "include"), "-I",
+                        os.path.join(_HERE, "host"), src, "-o", out, "-L", csrc, "-lm3t_b200", "-Wl,-rpath," + csrc],
+                       check=True)
+    return out
+
+
 def build_all(force=False, verbose=False):
     a, b = build_synth(force), build_cuda(force, verbose)
-    return a, b, build_host_example(force)
+    return a, b, build_host_example(force), build_pose_scoring_example(force)

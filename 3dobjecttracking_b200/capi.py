@@ -156,7 +156,8 @@ SYMBOLS = [
     "m3tb_get_texture_feature_flags", "m3tb_orb_params_default", "m3tb_texture_detect_orb",
     "m3tb_get_texture_detections", "m3tb_get_texture_orb_keypoints", "m3tb_refine_poses_orb", "m3tb_debug_bin_image",
     "m3tb_set_focused_normal_renderer", "m3tb_render_focused_normals", "m3tb_get_focused_normal_rendering",
-    "m3tb_get_normalized_depth_image",
+    "m3tb_get_normalized_depth_image", "m3tb_set_evaluation_model", "m3tb_set_body_evaluation_model",
+    "m3tb_get_evaluation_vertices", "m3tb_score_params_default", "m3tb_score_poses", "m3tb_calculate_diameters",
 ]
 
 KERNEL_NAMES = {0: None, 1: "k_track", 2: "k_track2"}
@@ -189,6 +190,29 @@ class ModelParams(C.Structure):
     _fields_ = [("sphere_radius", C.c_float), ("n_divides", C.c_int32), ("n_points", C.c_int32),
                 ("max_radius_depth_offset", C.c_float), ("stride_depth_offset", C.c_float),
                 ("use_random_seed", C.c_int32), ("image_size", C.c_int32)]
+
+
+class ScoreParams(C.Structure):
+    """m3tb_score_params: curve / AUC scale and the RBOT thresholds."""
+    _fields_ = [("threshold_max", C.c_float), ("curve_scale", C.c_float), ("auc_scale", C.c_float),
+                ("translation_error_threshold", C.c_float), ("rotation_error_threshold", C.c_float)]
+
+
+N_CURVE_VALUES = 100  # M3TB_N_CURVE_VALUES
+POSE_SCORE_DTYPE = np.dtype([("add_error", "<f4"), ("adds_error", "<f4"), ("add_auc", "<f4"), ("adds_auc", "<f4"),
+                             ("translation_error", "<f4"), ("rotation_error", "<f4"), ("tracking_success", "<f4")])
+
+
+def score_params(**kw) -> ScoreParams:
+    """m3tb_score_params_default (YCB: threshold_max 0.1, scales 1, RBOT thresholds 0.05 m / 5 deg) with the given
+    fields replaced."""
+    p = ScoreParams()
+    lib().m3tb_score_params_default(C.byref(p))
+    for k, v in kw.items():
+        if k not in dict(ScoreParams._fields_):
+            raise TypeError(f"unknown score parameter {k}")
+        setattr(p, k, v)
+    return p
 
 
 _lib = None
@@ -319,6 +343,13 @@ def lib():
     L.m3tb_render_focused_normals.argtypes = [vp]
     L.m3tb_get_focused_normal_rendering.argtypes = [vp, ci, vp, vp, fp, fp, fp, fp, fp, ip]
     L.m3tb_get_normalized_depth_image.argtypes = [vp, ci, ci, C.c_float, C.c_float, vp, C.c_size_t]
+    L.m3tb_set_evaluation_model.argtypes = [vp, ci, vp, ci, ci]
+    L.m3tb_set_body_evaluation_model.argtypes = [vp, ci, ci, vp]
+    L.m3tb_get_evaluation_vertices.argtypes = [vp, ci, vp, ci, ip]
+    L.m3tb_score_params_default.argtypes = [C.POINTER(ScoreParams)]
+    L.m3tb_score_params_default.restype = None
+    L.m3tb_score_poses.argtypes = [vp, vp, ci, vp, ci, C.POINTER(ScoreParams), vp, vp, vp, ci]
+    L.m3tb_calculate_diameters.argtypes = [vp, vp, ci, vp]
     _lib = L
     return L
 
@@ -446,6 +477,7 @@ class Context:
         if rc != 0:
             raise M3TBError(f"m3tb_create failed with status {rc} (no usable sm_90 CUDA device?)")
         self.h = h
+        self.device = device
         self.n_bodies = 0
         self._texture_length = {}  # SIFT / DAISY bodies: descriptor length of their uploads (0 before the first)
         self._texture_bytes = {}   # ORB / BRISK / FREAK bodies: bytes per binary descriptor
@@ -717,6 +749,68 @@ class Context:
         src = {"camera": 0, "full_renderer": 1}.get(source, source)
         self._ck(self.L.m3tb_get_normalized_depth_image(self.h, int(src), id, min_depth, max_depth, C.c_void_p(ptr),
                                                         pitch))
+
+    def set_evaluation_model(self, model, vertices, n_vertices_evaluation=0):
+        """Evaluation model `model`: the full vertex set [n, 3] and the reduced set of GenderateReducedVertices
+        (std::mt19937{7} draws when 0 < n_vertices_evaluation < n, otherwise every vertex)."""
+        v = _f32(vertices).reshape(-1, 3)
+        self._ck(self.L.m3tb_set_evaluation_model(self.h, model, v.ctypes.data, len(v), int(n_vertices_evaluation)))
+
+    def set_body_evaluation_model(self, body, model, geometry2body=None):
+        """Scores `body` against evaluation model `model`; geometry2body [3, 4] is the OPT evaluator's term."""
+        g = None if geometry2body is None else _f32(geometry2body).reshape(12)
+        self._ck(self.L.m3tb_set_body_evaluation_model(self.h, body, model, None if g is None else g.ctypes.data))
+
+    def get_evaluation_vertices(self, model):
+        """The reduced set of evaluation model `model`, read back from the device: [m, 3] float32."""
+        n = C.c_int(0)
+        self._ck(self.L.m3tb_get_evaluation_vertices(self.h, model, None, 0, C.byref(n)))
+        out = np.zeros((n.value, 3), np.float32)
+        self._ck(self.L.m3tb_get_evaluation_vertices(self.h, model, out.ctypes.data, n.value, C.byref(n)))
+        return out
+
+    def score_poses(self, bodies, gt_body2world, params=None, curves=True):
+        """Scores the current device poses of `bodies` against ground truth [n, 3, 4] (numpy, or a float32 tensor on
+        the context's device, read in place; another dtype, size or device raises M3TBError). Returns a POSE_SCORE_DTYPE record array [n] and, with curves, the ADD and ADD-S curves
+        [n, 100] each."""
+        b = np.ascontiguousarray(bodies, np.int32).reshape(-1)
+        n = len(b)
+        p = params if params is not None else score_params()
+        if hasattr(gt_body2world, "is_cuda") and gt_body2world.is_cuda:
+            import torch
+            gt = gt_body2world
+            if gt.dtype != torch.float32 or gt.numel() != 12 * n or gt.device.index != self.device:
+                raise M3TBError(f"ground truth on the device must be {n} x 12 float32 values on cuda:{self.device}, "
+                                f"not {tuple(gt.shape)} {gt.dtype} on {gt.device}")
+            gt = gt.contiguous()
+            gt_ptr, gt_dev = gt.data_ptr(), 1
+        else:
+            gt = _f32(gt_body2world).reshape(n, 12)
+            gt_ptr, gt_dev = gt.ctypes.data, 0
+        out = np.zeros(n, POSE_SCORE_DTYPE)
+        ca = np.zeros((n, N_CURVE_VALUES), np.float32) if curves else None
+        cs = np.zeros((n, N_CURVE_VALUES), np.float32) if curves else None
+        self._ck(self.L.m3tb_score_poses(self.h, b.ctypes.data, n, C.c_void_p(gt_ptr), gt_dev, C.byref(p),
+                                         out.ctypes.data, None if ca is None else ca.ctypes.data,
+                                         None if cs is None else cs.ctypes.data, 0))
+        return (out, ca, cs) if curves else out
+
+    def score_poses_to(self, bodies, gt_ptr, gt_on_device, out_ptr, add_curve_ptr=None, adds_curve_ptr=None,
+                       params=None):
+        """m3tb_score_poses into device memory (e.g. torch tensors' data_ptr(): out [n, 7] float32, curves [n, 100]);
+        nothing is synchronised. gt_ptr: [n, 12] float32, device memory when gt_on_device."""
+        b = np.ascontiguousarray(bodies, np.int32).reshape(-1)
+        p = params if params is not None else score_params()
+        self._ck(self.L.m3tb_score_poses(self.h, b.ctypes.data, len(b), C.c_void_p(gt_ptr), int(gt_on_device),
+                                         C.byref(p), C.c_void_p(out_ptr), C.c_void_p(add_curve_ptr),
+                                         C.c_void_p(adds_curve_ptr), 1))
+
+    def calculate_diameters(self, models):
+        """OPTEvaluator::CalculateDiameters: the largest vertex distance of each evaluation model, float32 [n]."""
+        m = np.ascontiguousarray(models, np.int32).reshape(-1)
+        out = np.zeros(len(m), np.float32)
+        self._ck(self.L.m3tb_calculate_diameters(self.h, m.ctypes.data, len(m), out.ctypes.data))
+        return out
 
     def generate_depth_model(self, model_id, body, occlusion_bodies=(), params=None):
         """DepthModel::GenerateModel on the device from the geometry of m3tb_set_body_geometry (params: ModelParams,

@@ -14,6 +14,7 @@
 #include <set>
 #include <cstring>
 #include <memory>
+#include <random>
 #include <string>
 #include <vector>
 
@@ -26,6 +27,7 @@
 #include "m3t_b200_view.cuh"
 #include "m3t_b200_undistort.cuh"
 #include "m3t_b200_texture.cuh"
+#include "m3t_b200_score.cuh"
 
 #include "m3t_b200_track_variants.h"
 #include "m3t_b200_track2.cuh"
@@ -333,6 +335,23 @@ struct m3tb_ctx {
   // pose refinement (m3tb_refine_poses): the lists of RefineSelection, grown on demand; `refine` is set while it runs
   DeviceBuffer<int> d_refine;
   RefineSelection* refine = nullptr;
+
+  // pose scoring (m3tb_set_evaluation_model / m3tb_score_poses / m3tb_calculate_diameters, k_score / k_diameter):
+  // evaluation models with dense ids, per body its model (-1: none) and geometry2body term; the device tables are
+  // uploaded by the next scoring call after a change, the per-call scratch grows lazily, each all or nothing
+  struct EvalModelHost {
+    DeviceBuffer<float4> full, reduced;
+    int n_full = 0, n_reduced = 0;
+  };
+  std::vector<EvalModelHost> eval_models;
+  std::vector<EvalBodyDev> h_eval_bodies;  // [max_bodies]
+  bool eval_dirty = true;
+  DeviceBuffer<EvalModelDev> d_eval_models;
+  DeviceBuffer<EvalBodyDev> d_eval_bodies;
+  DeviceBuffer<int> d_score_ids;           // bodies or models of the call
+  DeviceBuffer<float> d_score_gt, d_score_partial, d_score_curves;
+  DeviceBuffer<m3tb_pose_score> d_score_out;
+  DeviceBuffer<unsigned> d_diameter;
 };
 
 namespace {
@@ -5540,6 +5559,269 @@ int m3tb_get_texture_keyframes(m3tb_ctx* ctx, int body, int* n_keyframes, int* s
 int m3tb_debug_resources(int fail_after, long long* live) {
   if (fail_after >= 0) g_fail_after.store(fail_after);
   if (live) *live = g_live_resources.load();
+  return M3TB_OK;
+}
+
+// ---- pose scoring ------------------------------------------------------------------------------------------------
+
+static std::vector<EvalBodyDev>& EvalBodies(m3tb_ctx* ctx) {
+  if (ctx->h_eval_bodies.empty()) {
+    EvalBodyDev none = {};
+    none.model = -1;
+    ctx->h_eval_bodies.assign(size_t(ctx->max_bodies), none);
+  }
+  return ctx->h_eval_bodies;
+}
+
+// Uploads the model and body tables when they changed; on failure they keep what they held and stay dirty.
+static int SyncEvalTables(m3tb_ctx* ctx) {
+  if (!ctx->eval_dirty) return M3TB_OK;
+  std::vector<EvalModelDev> models(ctx->eval_models.size());
+  for (size_t i = 0; i < models.size(); ++i) {
+    const auto& h = ctx->eval_models[i];
+    models[i] = {h.full, h.reduced, h.n_full, h.n_reduced};
+  }
+  const auto& bodies = EvalBodies(ctx);
+  DeviceBuffer<EvalModelDev> gm;
+  DeviceBuffer<EvalBodyDev> gb;
+  int rc = GrowTable(ctx, ctx->d_eval_models, gm, models.size());
+  if (!rc) rc = GrowTable(ctx, ctx->d_eval_bodies, gb, bodies.size());
+  if (rc) return rc;
+  if (gm || gb) CU(cudaStreamSynchronize(ctx->stream));  // a scoring launch in flight may still read the old tables
+  if (gm) ctx->d_eval_models = std::move(gm);
+  if (gb) ctx->d_eval_bodies = std::move(gb);
+  CU(cudaMemcpyAsync(ctx->d_eval_models, models.data(), sizeof(EvalModelDev) * models.size(), cudaMemcpyHostToDevice,
+                     ctx->stream));
+  CU(cudaMemcpyAsync(ctx->d_eval_bodies, bodies.data(), sizeof(EvalBodyDev) * bodies.size(), cudaMemcpyHostToDevice,
+                     ctx->stream));
+  ctx->eval_dirty = false;
+  return M3TB_OK;
+}
+
+// Grows the per-call scratch tables, all or nothing.
+static int GrowScoreScratch(m3tb_ctx* ctx, size_t n_ids, size_t n_gt, size_t n_partial, size_t n_out, size_t n_curves,
+                            size_t n_diameter) {
+  DeviceBuffer<int> ids;
+  DeviceBuffer<float> gt, partial, curves;
+  DeviceBuffer<m3tb_pose_score> out;
+  DeviceBuffer<unsigned> diameter;
+  int rc = GrowTable(ctx, ctx->d_score_ids, ids, n_ids);
+  if (!rc) rc = GrowTable(ctx, ctx->d_score_gt, gt, n_gt);
+  if (!rc) rc = GrowTable(ctx, ctx->d_score_partial, partial, n_partial);
+  if (!rc) rc = GrowTable(ctx, ctx->d_score_out, out, n_out);
+  if (!rc) rc = GrowTable(ctx, ctx->d_score_curves, curves, n_curves);
+  if (!rc) rc = GrowTable(ctx, ctx->d_diameter, diameter, n_diameter);
+  if (rc) return rc;
+  if (ids || gt || partial || out || curves || diameter) CU(cudaStreamSynchronize(ctx->stream));
+  if (ids) ctx->d_score_ids = std::move(ids);
+  if (gt) ctx->d_score_gt = std::move(gt);
+  if (partial) ctx->d_score_partial = std::move(partial);
+  if (out) ctx->d_score_out = std::move(out);
+  if (curves) ctx->d_score_curves = std::move(curves);
+  if (diameter) ctx->d_diameter = std::move(diameter);
+  return M3TB_OK;
+}
+
+// Slices of the full set so that small batches still fill the device: (n_chunks, chunk) for `ctas` blocks per slice.
+static void ScoreSlices(const m3tb_ctx* ctx, long long ctas, int max_full, int* n_chunks, int* chunk) {
+  const int tiles = (max_full + kScoreTile - 1) / kScoreTile;
+  long long want = (2LL * ctx->sm_count + ctas - 1) / ctas;
+  const int c = int(std::max(1LL, std::min<long long>(want, tiles)));
+  const int tiles_per_chunk = (tiles + c - 1) / c;
+  *chunk = tiles_per_chunk * kScoreTile;
+  *n_chunks = (tiles + tiles_per_chunk - 1) / tiles_per_chunk;
+}
+
+void m3tb_score_params_default(m3tb_score_params* p) {
+  if (!p) return;
+  p->threshold_max = 0.1f;    // ycb_evaluator.h:46
+  p->curve_scale = 1.0f;
+  p->auc_scale = 1.0f;
+  p->translation_error_threshold = 0.05f;  // rbot_evaluator.h:192-193, kPi of common.h
+  p->rotation_error_threshold = 5.0f * 3.1415926535897f / 180.0f;
+}
+
+int m3tb_set_evaluation_model(m3tb_ctx* ctx, int model, const float* vertices, int n_vertices, int n_vertices_evaluation) {
+  CHECK_CTX();
+  if (model < 0 || model >= ctx->max_models || model > int(ctx->eval_models.size()))
+    return Fail(ctx, M3TB_ERR_INVALID, "evaluation model ids are dense (0..n) and below max_models");
+  if (!vertices || n_vertices < 1) return Fail(ctx, M3TB_ERR_INVALID, "an evaluation model needs vertices");
+  std::vector<float4> full(static_cast<size_t>(n_vertices));
+  for (int i = 0; i < n_vertices; ++i) {
+    const float* v = vertices + 3 * size_t(i);
+    if (!std::isfinite(v[0]) || !std::isfinite(v[1]) || !std::isfinite(v[2]))
+      return Fail(ctx, M3TB_ERR_INVALID, "evaluation vertex " + std::to_string(i) + " is not finite");
+    full[i] = make_float4(v[0], v[1], v[2], 0.0f);
+  }
+  // GenderateReducedVertices (ycb_evaluator.cpp:1222-1248)
+  std::vector<float4> reduced;
+  if (n_vertices_evaluation <= 0 || n_vertices_evaluation >= n_vertices) {
+    reduced = full;
+  } else {
+    std::mt19937 generator{7};
+    reduced.resize(size_t(n_vertices_evaluation));
+    for (auto& v : reduced) v = full[int(generator() % n_vertices)];
+  }
+  m3tb_ctx::EvalModelHost h;
+  CU(h.full.create(full.size()));
+  CU(h.reduced.create(reduced.size()));
+  h.n_full = int(full.size());
+  h.n_reduced = int(reduced.size());
+  CU(cudaMemcpyAsync(h.full, full.data(), sizeof(float4) * full.size(), cudaMemcpyHostToDevice, ctx->stream));
+  CU(cudaMemcpyAsync(h.reduced, reduced.data(), sizeof(float4) * reduced.size(), cudaMemcpyHostToDevice, ctx->stream));
+  CU(cudaStreamSynchronize(ctx->stream));  // the staging vectors end with this call
+  if (model == int(ctx->eval_models.size())) ctx->eval_models.push_back(std::move(h));
+  else ctx->eval_models[model] = std::move(h);
+  ctx->eval_dirty = true;
+  return M3TB_OK;
+}
+
+int m3tb_set_body_evaluation_model(m3tb_ctx* ctx, int body, int model, const float geometry2body[12]) {
+  CHECK_CTX();
+  if (body < 0 || body >= ctx->max_bodies) return Fail(ctx, M3TB_ERR_INVALID, "body index out of range");
+  if (model < 0 || model >= int(ctx->eval_models.size())) return Fail(ctx, M3TB_ERR_INVALID, "evaluation model not set");
+  EvalBodyDev e = {};
+  e.model = model;
+  e.has_geometry2body = geometry2body ? 1 : 0;
+  if (geometry2body) std::memcpy(e.geometry2body, geometry2body, sizeof(e.geometry2body));
+  EvalBodies(ctx)[body] = e;
+  ctx->eval_dirty = true;
+  return M3TB_OK;
+}
+
+int m3tb_get_evaluation_vertices(m3tb_ctx* ctx, int model, float* vertices, int capacity, int* n_vertices) {
+  CHECK_CTX();
+  if (model < 0 || model >= int(ctx->eval_models.size())) return Fail(ctx, M3TB_ERR_INVALID, "evaluation model not set");
+  if (capacity < 0 || (capacity > 0 && !vertices)) return Fail(ctx, M3TB_ERR_INVALID, "bad capacity");
+  const auto& h = ctx->eval_models[model];
+  if (n_vertices) *n_vertices = h.n_reduced;
+  const int n = std::min(capacity, h.n_reduced);
+  if (n == 0) return M3TB_OK;
+  std::vector<float4> v(static_cast<size_t>(n));
+  CU(cudaMemcpyAsync(v.data(), h.reduced, sizeof(float4) * n, cudaMemcpyDeviceToHost, ctx->stream));
+  CU(cudaStreamSynchronize(ctx->stream));
+  for (int i = 0; i < n; ++i) {
+    vertices[3 * i + 0] = v[i].x;
+    vertices[3 * i + 1] = v[i].y;
+    vertices[3 * i + 2] = v[i].z;
+  }
+  return M3TB_OK;
+}
+
+int m3tb_score_poses(m3tb_ctx* ctx, const int* bodies, int n, const float* gt_body2world, int gt_on_device,
+                     const m3tb_score_params* params, m3tb_pose_score* out, float* add_curve, float* adds_curve,
+                     int out_on_device) {
+  CHECK_CTX();
+  if (!bodies || n < 1 || !gt_body2world || !params || !out || (!add_curve) != (!adds_curve))
+    return Fail(ctx, M3TB_ERR_INVALID, "bad scoring arguments");
+  if (!(params->threshold_max > 0.0f) || !std::isfinite(params->threshold_max) || !(params->curve_scale > 0.0f) ||
+      !std::isfinite(params->curve_scale))
+    return Fail(ctx, M3TB_ERR_INVALID, "threshold_max and curve_scale must be finite and positive");
+  const auto& eb = EvalBodies(ctx);
+  int max_full = 0, max_reduced = 0;
+  for (int q = 0; q < n; ++q) {
+    const int b = bodies[q];
+    if (b < 0 || b >= ctx->max_bodies) return Fail(ctx, M3TB_ERR_INVALID, "body index out of range");
+    if (eb[b].model < 0) return Fail(ctx, M3TB_ERR_NOT_SET_UP, "body " + std::to_string(b) + " has no evaluation model");
+    const auto& m = ctx->eval_models[eb[b].model];
+    max_full = std::max(max_full, m.n_full);
+    max_reduced = std::max(max_reduced, m.n_reduced);
+  }
+  const int blocks = (max_reduced + kScoreBlock - 1) / kScoreBlock;
+  int n_chunks = 1, chunk = 0;
+  ScoreSlices(ctx, (long long)n * blocks, max_full, &n_chunks, &chunk);
+  const bool curves = add_curve != nullptr;
+  const size_t nq = size_t(n);
+  int rc = GrowScoreScratch(ctx, nq, gt_on_device ? 0 : 12 * nq, nq * size_t(n_chunks) * size_t(max_reduced),
+                            out_on_device ? 0 : nq, (out_on_device || !curves) ? 0 : 2 * M3TB_N_CURVE_VALUES * nq, 0);
+  if (!rc) rc = SyncEvalTables(ctx);
+  if (rc) return rc;
+  ScoreArgs a = {};
+  a.models = ctx->d_eval_models;
+  a.eval_bodies = ctx->d_eval_bodies;
+  a.poses = ctx->d_poses;
+  a.bodies = ctx->d_score_ids;
+  a.n = n;
+  a.n_chunks = n_chunks;
+  a.chunk = chunk;
+  a.max_reduced = max_reduced;
+  a.partial = ctx->d_score_partial;
+  a.threshold_max = params->threshold_max;
+  a.curve_scale = params->curve_scale;
+  a.auc_scale = params->auc_scale;
+  a.translation_threshold = params->translation_error_threshold;
+  a.rotation_threshold = params->rotation_error_threshold;
+  CU(cudaMemcpyAsync(ctx->d_score_ids, bodies, sizeof(int) * nq, cudaMemcpyHostToDevice, ctx->stream));
+  if (gt_on_device) {
+    a.gt = gt_body2world;
+  } else {
+    CU(cudaMemcpyAsync(ctx->d_score_gt, gt_body2world, sizeof(float) * 12 * nq, cudaMemcpyHostToDevice, ctx->stream));
+    a.gt = ctx->d_score_gt;
+  }
+  if (out_on_device) {
+    a.out = out;
+    a.add_curve = add_curve;
+    a.adds_curve = adds_curve;
+  } else {
+    a.out = ctx->d_score_out;
+    if (curves) {
+      a.add_curve = ctx->d_score_curves;
+      a.adds_curve = ctx->d_score_curves + M3TB_N_CURVE_VALUES * nq;
+    }
+  }
+  k_score<<<dim3(unsigned(n), unsigned(n_chunks), unsigned(blocks)), kScoreThreads, 0, ctx->stream>>>(a);
+  CU(cudaGetLastError());
+  ctx->launches++;
+  k_score_finish<<<unsigned(n), kScoreThreads, 0, ctx->stream>>>(a);
+  CU(cudaGetLastError());
+  ctx->launches++;
+  if (!out_on_device) {
+    CU(cudaMemcpyAsync(out, a.out, sizeof(m3tb_pose_score) * nq, cudaMemcpyDeviceToHost, ctx->stream));
+    if (curves) {
+      CU(cudaMemcpyAsync(add_curve, a.add_curve, sizeof(float) * M3TB_N_CURVE_VALUES * nq, cudaMemcpyDeviceToHost,
+                         ctx->stream));
+      CU(cudaMemcpyAsync(adds_curve, a.adds_curve, sizeof(float) * M3TB_N_CURVE_VALUES * nq, cudaMemcpyDeviceToHost,
+                         ctx->stream));
+    }
+    CU(cudaStreamSynchronize(ctx->stream));
+  }
+  return M3TB_OK;
+}
+
+int m3tb_calculate_diameters(m3tb_ctx* ctx, const int* models, int n, float* out) {
+  CHECK_CTX();
+  if (!models || n < 1 || !out) return Fail(ctx, M3TB_ERR_INVALID, "bad diameter arguments");
+  int max_full = 0;
+  for (int q = 0; q < n; ++q) {
+    if (models[q] < 0 || models[q] >= int(ctx->eval_models.size()))
+      return Fail(ctx, M3TB_ERR_INVALID, "evaluation model not set");
+    max_full = std::max(max_full, ctx->eval_models[models[q]].n_full);
+  }
+  const int blocks = (max_full + kScoreBlock - 1) / kScoreBlock;
+  int n_chunks = 1, chunk = 0;
+  ScoreSlices(ctx, (long long)n * blocks, max_full, &n_chunks, &chunk);
+  int rc = GrowScoreScratch(ctx, size_t(n), 0, 0, 0, 0, size_t(n));
+  if (!rc) rc = SyncEvalTables(ctx);
+  if (rc) return rc;
+  DiameterArgs a = {};
+  a.models = ctx->d_eval_models;
+  a.model_ids = ctx->d_score_ids;
+  a.n_chunks = n_chunks;
+  a.chunk = chunk;
+  a.max_sq = ctx->d_diameter;
+  CU(cudaMemcpyAsync(ctx->d_score_ids, models, sizeof(int) * size_t(n), cudaMemcpyHostToDevice, ctx->stream));
+  CU(cudaMemsetAsync(a.max_sq, 0, sizeof(unsigned) * size_t(n), ctx->stream));
+  k_diameter<<<dim3(unsigned(n), unsigned(n_chunks), unsigned(blocks)), kScoreThreads, 0, ctx->stream>>>(a);
+  CU(cudaGetLastError());
+  ctx->launches++;
+  std::vector<unsigned> bits(static_cast<size_t>(n));
+  CU(cudaMemcpyAsync(bits.data(), a.max_sq, sizeof(unsigned) * size_t(n), cudaMemcpyDeviceToHost, ctx->stream));
+  CU(cudaStreamSynchronize(ctx->stream));
+  for (int q = 0; q < n; ++q) {
+    float sq;
+    std::memcpy(&sq, &bits[q], sizeof(sq));
+    out[q] = std::sqrt(sq);
+  }
   return M3TB_OK;
 }
 

@@ -102,6 +102,7 @@ class Batch {
   int NextViewer() { return n_viewers_++; }
   int NextFullRenderer() { return n_full_renderers_++; }
   int NextFocusedNormalRenderer() { return n_focused_normal_renderers_++; }
+  int NextEvaluationModel() { return n_evaluation_models_++; }
   // every m3tb_update_viewers renders all viewers of the batch: read-backs older than the last update are stale
   void ViewersUpdated() { ++viewer_version_; }
   long viewer_version() const { return viewer_version_; }
@@ -137,7 +138,7 @@ class Batch {
  private:
   m3tb_ctx* ctx_ = nullptr;
   int max_bodies_ = 0, n_bodies_ = 0, n_renderers_ = 0, n_color_ = 0, n_depth_ = 0, n_rmodels_ = 0, n_dmodels_ = 0, n_structures_ = 0;
-  int n_viewers_ = 0, n_full_renderers_ = 0, n_focused_normal_renderers_ = 0;
+  int n_viewers_ = 0, n_full_renderers_ = 0, n_focused_normal_renderers_ = 0, n_evaluation_models_ = 0;
   long viewer_version_ = 0;
   long pose_version_ = 0;
   Key done_[kNPhases];
@@ -153,6 +154,7 @@ class Body {
   }
   const std::string& name() const { return name_; }
   int index() const { return index_; }
+  const std::shared_ptr<Batch>& batch() const { return batch_; }
   // Body::set_body2world_pose (body.cpp:85-90)
   bool set_body2world_pose(const Transform3fA& pose) {
     body2world_pose_ = pose;
@@ -2601,6 +2603,222 @@ class Refiner {
   int n_corr_iterations_, n_update_iterations_;
   std::vector<std::shared_ptr<Optimizer>> optimizer_ptrs_;
   bool set_up_ = false;
+};
+
+// ---- the evaluators' pose scoring (examples/{ycb,rtb,opt,rbot}_evaluator.cpp) -----------------------------------------
+// The evaluators' model data: the vertices of a body (Body::vertices()), the reduced set GenderateReducedVertices
+// draws from them, and the diameter CalculateDiameters computes. Bodies sharing a mesh share one EvaluationModel.
+class EvaluationModel {
+ public:
+  EvaluationModel(const std::string& name, const std::shared_ptr<Batch>& batch) : name_(name), batch_(batch) {
+    index_ = batch->NextEvaluationModel();
+  }
+  const std::string& name() const { return name_; }
+  int index() const { return index_; }
+  void set_n_vertices_evaluation(int n) { n_vertices_evaluation_ = n; }
+  void set_vertices(const std::vector<float>& vertices) { vertices_ = vertices; }  // [n][3], Body::vertices() order
+  bool SetUp() {
+    return Check(batch_->ctx(),
+                 m3tb_set_evaluation_model(batch_->ctx(), index_, vertices_.data(), int(vertices_.size() / 3),
+                                           n_vertices_evaluation_),
+                 "EvaluationModel::SetUp");
+  }
+  // scores `body` against this model; geometry2body: OPTEvaluator's kBody2Geometry2BodyPoseMap entry
+  bool AddBody(const Body& body, const Transform3fA* geometry2body = nullptr) {
+    return Check(batch_->ctx(),
+                 m3tb_set_body_evaluation_model(batch_->ctx(), body.index(), index_,
+                                                geometry2body ? geometry2body->data() : nullptr),
+                 "EvaluationModel::AddBody");
+  }
+  // the reduced set, read back from the device ([n][3])
+  std::vector<float> reduced_vertices() const {
+    int n = 0;
+    if (!Check(batch_->ctx(), m3tb_get_evaluation_vertices(batch_->ctx(), index_, nullptr, 0, &n), "reduced_vertices"))
+      return {};
+    std::vector<float> v(size_t(n) * 3);
+    Check(batch_->ctx(), m3tb_get_evaluation_vertices(batch_->ctx(), index_, v.data(), n, &n), "reduced_vertices");
+    return v;
+  }
+  // OPTEvaluator::CalculateDiameters for this model
+  bool CalculateDiameter(float* diameter) const {
+    return Check(batch_->ctx(), m3tb_calculate_diameters(batch_->ctx(), &index_, 1, diameter), "CalculateDiameters");
+  }
+
+ private:
+  std::string name_;
+  std::shared_ptr<Batch> batch_;
+  int index_ = 0;
+  int n_vertices_evaluation_ = -1;
+  std::vector<float> vertices_;
+};
+
+namespace detail {
+// One m3tb_score_poses call for bodies that share a batch, scored at their current device poses.
+inline bool ScorePoses(const std::vector<std::shared_ptr<Body>>& bodies, const std::vector<Transform3fA>& gt_body2world_poses,
+                       const m3tb_score_params& params, std::vector<m3tb_pose_score>* scores,
+                       std::vector<float>* add_curves, std::vector<float>* adds_curves, const char* what) {
+  if (bodies.empty() || bodies.size() != gt_body2world_poses.size()) {
+    std::cerr << what << ": one ground-truth pose per body" << std::endl;
+    return false;
+  }
+  m3tb_ctx* ctx = bodies[0]->batch()->ctx();
+  for (const auto& b : bodies)
+    if (b->batch() != bodies[0]->batch()) {
+      std::cerr << what << ": body " << b->name() << " belongs to another Batch than body " << bodies[0]->name()
+                << std::endl;
+      return false;
+    }
+  std::vector<int> ids;
+  std::vector<float> gt;
+  for (size_t i = 0; i < bodies.size(); ++i) {
+    ids.push_back(bodies[i]->index());
+    gt.insert(gt.end(), gt_body2world_poses[i].m, gt_body2world_poses[i].m + 12);
+  }
+  scores->resize(bodies.size());
+  if (add_curves) {
+    add_curves->resize(bodies.size() * M3TB_N_CURVE_VALUES);
+    adds_curves->resize(bodies.size() * M3TB_N_CURVE_VALUES);
+  }
+  return Check(ctx,
+               m3tb_score_poses(ctx, ids.data(), int(ids.size()), gt.data(), 0, &params, scores->data(),
+                                add_curves ? add_curves->data() : nullptr, add_curves ? adds_curves->data() : nullptr, 0),
+               what);
+}
+}  // namespace detail
+
+// YCBEvaluator::CalculatePoseResults (ycb_evaluator.cpp:803-848) for many bodies in one call: ADD / ADD-S AUC and curves
+// of each body's current pose against its ground truth.
+class YCBEvaluator {
+ public:
+  static constexpr size_t kNCurveValues = M3TB_N_CURVE_VALUES;
+  static constexpr float kThresholdMax = 0.1f;
+  struct Result {
+    float add_auc = 0.0f, adds_auc = 0.0f;
+    std::array<float, kNCurveValues> add_curve{}, adds_curve{};
+  };
+  static bool CalculatePoseResults(const std::vector<std::shared_ptr<Body>>& bodies,
+                                   const std::vector<Transform3fA>& gt_body2world_poses, std::vector<Result>* results) {
+    m3tb_score_params p;
+    m3tb_score_params_default(&p);
+    p.threshold_max = kThresholdMax;
+    std::vector<m3tb_pose_score> s;
+    std::vector<float> ca, cs;
+    if (!detail::ScorePoses(bodies, gt_body2world_poses, p, &s, &ca, &cs, "YCBEvaluator::CalculatePoseResults"))
+      return false;
+    results->resize(bodies.size());
+    for (size_t i = 0; i < bodies.size(); ++i) {
+      auto& r = (*results)[i];
+      r.add_auc = s[i].add_auc;
+      r.adds_auc = s[i].adds_auc;
+      std::copy(ca.begin() + i * kNCurveValues, ca.begin() + (i + 1) * kNCurveValues, r.add_curve.begin());
+      std::copy(cs.begin() + i * kNCurveValues, cs.begin() + (i + 1) * kNCurveValues, r.adds_curve.begin());
+    }
+    return true;
+  }
+};
+
+// RTBEvaluator::CalculatePoseResults (rtb_evaluator.cpp:930-989): per-body errors on the device, then the averages
+// over each combined body and over the combined bodies on the host, in the reference's order. `bodies` holds every
+// body the ids of ids_combined_bodies index, with its ground truth at the same position.
+class RTBEvaluator {
+ public:
+  static constexpr size_t kNCurveValues = M3TB_N_CURVE_VALUES;
+  struct Result {
+    float add_auc = 0.0f, adds_auc = 0.0f;
+    std::array<float, kNCurveValues> add_curve{}, adds_curve{};
+  };
+  static bool CalculatePoseResults(const std::vector<std::shared_ptr<Body>>& bodies,
+                                   const std::vector<Transform3fA>& gt_body2world_poses,
+                                   const std::vector<std::vector<int>>& ids_combined_bodies, float error_threshold,
+                                   Result* result) {
+    m3tb_score_params p;
+    m3tb_score_params_default(&p);
+    p.threshold_max = error_threshold;
+    std::vector<m3tb_pose_score> s;
+    if (!detail::ScorePoses(bodies, gt_body2world_poses, p, &s, nullptr, nullptr, "RTBEvaluator::CalculatePoseResults"))
+      return false;
+    float add_auc = 0.0f, adds_auc = 0.0f;
+    for (const auto& ids_combined_body : ids_combined_bodies) {
+      float add_error_combined_body = 0.0f, adds_error_combined_body = 0.0f;
+      for (int id : ids_combined_body) {
+        add_error_combined_body += s[size_t(id)].add_error;
+        adds_error_combined_body += s[size_t(id)].adds_error;
+      }
+      add_error_combined_body /= ids_combined_body.size();
+      adds_error_combined_body /= ids_combined_body.size();
+      add_auc += 1.0f - std::min(add_error_combined_body / error_threshold, 1.0f);
+      adds_auc += 1.0f - std::min(adds_error_combined_body / error_threshold, 1.0f);
+    }
+    add_auc /= ids_combined_bodies.size();
+    adds_auc /= ids_combined_bodies.size();
+    result->add_auc = add_auc;
+    result->adds_auc = adds_auc;
+    const float threshold_step = 1.0f / float(kNCurveValues);
+    std::fill(begin(result->add_curve), end(result->add_curve), 1.0f);
+    for (size_t i = 0; i < kNCurveValues; ++i) {
+      if (add_auc < threshold_step * (0.5f + float(i))) break;
+      result->add_curve[i] = 0.0f;
+    }
+    std::fill(begin(result->adds_curve), end(result->adds_curve), 1.0f);
+    for (size_t i = 0; i < kNCurveValues; ++i) {
+      if (adds_auc < threshold_step * (0.5f + float(i))) break;
+      result->adds_curve[i] = 0.0f;
+    }
+    return true;
+  }
+};
+
+// OPTEvaluator::CalculatePoseResults (opt_evaluator.cpp:462-488): the ADD curve and area under it, scaled by the
+// diameter of the body's evaluation model (CalculateDiameter) and with the geometry2body term given to AddBody. One call
+// scores bodies of one diameter.
+class OPTEvaluator {
+ public:
+  static constexpr size_t kNCurveValues = M3TB_N_CURVE_VALUES;
+  static constexpr float kThresholdMax = 0.2f;
+  struct Result {
+    float area_under_curve = 0.0f;
+    std::array<float, kNCurveValues> curve_values{};
+  };
+  static bool CalculatePoseResults(const std::vector<std::shared_ptr<Body>>& bodies,
+                                   const std::vector<Transform3fA>& gt_body2world_poses, float diameter,
+                                   std::vector<Result>* results) {
+    m3tb_score_params p;
+    m3tb_score_params_default(&p);
+    p.threshold_max = kThresholdMax;
+    p.curve_scale = diameter;
+    p.auc_scale = kThresholdMax;
+    std::vector<m3tb_pose_score> s;
+    std::vector<float> ca, cs;
+    if (!detail::ScorePoses(bodies, gt_body2world_poses, p, &s, &ca, &cs, "OPTEvaluator::CalculatePoseResults"))
+      return false;
+    results->resize(bodies.size());
+    for (size_t i = 0; i < bodies.size(); ++i) {
+      (*results)[i].area_under_curve = s[i].add_auc;
+      std::copy(ca.begin() + i * kNCurveValues, ca.begin() + (i + 1) * kNCurveValues, (*results)[i].curve_values.begin());
+    }
+    return true;
+  }
+};
+
+// RBOTEvaluator::CalculatePoseResults (rbot_evaluator.cpp:416-433): translation and rotation error and tracking success
+// (thresholds 0.05 m and 5 degrees).
+class RBOTEvaluator {
+ public:
+  struct Result {
+    float translation_error = 0.0f, rotation_error = 0.0f, tracking_success = 0.0f;
+  };
+  static bool CalculatePoseResults(const std::vector<std::shared_ptr<Body>>& bodies,
+                                   const std::vector<Transform3fA>& gt_body2world_poses, std::vector<Result>* results) {
+    m3tb_score_params p;
+    m3tb_score_params_default(&p);
+    std::vector<m3tb_pose_score> s;
+    if (!detail::ScorePoses(bodies, gt_body2world_poses, p, &s, nullptr, nullptr, "RBOTEvaluator::CalculatePoseResults"))
+      return false;
+    results->resize(bodies.size());
+    for (size_t i = 0; i < bodies.size(); ++i)
+      (*results)[i] = {s[i].translation_error, s[i].rotation_error, s[i].tracking_success};
+    return true;
+  }
 };
 
 }  // namespace m3t_b200

@@ -984,6 +984,60 @@ int m3tb_debug_region_model_view(m3tb_ctx* ctx, int body, const m3tb_associated_
 int m3tb_debug_closest_view(const float* orientations, int n_views, const float* queries, int n_queries,
                             const int* prev, int* out_scan, int* out_pruned, int* out_evaluated);
 
+/* ---- pose scoring (the evaluators' CalculatePoseResults, examples/{ycb,rtb,opt,rbot}_evaluator.cpp) ---------------- */
+#define M3TB_N_CURVE_VALUES 100  /* kNCurveValues of every evaluator */
+/* Stores evaluation model `model` (ids dense: 0 .. the number set, below max_models; bodies share models): the full
+ * vertex set `vertices` [n_vertices][3] in Body::vertices() order, which the nearest-neighbour search of ADD-S runs
+ * against, and the reduced set of GenderateReducedVertices (ycb_evaluator.cpp:1222-1248): every vertex when
+ * n_vertices_evaluation <= 0 or >= n_vertices, otherwise n_vertices_evaluation draws vertices[int(g() % n_vertices)]
+ * of a fresh std::mt19937 g{7}. The reference's use_random_seed seeds from the clock and is not offered. Refused
+ * (M3TB_ERR_INVALID, the model unchanged): bad id, NULL vertices, n_vertices < 1, a non-finite coordinate. */
+int m3tb_set_evaluation_model(m3tb_ctx* ctx, int model, const float* vertices, int n_vertices, int n_vertices_evaluation);
+/* Scores body `body` against evaluation model `model`; geometry2body (NULL: none) is the OPT evaluator's
+ * kBody2Geometry2BodyPoseMap term of its delta pose. */
+int m3tb_set_body_evaluation_model(m3tb_ctx* ctx, int body, int model, const float geometry2body[12]);
+/* Reads the reduced set back: *n_vertices receives its size, at most `capacity` vertices [.][3] are written (vertices
+ * may be NULL). */
+int m3tb_get_evaluation_vertices(m3tb_ctx* ctx, int model, float* vertices, int capacity, int* n_vertices);
+
+/* Curve and AUC scale, RBOT thresholds. YCB: threshold_max 0.1, curve_scale 1, auc_scale 1. OPT: threshold_max 0.2,
+ * curve_scale = the body's diameter, auc_scale 0.2. RTB scores each body with threshold_max = ErrorThreshold and
+ * averages on the host. */
+typedef struct m3tb_score_params {
+  float threshold_max;                /* 0.1 (YCBEvaluator::kThresholdMax) */
+  float curve_scale;                  /* 1 */
+  float auc_scale;                    /* 1 */
+  float translation_error_threshold;  /* 0.05 m (rbot_evaluator.h:192) */
+  float rotation_error_threshold;     /* 5 * kPi / 180 (rbot_evaluator.h:193) */
+} m3tb_score_params;
+void m3tb_score_params_default(m3tb_score_params* p);
+
+typedef struct m3tb_pose_score {
+  float add_error;          /* sum ||v - delta v|| / float(size) over the reduced set */
+  float adds_error;         /* sum sqrt(min_w ||delta v - w||^2) / float(size), w over the full set */
+  float add_auc;            /* auc_scale * (1 - std::min(error / (curve_scale * threshold_max), 1.0f)) */
+  float adds_auc;
+  float translation_error;  /* ||t - t_gt|| */
+  float rotation_error;     /* acos((trace(R^T R_gt) - 1) / 2), R = Transform3fA::rotation() */
+  float tracking_success;   /* 0 when either error is above its threshold, otherwise 1 (also for NaN errors) */
+} m3tb_pose_score;
+/* Scores the current device poses of bodies[0..n) against ground-truth body2world poses gt_body2world [n][12] (device
+ * memory when gt_on_device != 0), on the context's stream after the work enqueued before it (no read-back of the
+ * poses). delta = body2world.inverse() * gt, or (body2world * g2b).inverse() * gt * g2b with a geometry2body term. The
+ * curves [n][M3TB_N_CURVE_VALUES] start at 1 and are 0 up to the first threshold
+ * curve_scale * (threshold_max / 100) * (0.5 + i) the error falls below; add_curve / adds_curve may be NULL (both or
+ * neither). out and the curves are device memory when out_on_device != 0; otherwise the call synchronises. A NaN error
+ * gives a NaN AUC and a zero curve. As in nanoflann, a moved vertex whose distances are all NaN or infinite (a NaN or
+ * infinite pose) takes FLT_MAX as its squared ADD-S distance. Refused (M3TB_ERR_INVALID, nothing launched): bad body ids, a body without an
+ * evaluation model, n < 1, NULL gt / out / params, one curve pointer without the other, threshold_max or curve_scale
+ * not finite and positive. DESIGN.md §3 "k_score / k_score_finish / k_diameter" states what is computed. */
+int m3tb_score_poses(m3tb_ctx* ctx, const int* bodies, int n, const float* gt_body2world, int gt_on_device,
+                     const m3tb_score_params* params, m3tb_pose_score* out, float* add_curve, float* adds_curve,
+                     int out_on_device);
+/* OPTEvaluator::CalculateDiameters (opt_evaluator.cpp:580-599): the largest (v_i - v_j).norm() over all pairs of each
+ * model's full vertex set into out[n] (host memory; synchronises). Refused: bad or unset model ids, n < 1, NULL. */
+int m3tb_calculate_diameters(m3tb_ctx* ctx, const int* models, int n, float* out);
+
 #ifdef __cplusplus
 }
 #endif
